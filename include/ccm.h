@@ -285,10 +285,20 @@ uint64_t ccm_kernel_launches(void);
 int ccm_sim_topology(int n_gpus, int n_switches);
 /* key: "cc_mode" "ppcie_mode" "cc_supported" "ppcie_supported" "reset_ms"
  *      "boot_ms" "fail_op" (bitmask of ccm_sim_op) "stuck" (reset ignores staged)
- *      "cuda_ordinal" "scrub_inject" (fault drill: ccm_scrub_verify poisons that many bytes
- *      between the scrub and the read-back — first, unaligned, middle and last byte of each
- *      chunk — so the call must come back CCM_ERR_DIRTY with nonzero_bytes == min(value, 4 x
- *      chunks)).   dev = -1 applies to every device. */
+ *      "cuda_ordinal", and three fault drills of ccm_scrub_verify (0 = off; they only ever add
+ *      dirt, and only inside memory the call has mapped or allocated):
+ *      "scrub_inject"  dirties that many bytes between the scrub and the read-back: the first,
+ *                      byte 17, the middle + 3 and the last byte of each enqueued range (each once,
+ *                      in enqueue order).  The VMM path enqueues one range per main-zone chunk and
+ *                      one for all tail granules, or ONE range for the whole mapping when it maps
+ *                      first; the arena path one range per segment.  So the call comes back
+ *                      CCM_ERR_DIRTY with nonzero_bytes == min(value, 4 x ranges), fewer when a
+ *                      range is too short for four distinct bytes;
+ *      "scrub_poison"  (byte value) fills every physical chunk (arena: segment) right after it is
+ *                      mapped, before any scrub — the previous tenant: the call must stay clean;
+ *      "scrub_flood"   (byte value) fills every enqueued range between its scrub and its
+ *                      read-back: CCM_ERR_DIRTY with nonzero_bytes == bytes_scrubbed.
+ *      dev = -1 applies to every device. */
 int ccm_sim_set(int dev, const char* key, int64_t value);
 int ccm_sim_get(int dev, const char* key, int64_t* value);
 typedef enum ccm_sim_op {

@@ -56,7 +56,7 @@ struct Device {
   int reset_ms = 0, boot_ms = 0;
   uint32_t fail_mask = 0;  // ccm_sim_op bits that return CCM_ERR_FAULT
   bool stuck = false;      // reset does not apply staged values
-  uint64_t scrub_inject = 0;  // fault drill: bytes poisoned between scrub and read-back
+  ScrubDrill drill;        // fault drills of the scrub gate (ccm_internal.h)
   std::string sysfs_path;  // sysfs backend
 };
 
@@ -267,10 +267,13 @@ int cuda_ordinal_of(int dev) {
   return ord;
 }
 
-int sim_scrub_hook(int dev, uint64_t* inject) {
+static thread_local ScrubDrill t_scrub_drill;  // set for the duration of one scrub_verify_one
+const ScrubDrill& current_scrub_drill() { return t_scrub_drill; }
+
+int sim_scrub_hook(int dev, ScrubDrill* drill) {
   return with_dev(dev, [&](Device& d) {
     trace(d, "scrub", nullptr);
-    if (inject) *inject = g_backend == CCM_BACKEND_SYSFS ? 0 : d.scrub_inject;
+    if (drill) *drill = g_backend == CCM_BACKEND_SYSFS ? ScrubDrill() : d.drill;
     if (d.fail_mask & CCM_OP_SCRUB) { set_error("injected fault: scrub on %s", d.info.bdf); return (int)CCM_ERR_FAULT; }
     return (int)CCM_OK;
   });
@@ -484,11 +487,14 @@ static ScrubEngine* engine_of_ordinal(int ordinal, int* rc) {
 
 static int scrub_verify_one(int dev, uint64_t bytes, bool node_fanout, ccm_scrub_result* out) {
   if (out) { memset(out, 0, sizeof *out); out->bytes_requested = bytes; }
-  uint64_t inject = 0;
-  int rc = sim_scrub_hook(dev, &inject);
+  ScrubDrill drill;
+  int rc = sim_scrub_hook(dev, &drill);
   ScrubEngine* e = rc ? nullptr : engine_of_dev(dev, &rc);
   if (!e) { if (out) out->status = rc; return rc; }
-  return engine_scrub_verify(e, bytes, inject, node_fanout, out);
+  t_scrub_drill = drill;
+  rc = engine_scrub_verify(e, bytes, drill.inject, node_fanout, out);
+  t_scrub_drill = ScrubDrill();
+  return rc;
 }
 
 int ccm_scrub_verify(int dev, uint64_t bytes, ccm_scrub_result* out) { return scrub_verify_one(dev, bytes, false, out); }
@@ -633,7 +639,11 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
   else if (k == "stuck") d.stuck = v != 0;
   else if (k == "cuda_ordinal") d.info.cuda_ordinal = (int)v;
   else if (k == "booted") d.booted = v != 0;
-  else if (k == "scrub_inject") d.scrub_inject = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "scrub_inject") d.drill.inject = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "scrub_poison" || k == "scrub_flood") {
+    if (v < 0 || v > 255) { set_error("sim key '%s' takes a byte value (0 = off), not %lld", k.c_str(), (long long)v); return CCM_ERR_INVALID; }
+    (k == "scrub_poison" ? d.drill.poison : d.drill.flood) = (int)v;
+  }
   else { set_error("unknown sim key '%s'", k.c_str()); return CCM_ERR_INVALID; }
   return CCM_OK;
 }
@@ -669,7 +679,9 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "fail_op") *value = d.fail_mask;
     else if (k == "stuck") *value = d.stuck;
     else if (k == "cuda_ordinal") *value = d.info.cuda_ordinal;
-    else if (k == "scrub_inject") *value = (int64_t)d.scrub_inject;
+    else if (k == "scrub_inject") *value = (int64_t)d.drill.inject;
+    else if (k == "scrub_poison") *value = d.drill.poison;
+    else if (k == "scrub_flood") *value = d.drill.flood;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

@@ -35,8 +35,22 @@ int engine_arena_step_times(ScrubEngine*, int cap, float* scrub_ms, float* verif
 int engine_arena_fill(ScrubEngine*, int byte_value, void* stream);
 int engine_arena_fill_random(ScrubEngine*, uint64_t seed, void* stream);
 int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, bool write);
-// inject: fault drill (sim key "scrub_inject") — that many bytes are poisoned AFTER the scrub and
-// BEFORE the read-back (first / unaligned / middle / last byte of each chunk), so the verdict must be DIRTY.
+// Fault drills of the product call (sim keys "scrub_inject", "scrub_poison", "scrub_flood"; 0 = off).
+// They only ever ADD dirt, and only inside memory the call has already mapped (or allocated):
+//   inject: that many bytes are dirtied AFTER the scrub and BEFORE the read-back — first, +17,
+//           middle + 3 and last byte of each enqueued range (arena path: of each segment);
+//   poison: every physical chunk (arena path: segment) is filled with this byte right after it is
+//           mapped, before any scrub of it — the previous tenant; the verdict must be CLEAN;
+//   flood:  every enqueued range (arena path: segment) is filled with this byte between its scrub
+//           and its read-back; the verdict must be DIRTY with nonzero_bytes == bytes_scrubbed.
+struct ScrubDrill {
+  uint64_t inject = 0;
+  int poison = 0;
+  int flood = 0;
+};
+// inject: the call's "scrub_inject" budget.  Its poison and flood drills are those current_scrub_drill()
+// returns on the calling thread.  (The engine entry points keep the signatures that host-only builds of
+// ccm_core.cpp stub, tests/native/no_cuda_stub.cpp.)
 // node_fanout: the call is one of several running concurrently in THIS process (ccm_scrub_verify_many).
 int engine_scrub_verify(ScrubEngine*, uint64_t bytes, uint64_t inject, bool node_fanout, ccm_scrub_result* out);
 // Joins the background release of the last product call (no-op when none is pending).
@@ -55,8 +69,11 @@ int engine_teardown(int ordinal);
 // ---- implemented in ccm_core.cpp -------------------------------------------
 // Maps a device-table index to its CUDA ordinal (or a negative ccm_status).
 int cuda_ordinal_of(int dev);
-// sim fault hook for the scrub op (returns CCM_OK or CCM_ERR_FAULT) + trace line; *inject = the
-// device's "scrub_inject" drill value.
-int sim_scrub_hook(int dev, uint64_t* inject);
+// sim fault hook for the scrub op (returns CCM_OK or CCM_ERR_FAULT) + trace line; *drill = the
+// device's scrub drills (all off on the sysfs backend).
+int sim_scrub_hook(int dev, ScrubDrill* drill);
+// The drills of the product call running on this thread (all off outside such a call): the product
+// call is synchronous, one host thread per device call, so the thread identifies the call.
+const ScrubDrill& current_scrub_drill();
 
 }  // namespace ccm

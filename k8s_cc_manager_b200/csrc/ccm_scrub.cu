@@ -775,6 +775,37 @@ int engine_arena_rw(ScrubEngine* e, uint64_t offset, void* host, uint64_t bytes,
   return CCM_OK;
 }
 
+// Fault drill "scrub_inject" on one range [p, p+n): its first byte, byte 17, byte n/2 + 3 and its last
+// byte (each once, in that order) are dirtied while *budget lasts.  Writes only inside the range.
+static cudaError_t inject_dirt(uint8_t* p, uint64_t n, uint64_t* budget, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  const uint64_t cand[4] = {0, 17 < n ? uint64_t{17} : 0, n / 2 + 3 < n ? n / 2 + 3 : 0, n - 1};
+  for (int i = 0; i < 4 && *budget; ++i) {
+    bool dup = false;
+    for (int j = 0; j < i; ++j) dup |= cand[j] == cand[i];
+    if (dup) continue;
+    cudaError_t err = cudaMemsetAsync(p + cand[i], 0xA5, 1, st);
+    if (err != cudaSuccess) return err;
+    --*budget;
+  }
+  return cudaSuccess;
+}
+
+// Fault drills on the segments of the arena the product call's fallback path holds: every segment is
+// filled with `fill` (0 = no fill), then up to `inject` bytes are dirtied, 4 candidates per segment.
+static int arena_drill(ScrubEngine* e, int fill, uint64_t inject) {
+  if (!fill && !inject) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  int rc = need_arena(e); if (rc) return rc;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  for (auto& s : e->segs) {
+    if (fill) CCM_CUDA(cudaMemsetAsync(s.ptr, fill, s.bytes, e->stream));
+    if (inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &inject, e->stream));
+  }
+  return CCM_OK;
+}
+
 // ------------------------------------------------------- VMM (driver API, lazy)
 // The product call maps HBM in chunks through the virtual-memory-management API so
 // that (a) the chunks sit in ONE contiguous virtual range (one verify launch) and (b)
@@ -843,7 +874,8 @@ static bool async_release_enabled() { return env_u64("CCM_ASYNC_RELEASE", 1) != 
 //   next one (the GPU would otherwise idle while the driver maps);
 // * the verdict is returned as soon as the 8-byte count is on the host; cuMemUnmap/cuMemRelease
 //   (serialised node-wide by the driver) run on the engine's reaper thread.
-static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool node_fanout, ccm_scrub_result* r) {
+static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDrill& drill, bool node_fanout,
+                                  ccm_scrub_result* r) {
   const VmmApi& api = vmm();
   if (!api.ok) return CCM_ERR_UNSUPPORTED;
   std::lock_guard<std::mutex> g(e->mu);
@@ -897,6 +929,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, uint64_t injec
   int rc = CCM_OK;
   double host_acquire = 0;
   int timed = 0;  // chunks with an event triple (the first kMaxPipeChunks; a badly fragmented HBM may produce more)
+  uint64_t inject = drill.inject;  // one budget for all enqueued ranges, spent in enqueue order
 
   // enqueue scrub (+ read-back) of [off, off+n) with CUDA events around each kernel
   auto enqueue = [&](uint64_t off, uint64_t n) -> int {
@@ -904,16 +937,11 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, uint64_t injec
     if (evs) cudaEventRecord(evs[0], st);
     int rc2 = scrub_range(e, (void*)(m.base + off), n, CCM_SCRUB_AUTO, nullptr, st);
     if (evs) cudaEventRecord(evs[1], st);
-    if (inject) {  // fault drill: dirty bytes the read-back below MUST find
-      const uint64_t cand[4] = {off, off + 17 < off + n ? off + 17 : off, off + n / 2 + 3 < off + n ? off + n / 2 + 3 : off, off + n - 1};
-      for (int i = 0; i < 4 && inject; ++i) {
-        bool dup = false;
-        for (int j = 0; j < i; ++j) dup |= cand[j] == cand[i];
-        if (dup) continue;
-        cudaMemsetAsync((void*)(m.base + cand[i]), 0xA5, 1, st);
-        --inject;
-      }
-    }
+    // fault drills: dirt the read-back of this range MUST find
+    cudaError_t derr = cudaSuccess;
+    if (rc2 == CCM_OK && drill.flood) derr = cudaMemsetAsync((void*)(m.base + off), drill.flood, n, st);
+    if (rc2 == CCM_OK && derr == cudaSuccess && inject) derr = inject_dirt((uint8_t*)(m.base + off), n, &inject, st);
+    if (derr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(derr)); rc2 = CCM_ERR_CUDA; }
     if (rc2 == CCM_OK && interleave) rc2 = verify_range(e, (const void*)(m.base + off), n, CCM_VERIFY_AUTO, nullptr, st);
     if (evs) { cudaEventRecord(evs[2], st); ++timed; }
     return rc2;
@@ -957,6 +985,11 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, uint64_t injec
     host_acquire += now_ms() - t0;
     m.handles.push_back(h);
     m.mapped = off + n;
+    // fault drill: the previous tenant's data, in place before anything scrubs this chunk
+    if (drill.poison) {
+      cudaError_t perr = cudaMemsetAsync((void*)(m.base + off), drill.poison, n, st);
+      if (perr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(perr)); rc = CCM_ERR_CUDA; break; }
+    }
     // tail-zone granules are scrubbed with ONE launch pair once the zone is mapped
     if (!in_tail && !map_first) rc = enqueue(off, n);
     off += n;
@@ -1025,6 +1058,8 @@ int engine_release_wait(ScrubEngine* e, double* ms_release, double* ms_waited) {
 // --------------------------------------------------------------- product call
 int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool node_fanout, ccm_scrub_result* out) {
   const double t0 = now_ms();
+  ScrubDrill drill = current_scrub_drill();
+  drill.inject = inject;
   ccm_scrub_result r;
   memset(&r, 0, sizeof r);
   r.bytes_requested = bytes;
@@ -1032,9 +1067,10 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   r.scrub_variant = resolve_scrub_variant(CCM_SCRUB_AUTO);
   r.verify_variant = resolve_verify_variant(CCM_VERIFY_AUTO);
   int rc = CCM_ERR_UNSUPPORTED;
-  if (env_u64("CCM_PIPELINE", 1) != 0) rc = scrub_verify_pipelined(e, bytes, inject, node_fanout, &r);
+  if (env_u64("CCM_PIPELINE", 1) != 0) rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r);
   if (rc == CCM_ERR_UNSUPPORTED) {
-    // plain path: one cudaMalloc'ed arena, whole-arena scrub, whole-arena verify
+    // plain path: one cudaMalloc'ed arena, whole-arena scrub, whole-arena verify (the drills act per
+    // segment: poison before the scrub, flood + inject between the scrub and the verify)
     ccm_arena_info ai;
     rc = engine_arena_acquire(e, bytes, &ai);
     if (rc == CCM_OK) {
@@ -1046,7 +1082,9 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       r.segments = ai.segments;
       float ms_s = 0, ms_v = 0;
       uint64_t nz = 0;
-      rc = engine_arena_scrub(e, CCM_SCRUB_AUTO, nullptr, nullptr, &ms_s);
+      rc = arena_drill(e, drill.poison, 0);
+      if (rc == CCM_OK) rc = engine_arena_scrub(e, CCM_SCRUB_AUTO, nullptr, nullptr, &ms_s);
+      if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
       if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
       r.ms_scrub = ms_s;
       r.ms_verify = ms_v;
