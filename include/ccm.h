@@ -58,7 +58,8 @@ typedef enum ccm_status {
   CCM_ERR_NO_CUDA = -9,     /* no usable CUDA device behind this entry         */
   CCM_ERR_STATE = -10,      /* call out of order (e.g. no arena held)          */
   CCM_ERR_FAULT = -11,      /* fault injected by the sim backend               */
-  CCM_ERR_NOT_BOOTED = -12  /* device was reset and has not been waited for    */
+  CCM_ERR_NOT_BOOTED = -12, /* device was reset and has not been waited for    */
+  CCM_ERR_MISMATCH = -13    /* tagged gate: bytes did not hold their tag       */
 } ccm_status;
 
 /* ---- modes (string values of the reference: 'off' 'on' 'devtools') ------ */
@@ -214,6 +215,34 @@ int ccm_scrub_release_wait(int dev, double* ms_release, double* ms_waited);
 int ccm_scrub_verify_many(int n, const int* devs, uint64_t bytes,
                           ccm_scrub_result* out, double* wall_ms);
 
+/* ---- tagged gate: an address-tagged known answer before the zeroing -------
+ * A zero read-back cannot tell a byte the scrub zeroed from a byte that was already zero, or
+ * from a second virtual view of a physical byte zeroed elsewhere.  The tagged calls first write
+ * every mapped byte with a tag that depends on its virtual address and on a per-call seed (the
+ * word at address a holds lo32(a>>2)*0x9E3779B1 ^ hi32(a>>2)*0x85EBCA77 ^ seed; byte x is byte
+ * x&3 of the word at x&~3), each range as soon as it is mapped.  After the last mapping every
+ * range, in mapping order, is read back against its tags and zeroed in the same pass, and then
+ * read back for zeros as in ccm_scrub_verify.  A view that aliases another one, a store that
+ * does not land, or memory that was never written cannot hold the tag.  HBM traffic is about 4R
+ * instead of 2R (R = bytes mapped). */
+typedef struct ccm_tag_result {
+  uint32_t seed;               /* in: 0 = draw one (std::random_device); out: the seed used */
+  uint32_t reserved;
+  uint64_t mismatch_bytes;     /* EXACT count of bytes that did not hold their tag */
+  double ms_tag;               /* sum of the tag-fill kernels' CUDA-event times    */
+  double ms_check;             /* sum of the check-and-zero kernels' times          */
+  uint64_t va_base;            /* virtual address of the first byte scrubbed (the tags
+                                  are a function of it; 0 when nothing was mapped) */
+} ccm_tag_result;
+
+/* ccm_scrub_verify with the tagged check.  Returns CCM_ERR_MISMATCH when
+ * tag->mismatch_bytes != 0 (it takes precedence over CCM_ERR_DIRTY; both counts are
+ * reported), otherwise what ccm_scrub_verify returns. */
+int ccm_scrub_verify_tagged(int dev, uint64_t bytes, ccm_tag_result* tag, ccm_scrub_result* out);
+/* ccm_scrub_verify_many with the tagged check; tag[i] belongs to devs[i]. */
+int ccm_scrub_verify_many_tagged(int n, const int* devs, uint64_t bytes, ccm_tag_result* tag,
+                                 ccm_scrub_result* out, double* wall_ms);
+
 /* -- arena: the device-resident region, held across calls (bench / tests) -- */
 typedef struct ccm_arena_info {
   uint64_t bytes;              /* total bytes held                              */
@@ -253,6 +282,11 @@ int ccm_region_scrub(int cuda_ordinal, void* dptr, uint64_t bytes, int variant,
                      const ccm_launch_cfg* cfg, void* stream, float* ms);
 int ccm_region_verify(int cuda_ordinal, const void* dptr, uint64_t bytes, int variant,
                       const ccm_launch_cfg* cfg, void* stream, uint64_t* nonzero, float* ms);
+/* The tagged gate's two kernels on caller-owned memory: write the tags of `seed`, or count the
+ * bytes that differ from them (exact, synchronises) and zero the region in the same pass. */
+int ccm_region_tag_fill(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream, float* ms);
+int ccm_region_tag_check_zero(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream,
+                              uint64_t* mismatch, float* ms);
 /* Host-buffer round trip through the public path (tests, e2e): copies `bytes`
  * from host_buf to the device, counts non-zero bytes BEFORE (pre_nonzero, may be
  * NULL), scrubs, verifies, copies the region back into host_buf. */
@@ -298,6 +332,16 @@ int ccm_sim_topology(int n_gpus, int n_switches);
  *                      mapped, before any scrub — the previous tenant: the call must stay clean;
  *      "scrub_flood"   (byte value) fills every enqueued range between its scrub and its
  *                      read-back: CCM_ERR_DIRTY with nonzero_bytes == bytes_scrubbed.
+ *      Two drills of the tagged calls (ccm_scrub_verify_tagged; the zero-only call ignores them):
+ *      "tag_inject"    XORs that many bytes between the tag fill and the check, the same four
+ *                      candidates per enqueued range as "scrub_inject": CCM_ERR_MISMATCH with
+ *                      mismatch_bytes == min(value, 4 x ranges) and a clean zero read-back;
+ *      "scrub_alias"   (1 = on) maps the first n0 bytes of the second main-zone chunk from the
+ *                      first chunk's handle (n0 = the first chunk's size; when the second chunk
+ *                      is at least that large) instead of from fresh
+ *                      memory: two virtual views of one physical range, legal VMM use, no extra
+ *                      memory.  The zero gate passes it; the tagged gate must not.  VMM path only
+ *                      (the cudaMalloc fallback accepts the key and ignores it).
  *      dev = -1 applies to every device. */
 int ccm_sim_set(int dev, const char* key, int64_t value);
 int ccm_sim_get(int dev, const char* key, int64_t* value);

@@ -20,6 +20,7 @@
 #include <fstream>
 #include <memory>
 #include <mutex>
+#include <random>
 #include <shared_mutex>
 #include <sstream>
 #include <string>
@@ -269,6 +270,8 @@ int cuda_ordinal_of(int dev) {
 
 static thread_local ScrubDrill t_scrub_drill;  // set for the duration of one scrub_verify_one
 const ScrubDrill& current_scrub_drill() { return t_scrub_drill; }
+static thread_local ccm_tag_result* t_tag_call = nullptr;  // likewise; nullptr = zero-only call
+ccm_tag_result* current_tag_call() { return t_tag_call; }
 
 int sim_scrub_hook(int dev, ScrubDrill* drill) {
   return with_dev(dev, [&](Device& d) {
@@ -427,6 +430,7 @@ const char* ccm_strerror(int status) {
     case CCM_ERR_STATE: return "call out of order";
     case CCM_ERR_FAULT: return "injected fault";
     case CCM_ERR_NOT_BOOTED: return "device not booted since its last reset";
+    case CCM_ERR_MISMATCH: return "HBM bytes did not hold their address tag (tagged scrub gate)";
   }
   return "unknown ccm status";
 }
@@ -485,19 +489,38 @@ static ScrubEngine* engine_of_ordinal(int ordinal, int* rc) {
   return e;
 }
 
-static int scrub_verify_one(int dev, uint64_t bytes, bool node_fanout, ccm_scrub_result* out) {
+// tag: nullptr for the zero-only gate; otherwise the tagged gate runs, with tag->seed drawn here when 0.
+static int scrub_verify_one(int dev, uint64_t bytes, bool node_fanout, ccm_tag_result* tag, ccm_scrub_result* out) {
   if (out) { memset(out, 0, sizeof *out); out->bytes_requested = bytes; }
+  if (tag) {
+    const uint32_t seed = tag->seed;
+    memset(tag, 0, sizeof *tag);
+    tag->seed = seed;
+    if (tag->seed == 0) {
+      std::random_device rd;
+      while (tag->seed == 0) tag->seed = (uint32_t)rd();
+    }
+  }
   ScrubDrill drill;
   int rc = sim_scrub_hook(dev, &drill);
   ScrubEngine* e = rc ? nullptr : engine_of_dev(dev, &rc);
   if (!e) { if (out) out->status = rc; return rc; }
   t_scrub_drill = drill;
+  t_tag_call = tag;
   rc = engine_scrub_verify(e, bytes, drill.inject, node_fanout, out);
+  t_tag_call = nullptr;
   t_scrub_drill = ScrubDrill();
   return rc;
 }
 
-int ccm_scrub_verify(int dev, uint64_t bytes, ccm_scrub_result* out) { return scrub_verify_one(dev, bytes, false, out); }
+int ccm_scrub_verify(int dev, uint64_t bytes, ccm_scrub_result* out) {
+  return scrub_verify_one(dev, bytes, false, nullptr, out);
+}
+
+int ccm_scrub_verify_tagged(int dev, uint64_t bytes, ccm_tag_result* tag, ccm_scrub_result* out) {
+  if (!tag) return CCM_ERR_INVALID;
+  return scrub_verify_one(dev, bytes, false, tag, out);
+}
 
 int ccm_scrub_release_wait(int dev, double* ms_release, double* ms_waited) {
   if (ms_release) *ms_release = 0;
@@ -508,7 +531,8 @@ int ccm_scrub_release_wait(int dev, double* ms_release, double* ms_waited) {
   return e ? engine_release_wait(e, ms_release, ms_waited) : (int)CCM_OK;  // must not re-create a CUDA context
 }
 
-int ccm_scrub_verify_many(int n, const int* devs, uint64_t bytes, ccm_scrub_result* out, double* wall_ms) {
+static int scrub_verify_many(int n, const int* devs, uint64_t bytes, ccm_tag_result* tag, ccm_scrub_result* out,
+                             double* wall_ms) {
   if (n < 0 || (n > 0 && (!devs || !out))) return CCM_ERR_INVALID;
   const auto t0 = Clock::now();
   std::vector<std::thread> th;
@@ -516,7 +540,7 @@ int ccm_scrub_verify_many(int n, const int* devs, uint64_t bytes, ccm_scrub_resu
   th.reserve(n);
   for (int i = 0; i < n; ++i)
     th.emplace_back([&, i] {
-      int rc = scrub_verify_one(devs[i], bytes, n > 1, &out[i]);
+      int rc = scrub_verify_one(devs[i], bytes, n > 1, tag ? &tag[i] : nullptr, &out[i]);
       if (rc) errs[i] = last_error();
     });
   for (auto& t : th) t.join();
@@ -524,6 +548,16 @@ int ccm_scrub_verify_many(int n, const int* devs, uint64_t bytes, ccm_scrub_resu
   for (int i = 0; i < n; ++i)
     if (out[i].status != CCM_OK) { set_error("%s", errs[i].c_str()); return out[i].status; }
   return CCM_OK;
+}
+
+int ccm_scrub_verify_many(int n, const int* devs, uint64_t bytes, ccm_scrub_result* out, double* wall_ms) {
+  return scrub_verify_many(n, devs, bytes, nullptr, out, wall_ms);
+}
+
+int ccm_scrub_verify_many_tagged(int n, const int* devs, uint64_t bytes, ccm_tag_result* tag, ccm_scrub_result* out,
+                                 double* wall_ms) {
+  if (n > 0 && !tag) return CCM_ERR_INVALID;
+  return scrub_verify_many(n, devs, bytes, tag, out, wall_ms);
 }
 
 int ccm_arena_acquire(int dev, uint64_t bytes, ccm_arena_info* out) {
@@ -640,6 +674,8 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
   else if (k == "cuda_ordinal") d.info.cuda_ordinal = (int)v;
   else if (k == "booted") d.booted = v != 0;
   else if (k == "scrub_inject") d.drill.inject = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "tag_inject") d.drill.tag_inject = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "scrub_alias") d.drill.alias = v != 0;
   else if (k == "scrub_poison" || k == "scrub_flood") {
     if (v < 0 || v > 255) { set_error("sim key '%s' takes a byte value (0 = off), not %lld", k.c_str(), (long long)v); return CCM_ERR_INVALID; }
     (k == "scrub_poison" ? d.drill.poison : d.drill.flood) = (int)v;
@@ -682,6 +718,8 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "scrub_inject") *value = (int64_t)d.drill.inject;
     else if (k == "scrub_poison") *value = d.drill.poison;
     else if (k == "scrub_flood") *value = d.drill.flood;
+    else if (k == "tag_inject") *value = (int64_t)d.drill.tag_inject;
+    else if (k == "scrub_alias") *value = d.drill.alias;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

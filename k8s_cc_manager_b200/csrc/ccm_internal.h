@@ -43,10 +43,15 @@ int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, b
 //           mapped, before any scrub of it — the previous tenant; the verdict must be CLEAN;
 //   flood:  every enqueued range (arena path: segment) is filled with this byte between its scrub
 //           and its read-back; the verdict must be DIRTY with nonzero_bytes == bytes_scrubbed.
+// Drills of the tagged call (sim keys "tag_inject", "scrub_alias"; ccm.h):
+//   tag_inject: that many bytes are XORed between the tag fill and the check, same candidates as inject;
+//   alias:      the second main-zone chunk starts with a second view of the first chunk (VMM path only).
 struct ScrubDrill {
   uint64_t inject = 0;
   int poison = 0;
   int flood = 0;
+  uint64_t tag_inject = 0;
+  int alias = 0;
 };
 // inject: the call's "scrub_inject" budget.  Its poison and flood drills are those current_scrub_drill()
 // returns on the calling thread.  (The engine entry points keep the signatures that host-only builds of
@@ -75,5 +80,8 @@ int sim_scrub_hook(int dev, ScrubDrill* drill);
 // The drills of the product call running on this thread (all off outside such a call): the product
 // call is synchronous, one host thread per device call, so the thread identifies the call.
 const ScrubDrill& current_scrub_drill();
+// The tag block of the tagged product call running on this thread (its seed already drawn), or nullptr
+// for the zero-only call.  The engine writes the call's mismatch count and kernel times into it.
+ccm_tag_result* current_tag_call();
 
 }  // namespace ccm

@@ -87,10 +87,13 @@ static constexpr int kMaxPipeChunks = 32;
 // Word indices inside the engine's device control block (each on its own 64-byte line):
 //   [0] non-zero byte count of the current verify        [8] grab counter of the GENERIC kernels
 //   [16]/[24] grab + done of scrub_st256_fast_kernel      [32]/[40] grab + done of verify_ld256_fast_kernel
+//   [48]/[56] grab + done of tag_fill_kernel              [64]/[72] grab + done of tag_check_zero_kernel
+//   [80] mismatched byte count of the current tag check
 // The fast kernels hand their pair back zeroed (GrabCtl), so they never share words with the
 // generic kernels, whose counter is memset by the host before every launch.
-static constexpr int kCtlWords = 64;
+static constexpr int kCtlWords = 96;
 static constexpr int kGenericGrab = 8, kScrubGrab = 16, kScrubDone = 24, kVerifyGrab = 32, kVerifyDone = 40;
+static constexpr int kTagFillGrab = 48, kTagFillDone = 56, kTagCheckGrab = 64, kTagCheckDone = 72, kMismatch = 80;
 
 // One contiguous virtual range backed by VMM chunks (cuMemCreate / cuMemMap).
 struct VmmMapping {
@@ -106,9 +109,10 @@ struct ScrubEngine {
   int sm_count = 0;
   size_t smem_optin = 0;
   cudaStream_t stream = nullptr;   // the engine's own non-blocking stream
-  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t step_ev[kMaxSteps][3] = {};
   cudaEvent_t pipe_ev[kMaxPipeChunks][3] = {};
+  cudaEvent_t tag_ev[kMaxPipeChunks][2] = {};  // around the tag fills of the tagged product call
   int step_count = 0;
   unsigned long long* d_counter = nullptr;
   unsigned long long* h_counter = nullptr;  // pinned
@@ -126,6 +130,8 @@ struct ScrubEngine {
   cudaStream_t pick(void* s) const { return s ? (cudaStream_t)s : stream; }
   GrabCtl scrub_ctl() const { return GrabCtl{d_counter + kScrubGrab, d_counter + kScrubDone}; }
   GrabCtl verify_ctl() const { return GrabCtl{d_counter + kVerifyGrab, d_counter + kVerifyDone}; }
+  GrabCtl tag_fill_ctl() const { return GrabCtl{d_counter + kTagFillGrab, d_counter + kTagFillDone}; }
+  GrabCtl tag_check_ctl() const { return GrabCtl{d_counter + kTagCheckGrab, d_counter + kTagCheckDone}; }
   // Waits for the background release of the previous gate (no-op when none is pending).
   double join_reaper() {
     if (!reaper.joinable()) return 0.0;
@@ -141,6 +147,10 @@ static constexpr int kFastScrubThreads = 512, kFastScrubPer = 16;
 static constexpr int kFastVerifyThreads = 1024, kFastVerifyPer = 8;
 #define CCM_FAST_SCRUB scrub_st128_fast_kernel<kFastScrubThreads, kFastScrubPer, kPolDefault>
 #define CCM_FAST_VERIFY verify_ld128_fast_kernel<kFastVerifyThreads, kFastVerifyPer, kPolStreaming>
+// The tagged gate's kernels: 128 KiB per grab, one persistent 512-thread CTA per SM, 16 vectors per thread.
+static constexpr int kTagThreads = 512, kTagPer = 16;
+#define CCM_TAG_FILL tag_fill_kernel<kTagThreads, kTagPer>
+#define CCM_TAG_CHECK tag_check_zero_kernel<kTagThreads, kTagPer>
 
 const char* default_kernel_names() {
   static const std::string names = [] {
@@ -166,6 +176,7 @@ int ScrubEngine::init() {
   for (auto& e : ev) CCM_CUDA(cudaEventCreate(&e));
   for (auto& s : step_ev) for (auto& e : s) CCM_CUDA(cudaEventCreate(&e));
   for (auto& s : pipe_ev) for (auto& e : s) CCM_CUDA(cudaEventCreate(&e));
+  for (auto& s : tag_ev) for (auto& e : s) CCM_CUDA(cudaEventCreate(&e));
   CCM_CUDA(cudaMalloc(&d_counter, kCtlWords * sizeof(unsigned long long)));
   CCM_CUDA(cudaMemset(d_counter, 0, kCtlWords * sizeof(unsigned long long)));
   CCM_CUDA(cudaHostAlloc(&h_counter, 64, cudaHostAllocDefault));
@@ -174,6 +185,9 @@ int ScrubEngine::init() {
   cudaFuncAttributes fa;
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_FAST_SCRUB));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_FAST_VERIFY));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_TAG_FILL));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_TAG_CHECK));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, xor_byte_kernel));
   size_t fr = 0;
   CCM_CUDA(cudaMemGetInfo(&fr, &total_bytes));
   ready = true;
@@ -238,6 +252,7 @@ int engine_teardown(int ordinal) {
   for (auto& ev : e->ev) { if (ev) cudaEventDestroy(ev); ev = nullptr; }
   for (auto& st : e->step_ev) for (auto& ev : st) { if (ev) cudaEventDestroy(ev); ev = nullptr; }
   for (auto& st : e->pipe_ev) for (auto& ev : st) { if (ev) cudaEventDestroy(ev); ev = nullptr; }
+  for (auto& st : e->tag_ev) for (auto& ev : st) { if (ev) cudaEventDestroy(ev); ev = nullptr; }
   e->step_count = 0;
   if (e->d_counter) cudaFree(e->d_counter);
   if (e->h_counter) cudaFreeHost(e->h_counter);
@@ -525,6 +540,30 @@ static int verify_range(ScrubEngine* e, const void* p, uint64_t n, int variant, 
   return CCM_OK;
 }
 
+// Write the tags of `seed` over one range on `st` (no sync).
+static int tag_fill_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cudaStream_t st) {
+  if (n == 0) return CCM_OK;
+  const RegionSplit s = split_region(p, n, 16, 128);
+  const uint64_t nchunks = s.body_vecs * 16 / ((uint64_t)kTagThreads * kTagPer * 16);
+  const cudaError_t err = launch_fast(CCM_TAG_FILL, e->sm_count, kTagThreads, st, s, nchunks, e->tag_fill_ctl(), seed);
+  g_launches++;
+  if (err != cudaSuccess) { set_error("tag fill launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
+  return CCM_OK;
+}
+
+// Check one range against the tags of `seed` and zero it (no sync); the mismatch count accumulates
+// into d_counter[kMismatch].
+static int tag_check_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cudaStream_t st) {
+  if (n == 0) return CCM_OK;
+  const RegionSplit s = split_region(p, n, 16, 128);
+  const uint64_t nchunks = s.body_vecs * 16 / ((uint64_t)kTagThreads * kTagPer * 16);
+  const cudaError_t err = launch_fast(CCM_TAG_CHECK, e->sm_count, kTagThreads, st, s, nchunks, e->tag_check_ctl(),
+                                      seed, e->d_counter + kMismatch);
+  g_launches++;
+  if (err != cudaSuccess) { set_error("tag check launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
+  return CCM_OK;
+}
+
 // ----------------------------------------------------------------------- arena
 static constexpr uint64_t kMiB = 1ull << 20;
 
@@ -777,14 +816,23 @@ int engine_arena_rw(ScrubEngine* e, uint64_t offset, void* host, uint64_t bytes,
 
 // Fault drill "scrub_inject" on one range [p, p+n): its first byte, byte 17, byte n/2 + 3 and its last
 // byte (each once, in that order) are dirtied while *budget lasts.  Writes only inside the range.
-static cudaError_t inject_dirt(uint8_t* p, uint64_t n, uint64_t* budget, cudaStream_t st) {
+// xor_bytes ("tag_inject"): the bytes are XORed with 0xA5 instead of set to it, so a byte that held its
+// tag no longer does, whatever the tag.
+static cudaError_t inject_dirt(uint8_t* p, uint64_t n, uint64_t* budget, cudaStream_t st, bool xor_bytes = false) {
   if (n == 0) return cudaSuccess;
   const uint64_t cand[4] = {0, 17 < n ? uint64_t{17} : 0, n / 2 + 3 < n ? n / 2 + 3 : 0, n - 1};
   for (int i = 0; i < 4 && *budget; ++i) {
     bool dup = false;
     for (int j = 0; j < i; ++j) dup |= cand[j] == cand[i];
     if (dup) continue;
-    cudaError_t err = cudaMemsetAsync(p + cand[i], 0xA5, 1, st);
+    cudaError_t err = cudaSuccess;
+    if (xor_bytes) {
+      xor_byte_kernel<<<1, 1, 0, st>>>(p + cand[i]);
+      g_launches++;
+      err = cudaGetLastError();
+    } else {
+      err = cudaMemsetAsync(p + cand[i], 0xA5, 1, st);
+    }
     if (err != cudaSuccess) return err;
     --*budget;
   }
@@ -803,6 +851,35 @@ static int arena_drill(ScrubEngine* e, int fill, uint64_t inject) {
     if (fill) CCM_CUDA(cudaMemsetAsync(s.ptr, fill, s.bytes, e->stream));
     if (inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &inject, e->stream));
   }
+  return CCM_OK;
+}
+
+// Tagged pass of the product call's fallback path: tag every segment, then (after the "tag_inject"
+// drill) check and zero every segment.  Fills tag->mismatch_bytes, ->ms_tag, ->ms_check, ->va_base.
+static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inject) {
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  int rc = need_arena(e); if (rc) return rc;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  cudaStream_t st = e->stream;
+  CCM_CUDA(cudaMemsetAsync(e->d_counter + kMismatch, 0, sizeof(unsigned long long), st));
+  CCM_CUDA(cudaEventRecord(e->ev[0], st));
+  for (auto& s : e->segs) { rc = tag_fill_range(e, s.ptr, s.bytes, tag->seed, st); if (rc) return rc; }
+  CCM_CUDA(cudaEventRecord(e->ev[1], st));
+  for (auto& s : e->segs)
+    if (tag_inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &tag_inject, st, true));
+  CCM_CUDA(cudaEventRecord(e->ev[2], st));
+  for (auto& s : e->segs) { rc = tag_check_range(e, s.ptr, s.bytes, tag->seed, st); if (rc) return rc; }
+  CCM_CUDA(cudaEventRecord(e->ev[3], st));
+  CCM_CUDA(cudaMemcpyAsync(e->h_counter, e->d_counter + kMismatch, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  tag->mismatch_bytes = (uint64_t)*e->h_counter;
+  float a = 0, b = 0;
+  CCM_CUDA(cudaEventElapsedTime(&a, e->ev[0], e->ev[1]));
+  CCM_CUDA(cudaEventElapsedTime(&b, e->ev[2], e->ev[3]));
+  tag->ms_tag = a;
+  tag->ms_check = b;
+  tag->va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
   return CCM_OK;
 }
 
@@ -930,12 +1007,31 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   double host_acquire = 0;
   int timed = 0;  // chunks with an event triple (the first kMaxPipeChunks; a badly fragmented HBM may produce more)
   uint64_t inject = drill.inject;  // one budget for all enqueued ranges, spent in enqueue order
+  // Tagged gate: every mapping is tagged as soon as it is mapped, and the ranges are checked only after
+  // the LAST mapping — a view that aliases an earlier chunk has overwritten that chunk's tags by then.
+  ccm_tag_result* tag = current_tag_call();
+  uint64_t tag_inject = drill.tag_inject;
+  int tag_timed = 0;
+  std::vector<std::pair<uint64_t, uint64_t>> deferred;  // tagged: main-zone ranges, checked after the last mapping
+  auto tag_fill = [&](uint64_t off, uint64_t n) -> int {
+    cudaEvent_t* evs = tag_timed < kMaxPipeChunks ? e->tag_ev[tag_timed] : nullptr;
+    if (evs) cudaEventRecord(evs[0], st);
+    const int rc2 = tag_fill_range(e, (void*)(m.base + off), n, tag->seed, st);
+    if (evs) { cudaEventRecord(evs[1], st); ++tag_timed; }
+    return rc2;
+  };
 
-  // enqueue scrub (+ read-back) of [off, off+n) with CUDA events around each kernel
+  // enqueue scrub (+ read-back) of [off, off+n) with CUDA events around each kernel; in the tagged gate the
+  // scrub is the check-and-zero pass
   auto enqueue = [&](uint64_t off, uint64_t n) -> int {
+    if (tag && tag_inject) {
+      const cudaError_t ierr = inject_dirt((uint8_t*)(m.base + off), n, &tag_inject, st, true);
+      if (ierr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(ierr)); return CCM_ERR_CUDA; }
+    }
     cudaEvent_t* evs = timed < kMaxPipeChunks ? e->pipe_ev[timed] : nullptr;
     if (evs) cudaEventRecord(evs[0], st);
-    int rc2 = scrub_range(e, (void*)(m.base + off), n, CCM_SCRUB_AUTO, nullptr, st);
+    int rc2 = tag ? tag_check_range(e, (void*)(m.base + off), n, tag->seed, st)
+                  : scrub_range(e, (void*)(m.base + off), n, CCM_SCRUB_AUTO, nullptr, st);
     if (evs) cudaEventRecord(evs[1], st);
     // fault drills: dirt the read-back of this range MUST find
     cudaError_t derr = cudaSuccess;
@@ -948,6 +1044,8 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   };
 
   if (cudaMemsetAsync(e->d_counter, 0, sizeof(unsigned long long), st) != cudaSuccess) rc = CCM_ERR_CUDA;
+  if (tag && cudaMemsetAsync(e->d_counter + kMismatch, 0, sizeof(unsigned long long), st) != cudaSuccess) rc = CCM_ERR_CUDA;
+  bool aliased = false;  // "scrub_alias" drill done
   cudaEventRecord(e->ev[0], st);
   uint64_t off = 0, tail_start = 0;
   bool in_tail = false;
@@ -957,8 +1055,10 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     uint64_t& ck = in_tail ? tail_chunk : chunk;
     const uint64_t n = limit - off < ck ? limit - off : ck;
     const double t0 = now_ms();
-    CUmemGenericAllocationHandle h;
-    CUresult cr = api.Create(&h, n, &prop, 0);
+    // "scrub_alias" drill: the first chunk's handle backs the start of the second chunk as well
+    const uint64_t alias = drill.alias && !aliased && !in_tail && m.handles.size() == 1 && m.mapped <= n ? m.mapped : 0;
+    CUmemGenericAllocationHandle h = 0;
+    CUresult cr = alias == n ? CUDA_SUCCESS : api.Create(&h, n - alias, &prop, 0);
     if (cr == CUDA_ERROR_OUT_OF_MEMORY) {
       const uint64_t floor_bytes = in_tail ? gran : (64 * kMiB > gran ? 64 * kMiB : gran);
       if (ck > floor_bytes) { ck = (ck / 2) / gran * gran; if (ck < gran) ck = gran; continue; }  // fragmented / less free than reported
@@ -970,31 +1070,38 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
       rc = cr == CUDA_ERROR_OUT_OF_MEMORY ? CCM_ERR_NOMEM : CCM_ERR_CUDA;
       break;
     }
-    CUresult mr = api.Map(m.base + off, n, 0, h, 0);
-    if (mr == CUDA_SUCCESS) {
-      mr = api.SetAccess(m.base + off, n, &acc, 1);
-      if (mr != CUDA_SUCCESS) api.Unmap(m.base + off, n);
-    }
+    CUresult mr = CUDA_SUCCESS;
+    uint64_t in_map = 0;
+    if (alias) { mr = api.Map(m.base + off, alias, 0, m.handles[0], 0); if (mr == CUDA_SUCCESS) in_map = alias; }
+    if (mr == CUDA_SUCCESS && n > alias) { mr = api.Map(m.base + off + alias, n - alias, 0, h, 0); if (mr == CUDA_SUCCESS) in_map = n; }
+    if (mr == CUDA_SUCCESS) mr = api.SetAccess(m.base + off, n, &acc, 1);
     if (mr != CUDA_SUCCESS) {
-      api.Release(h);
+      if (in_map) api.Unmap(m.base + off, in_map);
+      if (n > alias) api.Release(h);
       if (mr == CUDA_ERROR_OUT_OF_MEMORY && in_tail) break;  // no room left for page tables: the region ends here
       set_error("cuMemMap/cuMemSetAccess failed: %d", (int)mr);
       rc = CCM_ERR_CUDA;
       break;
     }
     host_acquire += now_ms() - t0;
-    m.handles.push_back(h);
+    if (n > alias) m.handles.push_back(h);
+    aliased |= alias != 0;
     m.mapped = off + n;
     // fault drill: the previous tenant's data, in place before anything scrubs this chunk
     if (drill.poison) {
       cudaError_t perr = cudaMemsetAsync((void*)(m.base + off), drill.poison, n, st);
       if (perr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(perr)); rc = CCM_ERR_CUDA; break; }
     }
+    if (tag) rc = tag_fill(off, n);
     // tail-zone granules are scrubbed with ONE launch pair once the zone is mapped
-    if (!in_tail && !map_first) rc = enqueue(off, n);
+    if (rc == CCM_OK && !in_tail && !map_first) {
+      if (tag) deferred.emplace_back(off, n);
+      else rc = enqueue(off, n);
+    }
     off += n;
     if (!in_tail && chunk < max_chunk) { chunk *= 2; if (chunk > max_chunk) chunk = max_chunk; }
   }
+  for (const auto& d : deferred) if (rc == CCM_OK) rc = enqueue(d.first, d.second);
   if (rc == CCM_OK && map_first) { if (m.mapped) rc = enqueue(0, m.mapped); }
   else if (rc == CCM_OK && in_tail && m.mapped > tail_start) rc = enqueue(tail_start, m.mapped - tail_start);
   if (rc == CCM_OK && !interleave) {
@@ -1004,6 +1111,10 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   cudaEventRecord(e->ev[2], st);
   if (rc == CCM_OK &&
       cudaMemcpyAsync(e->h_counter, e->d_counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st) != cudaSuccess)
+    rc = CCM_ERR_CUDA;
+  if (rc == CCM_OK && tag &&
+      cudaMemcpyAsync(e->h_counter + 1, e->d_counter + kMismatch, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                      st) != cudaSuccess)
     rc = CCM_ERR_CUDA;
   cudaError_t serr = cudaStreamSynchronize(st);  // nothing may still touch the mapping below
   if (rc == CCM_OK && serr != cudaSuccess) { set_error("stream sync failed: %s", cudaGetErrorString(serr)); rc = CCM_ERR_CUDA; }
@@ -1029,6 +1140,18 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     r->ms_verify = ms_v;
     r->ms_gpu_span = span;
     r->nonzero_bytes = (uint64_t)*e->h_counter;
+    if (tag) {
+      float ms_t = 0;
+      for (int i = 0; i < tag_timed; ++i) {
+        float a = 0;
+        cudaEventElapsedTime(&a, e->tag_ev[i][0], e->tag_ev[i][1]);
+        ms_t += a;
+      }
+      tag->mismatch_bytes = (uint64_t)e->h_counter[1];
+      tag->ms_tag = ms_t;
+      tag->ms_check = ms_s;
+      tag->va_base = mapped ? (uint64_t)m.base : 0;
+    }
   }
   // ---- give the HBM back: on the reaper (default) or right here -----------------------
   if (rc == CCM_OK && async_release_enabled()) {
@@ -1060,6 +1183,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   const double t0 = now_ms();
   ScrubDrill drill = current_scrub_drill();
   drill.inject = inject;
+  ccm_tag_result* tag = current_tag_call();
   ccm_scrub_result r;
   memset(&r, 0, sizeof r);
   r.bytes_requested = bytes;
@@ -1083,7 +1207,12 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       float ms_s = 0, ms_v = 0;
       uint64_t nz = 0;
       rc = arena_drill(e, drill.poison, 0);
-      if (rc == CCM_OK) rc = engine_arena_scrub(e, CCM_SCRUB_AUTO, nullptr, nullptr, &ms_s);
+      if (rc == CCM_OK && tag) {
+        rc = arena_tag_check(e, tag, drill.tag_inject);
+        ms_s = (float)tag->ms_check;
+      } else if (rc == CCM_OK) {
+        rc = engine_arena_scrub(e, CCM_SCRUB_AUTO, nullptr, nullptr, &ms_s);
+      }
       if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
       if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
       r.ms_scrub = ms_s;
@@ -1093,7 +1222,11 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       if (rc == CCM_OK) rc = rc2;
     }
   }
-  if (rc == CCM_OK && r.nonzero_bytes != 0) {
+  if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) {
+    set_error("tagged scrub found %llu bytes that did not hold their tag (and %llu non-zero bytes after the zeroing) "
+              "on CUDA device %d", (unsigned long long)tag->mismatch_bytes, (unsigned long long)r.nonzero_bytes, e->ordinal);
+    rc = CCM_ERR_MISMATCH;
+  } else if (rc == CCM_OK && r.nonzero_bytes != 0) {
     set_error("scrub verify found %llu non-zero bytes on CUDA device %d", (unsigned long long)r.nonzero_bytes, e->ordinal);
     rc = CCM_ERR_DIRTY;
   }
@@ -1185,3 +1318,45 @@ int engine_host_roundtrip(ScrubEngine* e, void* host_buf, uint64_t bytes, uint64
 }
 
 }  // namespace ccm
+
+// ---------------------------------------------------- tagged kernels on raw regions
+// Defined here, next to the engine, rather than in ccm_core.cpp: they need nothing of the device table.
+using namespace ccm;
+
+extern "C" int ccm_region_tag_fill(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream, float* ms) {
+  ScrubEngine* e = engine_for(cuda_ordinal);
+  if (!e) return CCM_ERR_NO_CUDA;
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  cudaStream_t st = e->pick(stream);
+  if (ms) CCM_CUDA(cudaEventRecord(e->ev[0], st));
+  int rc = tag_fill_range(e, dptr, bytes, seed, st);
+  if (rc) return rc;
+  if (ms) {
+    CCM_CUDA(cudaEventRecord(e->ev[1], st));
+    CCM_CUDA(cudaEventSynchronize(e->ev[1]));
+    CCM_CUDA(cudaEventElapsedTime(ms, e->ev[0], e->ev[1]));
+  }
+  return CCM_OK;
+}
+
+extern "C" int ccm_region_tag_check_zero(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream,
+                                         uint64_t* mismatch, float* ms) {
+  ScrubEngine* e = engine_for(cuda_ordinal);
+  if (!e) return CCM_ERR_NO_CUDA;
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  cudaStream_t st = e->pick(stream);
+  CCM_CUDA(cudaMemsetAsync(e->d_counter + kMismatch, 0, sizeof(unsigned long long), st));
+  CCM_CUDA(cudaEventRecord(e->ev[0], st));
+  int rc = tag_check_range(e, dptr, bytes, seed, st);
+  if (rc) return rc;
+  CCM_CUDA(cudaEventRecord(e->ev[1], st));
+  CCM_CUDA(cudaMemcpyAsync(e->h_counter, e->d_counter + kMismatch, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  if (mismatch) *mismatch = (uint64_t)*e->h_counter;
+  if (ms) CCM_CUDA(cudaEventElapsedTime(ms, e->ev[0], e->ev[1]));
+  return CCM_OK;
+}

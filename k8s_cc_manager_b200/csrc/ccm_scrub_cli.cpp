@@ -1,9 +1,10 @@
 // ccm-scrub — native command-line front end of the HBM scrub gate (links libccm.so).
 //
-//   ccm-scrub [--bytes N] [--backend sim|cudasim|sysfs] (--all | --bdf <pci address> ...)
+//   ccm-scrub [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] (--all | --bdf <pci address> ...)
 //
-// Runs the concurrent gate (ccm_scrub_verify_many) and prints ONE JSON line with the same
-// fields as k8s_cc_manager_b200.devices.ScrubReport.  Exit 0: every GPU clean; 3: gate failed;
+// Runs the concurrent gate (ccm_scrub_verify_many, or ccm_scrub_verify_many_tagged with --check tagged)
+// and prints ONE JSON line with the same fields as k8s_cc_manager_b200.devices.ScrubReport (the
+// tagged-gate fields only with --check tagged).  Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
 // post-reset step.
@@ -16,19 +17,25 @@
 #include "ccm.h"
 
 static int usage(const char* argv0) {
-  fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] (--all | --bdf <bdf> ...)\n", argv0);
+  fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] (--all | --bdf <bdf> ...)\n",
+          argv0);
   return 2;
 }
 
 int main(int argc, char** argv) {
   std::vector<std::string> bdfs;
   unsigned long long bytes = 0;
-  bool all = false;
+  bool all = false, tagged = false;
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     if (a == "--all") all = true;
     else if (a == "--bdf" && i + 1 < argc) bdfs.emplace_back(argv[++i]);
     else if (a == "--bytes" && i + 1 < argc) bytes = strtoull(argv[++i], nullptr, 10);
+    else if (a == "--check" && i + 1 < argc) {
+      std::string c = argv[++i];
+      if (c != "zero" && c != "tagged") return usage(argv[0]);
+      tagged = c == "tagged";
+    }
     else if (a == "--backend" && i + 1 < argc) {
       std::string b = argv[++i];
       int be = b == "sim" ? CCM_BACKEND_SIM : b == "cudasim" ? CCM_BACKEND_CUDASIM : b == "sysfs" ? CCM_BACKEND_SYSFS : -1;
@@ -58,8 +65,10 @@ int main(int argc, char** argv) {
     }
   }
   std::vector<ccm_scrub_result> res(devs.size() ? devs.size() : 1);
+  std::vector<ccm_tag_result> tags(res.size());
   double wall_ms = 0;
-  ccm_scrub_verify_many((int)devs.size(), devs.data(), bytes, res.data(), &wall_ms);
+  if (tagged) ccm_scrub_verify_many_tagged((int)devs.size(), devs.data(), bytes, tags.data(), res.data(), &wall_ms);
+  else ccm_scrub_verify_many((int)devs.size(), devs.data(), bytes, res.data(), &wall_ms);
   bool clean = true;
   printf("{\"wall_ms\": %.3f, \"reports\": [", wall_ms);
   for (size_t i = 0; i < devs.size(); ++i) {
@@ -68,11 +77,18 @@ int main(int argc, char** argv) {
     printf("%s{\"bdf\": \"%s\", \"bytes_requested\": %llu, \"bytes_scrubbed\": %llu, \"device_total_bytes\": %llu, "
            "\"nonzero_bytes\": %llu, \"ms_acquire\": %.3f, \"ms_scrub\": %.3f, \"ms_verify\": %.3f, \"ms_release\": %.3f, "
            "\"ms_total\": %.3f, \"segments\": %d, \"status\": %d, \"release_deferred\": %d, "
-           "\"device_free_before\": %llu, \"bytes_unreached\": %llu, \"ms_release_wait\": %.3f, \"ms_gpu_span\": %.3f}",
+           "\"device_free_before\": %llu, \"bytes_unreached\": %llu, \"ms_release_wait\": %.3f, \"ms_gpu_span\": %.3f",
            i ? ", " : "", names[i].c_str(), (unsigned long long)r.bytes_requested, (unsigned long long)r.bytes_scrubbed,
            (unsigned long long)r.device_total_bytes, (unsigned long long)r.nonzero_bytes, r.ms_acquire, r.ms_scrub,
            r.ms_verify, r.ms_release, r.ms_total, r.segments, r.status, r.release_deferred,
            (unsigned long long)r.device_free_before, (unsigned long long)r.bytes_unreached, r.ms_release_wait, r.ms_gpu_span);
+    if (tagged) {
+      const ccm_tag_result& t = tags[i];
+      clean = clean && t.mismatch_bytes == 0;
+      printf(", \"check\": \"tagged\", \"tag_seed\": %u, \"mismatch_bytes\": %llu, \"ms_tag\": %.3f, \"ms_check\": %.3f",
+             t.seed, (unsigned long long)t.mismatch_bytes, t.ms_tag, t.ms_check);
+    }
+    printf("}");
   }
   printf("]}\n");
   fflush(stdout);  // the verdict is out BEFORE the contexts are torn down: a parent can act on it right away

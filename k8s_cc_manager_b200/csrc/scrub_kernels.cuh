@@ -27,6 +27,7 @@
 //   scrub_st128_fast_kernel / verify_ld128_fast_kernel   what AUTO launches (compile-time shape)
 //   scrub_st_kernel / verify_ld_kernel                   any shape / width / policy / schedule
 //   scrub_tma_kernel                                     cp.async.bulk stores from one zero tile
+//   tag_fill_kernel / tag_check_zero_kernel              the tagged gate's known-answer pass
 //   fill_pattern_kernel                                  seeded test pattern (tests only)
 #pragma once
 #include <cstdint>
@@ -554,6 +555,162 @@ verify_ld128_fast_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, unsigned 
   }
   block_accumulate(cnt, counter);
 }
+
+// ------------------------------------------------- address-tagged known answer
+// A zero read-back cannot tell a byte the scrub zeroed from one that was already zero, or from a
+// second virtual view of a byte zeroed elsewhere.  The tagged gate first writes a pattern that only
+// this call, at this virtual address, could have produced, and checks it before zeroing.
+//
+// tag(seed, a) of the 4-byte word at device address a (i = a >> 2):
+//     lo32(i) * kTagK1  ^  hi32(i) * kTagK2  ^  seed
+// A byte at address x is byte (x & 3) (little-endian) of tag(seed, x & ~3).  Both constants are odd,
+// so multiplying by them is a bijection mod 2^32:
+//   * within one 16 GiB-aligned window (hi32 fixed) distinct words get distinct tags;
+//   * a word and its alias at any non-zero multiple of 16 GiB (lo32 fixed) get distinct tags;
+//   * two seeds differ in every word by seed1 ^ seed2.
+// oracle/scrub_oracle.py (tag_bytes) restates this formula.
+constexpr uint32_t kTagK1 = 0x9E3779B1u;
+constexpr uint32_t kTagK2 = 0x85EBCA77u;
+
+__host__ __device__ __forceinline__ uint32_t tag_word(uint32_t seed, uint64_t a) {
+  const uint64_t i = a >> 2;
+  return ((uint32_t)i * kTagK1) ^ ((uint32_t)(i >> 32) * kTagK2) ^ seed;
+}
+
+__host__ __device__ __forceinline__ uint8_t tag_byte(uint32_t seed, uint64_t x) {
+  return (uint8_t)(tag_word(seed, x & ~3ull) >> (8 * (x & 3)));
+}
+
+// The four words of the 16-byte vector at the 16-aligned address a: one 32-bit multiply per pair of
+// constants per vector, then one add and one xor per word (hi32 is the same for all four words).
+__device__ __forceinline__ uint4 tag_vec(uint32_t seed, uint64_t a) {
+  const uint64_t i = a >> 2;
+  const uint32_t b = (uint32_t)i * kTagK1;
+  const uint32_t h = ((uint32_t)(i >> 32) * kTagK2) ^ seed;
+  return make_uint4(b ^ h, (b + kTagK1) ^ h, (b + 2 * kTagK1) ^ h, (b + 3 * kTagK1) ^ h);
+}
+
+__device__ __forceinline__ void st16(void* p, uint4 v) {
+  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+
+// Coherent streaming load: the check kernel writes every address it reads, so the read-only (.nc)
+// path of the verifier is not used here.
+__device__ __forceinline__ uint4 ld16_cs(const void* p) {
+  uint4 v;
+  asm volatile("ld.global.cs.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+  return v;
+}
+
+// Writes the tags over a region.  Shape and bookkeeping of scrub_st128_fast_kernel: persistent CTAs,
+// one THREADS * PER_THREAD * 16-byte chunk per grab, self-resetting GrabCtl, CTA 0 takes the ragged bytes.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS)
+tag_fill_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed) {
+  constexpr uint64_t kChunk = (uint64_t)THREADS * PER_THREAD * 16;
+  uint8_t* body = s.base + s.head;
+  __shared__ unsigned long long s_chunk[2];
+  pdl_wait();
+  if (threadIdx.x == 0) s_chunk[0] = atomicAdd(ctl.grab, 1ull);
+  __syncthreads();
+  int buf = 0;
+  for (;;) {
+    const uint64_t c = s_chunk[buf];
+    if (c >= nchunks) break;
+    unsigned long long nxt = 0;
+    if (threadIdx.x == 0) nxt = atomicAdd(ctl.grab, 1ull);
+    uint8_t* p = body + c * kChunk + threadIdx.x * 16u;
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) {
+      uint8_t* q = p + (uint32_t)u * THREADS * 16u;
+      st16(q, tag_vec(seed, (uint64_t)(uintptr_t)q));
+    }
+    if (threadIdx.x == 0) s_chunk[buf ^ 1] = nxt;
+    __syncthreads();
+    buf ^= 1;
+  }
+  pdl_launch_dependents();
+  if (threadIdx.x == 0) grab_release(ctl, nullptr);
+  for (uint64_t i = nchunks * (kChunk / 16) + (uint64_t)blockIdx.x * THREADS + threadIdx.x;
+       i < s.body_vecs; i += (uint64_t)gridDim.x * THREADS) {
+    uint8_t* q = body + i * 16;
+    st16(q, tag_vec(seed, (uint64_t)(uintptr_t)q));
+  }
+  if (blockIdx.x == 0) {
+    for (uint64_t i = threadIdx.x; i < s.head; i += THREADS) s.base[i] = tag_byte(seed, (uint64_t)(uintptr_t)(s.base + i));
+    uint8_t* t = body + s.body_vecs * 16;
+    for (uint64_t i = threadIdx.x; i < s.tail; i += THREADS) t[i] = tag_byte(seed, (uint64_t)(uintptr_t)(t + i));
+  }
+}
+
+// Reads the tags back, counts every byte that differs from them (exact, u64, one atomic per CTA into
+// *mismatch) and stores zero over the same addresses.  All PER_THREAD loads are in flight before any use.
+// The exact per-byte count is computed for every batch, branch-free, and the loaded words die before the
+// stores: on H100 this runs at 0.97x of a same-run device-to-device copy, where counting only batches whose
+// XOR is non-zero (verify_ld128_fast_kernel's trick) keeps the loaded words live across the stores and
+// runs at 0.75x (one H100 80GB HBM3, 700 W, 32 GiB region).  Chunks are taken in ascending order, so the
+// last stretch this kernel writes is the first one the descending zero read-back reads.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS)
+tag_check_zero_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed, unsigned long long* mismatch) {
+  constexpr uint64_t kChunk = (uint64_t)THREADS * PER_THREAD * 16;
+  uint8_t* body = s.base + s.head;
+  uint64_t cnt = 0;
+  __shared__ unsigned long long s_chunk[2];
+  pdl_wait();
+  if (threadIdx.x == 0) s_chunk[0] = atomicAdd(ctl.grab, 1ull);
+  __syncthreads();
+  int buf = 0;
+  for (;;) {
+    const uint64_t c = s_chunk[buf];
+    if (c >= nchunks) break;
+    unsigned long long nxt = 0;
+    if (threadIdx.x == 0) nxt = atomicAdd(ctl.grab, 1ull);
+    uint8_t* p = body + c * kChunk + threadIdx.x * 16u;
+    uint4 v[PER_THREAD];
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16_cs(p + (uint32_t)u * THREADS * 16u);  // all loads first
+    uint32_t n = 0;
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) {
+      const uint4 t = tag_vec(seed, (uint64_t)(uintptr_t)(p + (uint32_t)u * THREADS * 16u));
+      n += nonzero_bytes_in_word(v[u].x ^ t.x) + nonzero_bytes_in_word(v[u].y ^ t.y) +
+           nonzero_bytes_in_word(v[u].z ^ t.z) + nonzero_bytes_in_word(v[u].w ^ t.w);
+    }
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) st16(p + (uint32_t)u * THREADS * 16u, make_uint4(0, 0, 0, 0));
+    cnt += n;
+    if (threadIdx.x == 0) s_chunk[buf ^ 1] = nxt;
+    __syncthreads();
+    buf ^= 1;
+  }
+  pdl_launch_dependents();
+  if (threadIdx.x == 0) grab_release(ctl, nullptr);
+  for (uint64_t i = nchunks * (kChunk / 16) + (uint64_t)blockIdx.x * THREADS + threadIdx.x;
+       i < s.body_vecs; i += (uint64_t)gridDim.x * THREADS) {
+    uint8_t* q = body + i * 16;
+    uint4 v = ld16_cs(q);
+    const uint4 t = tag_vec(seed, (uint64_t)(uintptr_t)q);
+    st16(q, make_uint4(0, 0, 0, 0));
+    cnt += nonzero_bytes_in_word(v.x ^ t.x) + nonzero_bytes_in_word(v.y ^ t.y) + nonzero_bytes_in_word(v.z ^ t.z) +
+           nonzero_bytes_in_word(v.w ^ t.w);
+  }
+  if (blockIdx.x == 0) {
+    for (uint64_t i = threadIdx.x; i < s.head; i += THREADS) {
+      cnt += s.base[i] != tag_byte(seed, (uint64_t)(uintptr_t)(s.base + i));
+      s.base[i] = 0;
+    }
+    uint8_t* t = body + s.body_vecs * 16;
+    for (uint64_t i = threadIdx.x; i < s.tail; i += THREADS) {
+      cnt += t[i] != tag_byte(seed, (uint64_t)(uintptr_t)(t + i));
+      t[i] = 0;
+    }
+  }
+  block_accumulate(cnt, mismatch);
+}
+
+// Fault drill "tag_inject": flips bits of single bytes (XOR, so the byte can never keep its tag).
+__global__ void xor_byte_kernel(uint8_t* p) { *p ^= 0xA5; }
 
 // ------------------------------------------------------------ test scaffolding
 __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {

@@ -20,6 +20,7 @@ Errors: every non-zero ccm_status becomes a GpuError carrying `.status`.
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 from dataclasses import dataclass
 from typing import List, Sequence, Tuple
 
@@ -61,10 +62,16 @@ class ScrubReport:
     bytes_unreached: int = 0         # free HBM that could not be mapped (hence not scrubbed)
     ms_release_wait: float = 0.0     # waited for the previous call's deferred release
     ms_gpu_span: float = 0.0         # first scrub launch .. last verify done
+    # tagged gate only (check="tagged"; include/ccm.h: ccm_tag_result)
+    check: str = "zero"
+    tag_seed: int = 0                # seed of the address tags this call wrote
+    mismatch_bytes: int = 0          # bytes that did not hold their tag
+    ms_tag: float = 0.0              # tag-fill kernels
+    ms_check: float = 0.0            # check-and-zero kernels
 
     @property
     def clean(self) -> bool:
-        return self.status == N.OK and self.nonzero_bytes == 0
+        return self.status == N.OK and self.nonzero_bytes == 0 and self.mismatch_bytes == 0
 
     @property
     def coverage(self) -> float:
@@ -86,10 +93,34 @@ class ScrubReport:
         return self.bytes_scrubbed / self.ms_verify / 1e6 if self.ms_verify > 0 else 0.0
 
     @classmethod
-    def from_native(cls, bdf: str, r: N.ScrubResult) -> "ScrubReport":
-        return cls(bdf, r.bytes_requested, r.bytes_scrubbed, r.device_total_bytes, r.nonzero_bytes,
-                   r.ms_acquire, r.ms_scrub, r.ms_verify, r.ms_release, r.ms_total, r.segments, r.status,
-                   r.release_deferred, r.device_free_before, r.bytes_unreached, r.ms_release_wait, r.ms_gpu_span)
+    def from_native(cls, bdf: str, r: N.ScrubResult, tag: "N.TagResult | None" = None) -> "ScrubReport":
+        rep = cls(bdf, r.bytes_requested, r.bytes_scrubbed, r.device_total_bytes, r.nonzero_bytes,
+                  r.ms_acquire, r.ms_scrub, r.ms_verify, r.ms_release, r.ms_total, r.segments, r.status,
+                  r.release_deferred, r.device_free_before, r.bytes_unreached, r.ms_release_wait, r.ms_gpu_span)
+        if tag is not None:
+            rep.check, rep.tag_seed, rep.mismatch_bytes = "tagged", tag.seed, tag.mismatch_bytes
+            rep.ms_tag, rep.ms_check = tag.ms_tag, tag.ms_check
+        return rep
+
+    def as_json(self) -> dict:
+        """The report as the scrub workers print it: the tagged-gate fields only for a tagged call."""
+        d = dataclasses.asdict(self)
+        if self.check == "zero":
+            for name in TAG_FIELDS:
+                del d[name]
+        return d
+
+
+# ScrubReport fields that only a tagged call reports
+TAG_FIELDS = ("check", "tag_seed", "mismatch_bytes", "ms_tag", "ms_check")
+CHECKS = ("zero", "tagged")
+
+
+def _check_mode(check: str) -> bool:
+    """True for the tagged gate; ValueError for anything but 'zero' / 'tagged'."""
+    if check not in CHECKS:
+        raise ValueError(f"scrub check must be 'zero' or 'tagged', not {check!r}")
+    return check == "tagged"
 
 
 class NvidiaDevice:
@@ -144,13 +175,20 @@ class NvidiaDevice:
         _check(N.lib().ccm_wait_for_boot(self.index, timeout_ms), "wait_for_boot", self.bdf)
 
     # -- NEW: HBM scrub-and-verify ---------------------------------------------
-    def scrub_and_verify(self, nbytes: int = 0) -> ScrubReport:
+    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero") -> ScrubReport:
         """Zero-fills and reads back this GPU's HBM (nbytes=0: all the context can map).
+        check="tagged" first writes and checks an address-tagged known answer
+        (include/ccm.h: ccm_scrub_verify_tagged).
 
-        Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error)
-        or if any byte reads back non-zero.
+        Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
+        if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.
         """
         res = N.ScrubResult()
+        if _check_mode(check):
+            tag = N.TagResult()
+            rc = N.lib().ccm_scrub_verify_tagged(self.index, nbytes, C.byref(tag), C.byref(res))
+            _check(rc, "scrub_and_verify", self.bdf)
+            return ScrubReport.from_native(self.bdf, res, tag)
         rc = N.lib().ccm_scrub_verify(self.index, nbytes, C.byref(res))
         _check(rc, "scrub_and_verify", self.bdf)
         return ScrubReport.from_native(self.bdf, res)
@@ -195,17 +233,24 @@ def find_gpus() -> Tuple[List[NvidiaDevice], int]:
     return devices, len(devices)
 
 
-def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0) -> Tuple[List[ScrubReport], float]:
+def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
+                          check: str = "zero") -> Tuple[List[ScrubReport], float]:
     """Concurrent multi-context scrub of several GPUs through ONE native call
     (ccm_scrub_verify_many: one host thread + primary context + stream per GPU, no
-    peer access, no collective).  Returns (reports, wall_ms); never raises for a
-    per-device failure — inspect report.status / report.clean."""
+    peer access, no collective; check="tagged": ccm_scrub_verify_many_tagged).  Returns
+    (reports, wall_ms); never raises for a per-device failure — inspect report.status /
+    report.clean."""
+    tagged = _check_mode(check)
     n = len(devices)
     if n == 0:
         return [], 0.0
     idx = (C.c_int * n)(*[d.index for d in devices])
     res = (N.ScrubResult * n)()
     wall = C.c_double(0.0)
+    if tagged:
+        tags = (N.TagResult * n)()
+        N.lib().ccm_scrub_verify_many_tagged(n, idx, nbytes, tags, res, C.byref(wall))
+        return [ScrubReport.from_native(d.bdf, res[i], tags[i]) for i, d in enumerate(devices)], wall.value
     N.lib().ccm_scrub_verify_many(n, idx, nbytes, res, C.byref(wall))
     return [ScrubReport.from_native(d.bdf, res[i]) for i, d in enumerate(devices)], wall.value
 
@@ -258,11 +303,13 @@ class ScrubbingProxy:
         native = object.__getattribute__(self, "_native")
         return native.wait_scrub_released() if native is not None else (0.0, 0.0)
 
-    def scrub_and_verify(self, nbytes: int = 0) -> ScrubReport:
+    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero") -> ScrubReport:
         native = object.__getattribute__(self, "_native")
         if native is None:
             raise GpuError(f"no CUDA device with PCI address {self._foreign.bdf}: HBM scrub cannot run", N.ERR_NO_CUDA)
-        return native.scrub_and_verify(nbytes)
+        if check == "zero":
+            return native.scrub_and_verify(nbytes)   # exactly the call a zero-only device takes
+        return native.scrub_and_verify(nbytes, check=check)
 
 
 def _norm_bdf(bdf: str) -> str:

@@ -32,6 +32,7 @@ and never validates the mode string before touching hardware.
 from __future__ import annotations
 
 import argparse
+import inspect
 import logging
 import os
 import sys
@@ -101,7 +102,7 @@ class CCManager:
                  kubeconfig: str = "", v1=None,
                  device_source: Optional[Callable[[], tuple]] = None,
                  scrub_mode: Optional[str] = None, scrub_bytes: Optional[int] = None,
-                 max_parallel: Optional[int] = None):
+                 max_parallel: Optional[int] = None, scrub_check: Optional[str] = None):
         env = os.environ
         self.operator_namespace = env.get("OPERATOR_NAMESPACE", "gpu-operator")
         self.evict_operator_components = env.get("EVICT_OPERATOR_COMPONENTS", "true").lower() == "true"
@@ -129,6 +130,13 @@ class CCManager:
             raise ValueError("CC_SCRUB_BYTES != 0 scrubs only part of HBM; set CC_SCRUB_ALLOW_PARTIAL=true "
                              "to accept that (tests / drills), or leave it 0 for the full-HBM gate")
         self.scrub_bytes = int(scrub_bytes if scrub_bytes is not None else env.get("CC_SCRUB_BYTES", "0"))
+        # zero:   zero-fill + read-back.
+        # tagged: an address-tagged known answer is written and checked before the zeroing, so memory
+        #         the zeroing never reached (a second virtual view of one physical range, a store that
+        #         does not land) fails the gate too.  About twice the HBM traffic of 'zero'.
+        self.scrub_check = (scrub_check or env.get("CC_SCRUB_CHECK", "zero")).lower()
+        if self.scrub_check not in _devices.CHECKS:
+            raise ValueError(f"CC_SCRUB_CHECK must be 'zero' or 'tagged', not {self.scrub_check!r}")
         self.max_parallel = int(max_parallel if max_parallel is not None else env.get("CC_MAX_PARALLEL", "0"))
         # "full-HBM" is enforced, not assumed: when scrubbing everything (scrub_bytes == 0) a GPU on
         # which less than this fraction of DEVICE memory was zeroed and read back fails the gate
@@ -163,8 +171,8 @@ class CCManager:
             self.v1 = self._connect(kubeconfig)
         logger.info("Initialized CC Manager for node: %s", node_name)
         logger.info("Default CC mode: %s", default_mode or "(none)")
-        logger.info("HBM scrub gate: %s (bytes=%s, max_parallel=%s)", self.scrub_mode,
-                    self.scrub_bytes or "max", self.max_parallel or "all")
+        logger.info("HBM scrub gate: %s (bytes=%s, max_parallel=%s, check=%s)", self.scrub_mode,
+                    self.scrub_bytes or "max", self.max_parallel or "all", self.scrub_check)
 
     @staticmethod
     def _connect(kubeconfig: str):
@@ -510,6 +518,8 @@ class CCManager:
             cmd = [str(native_cli), "--bytes", str(self.scrub_bytes)]   # no interpreter start-up in the child
         else:
             cmd = [sys.executable, "-m", "k8s_cc_manager_b200.scrub_worker", "--bytes", str(self.scrub_bytes)]
+        if self.scrub_check != "zero":
+            cmd += ["--check", self.scrub_check]
         for gpu in gpus:
             cmd += ["--bdf", gpu.bdf]
         env = dict(os.environ)
@@ -523,6 +533,20 @@ class CCManager:
         payload = _json.loads(lines[-1])
         return [_devices.ScrubReport(**r) for r in payload["reports"]]
 
+    def _scrub_checked(self, gpu):
+        """The tagged gate on one device.  A device that cannot run it fails the gate: it is never
+        scrubbed zero-only in its place."""
+        try:
+            inspect.signature(gpu.scrub_and_verify).bind(self.scrub_bytes, check=self.scrub_check)
+        except (TypeError, ValueError):
+            raise ScrubFailure(f"device {gpu.bdf} cannot run the {self.scrub_check} HBM check "
+                               f"(CC_SCRUB_CHECK={self.scrub_check}); refusing to release it") from None
+        rep = gpu.scrub_and_verify(self.scrub_bytes, check=self.scrub_check)
+        if getattr(rep, "check", "zero") != self.scrub_check:
+            raise ScrubFailure(f"device {gpu.bdf} returned a {getattr(rep, 'check', 'zero')} scrub report for "
+                               f"CC_SCRUB_CHECK={self.scrub_check}; refusing to release it")
+        return rep
+
     def _run_scrub(self, gpus: list) -> None:
         started = time.perf_counter()
         if self.scrub_isolation == "process":
@@ -530,23 +554,32 @@ class CCManager:
         elif all(self._native_of(g) is not None for g in gpus) and self._workers(len(gpus)) == len(gpus):
             # ONE native call for the whole node (maps first, then launches: DESIGN.md §6) — also when the
             # register work belongs to a foreign library and libccm only scrubs (ScrubbingProxy)
-            reports, _ = _devices.scrub_and_verify_many([self._native_of(g) for g in gpus], self.scrub_bytes)
+            natives = [self._native_of(g) for g in gpus]
+            if self.scrub_check == "zero":
+                reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes)
+            else:
+                reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes, check=self.scrub_check)
             for rep, gpu in zip(reports, gpus):
                 rep.bdf = gpu.bdf
         else:
             def one(gpu):
                 if not hasattr(gpu, "scrub_and_verify"):
                     raise ScrubFailure(f"device {gpu.bdf} offers no HBM scrub; refusing to release it")
-                return gpu.scrub_and_verify(self.scrub_bytes)
+                if self.scrub_check == "zero":
+                    return gpu.scrub_and_verify(self.scrub_bytes)   # the call every scrubbing device takes
+                return self._scrub_checked(gpu)
             reports = self._fan_out(gpus, one, "scrub")
         elapsed = time.perf_counter() - started
         self.last_transition.setdefault("phase_seconds", {})["scrub"] = elapsed
         self.last_transition["scrub"] = reports
         for rep in reports:
-            if rep.status != 0 or rep.nonzero_bytes != 0:
+            mismatch = getattr(rep, "mismatch_bytes", 0)
+            if rep.status != 0 or rep.nonzero_bytes != 0 or mismatch != 0:
                 raise ScrubFailure(
                     f"HBM scrub failed on {rep.bdf}: status={rep.status} "
-                    f"nonzero_bytes={rep.nonzero_bytes} of {rep.bytes_scrubbed}")
+                    f"nonzero_bytes={rep.nonzero_bytes} of {rep.bytes_scrubbed}"
+                    + (f" mismatch_bytes={mismatch} (bytes that did not hold their address tag)"
+                       if self.scrub_check == "tagged" else ""))
             if self.scrub_bytes == 0 and rep.coverage < self.scrub_min_coverage:
                 raise ScrubFailure(
                     f"HBM scrub on {rep.bdf} covered only {100 * rep.coverage:.2f}% of device memory "
@@ -799,6 +832,9 @@ def build_arg_parser() -> argparse.ArgumentParser:
     parser.add_argument("--debug", action="store_true", help="Enable debug logging")
     parser.add_argument("--scrub-mode", default=None, choices=("require", "auto", "skip"),
                         help="HBM scrub gate after every CC transition (default: $CC_SCRUB_MODE or require)")
+    parser.add_argument("--scrub-check", default=None, choices=("zero", "tagged"),
+                        help="what the scrub gate checks: zero read-back, or an address-tagged known answer "
+                             "before it (default: $CC_SCRUB_CHECK or zero)")
     return parser
 
 
@@ -822,7 +858,7 @@ def main(argv: Optional[List[str]] = None) -> None:
 
     try:
         CCManager(node_name=args.node_name, default_mode=default_mode, host_cc=host_cc,
-                  kubeconfig=args.kubeconfig, scrub_mode=args.scrub_mode,
+                  kubeconfig=args.kubeconfig, scrub_mode=args.scrub_mode, scrub_check=args.scrub_check,
                   device_source=_device_source_from_env()).run()
     except KeyboardInterrupt:
         logger.info("Shutting down...")

@@ -8,12 +8,12 @@ concurrent gate (ccm_scrub_verify_many: one host thread + context + stream per G
 short-lived process and reads ONE JSON line back; the process exit returns every CUDA resource.
 
 Output (stdout, last line):  {"wall_ms": ..., "reports": [ {ScrubReport fields}, ... ]}
+(the tagged-gate fields only with --check tagged).
 Exit code: 0 if every GPU is clean, 3 if the gate failed, 2 on usage errors.
 """
 from __future__ import annotations
 
 import argparse
-import dataclasses
 import json
 import sys
 from typing import List, Optional
@@ -22,13 +22,13 @@ from . import _native as N
 from . import devices as D
 
 
-def run(bdfs: List[str], nbytes: int) -> dict:
+def run(bdfs: List[str], nbytes: int, check: str = "zero") -> dict:
     by_bdf = {d.bdf: d for d in D.find_gpus()[0] if d.is_gpu()}
     missing = [b for b in bdfs if b not in by_bdf]
     if missing:
         raise SystemExit(f"unknown GPU(s): {', '.join(missing)} (known: {', '.join(sorted(by_bdf))})")
-    reports, wall_ms = D.scrub_and_verify_many([by_bdf[b] for b in bdfs], nbytes)
-    return {"wall_ms": wall_ms, "reports": [dataclasses.asdict(r) for r in reports]}
+    reports, wall_ms = D.scrub_and_verify_many([by_bdf[b] for b in bdfs], nbytes, check=check)
+    return {"wall_ms": wall_ms, "reports": [r.as_json() for r in reports]}
 
 
 def main(argv: Optional[List[str]] = None) -> int:
@@ -36,14 +36,17 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap.add_argument("--bdf", action="append", default=[], help="PCI address of a GPU to scrub (repeatable)")
     ap.add_argument("--bytes", type=int, default=0, help="bytes per GPU (0 = all mappable HBM)")
     ap.add_argument("--backend", choices=sorted(N.BACKENDS), default=None)
+    ap.add_argument("--check", choices=D.CHECKS, default="zero",
+                    help="zero: zero-fill + read-back; tagged: an address-tagged known answer first")
     args = ap.parse_args(argv)
     if not args.bdf:
         ap.error("at least one --bdf is required")
     if args.backend:
         D.select_backend(args.backend)
-    out = run([b.lower() for b in args.bdf], args.bytes)
+    out = run([b.lower() for b in args.bdf], args.bytes, args.check)
     print(json.dumps(out), flush=True)
-    return 0 if all(r["status"] == 0 and r["nonzero_bytes"] == 0 for r in out["reports"]) else 3
+    return 0 if all(r["status"] == 0 and r["nonzero_bytes"] == 0 and r.get("mismatch_bytes", 0) == 0
+                    for r in out["reports"]) else 3
 
 
 if __name__ == "__main__":
