@@ -86,14 +86,14 @@ static constexpr int kMaxPipeChunks = 32;
 
 // Word indices inside the engine's device control block (each on its own 64-byte line):
 //   [0] non-zero byte count of the current verify        [8] grab counter of the GENERIC kernels
-//   [16]/[24] grab + done of scrub_st256_fast_kernel      [32]/[40] grab + done of verify_ld256_fast_kernel
+//   [16]/[24] grab + done of scrub_st128_fast_kernel      [32]/[40] grab + done of verify_ld128_fast_kernel
 //   [48]/[56] grab + done of tag_fill_kernel              [64]/[72] grab + done of tag_check_zero_kernel
 //   [80] mismatched byte count of the current tag check
-// The fast kernels hand their pair back zeroed (GrabCtl), so they never share words with the
+// The default kernels hand their pair back zeroed (GrabCtl), so they never share words with the
 // generic kernels, whose counter is memset by the host before every launch.
 static constexpr int kCtlWords = 96;
-static constexpr int kGenericGrab = 8, kScrubGrab = 16, kScrubDone = 24, kVerifyGrab = 32, kVerifyDone = 40;
-static constexpr int kTagFillGrab = 48, kTagFillDone = 56, kTagCheckGrab = 64, kTagCheckDone = 72, kMismatch = 80;
+static constexpr int kNonzero = 0, kGenericGrab = 8, kScrubGrab = 16, kVerifyGrab = 32, kTagFillGrab = 48,
+                     kTagCheckGrab = 64, kMismatch = 80;
 
 // One contiguous virtual range backed by VMM chunks (cuMemCreate / cuMemMap).
 struct VmmMapping {
@@ -128,10 +128,8 @@ struct ScrubEngine {
 
   int init();
   cudaStream_t pick(void* s) const { return s ? (cudaStream_t)s : stream; }
-  GrabCtl scrub_ctl() const { return GrabCtl{d_counter + kScrubGrab, d_counter + kScrubDone}; }
-  GrabCtl verify_ctl() const { return GrabCtl{d_counter + kVerifyGrab, d_counter + kVerifyDone}; }
-  GrabCtl tag_fill_ctl() const { return GrabCtl{d_counter + kTagFillGrab, d_counter + kTagFillDone}; }
-  GrabCtl tag_check_ctl() const { return GrabCtl{d_counter + kTagCheckGrab, d_counter + kTagCheckDone}; }
+  // the grab word of a default kernel and its done word, one line further on
+  GrabCtl ctl(int grab) const { return GrabCtl{d_counter + grab, d_counter + grab + 8}; }
   // Waits for the background release of the previous gate (no-op when none is pending).
   double join_reaper() {
     if (!reaper.joinable()) return 0.0;
@@ -268,35 +266,25 @@ int engine_teardown(int ordinal) {
 // ------------------------------------------------------------- launch shapes
 struct Shape { int ctas_per_sm, threads, unroll, policy, tile_bytes, schedule; };  // schedule: 1 static, 2 dynamic
 
+// The defaults `s` with every field that `c` sets taken from `c`.
+static Shape with_cfg(Shape s, const ccm_launch_cfg* c) {
+  if (c) {
+    if (c->ctas_per_sm > 0) s.ctas_per_sm = c->ctas_per_sm;
+    if (c->threads_per_cta > 0) s.threads = c->threads_per_cta;
+    if (c->unroll > 0) s.unroll = c->unroll;
+    if (c->cache_policy >= 1 && c->cache_policy <= 4) s.policy = c->cache_policy - 1;
+    if (c->tile_bytes > 0) s.tile_bytes = c->tile_bytes;
+    if (c->schedule >= 1 && c->schedule <= 3) s.schedule = c->schedule;
+  }
+  return s;
+}
+
 // Defaults of the generic kernels: persistent CTAs + dynamic chunk grabs (benchmarks/tune_scrub.py
 // sweeps the alternatives).
 static Shape scrub_shape(int variant, const ccm_launch_cfg* c) {
-  Shape s;
-  if (variant == CCM_SCRUB_TMA) s = Shape{1, 32, 1, kPolDefault, 65536, 2};
-  else s = Shape{1, 512, 4, kPolDefault, 131072, 2};
-  if (c) {
-    if (c->ctas_per_sm > 0) s.ctas_per_sm = c->ctas_per_sm;
-    if (c->threads_per_cta > 0) s.threads = c->threads_per_cta;
-    if (c->unroll > 0) s.unroll = c->unroll;
-    if (c->cache_policy >= 1 && c->cache_policy <= 4) s.policy = c->cache_policy - 1;
-    if (c->tile_bytes > 0) s.tile_bytes = c->tile_bytes;
-    if (c->schedule >= 1 && c->schedule <= 3) s.schedule = c->schedule;
-  }
-  return s;
+  return with_cfg(variant == CCM_SCRUB_TMA ? Shape{1, 32, 1, kPolDefault, 65536, 2} : Shape{1, 512, 4, kPolDefault, 131072, 2}, c);
 }
-static Shape verify_shape(int variant, const ccm_launch_cfg* c) {
-  (void)variant;
-  Shape s = Shape{1, 1024, 4, kPolStreaming, 131072, 2};
-  if (c) {
-    if (c->ctas_per_sm > 0) s.ctas_per_sm = c->ctas_per_sm;
-    if (c->threads_per_cta > 0) s.threads = c->threads_per_cta;
-    if (c->unroll > 0) s.unroll = c->unroll;
-    if (c->cache_policy >= 1 && c->cache_policy <= 4) s.policy = c->cache_policy - 1;
-    if (c->tile_bytes > 0) s.tile_bytes = c->tile_bytes;
-    if (c->schedule >= 1 && c->schedule <= 3) s.schedule = c->schedule;
-  }
-  return s;
-}
+static Shape verify_shape(const ccm_launch_cfg* c) { return with_cfg(Shape{1, 1024, 4, kPolStreaming, 131072, 2}, c); }
 
 // AUTO = the compile-time-shape 128-bit kernels (CCM_FAST_SCRUB / CCM_FAST_VERIFY).  A deployment can
 // pin another variant with CCM_SCRUB_VARIANT (st128 | st256 | tma | memset) and CCM_VERIFY_VARIANT
@@ -401,11 +389,17 @@ static bool pdl_enabled() {
   static const bool on = [] { const char* v = getenv("CCM_PDL"); return v && *v && strcmp(v, "0") != 0; }();
   return on;
 }
+
+// Launches a default-shape kernel (default_kernel in scrub_kernels.cuh) over `s`, with that attribute when
+// enabled: one persistent CTA per SM, whole chunks of `threads` x `per_thread` 16-byte vectors, the GrabCtl
+// pair at control-block word `grab`.
 template <typename... KArgs, typename... Args>
-static cudaError_t launch_fast(void (*kernel)(KArgs...), int grid, int threads, cudaStream_t st, Args... args) {
+static cudaError_t launch_fast(void (*kernel)(RegionSplit, uint64_t, GrabCtl, KArgs...), int threads, int per_thread,
+                               ScrubEngine* e, int grab, cudaStream_t st, const RegionSplit& s, Args... args) {
+  const uint64_t nchunks = s.body_vecs * 16 / ((uint64_t)threads * per_thread * 16);
   cudaLaunchConfig_t lc;
   memset(&lc, 0, sizeof lc);
-  lc.gridDim = dim3((unsigned)grid);
+  lc.gridDim = dim3((unsigned)e->sm_count);
   lc.blockDim = dim3((unsigned)threads);
   lc.stream = st;
   cudaLaunchAttribute attr[1];
@@ -413,7 +407,7 @@ static cudaError_t launch_fast(void (*kernel)(KArgs...), int grid, int threads, 
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = attr;
   lc.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&lc, kernel, KArgs(args)...);
+  return cudaLaunchKernelEx(&lc, kernel, s, nchunks, e->ctl(grab), KArgs(args)...);
 }
 
 // True when (variant, cfg) resolves to the compile-time-shape default kernel.
@@ -442,8 +436,7 @@ static int scrub_range(ScrubEngine* e, void* p, uint64_t n, int variant, const c
       if (cfg == nullptr) {
         // library default: compile-time shape (one persistent 512-thread CTA per SM, 16 x STG.128 per
         // thread per 128 KiB grab) — scrub_st128_fast_kernel
-        const uint64_t nchunks = s.body_vecs * 16 / ((uint64_t)kFastScrubThreads * kFastScrubPer * 16);
-        err = launch_fast(CCM_FAST_SCRUB, e->sm_count, kFastScrubThreads, st, s, nchunks, e->scrub_ctl(), zero_on_exit);
+        err = launch_fast(CCM_FAST_SCRUB, kFastScrubThreads, kFastScrubPer, e, kScrubGrab, st, s, zero_on_exit);
         g_launches++;
         break;
       }
@@ -501,7 +494,7 @@ static int verify_range(ScrubEngine* e, const void* p, uint64_t n, int variant, 
                         cudaStream_t st) {
   if (n == 0) return CCM_OK;
   variant = resolve_verify_variant(variant);
-  Shape sh = verify_shape(variant, cfg);
+  Shape sh = verify_shape(cfg);
   sh.threads = clamp_threads(sh.threads);
   if (sh.unroll != 1 && sh.unroll != 2 && sh.unroll != 8) sh.unroll = 4;
   const int grid = e->sm_count * (sh.ctas_per_sm > 0 ? sh.ctas_per_sm : 1);
@@ -512,8 +505,7 @@ static int verify_range(ScrubEngine* e, const void* p, uint64_t n, int variant, 
       if (cfg == nullptr) {
         // library default: one persistent 1024-thread CTA per SM, 8 x LDG.128 in flight per thread
         // per 128 KiB grab — verify_ld128_fast_kernel
-        const uint64_t nchunks = s.body_vecs * 16 / ((uint64_t)kFastVerifyThreads * kFastVerifyPer * 16);
-        err = launch_fast(CCM_FAST_VERIFY, e->sm_count, kFastVerifyThreads, st, s, nchunks, e->verify_ctl(), e->d_counter);
+        err = launch_fast(CCM_FAST_VERIFY, kFastVerifyThreads, kFastVerifyPer, e, kVerifyGrab, st, s, e->d_counter + kNonzero);
         break;
       }
       Sched sc;
@@ -543,9 +535,7 @@ static int verify_range(ScrubEngine* e, const void* p, uint64_t n, int variant, 
 // Write the tags of `seed` over one range on `st` (no sync).
 static int tag_fill_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cudaStream_t st) {
   if (n == 0) return CCM_OK;
-  const RegionSplit s = split_region(p, n, 16, 128);
-  const uint64_t nchunks = s.body_vecs * 16 / ((uint64_t)kTagThreads * kTagPer * 16);
-  const cudaError_t err = launch_fast(CCM_TAG_FILL, e->sm_count, kTagThreads, st, s, nchunks, e->tag_fill_ctl(), seed);
+  const cudaError_t err = launch_fast(CCM_TAG_FILL, kTagThreads, kTagPer, e, kTagFillGrab, st, split_region(p, n, 16, 128), seed);
   g_launches++;
   if (err != cudaSuccess) { set_error("tag fill launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
   return CCM_OK;
@@ -555,9 +545,7 @@ static int tag_fill_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cu
 // into d_counter[kMismatch].
 static int tag_check_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cudaStream_t st) {
   if (n == 0) return CCM_OK;
-  const RegionSplit s = split_region(p, n, 16, 128);
-  const uint64_t nchunks = s.body_vecs * 16 / ((uint64_t)kTagThreads * kTagPer * 16);
-  const cudaError_t err = launch_fast(CCM_TAG_CHECK, e->sm_count, kTagThreads, st, s, nchunks, e->tag_check_ctl(),
+  const cudaError_t err = launch_fast(CCM_TAG_CHECK, kTagThreads, kTagPer, e, kTagCheckGrab, st, split_region(p, n, 16, 128),
                                       seed, e->d_counter + kMismatch);
   g_launches++;
   if (err != cudaSuccess) { set_error("tag check launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
@@ -651,14 +639,11 @@ static int need_arena(ScrubEngine* e) {
   return CCM_OK;
 }
 
-int engine_arena_scrub(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, void* stream, float* ms) {
-  std::lock_guard<std::mutex> g(e->mu);
-  CCM_ENSURE_READY(e);
-  int rc = need_arena(e); if (rc) return rc;
-  CCM_CUDA(cudaSetDevice(e->ordinal));
-  cudaStream_t st = e->pick(stream);
+// Runs enqueue() on `st`.  With `ms`: brackets it with the events ev[0] / ev[1], waits for it and reports its time.
+template <typename Enqueue>
+static int run_timed(ScrubEngine* e, cudaStream_t st, float* ms, Enqueue&& enqueue) {
   if (ms) CCM_CUDA(cudaEventRecord(e->ev[0], st));
-  for (auto& s : e->segs) { rc = scrub_range(e, s.ptr, s.bytes, variant, cfg, st); if (rc) return rc; }
+  if (int rc = enqueue()) return rc;
   if (ms) {
     CCM_CUDA(cudaEventRecord(e->ev[1], st));
     CCM_CUDA(cudaEventSynchronize(e->ev[1]));
@@ -667,11 +652,37 @@ int engine_arena_scrub(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, v
   return CCM_OK;
 }
 
-static int fetch_count_locked(ScrubEngine* e, cudaStream_t st, uint64_t* nonzero) {
-  CCM_CUDA(cudaMemcpyAsync(e->h_counter, e->d_counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+// Copies control-block word `word` to *count (if asked) and waits for the stream.
+static int fetch_count_locked(ScrubEngine* e, cudaStream_t st, uint64_t* count, int word = kNonzero) {
+  CCM_CUDA(cudaMemcpyAsync(e->h_counter, e->d_counter + word, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   CCM_CUDA(cudaStreamSynchronize(st));
-  if (nonzero) *nonzero = (uint64_t)*e->h_counter;
+  if (count) *count = (uint64_t)*e->h_counter;
   return CCM_OK;
+}
+
+// Zeroes control-block word `word`, runs enqueue() between the events ev[0] and ev[1] on `st`, then reads the
+// word back into *count.  With `ms`: the time between the two events.
+template <typename Enqueue>
+static int run_counted(ScrubEngine* e, cudaStream_t st, int word, uint64_t* count, float* ms, Enqueue&& enqueue) {
+  CCM_CUDA(cudaMemsetAsync(e->d_counter + word, 0, sizeof(unsigned long long), st));
+  CCM_CUDA(cudaEventRecord(e->ev[0], st));
+  if (int rc = enqueue()) return rc;
+  CCM_CUDA(cudaEventRecord(e->ev[1], st));
+  if (int rc = fetch_count_locked(e, st, count, word)) return rc;
+  if (ms) CCM_CUDA(cudaEventElapsedTime(ms, e->ev[0], e->ev[1]));
+  return CCM_OK;
+}
+
+int engine_arena_scrub(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, void* stream, float* ms) {
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  int rc = need_arena(e); if (rc) return rc;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  cudaStream_t st = e->pick(stream);
+  return run_timed(e, st, ms, [&]() -> int {
+    for (auto& s : e->segs) if (int rc2 = scrub_range(e, s.ptr, s.bytes, variant, cfg, st)) return rc2;
+    return CCM_OK;
+  });
 }
 
 int engine_arena_verify(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, void* stream,
@@ -681,13 +692,10 @@ int engine_arena_verify(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, 
   int rc = need_arena(e); if (rc) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->pick(stream);
-  CCM_CUDA(cudaMemsetAsync(e->d_counter, 0, sizeof(unsigned long long), st));
-  CCM_CUDA(cudaEventRecord(e->ev[0], st));
-  for (auto& s : e->segs) { rc = verify_range(e, s.ptr, s.bytes, variant, cfg, st); if (rc) return rc; }
-  CCM_CUDA(cudaEventRecord(e->ev[1], st));
-  rc = fetch_count_locked(e, st, nonzero); if (rc) return rc;
-  if (ms) CCM_CUDA(cudaEventElapsedTime(ms, e->ev[0], e->ev[1]));
-  return CCM_OK;
+  return run_counted(e, st, kNonzero, nonzero, ms, [&]() -> int {
+    for (auto& s : e->segs) if (int rc2 = verify_range(e, s.ptr, s.bytes, variant, cfg, st)) return rc2;
+    return CCM_OK;
+  });
 }
 
 int engine_arena_scrub_verify_async(ScrubEngine* e, int sv, int vv, const ccm_launch_cfg* scfg,
@@ -862,21 +870,20 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
   int rc = need_arena(e); if (rc) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->stream;
-  CCM_CUDA(cudaMemsetAsync(e->d_counter + kMismatch, 0, sizeof(unsigned long long), st));
-  CCM_CUDA(cudaEventRecord(e->ev[0], st));
-  for (auto& s : e->segs) { rc = tag_fill_range(e, s.ptr, s.bytes, tag->seed, st); if (rc) return rc; }
-  CCM_CUDA(cudaEventRecord(e->ev[1], st));
-  for (auto& s : e->segs)
-    if (tag_inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &tag_inject, st, true));
-  CCM_CUDA(cudaEventRecord(e->ev[2], st));
-  for (auto& s : e->segs) { rc = tag_check_range(e, s.ptr, s.bytes, tag->seed, st); if (rc) return rc; }
-  CCM_CUDA(cudaEventRecord(e->ev[3], st));
-  CCM_CUDA(cudaMemcpyAsync(e->h_counter, e->d_counter + kMismatch, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CCM_CUDA(cudaStreamSynchronize(st));
-  tag->mismatch_bytes = (uint64_t)*e->h_counter;
+  // fills between ev[0] and ev[2], the drill, checks between ev[3] and ev[1]
+  rc = run_counted(e, st, kMismatch, &tag->mismatch_bytes, nullptr, [&]() -> int {
+    for (auto& s : e->segs) if (int rc2 = tag_fill_range(e, s.ptr, s.bytes, tag->seed, st)) return rc2;
+    CCM_CUDA(cudaEventRecord(e->ev[2], st));
+    for (auto& s : e->segs)
+      if (tag_inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &tag_inject, st, true));
+    CCM_CUDA(cudaEventRecord(e->ev[3], st));
+    for (auto& s : e->segs) if (int rc2 = tag_check_range(e, s.ptr, s.bytes, tag->seed, st)) return rc2;
+    return CCM_OK;
+  });
+  if (rc) return rc;
   float a = 0, b = 0;
-  CCM_CUDA(cudaEventElapsedTime(&a, e->ev[0], e->ev[1]));
-  CCM_CUDA(cudaEventElapsedTime(&b, e->ev[2], e->ev[3]));
+  CCM_CUDA(cudaEventElapsedTime(&a, e->ev[0], e->ev[2]));
+  CCM_CUDA(cudaEventElapsedTime(&b, e->ev[3], e->ev[1]));
   tag->ms_tag = a;
   tag->ms_check = b;
   tag->va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
@@ -1244,15 +1251,7 @@ int engine_region_scrub(ScrubEngine* e, void* dptr, uint64_t bytes, int variant,
   CCM_ENSURE_READY(e);
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->pick(stream);
-  if (ms) CCM_CUDA(cudaEventRecord(e->ev[0], st));
-  int rc = scrub_range(e, dptr, bytes, variant, cfg, st);
-  if (rc) return rc;
-  if (ms) {
-    CCM_CUDA(cudaEventRecord(e->ev[1], st));
-    CCM_CUDA(cudaEventSynchronize(e->ev[1]));
-    CCM_CUDA(cudaEventElapsedTime(ms, e->ev[0], e->ev[1]));
-  }
-  return CCM_OK;
+  return run_timed(e, st, ms, [&] { return scrub_range(e, dptr, bytes, variant, cfg, st); });
 }
 
 int engine_region_verify(ScrubEngine* e, const void* dptr, uint64_t bytes, int variant,
@@ -1261,15 +1260,7 @@ int engine_region_verify(ScrubEngine* e, const void* dptr, uint64_t bytes, int v
   CCM_ENSURE_READY(e);
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->pick(stream);
-  CCM_CUDA(cudaMemsetAsync(e->d_counter, 0, sizeof(unsigned long long), st));
-  CCM_CUDA(cudaEventRecord(e->ev[0], st));
-  int rc = verify_range(e, dptr, bytes, variant, cfg, st);
-  if (rc) return rc;
-  CCM_CUDA(cudaEventRecord(e->ev[1], st));
-  rc = fetch_count_locked(e, st, nonzero);
-  if (rc) return rc;
-  if (ms) CCM_CUDA(cudaEventElapsedTime(ms, e->ev[0], e->ev[1]));
-  return CCM_OK;
+  return run_counted(e, st, kNonzero, nonzero, ms, [&] { return verify_range(e, dptr, bytes, variant, cfg, st); });
 }
 
 int engine_host_roundtrip(ScrubEngine* e, void* host_buf, uint64_t bytes, uint64_t dev_offset,
@@ -1330,15 +1321,7 @@ extern "C" int ccm_region_tag_fill(int cuda_ordinal, void* dptr, uint64_t bytes,
   CCM_ENSURE_READY(e);
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->pick(stream);
-  if (ms) CCM_CUDA(cudaEventRecord(e->ev[0], st));
-  int rc = tag_fill_range(e, dptr, bytes, seed, st);
-  if (rc) return rc;
-  if (ms) {
-    CCM_CUDA(cudaEventRecord(e->ev[1], st));
-    CCM_CUDA(cudaEventSynchronize(e->ev[1]));
-    CCM_CUDA(cudaEventElapsedTime(ms, e->ev[0], e->ev[1]));
-  }
-  return CCM_OK;
+  return run_timed(e, st, ms, [&] { return tag_fill_range(e, dptr, bytes, seed, st); });
 }
 
 extern "C" int ccm_region_tag_check_zero(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream,
@@ -1349,14 +1332,5 @@ extern "C" int ccm_region_tag_check_zero(int cuda_ordinal, void* dptr, uint64_t 
   CCM_ENSURE_READY(e);
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->pick(stream);
-  CCM_CUDA(cudaMemsetAsync(e->d_counter + kMismatch, 0, sizeof(unsigned long long), st));
-  CCM_CUDA(cudaEventRecord(e->ev[0], st));
-  int rc = tag_check_range(e, dptr, bytes, seed, st);
-  if (rc) return rc;
-  CCM_CUDA(cudaEventRecord(e->ev[1], st));
-  CCM_CUDA(cudaMemcpyAsync(e->h_counter, e->d_counter + kMismatch, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CCM_CUDA(cudaStreamSynchronize(st));
-  if (mismatch) *mismatch = (uint64_t)*e->h_counter;
-  if (ms) CCM_CUDA(cudaEventElapsedTime(ms, e->ev[0], e->ev[1]));
-  return CCM_OK;
+  return run_counted(e, st, kMismatch, mismatch, ms, [&] { return tag_check_range(e, dptr, bytes, seed, st); });
 }

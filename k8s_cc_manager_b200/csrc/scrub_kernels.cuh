@@ -29,6 +29,9 @@
 //   scrub_tma_kernel                                     cp.async.bulk stores from one zero tile
 //   tag_fill_kernel / tag_check_zero_kernel              the tagged gate's known-answer pass
 //   fill_pattern_kernel                                  seeded test pattern (tests only)
+// The grab loop (grab_chunks) and the epilogue after the last whole chunk or tile (finish_region,
+// ragged_bytes) are written once.  The four compile-time-shape kernels are one frame (default_kernel)
+// around an op struct that says what happens to each chunk, leftover vector and ragged byte.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -144,91 +147,86 @@ struct Sched {
                                 //    no block barrier, no shared memory in the hot loop
 };
 
-// ------------------------------------------------------------- scrub (stores)
-template <int VB, int UNROLL, int POL>
-__device__ __forceinline__ void scrub_tile(uint8_t* body, uint64_t tile, uint64_t tile_vecs, uint32_t idx,
-                                           uint64_t stride_bytes, uint64_t l2pol) {
-  if constexpr (VB == 32) {
-    // lane-contiguous halves: stride_bytes = group * 32, each half is group * 16 bytes
-    uint8_t* p = body + tile * tile_vecs * 32 + (uint64_t)idx * 16;
-    const uint64_t half = stride_bytes / 2;
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      st_zero16<POL>(p + u * stride_bytes, l2pol);
-      st_zero16<POL>(p + u * stride_bytes + half, l2pol);
-    }
-  } else {
-    uint8_t* p = body + (tile * tile_vecs + idx) * VB;
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) st_zero16<POL>(p + u * stride_bytes, l2pol);
+// One CTA grabs chunks [0, nchunks) off *counter and calls body(c) for each, with every thread of the
+// CTA.  Double-buffered: thread 0 has the grab for the next chunk in flight while the CTA works on this one,
+// and one block barrier per chunk publishes it.
+template <typename Body>
+__device__ __forceinline__ void grab_chunks(unsigned long long* counter, uint64_t nchunks, Body&& body) {
+  __shared__ unsigned long long s_chunk[2];
+  if (threadIdx.x == 0) s_chunk[0] = atomicAdd(counter, 1ull);
+  __syncthreads();
+  int buf = 0;
+  for (;;) {
+    const uint64_t c = s_chunk[buf];
+    if (c >= nchunks) break;
+    unsigned long long nxt = 0;
+    // next grab in flight while we work.  The raw result goes straight to shared memory at the end of
+    // the iteration: any arithmetic on it here would make warp 0 wait out the atomic's round trip
+    // before its stores.
+    if (threadIdx.x == 0) nxt = atomicAdd(counter, 1ull);
+    body(c);
+    if (threadIdx.x == 0) s_chunk[buf ^ 1] = nxt;
+    __syncthreads();
+    buf ^= 1;  // two slots: a slow warp may still be reading slot k when thread 0 already writes slot k+1
   }
 }
 
-template <int VB, int UNROLL, int POL>
-__global__ void __launch_bounds__(1024)
-scrub_st_kernel(RegionSplit s, Sched sched) {
-  uint8_t* body = s.base + s.head;
-  const uint32_t group = sched.per_warp ? 32u : blockDim.x;   // threads that share one tile
-  const uint32_t idx = sched.per_warp ? (threadIdx.x & 31u) : threadIdx.x;
-  const uint64_t tile_vecs = (uint64_t)group * UNROLL;
+// Calls tile_fn(tile) for every tile this thread's group covers under `sched`: grid-stride (static), chunks
+// grabbed by each warp, or chunks grabbed by each CTA.  idx: the thread's index in its group (the lane, when
+// every warp grabs); the kernel has it live anyway, and testing it rather than threadIdx.x & 31 keeps the
+// generic kernels' register counts and spills where they were.
+template <typename TileFn>
+__device__ __forceinline__ void for_each_tile(const Sched& sched, uint32_t idx, TileFn&& tile_fn) {
   const uint64_t ntiles = sched.ntiles;
-  const uint64_t stride_bytes = (uint64_t)group * VB;
-  const uint64_t l2pol = make_l2_policy<POL>();
-
+  auto chunk_tiles = [&](uint64_t c) {
+    const uint64_t t0 = c * sched.chunk_tiles;
+    const uint64_t t1 = t0 + sched.chunk_tiles < ntiles ? t0 + sched.chunk_tiles : ntiles;
+    for (uint64_t tile = t0; tile < t1; ++tile) tile_fn(tile);
+  };
   if (sched.counter == nullptr) {
-    for (uint64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
-      scrub_tile<VB, UNROLL, POL>(body, tile, tile_vecs, idx, stride_bytes, l2pol);
+    for (uint64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) tile_fn(tile);
   } else if (sched.per_warp) {
-    const uint64_t nchunks = sched.nchunks;
     unsigned long long c = 0;
     if (idx == 0) c = atomicAdd(sched.counter, 1ull);
     c = __shfl_sync(0xffffffffu, c, 0);
-    while (c < nchunks) {
+    while (c < sched.nchunks) {
       unsigned long long nxt = 0;
       if (idx == 0) nxt = atomicAdd(sched.counter, 1ull);  // prefetch the next grab
-      const uint64_t t0 = c * sched.chunk_tiles;
-      const uint64_t t1 = t0 + sched.chunk_tiles < ntiles ? t0 + sched.chunk_tiles : ntiles;
-      for (uint64_t tile = t0; tile < t1; ++tile)
-        scrub_tile<VB, UNROLL, POL>(body, tile, tile_vecs, idx, stride_bytes, l2pol);
+      chunk_tiles(c);
       c = __shfl_sync(0xffffffffu, nxt, 0);
     }
   } else {
-    __shared__ unsigned long long s_chunk[2];
-    const uint64_t nchunks = sched.nchunks;
-    if (threadIdx.x == 0) s_chunk[0] = atomicAdd(sched.counter, 1ull);
-    __syncthreads();
-    int buf = 0;
-    for (;;) {
-      const uint64_t c = s_chunk[buf];
-      if (c >= nchunks) break;
-      unsigned long long nxt = 0;
-      if (threadIdx.x == 0) nxt = atomicAdd(sched.counter, 1ull);  // prefetch the next grab
-      const uint64_t t0 = c * sched.chunk_tiles;
-      const uint64_t t1 = t0 + sched.chunk_tiles < ntiles ? t0 + sched.chunk_tiles : ntiles;
-      for (uint64_t tile = t0; tile < t1; ++tile)
-        scrub_tile<VB, UNROLL, POL>(body, tile, tile_vecs, idx, stride_bytes, l2pol);
-      if (threadIdx.x == 0) s_chunk[buf ^ 1] = nxt;
-      __syncthreads();
-      buf ^= 1;
-    }
-  }
-  // remainder vectors (< one tile), spread over the grid
-  for (uint64_t i = ntiles * tile_vecs + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-       i < s.body_vecs; i += (uint64_t)gridDim.x * blockDim.x)
-    st_zero<VB, POL>(body + i * VB, l2pol);
-  // ragged head / tail bytes
-  if (blockIdx.x == 0) {
-    for (uint64_t i = threadIdx.x; i < s.head; i += blockDim.x) s.base[i] = 0;
-    uint8_t* t = body + s.body_vecs * VB;
-    for (uint64_t i = threadIdx.x; i < s.tail; i += blockDim.x) t[i] = 0;
+    grab_chunks(sched.counter, sched.nchunks, chunk_tiles);
   }
 }
 
+// ------------------------------------------------------------------ epilogue
+// CTA 0 takes the ragged head and tail bytes, op.byte(p) for each.
+template <int VB, typename Op>
+__device__ __forceinline__ void ragged_bytes(const RegionSplit& s, uint32_t nthreads, Op& op) {
+  if (blockIdx.x == 0) {
+    for (uint64_t i = threadIdx.x; i < s.head; i += nthreads) op.byte(s.base + i);
+    uint8_t* t = s.base + s.head + s.body_vecs * VB;
+    for (uint64_t i = threadIdx.x; i < s.tail; i += nthreads) op.byte(t + i);
+  }
+}
+
+// The vectors from first_vec on (what is left after the last whole chunk or tile: less than one of them),
+// op.vec(p) spread over the grid, then the ragged head / tail bytes.
+template <int VB, typename Op>
+__device__ __forceinline__ void finish_region(const RegionSplit& s, uint64_t first_vec, uint32_t nthreads, Op& op) {
+  uint8_t* body = s.base + s.head;
+  for (uint64_t i = first_vec + (uint64_t)blockIdx.x * nthreads + threadIdx.x; i < s.body_vecs;
+       i += (uint64_t)gridDim.x * nthreads)
+    op.vec(body + i * VB);
+  ragged_bytes<VB>(s, nthreads, op);
+}
+
 // ----------------------------------------------------- default shapes, tight loops
-// The two kernels below are what AUTO launches.  Same algorithm as scrub_st_kernel /
-// verify_ld_kernel with a per-CTA dynamic schedule, but block size and vectors per thread
-// are compile-time constants, so one chunk = THREADS * PER_THREAD * 16 bytes is addressed
-// from ONE 64-bit base with immediate offsets: PER_THREAD STG.128 / LDG.128 per thread per
+// The four kernels built on default_kernel below are what AUTO and the tagged gate launch.  Same
+// algorithm as scrub_st_kernel / verify_ld_kernel with a per-CTA dynamic schedule, but block size and
+// vectors per thread are compile-time constants, so one chunk = THREADS * PER_THREAD * 16 bytes is
+// addressed from ONE 64-bit base with immediate offsets: PER_THREAD STG.128 / LDG.128 per thread per
 // chunk (consecutive lanes touch consecutive 16-byte vectors, so every warp instruction covers
 // four whole 128-byte lines) and a few instructions of bookkeeping, instead of a 64-bit add pair
 // per access in the generic kernel (runtime stride).
@@ -258,44 +256,79 @@ __device__ __forceinline__ void grab_release(const GrabCtl& g, unsigned long lon
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// zero_on_exit (may be null): a word the last CTA clears as well — the arena step passes the
-// verify counter, so "scrub" also resets the verdict of the previous read-back.
+// The frame of the four default kernels: persistent CTAs grab whole chunks (from the top of the region
+// down when DESCENDING) and hand each to op.chunk<THREADS, PER_THREAD>(p), where p is this thread's first
+// vector and its PER_THREAD vectors are at p + u * THREADS * 16; then the self-resetting GrabCtl, then the
+// vectors after the last whole chunk and the ragged bytes (finish_region).
+// zero_on_exit (may be null): a word the last CTA clears as well.
+template <int THREADS, int PER_THREAD, bool DESCENDING, typename Op>
+__device__ __forceinline__ void default_kernel(const RegionSplit& s, uint64_t nchunks, const GrabCtl& ctl,
+                                               unsigned long long* zero_on_exit, Op& op) {
+  constexpr uint64_t kChunk = (uint64_t)THREADS * PER_THREAD * 16;
+  uint8_t* body = s.base + s.head;
+  pdl_wait();
+  grab_chunks(ctl.grab, nchunks, [&](uint64_t c) {
+    op.template chunk<THREADS, PER_THREAD>(body + (DESCENDING ? nchunks - 1 - c : c) * kChunk + threadIdx.x * 16u);
+  });
+  pdl_launch_dependents();
+  if (threadIdx.x == 0) grab_release(ctl, zero_on_exit);
+  finish_region<16>(s, nchunks * (kChunk / 16), THREADS, op);
+}
+
+// ------------------------------------------------------------- scrub (stores)
+template <int VB, int POL>
+struct ZeroOp {
+  uint64_t l2pol;
+  template <int THREADS, int PER_THREAD>
+  __device__ __forceinline__ void chunk(uint8_t* p) {
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) st_zero16<POL>(p + (uint32_t)u * THREADS * 16u, l2pol);
+  }
+  __device__ __forceinline__ void vec(uint8_t* p) { st_zero<VB, POL>(p, l2pol); }
+  __device__ __forceinline__ void byte(uint8_t* p) { *p = 0; }
+};
+
+template <int VB, int UNROLL, int POL>
+__device__ __forceinline__ void scrub_tile(uint8_t* body, uint64_t tile, uint64_t tile_vecs, uint32_t idx,
+                                           uint64_t stride_bytes, uint64_t l2pol) {
+  if constexpr (VB == 32) {
+    // lane-contiguous halves: stride_bytes = group * 32, each half is group * 16 bytes
+    uint8_t* p = body + tile * tile_vecs * 32 + (uint64_t)idx * 16;
+    const uint64_t half = stride_bytes / 2;
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      st_zero16<POL>(p + u * stride_bytes, l2pol);
+      st_zero16<POL>(p + u * stride_bytes + half, l2pol);
+    }
+  } else {
+    uint8_t* p = body + (tile * tile_vecs + idx) * VB;
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) st_zero16<POL>(p + u * stride_bytes, l2pol);
+  }
+}
+
+template <int VB, int UNROLL, int POL>
+__global__ void __launch_bounds__(1024)
+scrub_st_kernel(RegionSplit s, Sched sched) {
+  uint8_t* body = s.base + s.head;
+  const uint32_t group = sched.per_warp ? 32u : blockDim.x;   // threads that share one tile
+  const uint32_t idx = sched.per_warp ? (threadIdx.x & 31u) : threadIdx.x;
+  const uint64_t tile_vecs = (uint64_t)group * UNROLL;
+  const uint64_t stride_bytes = (uint64_t)group * VB;
+  ZeroOp<VB, POL> op{make_l2_policy<POL>()};
+  for_each_tile(sched, idx, [&](uint64_t tile) {
+    scrub_tile<VB, UNROLL, POL>(body, tile, tile_vecs, idx, stride_bytes, op.l2pol);
+  });
+  finish_region<VB>(s, sched.ntiles * tile_vecs, blockDim.x, op);
+}
+
+// zero_on_exit (may be null): the arena step passes the verify counter, so "scrub" also resets the
+// verdict of the previous read-back.
 template <int THREADS, int PER_THREAD, int POL>
 __global__ void __launch_bounds__(THREADS)
 scrub_st128_fast_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, unsigned long long* zero_on_exit) {
-  constexpr uint64_t kChunk = (uint64_t)THREADS * PER_THREAD * 16;
-  uint8_t* body = s.base + s.head;
-  __shared__ unsigned long long s_chunk[2];
-  pdl_wait();
-  if (threadIdx.x == 0) s_chunk[0] = atomicAdd(ctl.grab, 1ull);
-  __syncthreads();
-  int buf = 0;
-  for (;;) {
-    const uint64_t c = s_chunk[buf];
-    if (c >= nchunks) break;
-    unsigned long long nxt = 0;
-    // next grab in flight while we store.  The raw result goes straight to shared memory at the end of
-    // the iteration: any arithmetic on it here would make warp 0 wait out the atomic's round trip
-    // before its stores.
-    if (threadIdx.x == 0) nxt = atomicAdd(ctl.grab, 1ull);
-    uint8_t* p = body + c * kChunk + threadIdx.x * 16u;
-#pragma unroll
-    for (int u = 0; u < PER_THREAD; ++u) st_zero16<POL>(p + (uint32_t)u * THREADS * 16u, 0);
-    if (threadIdx.x == 0) s_chunk[buf ^ 1] = nxt;
-    __syncthreads();
-    buf ^= 1;  // two slots: a slow warp may still be reading slot k when thread 0 already writes slot k+1
-  }
-  pdl_launch_dependents();
-  if (threadIdx.x == 0) grab_release(ctl, zero_on_exit);
-  // vectors after the last whole chunk (< kChunk bytes), then the ragged head / tail bytes
-  for (uint64_t i = nchunks * (kChunk / 16) + (uint64_t)blockIdx.x * THREADS + threadIdx.x;
-       i < s.body_vecs; i += (uint64_t)gridDim.x * THREADS)
-    st_zero16<POL>(body + i * 16, 0);
-  if (blockIdx.x == 0) {
-    for (uint64_t i = threadIdx.x; i < s.head; i += THREADS) s.base[i] = 0;
-    uint8_t* t = body + s.body_vecs * 16;
-    for (uint64_t i = threadIdx.x; i < s.tail; i += THREADS) t[i] = 0;
-  }
+  ZeroOp<16, POL> op{0};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, zero_on_exit, op);
 }
 
 // ------------------------------------------------------ scrub (TMA bulk store)
@@ -362,11 +395,8 @@ scrub_tma_kernel(RegionSplit s /* VB = 16 */, uint32_t tile_bytes, uint32_t ops_
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
-  if (blockIdx.x == 0) {
-    for (uint64_t i = threadIdx.x; i < s.head; i += blockDim.x) s.base[i] = 0;
-    uint8_t* t = body + body_bytes;
-    for (uint64_t i = threadIdx.x; i < s.tail; i += blockDim.x) t[i] = 0;
-  }
+  ZeroOp<16, POL> zero{0};
+  ragged_bytes<16>(s, blockDim.x, zero);
 }
 
 // ----------------------------------------------------------------- reductions
@@ -428,101 +458,16 @@ __device__ __forceinline__ uint32_t verify_tile(const uint8_t* body, uint64_t ti
   return c;
 }
 
-template <int VB, int UNROLL, int POL>
-__global__ void __launch_bounds__(1024)
-verify_ld_kernel(RegionSplit s, unsigned long long* counter, Sched sched) {
-  const uint8_t* body = s.base + s.head;
-  const uint32_t group = sched.per_warp ? 32u : blockDim.x;
-  const uint32_t idx = sched.per_warp ? (threadIdx.x & 31u) : threadIdx.x;
-  const uint64_t tile_vecs = (uint64_t)group * UNROLL;
-  const uint64_t ntiles = sched.ntiles;
-  const uint64_t stride_bytes = (uint64_t)group * VB;
-  constexpr int W = VB / 4;
+// Counts the non-zero bytes it reads into cnt.  chunk() batches like verify_tile.
+template <int VB, int POL>
+struct CountNonzeroOp {
+  uint64_t l2pol;
   uint64_t cnt = 0;
-  const uint64_t l2pol = make_l2_policy<POL>();
-  (void)l2pol;
-
-  if (sched.counter == nullptr) {
-    for (uint64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
-      cnt += verify_tile<VB, UNROLL, POL>(body, tile, tile_vecs, idx, stride_bytes, l2pol);
-  } else if (sched.per_warp) {
-    const uint64_t nchunks = sched.nchunks;
-    unsigned long long c = 0;
-    if (idx == 0) c = atomicAdd(sched.counter, 1ull);
-    c = __shfl_sync(0xffffffffu, c, 0);
-    while (c < nchunks) {
-      unsigned long long nxt = 0;
-      if (idx == 0) nxt = atomicAdd(sched.counter, 1ull);
-      const uint64_t t0 = c * sched.chunk_tiles;
-      const uint64_t t1 = t0 + sched.chunk_tiles < ntiles ? t0 + sched.chunk_tiles : ntiles;
-      for (uint64_t tile = t0; tile < t1; ++tile)
-        cnt += verify_tile<VB, UNROLL, POL>(body, tile, tile_vecs, idx, stride_bytes, l2pol);
-      c = __shfl_sync(0xffffffffu, nxt, 0);
-    }
-  } else {
-    __shared__ unsigned long long s_chunk[2];
-    const uint64_t nchunks = sched.nchunks;
-    if (threadIdx.x == 0) s_chunk[0] = atomicAdd(sched.counter, 1ull);
-    __syncthreads();
-    int buf = 0;
-    for (;;) {
-      const uint64_t c = s_chunk[buf];
-      if (c >= nchunks) break;
-      unsigned long long nxt = 0;
-      if (threadIdx.x == 0) nxt = atomicAdd(sched.counter, 1ull);
-      const uint64_t t0 = c * sched.chunk_tiles;
-      const uint64_t t1 = t0 + sched.chunk_tiles < ntiles ? t0 + sched.chunk_tiles : ntiles;
-      for (uint64_t tile = t0; tile < t1; ++tile)
-        cnt += verify_tile<VB, UNROLL, POL>(body, tile, tile_vecs, idx, stride_bytes, l2pol);
-      if (threadIdx.x == 0) s_chunk[buf ^ 1] = nxt;
-      __syncthreads();
-      buf ^= 1;
-    }
-  }
-  for (uint64_t i = ntiles * tile_vecs + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-       i < s.body_vecs; i += (uint64_t)gridDim.x * blockDim.x) {
-    if constexpr (VB == 32) {
-      Vec32 v = ld32<POL>(body + i * VB, l2pol);
-#pragma unroll
-      for (int k = 0; k < W; ++k) cnt += nonzero_bytes_in_word(v.w[k]);
-    } else {
-      Vec16 v = ld16<POL>(body + i * VB, l2pol);
-#pragma unroll
-      for (int k = 0; k < W; ++k) cnt += nonzero_bytes_in_word(v.w[k]);
-    }
-  }
-  if (blockIdx.x == 0) {
-    for (uint64_t i = threadIdx.x; i < s.head; i += blockDim.x) cnt += (s.base[i] != 0);
-    const uint8_t* t = body + s.body_vecs * VB;
-    for (uint64_t i = threadIdx.x; i < s.tail; i += blockDim.x) cnt += (t[i] != 0);
-  }
-  block_accumulate(cnt, counter);
-}
-
-template <int THREADS, int PER_THREAD, int POL>
-__global__ void __launch_bounds__(THREADS)
-verify_ld128_fast_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, unsigned long long* counter) {
-  constexpr uint64_t kChunk = (uint64_t)THREADS * PER_THREAD * 16;
-  const uint8_t* body = s.base + s.head;
-  uint64_t cnt = 0;
-  __shared__ unsigned long long s_chunk[2];
-  pdl_wait();
-  if (threadIdx.x == 0) s_chunk[0] = atomicAdd(ctl.grab, 1ull);
-  __syncthreads();
-  int buf = 0;
-  for (;;) {
-    const uint64_t c = s_chunk[buf];
-    if (c >= nchunks) break;
-    unsigned long long nxt = 0;
-    if (threadIdx.x == 0) nxt = atomicAdd(ctl.grab, 1ull);
-    // DESCENDING chunk order.  The scrub ran in ascending order and left the last L2-sized stretch it
-    // wrote (up to 50 MB on H100) dirty in L2.  Reading upwards would stream the whole region from DRAM
-    // and, on top of that, evict those dirty lines (extra write-back traffic); reading downwards takes
-    // them out of L2 first, so the DRAM traffic of a read-back is R again, not R + L2.
-    const uint8_t* p = body + (nchunks - 1 - c) * kChunk + threadIdx.x * 16u;
+  template <int THREADS, int PER_THREAD>
+  __device__ __forceinline__ void chunk(const uint8_t* p) {
     Vec16 v[PER_THREAD];
 #pragma unroll
-    for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16<POL>(p + (uint32_t)u * THREADS * 16u, 0);  // all loads first
+    for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16<POL>(p + (uint32_t)u * THREADS * 16u, l2pol);  // all loads first
     uint32_t any = 0;
 #pragma unroll
     for (int u = 0; u < PER_THREAD; ++u)
@@ -536,24 +481,47 @@ verify_ld128_fast_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, unsigned 
         for (int k = 0; k < 4; ++k) n += nonzero_bytes_in_word(v[u].w[k]);
       cnt += n;
     }
-    if (threadIdx.x == 0) s_chunk[buf ^ 1] = nxt;
-    __syncthreads();
-    buf ^= 1;
   }
-  pdl_launch_dependents();
-  if (threadIdx.x == 0) grab_release(ctl, nullptr);
-  for (uint64_t i = nchunks * (kChunk / 16) + (uint64_t)blockIdx.x * THREADS + threadIdx.x;
-       i < s.body_vecs; i += (uint64_t)gridDim.x * THREADS) {
-    Vec16 v = ld16<POL>(body + i * 16, 0);
+  __device__ __forceinline__ void vec(const uint8_t* p) {
+    if constexpr (VB == 32) {
+      Vec32 v = ld32<POL>(p, l2pol);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) cnt += nonzero_bytes_in_word(v.w[k]);
+      for (int k = 0; k < 8; ++k) cnt += nonzero_bytes_in_word(v.w[k]);
+    } else {
+      Vec16 v = ld16<POL>(p, l2pol);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) cnt += nonzero_bytes_in_word(v.w[k]);
+    }
   }
-  if (blockIdx.x == 0) {
-    for (uint64_t i = threadIdx.x; i < s.head; i += THREADS) cnt += (s.base[i] != 0);
-    const uint8_t* t = body + s.body_vecs * 16;
-    for (uint64_t i = threadIdx.x; i < s.tail; i += THREADS) cnt += (t[i] != 0);
-  }
-  block_accumulate(cnt, counter);
+  __device__ __forceinline__ void byte(const uint8_t* p) { cnt += (*p != 0); }
+};
+
+template <int VB, int UNROLL, int POL>
+__global__ void __launch_bounds__(1024)
+verify_ld_kernel(RegionSplit s, unsigned long long* counter, Sched sched) {
+  const uint8_t* body = s.base + s.head;
+  const uint32_t group = sched.per_warp ? 32u : blockDim.x;
+  const uint32_t idx = sched.per_warp ? (threadIdx.x & 31u) : threadIdx.x;
+  const uint64_t tile_vecs = (uint64_t)group * UNROLL;
+  const uint64_t stride_bytes = (uint64_t)group * VB;
+  CountNonzeroOp<VB, POL> op{make_l2_policy<POL>()};
+  for_each_tile(sched, idx, [&](uint64_t tile) {
+    op.cnt += verify_tile<VB, UNROLL, POL>(body, tile, tile_vecs, idx, stride_bytes, op.l2pol);
+  });
+  finish_region<VB>(s, sched.ntiles * tile_vecs, blockDim.x, op);
+  block_accumulate(op.cnt, counter);
+}
+
+// DESCENDING chunk order.  The scrub ran in ascending order and left the last L2-sized stretch it
+// wrote (up to 50 MB on H100) dirty in L2.  Reading upwards would stream the whole region from DRAM
+// and, on top of that, evict those dirty lines (extra write-back traffic); reading downwards takes
+// them out of L2 first, so the DRAM traffic of a read-back is R again, not R + L2.
+template <int THREADS, int PER_THREAD, int POL>
+__global__ void __launch_bounds__(THREADS)
+verify_ld128_fast_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, unsigned long long* counter) {
+  CountNonzeroOp<16, POL> op{0};
+  default_kernel<THREADS, PER_THREAD, true>(s, nchunks, ctl, nullptr, op);
+  block_accumulate(op.cnt, counter);
 }
 
 // ------------------------------------------------- address-tagged known answer
@@ -602,111 +570,75 @@ __device__ __forceinline__ uint4 ld16_cs(const void* p) {
   return v;
 }
 
+__device__ __forceinline__ uint64_t addr(const void* p) { return (uint64_t)(uintptr_t)p; }
+
+struct TagFillOp {
+  uint32_t seed;
+  template <int THREADS, int PER_THREAD>
+  __device__ __forceinline__ void chunk(uint8_t* p) {
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) vec(p + (uint32_t)u * THREADS * 16u);
+  }
+  __device__ __forceinline__ void vec(uint8_t* q) { st16(q, tag_vec(seed, addr(q))); }
+  __device__ __forceinline__ void byte(uint8_t* x) { *x = tag_byte(seed, addr(x)); }
+};
+
 // Writes the tags over a region.  Shape and bookkeeping of scrub_st128_fast_kernel: persistent CTAs,
 // one THREADS * PER_THREAD * 16-byte chunk per grab, self-resetting GrabCtl, CTA 0 takes the ragged bytes.
 template <int THREADS, int PER_THREAD>
 __global__ void __launch_bounds__(THREADS)
 tag_fill_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed) {
-  constexpr uint64_t kChunk = (uint64_t)THREADS * PER_THREAD * 16;
-  uint8_t* body = s.base + s.head;
-  __shared__ unsigned long long s_chunk[2];
-  pdl_wait();
-  if (threadIdx.x == 0) s_chunk[0] = atomicAdd(ctl.grab, 1ull);
-  __syncthreads();
-  int buf = 0;
-  for (;;) {
-    const uint64_t c = s_chunk[buf];
-    if (c >= nchunks) break;
-    unsigned long long nxt = 0;
-    if (threadIdx.x == 0) nxt = atomicAdd(ctl.grab, 1ull);
-    uint8_t* p = body + c * kChunk + threadIdx.x * 16u;
-#pragma unroll
-    for (int u = 0; u < PER_THREAD; ++u) {
-      uint8_t* q = p + (uint32_t)u * THREADS * 16u;
-      st16(q, tag_vec(seed, (uint64_t)(uintptr_t)q));
-    }
-    if (threadIdx.x == 0) s_chunk[buf ^ 1] = nxt;
-    __syncthreads();
-    buf ^= 1;
-  }
-  pdl_launch_dependents();
-  if (threadIdx.x == 0) grab_release(ctl, nullptr);
-  for (uint64_t i = nchunks * (kChunk / 16) + (uint64_t)blockIdx.x * THREADS + threadIdx.x;
-       i < s.body_vecs; i += (uint64_t)gridDim.x * THREADS) {
-    uint8_t* q = body + i * 16;
-    st16(q, tag_vec(seed, (uint64_t)(uintptr_t)q));
-  }
-  if (blockIdx.x == 0) {
-    for (uint64_t i = threadIdx.x; i < s.head; i += THREADS) s.base[i] = tag_byte(seed, (uint64_t)(uintptr_t)(s.base + i));
-    uint8_t* t = body + s.body_vecs * 16;
-    for (uint64_t i = threadIdx.x; i < s.tail; i += THREADS) t[i] = tag_byte(seed, (uint64_t)(uintptr_t)(t + i));
-  }
+  TagFillOp op{seed};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
 }
 
-// Reads the tags back, counts every byte that differs from them (exact, u64, one atomic per CTA into
-// *mismatch) and stores zero over the same addresses.  All PER_THREAD loads are in flight before any use.
+// Counts the bytes that differ from the tags into cnt and stores zero over them.
 // The exact per-byte count is computed for every batch, branch-free, and the loaded words die before the
 // stores: on H100 this runs at 0.97x of a same-run device-to-device copy, where counting only batches whose
 // XOR is non-zero (verify_ld128_fast_kernel's trick) keeps the loaded words live across the stores and
-// runs at 0.75x (one H100 80GB HBM3, 700 W, 32 GiB region).  Chunks are taken in ascending order, so the
-// last stretch this kernel writes is the first one the descending zero read-back reads.
-template <int THREADS, int PER_THREAD>
-__global__ void __launch_bounds__(THREADS)
-tag_check_zero_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed, unsigned long long* mismatch) {
-  constexpr uint64_t kChunk = (uint64_t)THREADS * PER_THREAD * 16;
-  uint8_t* body = s.base + s.head;
+// runs at 0.75x (one H100 80GB HBM3, 700 W, 32 GiB region).
+struct TagCheckZeroOp {
+  uint32_t seed;
   uint64_t cnt = 0;
-  __shared__ unsigned long long s_chunk[2];
-  pdl_wait();
-  if (threadIdx.x == 0) s_chunk[0] = atomicAdd(ctl.grab, 1ull);
-  __syncthreads();
-  int buf = 0;
-  for (;;) {
-    const uint64_t c = s_chunk[buf];
-    if (c >= nchunks) break;
-    unsigned long long nxt = 0;
-    if (threadIdx.x == 0) nxt = atomicAdd(ctl.grab, 1ull);
-    uint8_t* p = body + c * kChunk + threadIdx.x * 16u;
+  template <int THREADS, int PER_THREAD>
+  __device__ __forceinline__ void chunk(uint8_t* p) {
     uint4 v[PER_THREAD];
 #pragma unroll
     for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16_cs(p + (uint32_t)u * THREADS * 16u);  // all loads first
     uint32_t n = 0;
 #pragma unroll
     for (int u = 0; u < PER_THREAD; ++u) {
-      const uint4 t = tag_vec(seed, (uint64_t)(uintptr_t)(p + (uint32_t)u * THREADS * 16u));
+      const uint4 t = tag_vec(seed, addr(p + (uint32_t)u * THREADS * 16u));
       n += nonzero_bytes_in_word(v[u].x ^ t.x) + nonzero_bytes_in_word(v[u].y ^ t.y) +
            nonzero_bytes_in_word(v[u].z ^ t.z) + nonzero_bytes_in_word(v[u].w ^ t.w);
     }
 #pragma unroll
     for (int u = 0; u < PER_THREAD; ++u) st16(p + (uint32_t)u * THREADS * 16u, make_uint4(0, 0, 0, 0));
     cnt += n;
-    if (threadIdx.x == 0) s_chunk[buf ^ 1] = nxt;
-    __syncthreads();
-    buf ^= 1;
   }
-  pdl_launch_dependents();
-  if (threadIdx.x == 0) grab_release(ctl, nullptr);
-  for (uint64_t i = nchunks * (kChunk / 16) + (uint64_t)blockIdx.x * THREADS + threadIdx.x;
-       i < s.body_vecs; i += (uint64_t)gridDim.x * THREADS) {
-    uint8_t* q = body + i * 16;
+  __device__ __forceinline__ void vec(uint8_t* q) {
     uint4 v = ld16_cs(q);
-    const uint4 t = tag_vec(seed, (uint64_t)(uintptr_t)q);
+    const uint4 t = tag_vec(seed, addr(q));
     st16(q, make_uint4(0, 0, 0, 0));
     cnt += nonzero_bytes_in_word(v.x ^ t.x) + nonzero_bytes_in_word(v.y ^ t.y) + nonzero_bytes_in_word(v.z ^ t.z) +
            nonzero_bytes_in_word(v.w ^ t.w);
   }
-  if (blockIdx.x == 0) {
-    for (uint64_t i = threadIdx.x; i < s.head; i += THREADS) {
-      cnt += s.base[i] != tag_byte(seed, (uint64_t)(uintptr_t)(s.base + i));
-      s.base[i] = 0;
-    }
-    uint8_t* t = body + s.body_vecs * 16;
-    for (uint64_t i = threadIdx.x; i < s.tail; i += THREADS) {
-      cnt += t[i] != tag_byte(seed, (uint64_t)(uintptr_t)(t + i));
-      t[i] = 0;
-    }
+  __device__ __forceinline__ void byte(uint8_t* x) {
+    cnt += *x != tag_byte(seed, addr(x));
+    *x = 0;
   }
-  block_accumulate(cnt, mismatch);
+};
+
+// Reads the tags back, counts every byte that differs from them (exact, u64, one atomic per CTA into
+// *mismatch) and stores zero over the same addresses.  All PER_THREAD loads are in flight before any use.
+// Chunks are taken in ascending order, so the last stretch this kernel writes is the first one the
+// descending zero read-back reads.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS)
+tag_check_zero_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed, unsigned long long* mismatch) {
+  TagCheckZeroOp op{seed};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
+  block_accumulate(op.cnt, mismatch);
 }
 
 // Fault drill "tag_inject": flips bits of single bytes (XOR, so the byte can never keep its tag).
