@@ -42,7 +42,9 @@ extern "C" {
 #endif
 
 #define CCM_ABI_VERSION 2 /* v2: deferred release, coverage fields; ccm_transition_many and the
-                             TMA verify variant removed (one phase engine, one verify family) */
+                             TMA verify variant removed (one phase engine, one verify family).
+                             Additions that change no existing entry point or struct (the tagged
+                             gate, the dirt report) keep the version. */
 
 /* ---- status codes ------------------------------------------------------- */
 typedef enum ccm_status {
@@ -242,6 +244,50 @@ int ccm_scrub_verify_tagged(int dev, uint64_t bytes, ccm_tag_result* tag, ccm_sc
 /* ccm_scrub_verify_many with the tagged check; tag[i] belongs to devs[i]. */
 int ccm_scrub_verify_many_tagged(int n, const int* devs, uint64_t bytes, ccm_tag_result* tag,
                                  ccm_scrub_result* out, double* wall_ms);
+
+/* ---- where the dirt is: the report of a failed read-back ----------------------------------
+ * When the zero read-back of a product call (zero or tagged) counts nonzero_bytes != 0, the call runs one
+ * more kernel over what it mapped (one launch per segment on the cudaMalloc fallback) before the memory goes
+ * back to the driver, and keeps the result as the engine's dirt report; a clean call launches nothing more.
+ * Every product call on the device replaces the report.  The verdict and the status do not change.
+ *
+ * A dirty WINDOW is a 16-byte, 16-aligned address window that holds at least one non-zero byte.  Everything
+ * but the choice of records is exact: when there are more than CCM_DIRT_RECORDS dirty windows, the records
+ * are some CCM_DIRT_RECORDS of them, not necessarily the lowest. */
+#define CCM_DIRT_RECORDS 64
+typedef struct ccm_dirt_record {
+  uint64_t offset;     /* first byte of the window - va_base (product call: offset into the mapping, or into the
+                          concatenated segments on the fallback; a raw region that does not start 16-aligned
+                          has its head window begin before it: negative, two's complement) */
+  uint32_t chunk;      /* physical allocation behind the window, in creation order: the cuMemCreate handle
+                          (main-zone chunks and tail granules alike; the aliased view of "scrub_alias" reports
+                          handle 0), or the segment index on the fallback; 0 for a raw region */
+  uint16_t mask;       /* bit i: byte i of the window is non-zero (bytes outside the region count as 0) */
+  uint16_t reserved;
+  uint8_t bytes[16];   /* the window as the pass read it */
+} ccm_dirt_record;     /* 32 B */
+
+typedef struct ccm_dirt_report {
+  uint64_t nonzero_bytes;  /* non-zero bytes the locate pass counted: it recounts the read-back, and both
+                              are reported when something wrote the memory in between */
+  uint64_t dirty_windows;
+  uint64_t first_offset;   /* offset of the first / last non-zero byte from va_base */
+  uint64_t last_offset;
+  uint64_t va_base;        /* address of the first byte the pass read (fallback: of the first segment) */
+  double ms_locate;        /* CUDA-event time of the locate kernel(s) */
+  int32_t located;         /* 1: a locate pass ran; 0: the last call read back clean (or never ran) */
+  int32_t nrecords;        /* min(dirty_windows, CCM_DIRT_RECORDS), distinct windows sorted by offset */
+  int32_t truncated;       /* dirty_windows > CCM_DIRT_RECORDS */
+  int32_t reserved;
+  ccm_dirt_record records[CCM_DIRT_RECORDS];
+} ccm_dirt_report;
+
+/* The dirt report of the last product call on the CUDA device `cuda_ordinal` (located == 0 when it read
+ * back clean).  CCM_ERR_NO_CUDA when there is no such CUDA device. */
+int ccm_scrub_last_dirt(int cuda_ordinal, ccm_dirt_report* out);
+/* The locate pass on caller-owned memory (any alignment, any length; synchronises).  Reads the region and
+ * writes nothing into it; located == 1 and every record's chunk is 0. */
+int ccm_region_locate(int cuda_ordinal, const void* dptr, uint64_t bytes, void* stream, ccm_dirt_report* out);
 
 /* -- arena: the device-resident region, held across calls (bench / tests) -- */
 typedef struct ccm_arena_info {

@@ -7,8 +7,10 @@
 // verify-mode, reference main.py:521-529).  There is NO host fallback anywhere in
 // this file: without a usable CUDA device every entry point returns
 // CCM_ERR_NO_CUDA / CCM_ERR_CUDA.
+#include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cstddef>
 #include <cstring>
 #include <memory>
 #include <mutex>
@@ -89,11 +91,22 @@ static constexpr int kMaxPipeChunks = 32;
 //   [16]/[24] grab + done of scrub_st128_fast_kernel      [32]/[40] grab + done of verify_ld128_fast_kernel
 //   [48]/[56] grab + done of tag_fill_kernel              [64]/[72] grab + done of tag_check_zero_kernel
 //   [80] mismatched byte count of the current tag check
+//   [96]/[104] grab + done of locate_dirt_kernel           [112] .. [152] its six result words (LocateOut)
 // The default kernels hand their pair back zeroed (GrabCtl), so they never share words with the
 // generic kernels, whose counter is memset by the host before every launch.
-static constexpr int kCtlWords = 96;
+static constexpr int kCtlWords = 160;
 static constexpr int kNonzero = 0, kGenericGrab = 8, kScrubGrab = 16, kVerifyGrab = 32, kTagFillGrab = 48,
-                     kTagCheckGrab = 64, kMismatch = 80;
+                     kTagCheckGrab = 64, kMismatch = 80, kLocateGrab = 96, kLocateOut = 112;
+static constexpr int kLocateWords = kCtlWords - kLocateOut;  // LocateOut word k at kLocateOut + 8k
+
+// What a locate pass leaves for the host: its result words and records, copied back in one go.
+struct LocateHost {
+  unsigned long long words[kLocateWords];
+  DirtRecord records[kDirtRecords];
+};
+static_assert(sizeof(DirtRecord) == sizeof(ccm_dirt_record) && offsetof(ccm_dirt_record, bytes) == 16 &&
+              offsetof(ccm_dirt_record, mask) == 12 && kDirtRecords == CCM_DIRT_RECORDS,
+              "DirtRecord must match ccm_dirt_record");
 
 // One contiguous virtual range backed by VMM chunks (cuMemCreate / cuMemMap).
 struct VmmMapping {
@@ -116,6 +129,9 @@ struct ScrubEngine {
   int step_count = 0;
   unsigned long long* d_counter = nullptr;
   unsigned long long* h_counter = nullptr;  // pinned
+  DirtRecord* d_records = nullptr;          // the locate pass's records
+  LocateHost* h_locate = nullptr;           // pinned
+  ccm_dirt_report dirt{};                   // report of the last product call (ccm_scrub_last_dirt)
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -130,6 +146,10 @@ struct ScrubEngine {
   cudaStream_t pick(void* s) const { return s ? (cudaStream_t)s : stream; }
   // the grab word of a default kernel and its done word, one line further on
   GrabCtl ctl(int grab) const { return GrabCtl{d_counter + grab, d_counter + grab + 8}; }
+  LocateOut locate_out() const {
+    unsigned long long* w = d_counter + kLocateOut;
+    return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, d_records};
+  }
   // Waits for the background release of the previous gate (no-op when none is pending).
   double join_reaper() {
     if (!reaper.joinable()) return 0.0;
@@ -149,6 +169,9 @@ static constexpr int kFastVerifyThreads = 1024, kFastVerifyPer = 8;
 static constexpr int kTagThreads = 512, kTagPer = 16;
 #define CCM_TAG_FILL tag_fill_kernel<kTagThreads, kTagPer>
 #define CCM_TAG_CHECK tag_check_zero_kernel<kTagThreads, kTagPer>
+// The locate pass after a failed read-back: 128 KiB per grab, one persistent 512-thread CTA per SM.
+static constexpr int kLocateThreads = 512, kLocatePer = 16;
+#define CCM_LOCATE locate_dirt_kernel<kLocateThreads, kLocatePer>
 
 const char* default_kernel_names() {
   static const std::string names = [] {
@@ -178,13 +201,17 @@ int ScrubEngine::init() {
   CCM_CUDA(cudaMalloc(&d_counter, kCtlWords * sizeof(unsigned long long)));
   CCM_CUDA(cudaMemset(d_counter, 0, kCtlWords * sizeof(unsigned long long)));
   CCM_CUDA(cudaHostAlloc(&h_counter, 64, cudaHostAllocDefault));
+  // The locate pass runs with all HBM mapped: its records and their host copy are set aside now.
+  CCM_CUDA(cudaMalloc(&d_records, kDirtRecords * sizeof(DirtRecord)));
+  CCM_CUDA(cudaHostAlloc(&h_locate, sizeof(LocateHost), cudaHostAllocDefault));
   // The product call maps HBM down to the last granule; CUDA loads kernel code lazily at the
-  // first launch and that needs device memory — make the two default kernels resident now.
+  // first launch and that needs device memory — make the default kernels resident now.
   cudaFuncAttributes fa;
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_FAST_SCRUB));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_FAST_VERIFY));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_TAG_FILL));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_TAG_CHECK));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_LOCATE));
   CCM_CUDA(cudaFuncGetAttributes(&fa, xor_byte_kernel));
   size_t fr = 0;
   CCM_CUDA(cudaMemGetInfo(&fr, &total_bytes));
@@ -254,8 +281,12 @@ int engine_teardown(int ordinal) {
   e->step_count = 0;
   if (e->d_counter) cudaFree(e->d_counter);
   if (e->h_counter) cudaFreeHost(e->h_counter);
+  if (e->d_records) cudaFree(e->d_records);
+  if (e->h_locate) cudaFreeHost(e->h_locate);
   e->d_counter = nullptr;
   e->h_counter = nullptr;
+  e->d_records = nullptr;
+  e->h_locate = nullptr;
   if (e->stream) cudaStreamDestroy(e->stream);
   e->stream = nullptr;
   e->ready = false;
@@ -673,6 +704,54 @@ static int run_counted(ScrubEngine* e, cudaStream_t st, int word, uint64_t* coun
   return CCM_OK;
 }
 
+// ------------------------------------------------------------------ locate the dirt
+// One locate pass over [p, p+n) on `st` (synchronises; the caller holds e->mu).  What it found is added to `rep`
+// with its offsets moved by `shift` (the range's offset in what `rep` describes), and each new record gets the chunk
+// chunk_of(offset).  Records are kept while `rep` has room; finish_dirt() sorts them.
+template <typename ChunkOf>
+static int locate_range(ScrubEngine* e, const void* p, uint64_t n, uint64_t shift, cudaStream_t st,
+                        ccm_dirt_report* rep, ChunkOf&& chunk_of) {
+  rep->located = 1;
+  if (n == 0) return CCM_OK;
+  CCM_CUDA(cudaMemsetAsync(e->d_counter + kLocateOut, 0, kLocateWords * sizeof(unsigned long long), st));
+  float ms = 0;
+  int rc = run_timed(e, st, &ms, [&]() -> int {
+    const cudaError_t err = launch_fast(CCM_LOCATE, kLocateThreads, kLocatePer, e, kLocateGrab, st,
+                                        split_region(p, n, 16, 128), e->locate_out());
+    g_launches++;
+    if (err != cudaSuccess) { set_error("locate launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
+    return CCM_OK;
+  });
+  if (rc) return rc;
+  LocateHost& h = *e->h_locate;
+  CCM_CUDA(cudaMemcpyAsync(h.words, e->d_counter + kLocateOut, sizeof h.words, cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaMemcpyAsync(h.records, e->d_records, sizeof h.records, cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  const uint64_t nonzero = h.words[0], windows = h.words[8], first = ~h.words[16] + shift, last = h.words[24] + shift;
+  const uint64_t claimed = h.words[32] < (uint64_t)kDirtRecords ? h.words[32] : (uint64_t)kDirtRecords;
+  rep->ms_locate += ms;
+  if (windows == 0) return CCM_OK;
+  if (rep->dirty_windows == 0 || first < rep->first_offset) rep->first_offset = first;
+  if (rep->dirty_windows == 0 || last > rep->last_offset) rep->last_offset = last;
+  rep->nonzero_bytes += nonzero;
+  rep->dirty_windows += windows;
+  for (uint64_t i = 0; i < claimed && rep->nrecords < CCM_DIRT_RECORDS; ++i) {
+    ccm_dirt_record& r = rep->records[rep->nrecords++];
+    memcpy(&r, &h.records[i], sizeof r);
+    r.offset += shift;
+    r.chunk = chunk_of(r.offset);
+  }
+  return CCM_OK;
+}
+
+// Sorts the records by offset (signed: a head window that starts before the region comes first) and sets truncated.
+static void finish_dirt(ccm_dirt_report* rep) {
+  std::sort(rep->records, rep->records + rep->nrecords, [](const ccm_dirt_record& a, const ccm_dirt_record& b) {
+    return (int64_t)a.offset < (int64_t)b.offset;
+  });
+  rep->truncated = rep->dirty_windows > (uint64_t)CCM_DIRT_RECORDS;
+}
+
 int engine_arena_scrub(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, void* stream, float* ms) {
   std::lock_guard<std::mutex> g(e->mu);
   CCM_ENSURE_READY(e);
@@ -890,6 +969,24 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
   return CCM_OK;
 }
 
+// The dirt report of the fallback path: one locate pass per segment, offsets into the concatenated segments,
+// chunk = segment index.  A failure of the pass leaves the report empty; it never changes the verdict.
+static void arena_locate(ScrubEngine* e) {
+  std::lock_guard<std::mutex> g(e->mu);
+  if (!e->ready || e->segs.empty() || cudaSetDevice(e->ordinal) != cudaSuccess) return;
+  ccm_dirt_report rep;
+  memset(&rep, 0, sizeof rep);
+  rep.va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
+  uint64_t shift = 0;
+  for (size_t i = 0; i < e->segs.size(); ++i) {
+    if (locate_range(e, e->segs[i].ptr, e->segs[i].bytes, shift, e->stream, &rep, [i](uint64_t) { return (uint32_t)i; }))
+      return;
+    shift += e->segs[i].bytes;
+  }
+  finish_dirt(&rep);
+  e->dirt = rep;
+}
+
 // ------------------------------------------------------- VMM (driver API, lazy)
 // The product call maps HBM in chunks through the virtual-memory-management API so
 // that (a) the chunks sit in ONE contiguous virtual range (one verify launch) and (b)
@@ -1020,6 +1117,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   uint64_t tag_inject = drill.tag_inject;
   int tag_timed = 0;
   std::vector<std::pair<uint64_t, uint64_t>> deferred;  // tagged: main-zone ranges, checked after the last mapping
+  std::vector<std::pair<uint64_t, uint32_t>> pieces;    // (offset, handle index) of every mapped piece, ascending
   auto tag_fill = [&](uint64_t off, uint64_t n) -> int {
     cudaEvent_t* evs = tag_timed < kMaxPipeChunks ? e->tag_ev[tag_timed] : nullptr;
     if (evs) cudaEventRecord(evs[0], st);
@@ -1091,7 +1189,11 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
       break;
     }
     host_acquire += now_ms() - t0;
-    if (n > alias) m.handles.push_back(h);
+    if (alias) pieces.emplace_back(off, 0u);
+    if (n > alias) {
+      pieces.emplace_back(off + alias, (uint32_t)m.handles.size());
+      m.handles.push_back(h);
+    }
     aliased |= alias != 0;
     m.mapped = off + n;
     // fault drill: the previous tenant's data, in place before anything scrubs this chunk
@@ -1160,6 +1262,21 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
       tag->va_base = mapped ? (uint64_t)m.base : 0;
     }
   }
+  // ---- a failed read-back: where is the dirt?  One more launch, before the mapping goes back -------------
+  if (rc == CCM_OK && r->nonzero_bytes != 0) {
+    ccm_dirt_report rep;
+    memset(&rep, 0, sizeof rep);
+    rep.va_base = (uint64_t)m.base;
+    auto chunk_of = [&](uint64_t o) {
+      auto it = std::upper_bound(pieces.begin(), pieces.end(), o,
+                                 [](uint64_t v, const std::pair<uint64_t, uint32_t>& pc) { return v < pc.first; });
+      return it == pieces.begin() ? 0u : std::prev(it)->second;
+    };
+    if (locate_range(e, (const void*)m.base, mapped, 0, st, &rep, chunk_of) == CCM_OK) {  // never changes the verdict
+      finish_dirt(&rep);
+      e->dirt = rep;
+    }
+  }
   // ---- give the HBM back: on the reaper (default) or right here -----------------------
   if (rc == CCM_OK && async_release_enabled()) {
     r->release_deferred = 1;
@@ -1191,6 +1308,10 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   ScrubDrill drill = current_scrub_drill();
   drill.inject = inject;
   ccm_tag_result* tag = current_tag_call();
+  {
+    std::lock_guard<std::mutex> g(e->mu);
+    memset(&e->dirt, 0, sizeof e->dirt);  // every call replaces the report of the last one
+  }
   ccm_scrub_result r;
   memset(&r, 0, sizeof r);
   r.bytes_requested = bytes;
@@ -1222,6 +1343,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       }
       if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
       if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
+      if (rc == CCM_OK && nz != 0) arena_locate(e);
       r.ms_scrub = ms_s;
       r.ms_verify = ms_v;
       r.nonzero_bytes = nz;
@@ -1333,4 +1455,36 @@ extern "C" int ccm_region_tag_check_zero(int cuda_ordinal, void* dptr, uint64_t 
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->pick(stream);
   return run_counted(e, st, kMismatch, mismatch, ms, [&] { return tag_check_range(e, dptr, bytes, seed, st); });
+}
+
+// ------------------------------------------------------------------------- dirt report
+extern "C" int ccm_scrub_last_dirt(int cuda_ordinal, ccm_dirt_report* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  *out = e->dirt;
+  return CCM_OK;
+}
+
+extern "C" int ccm_region_locate(int cuda_ordinal, const void* dptr, uint64_t bytes, void* stream, ccm_dirt_report* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  ScrubEngine* e = engine_for(cuda_ordinal);
+  if (!e) return CCM_ERR_NO_CUDA;
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  ccm_dirt_report rep;
+  memset(&rep, 0, sizeof rep);
+  rep.va_base = (uint64_t)(uintptr_t)dptr;
+  if (int rc = locate_range(e, dptr, bytes, 0, e->pick(stream), &rep, [](uint64_t) { return 0u; })) return rc;
+  finish_dirt(&rep);
+  *out = rep;
+  return CCM_OK;
 }

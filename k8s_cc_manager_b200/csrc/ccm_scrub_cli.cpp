@@ -4,7 +4,8 @@
 //
 // Runs the concurrent gate (ccm_scrub_verify_many, or ccm_scrub_verify_many_tagged with --check tagged)
 // and prints ONE JSON line with the same fields as k8s_cc_manager_b200.devices.ScrubReport (the
-// tagged-gate fields only with --check tagged).  Exit 0: every GPU clean; 3: gate failed;
+// tagged-gate fields only with --check tagged, "dirt" only for a GPU whose read-back found non-zero bytes: where
+// they are, as ccm_scrub_last_dirt reports it).  Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
 // post-reset step.
@@ -15,6 +16,22 @@
 #include <vector>
 
 #include "ccm.h"
+
+// The "dirt" object: the fields of k8s_cc_manager_b200.devices.DirtReport, records with their bytes in hex.
+static void print_dirt(const ccm_dirt_report& d) {
+  printf(", \"dirt\": {\"nonzero_bytes\": %llu, \"dirty_windows\": %llu, \"first_offset\": %llu, \"last_offset\": %llu, "
+         "\"va_base\": %llu, \"ms_locate\": %.3f, \"located\": %d, \"truncated\": %d, \"records\": [",
+         (unsigned long long)d.nonzero_bytes, (unsigned long long)d.dirty_windows, (unsigned long long)d.first_offset,
+         (unsigned long long)d.last_offset, (unsigned long long)d.va_base, d.ms_locate, d.located, d.truncated);
+  for (int k = 0; k < d.nrecords; ++k) {
+    const ccm_dirt_record& w = d.records[k];
+    printf("%s{\"offset\": %lld, \"chunk\": %u, \"mask\": %u, \"bytes\": \"", k ? ", " : "", (long long)w.offset,
+           w.chunk, (unsigned)w.mask);
+    for (int b = 0; b < 16; ++b) printf("%02x", w.bytes[b]);
+    printf("\"}");
+  }
+  printf("]}");
+}
 
 static int usage(const char* argv0) {
   fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] (--all | --bdf <bdf> ...)\n",
@@ -48,19 +65,24 @@ int main(int argc, char** argv) {
   ccm_enumerate(nullptr, 0, &n);
   std::vector<ccm_dev_info> infos(n > 0 ? n : 1);
   ccm_enumerate(infos.data(), n, &n);
-  std::vector<int> devs;
+  std::vector<int> devs, ordinals;
   std::vector<std::string> names;
   if (all) {
     for (int i = 0; i < n; ++i)
-      if (infos[i].kind == CCM_KIND_GPU) { devs.push_back(infos[i].index); names.emplace_back(infos[i].bdf); }
+      if (infos[i].kind == CCM_KIND_GPU) {
+        devs.push_back(infos[i].index);
+        ordinals.push_back(infos[i].cuda_ordinal);
+        names.emplace_back(infos[i].bdf);
+      }
   } else {
     for (auto& want : bdfs) {
       for (auto& c : want) c = (char)tolower(c);
-      int found = -1;
+      int found = -1, ordinal = -1;
       for (int i = 0; i < n; ++i)
-        if (infos[i].kind == CCM_KIND_GPU && want == infos[i].bdf) found = infos[i].index;
+        if (infos[i].kind == CCM_KIND_GPU && want == infos[i].bdf) { found = infos[i].index; ordinal = infos[i].cuda_ordinal; }
       if (found < 0) { fprintf(stderr, "unknown GPU %s\n", want.c_str()); return 1; }
       devs.push_back(found);
+      ordinals.push_back(ordinal);
       names.push_back(want);
     }
   }
@@ -88,6 +110,8 @@ int main(int argc, char** argv) {
       printf(", \"check\": \"tagged\", \"tag_seed\": %u, \"mismatch_bytes\": %llu, \"ms_tag\": %.3f, \"ms_check\": %.3f",
              t.seed, (unsigned long long)t.mismatch_bytes, t.ms_tag, t.ms_check);
     }
+    ccm_dirt_report d;
+    if (r.nonzero_bytes != 0 && ccm_scrub_last_dirt(ordinals[i], &d) == CCM_OK) print_dirt(d);
     printf("}");
   }
   printf("]}\n");

@@ -28,9 +28,10 @@
 //   scrub_st_kernel / verify_ld_kernel                   any shape / width / policy / schedule
 //   scrub_tma_kernel                                     cp.async.bulk stores from one zero tile
 //   tag_fill_kernel / tag_check_zero_kernel              the tagged gate's known-answer pass
+//   locate_dirt_kernel                                   where the dirt is, after a failed read-back
 //   fill_pattern_kernel                                  seeded test pattern (tests only)
 // The grab loop (grab_chunks) and the epilogue after the last whole chunk or tile (finish_region,
-// ragged_bytes) are written once.  The four compile-time-shape kernels are one frame (default_kernel)
+// ragged_bytes) are written once.  The five compile-time-shape kernels are one frame (default_kernel)
 // around an op struct that says what happens to each chunk, leftover vector and ragged byte.
 #pragma once
 #include <cstdint>
@@ -643,6 +644,190 @@ tag_check_zero_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t see
 
 // Fault drill "tag_inject": flips bits of single bytes (XOR, so the byte can never keep its tag).
 __global__ void xor_byte_kernel(uint8_t* p) { *p ^= 0xA5; }
+
+// ------------------------------------------------------------ locate the dirt
+// When the zero read-back counted dirt, this pass says where it is.  A dirty WINDOW is a 16-byte, 16-aligned address
+// window holding at least one non-zero byte of the region; in the body a window is one vector.  Results: the exact
+// number of non-zero bytes and of dirty windows, the offsets (from the region base) of the first and the last
+// non-zero byte, and up to kDirtRecords records of (window offset, mask of its non-zero bytes, its 16 bytes).
+constexpr int kDirtRecords = 64;
+
+struct DirtRecord {       // layout of ccm_dirt_record (include/ccm.h); `chunk` is filled in by the host
+  uint64_t offset;        // window address - region base (negative, two's complement, for the head window of a
+                          // region that does not start 16-aligned)
+  uint32_t chunk;
+  uint16_t mask;          // bit i: byte i of the window is non-zero (bytes outside the region read as 0)
+  uint16_t reserved;
+  uint4 bytes;
+};
+
+// Result words of one pass, each on its own line of the engine's control block; zero before the launch.
+struct LocateOut {
+  unsigned long long* nonzero;    // += non-zero bytes
+  unsigned long long* windows;    // += dirty windows
+  unsigned long long* first_inv;  // max of ~offset of the first non-zero byte (0: none)
+  unsigned long long* last;       // max of the offset of the last non-zero byte
+  unsigned long long* slots;      // record slots claimed (may run past kDirtRecords)
+  unsigned long long* full;       // set once kDirtRecords slots are taken
+  DirtRecord* records;
+};
+
+// Bit 7 of each byte of the result is set iff that byte of w is non-zero (as in nonzero_bytes_in_word).
+__device__ __forceinline__ uint32_t nonzero_byte_flags(uint32_t w) {
+  return (((w & 0x7f7f7f7fu) + 0x7f7f7f7fu) | w) & 0x80808080u;
+}
+
+// 16-bit mask of the non-zero bytes of one vector.
+__device__ __forceinline__ uint32_t nonzero_mask16(const Vec16& v) {
+  uint32_t m = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint32_t f = nonzero_byte_flags(v.w[k]);
+    m |= (((f >> 7) & 1u) | ((f >> 14) & 2u) | ((f >> 21) & 4u) | ((f >> 28) & 8u)) << (4 * k);
+  }
+  return m;
+}
+
+// Counts, first / last offset and window count stay in registers; only records go through memory.  A record slot
+// is claimed with an atomicAdd only while the "records full" word is clear, and a thread that has seen it set (or
+// drew the last slot or a later one) never reads it again: a region that is dirty everywhere would otherwise serialise one
+// atomic per vector on a single address, about 5e9 of them at whole HBM.  The ragged head and tail are not taken
+// byte by byte (byte() does nothing): locate_dirt_kernel takes them window by window, so no window is counted or
+// recorded twice.
+struct LocateOp {
+  LocateOut out;
+  const uint8_t* base;
+  uint64_t bytes = 0, windows = 0, first_inv = 0, last = 0;
+  bool full_seen = false;
+
+  // A record slot (>= kDirtRecords: none left).
+  __device__ __forceinline__ uint64_t claim() {
+    if (*(volatile unsigned long long*)out.full) { full_seen = true; return kDirtRecords; }
+    const uint64_t slot = atomicAdd(out.slots, 1ull);
+    if (slot + 1 >= (uint64_t)kDirtRecords) { *(volatile unsigned long long*)out.full = 1; full_seen = true; }
+    return slot;
+  }
+
+  // Books one window at offset `off` whose non-zero bytes are `mask` (!= 0).
+  __device__ __forceinline__ void tally(uint64_t off, uint32_t mask) {
+    bytes += __popc(mask);
+    windows += 1;
+    const uint64_t lo = off + (uint64_t)(__ffs(mask) - 1), hi = off + (uint64_t)(31 - __clz(mask));
+    first_inv = max(first_inv, (uint64_t)~lo);
+    last = max(last, hi);
+  }
+
+  __device__ __forceinline__ void record(uint64_t slot, uint64_t off, uint32_t mask, const Vec16& v) {
+    DirtRecord r;
+    r.offset = off;
+    r.chunk = 0;
+    r.mask = (uint16_t)mask;
+    r.reserved = 0;
+    r.bytes = make_uint4(v.w[0], v.w[1], v.w[2], v.w[3]);
+    out.records[slot] = r;
+  }
+
+  template <int THREADS, int PER_THREAD>
+  __device__ __forceinline__ void chunk(const uint8_t* p) {
+    Vec16 v[PER_THREAD];
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16<kPolStreaming>(p + (uint32_t)u * THREADS * 16u, 0);  // all loads first
+    uint32_t any = 0;
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) any |= v[u].w[k];
+    if (any != 0) {  // rare except in a flood
+      const uint64_t off0 = (uint64_t)(p - base);
+#pragma unroll
+      for (int u = 0; u < PER_THREAD; ++u) window(off0 + (uint32_t)u * THREADS * 16u, nonzero_mask16(v[u]), v[u]);
+    }
+  }
+
+  // One window given as its aligned vector (a body vector, or a head / tail window from ragged_windows).
+  __device__ __forceinline__ void window(uint64_t off, uint32_t mask, const Vec16& v) {
+    if (mask == 0) return;
+    tally(off, mask);
+    if (full_seen) return;
+    const uint64_t slot = claim();
+    if (slot < (uint64_t)kDirtRecords) record(slot, off, mask, v);
+  }
+
+  __device__ __forceinline__ void vec(const uint8_t* p) {
+    const Vec16 v = ld16<kPolStreaming>(p, 0);
+    window((uint64_t)(p - base), nonzero_mask16(v), v);
+  }
+
+  __device__ __forceinline__ void byte(const uint8_t*) {}
+
+  // CTA 0: the windows of the ragged head and tail, one thread per window, bytes outside the region as 0.
+  __device__ __forceinline__ void ragged_windows(const RegionSplit& s) {
+    if (blockIdx.x != 0) return;
+    const uint64_t a0 = addr(s.base);
+    const uint64_t head_end = a0 + s.head, tail_start = head_end + s.body_vecs * 16, end = tail_start + s.tail;
+    const uint64_t first_win = a0 & ~15ull;
+    const uint64_t nhead = s.head ? (head_end - first_win + 15) / 16 : 0;   // at most 8
+    const uint64_t t = threadIdx.x;
+    uint64_t w0 = 0, lo = 0, hi = 0;
+    if (t < nhead) { w0 = first_win + 16 * t; lo = max(w0, a0); hi = min(w0 + 16, head_end); }
+    else if (t == nhead && s.tail) { w0 = tail_start; lo = tail_start; hi = end; }
+    else return;
+    Vec16 v = {{0, 0, 0, 0}};
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+      if (w0 + i >= lo && w0 + i < hi) v.w[i >> 2] |= (uint32_t)*(const uint8_t*)(uintptr_t)(w0 + i) << (8 * (i & 3));
+    window(w0 - a0, nonzero_mask16(v), v);
+  }
+
+  // One atomic per result word per CTA (skipped when the CTA found nothing), after a block reduction.
+  __device__ __forceinline__ void flush() {
+    __shared__ uint64_t part[4][32];
+    uint64_t a = bytes, b = windows, c = first_inv, d = last;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      a += __shfl_xor_sync(0xffffffffu, a, o);
+      b += __shfl_xor_sync(0xffffffffu, b, o);
+      c = max(c, __shfl_xor_sync(0xffffffffu, c, o));
+      d = max(d, __shfl_xor_sync(0xffffffffu, d, o));
+    }
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) { part[0][warp] = a; part[1][warp] = b; part[2][warp] = c; part[3][warp] = d; }
+    __syncthreads();
+    if (warp == 0) {
+      const bool in = lane < ((blockDim.x + 31) >> 5);
+      a = in ? part[0][lane] : 0;
+      b = in ? part[1][lane] : 0;
+      c = in ? part[2][lane] : 0;
+      d = in ? part[3][lane] : 0;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        a += __shfl_xor_sync(0xffffffffu, a, o);
+        b += __shfl_xor_sync(0xffffffffu, b, o);
+        c = max(c, __shfl_xor_sync(0xffffffffu, c, o));
+        d = max(d, __shfl_xor_sync(0xffffffffu, d, o));
+      }
+      if (lane == 0 && b != 0) {
+        atomicAdd(out.nonzero, (unsigned long long)a);
+        atomicAdd(out.windows, (unsigned long long)b);
+        atomicMax(out.first_inv, (unsigned long long)c);
+        atomicMax(out.last, (unsigned long long)d);
+      }
+    }
+  }
+};
+
+// Reads the region (writes nothing into it) and reports where its non-zero bytes are.  Frame, loads and batching of
+// verify_ld128_fast_kernel: persistent CTAs, one THREADS * PER_THREAD * 16-byte chunk per grab in ascending order, all
+// PER_THREAD loads in flight, then OR; only batches whose OR is non-zero do more work.  Minimum one CTA per SM in the
+// launch bounds: the compiler may then use the registers the flood path needs instead of spilling it.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS, 1)
+locate_dirt_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, LocateOut out) {
+  LocateOp op{out, s.base};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
+  op.ragged_windows(s);
+  op.flush();
+}
 
 // ------------------------------------------------------------ test scaffolding
 __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {

@@ -21,25 +21,102 @@ from __future__ import annotations
 
 import ctypes as C
 import dataclasses
-from dataclasses import dataclass
-from typing import List, Sequence, Tuple
+from dataclasses import dataclass, field
+from typing import List, Optional, Sequence, Tuple
 
 from . import _native as N
 
 
 class GpuError(Exception):
-    """Raised for any failed device operation (reference: gpu.GpuError)."""
+    """Raised for any failed device operation (reference: gpu.GpuError).  A scrub that read back dirt
+    carries its DirtReport as `.dirt`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
         self.status = status
+        self.dirt: "Optional[DirtReport]" = None
+
+
+def _error(rc: int, what: str, bdf: str = "") -> "Optional[GpuError]":
+    if rc == N.OK:
+        return None
+    detail = N.last_error()
+    where = f" on {bdf}" if bdf else ""
+    return GpuError(f"{what}{where}: {N.strerror(rc)}" + (f" ({detail})" if detail else ""), rc)
 
 
 def _check(rc: int, what: str, bdf: str = "") -> None:
-    if rc != N.OK:
-        detail = N.last_error()
-        where = f" on {bdf}" if bdf else ""
-        raise GpuError(f"{what}{where}: {N.strerror(rc)}" + (f" ({detail})" if detail else ""), rc)
+    err = _error(rc, what, bdf)
+    if err is not None:
+        raise err
+
+
+def _signed64(x: int) -> int:
+    return x - (1 << 64) if x >= 1 << 63 else x
+
+
+@dataclass
+class DirtWindow:
+    """One dirty 16-byte, 16-aligned window (include/ccm.h: ccm_dirt_record)."""
+    offset: int      # first byte of the window from the report's va_base (negative only for the head window
+                     # of a raw region that does not start 16-aligned)
+    chunk: int       # physical allocation behind it, in creation order (fallback: segment index)
+    mask: int        # bit i: byte i is non-zero
+    bytes: str       # the 16 bytes as read, hex
+
+    def describe(self) -> str:
+        return f"+{self.offset:#x} chunk {self.chunk} mask {self.mask:04x} [{self.bytes}]"
+
+
+@dataclass
+class DirtReport:
+    """Where the read-back of a failed scrub found its non-zero bytes (include/ccm.h: ccm_dirt_report).
+    Every field but the choice of `records` is exact; records are distinct windows sorted by offset, all of
+    them unless `truncated`."""
+    nonzero_bytes: int       # the locate pass's own recount
+    dirty_windows: int
+    first_offset: int        # first / last non-zero byte, from va_base
+    last_offset: int
+    va_base: int
+    ms_locate: float
+    located: int             # 0: no locate pass ran (the call read back clean)
+    truncated: int
+    records: List[DirtWindow] = field(default_factory=list)
+
+    @classmethod
+    def from_native(cls, d: N.DirtReport) -> "DirtReport":
+        recs = [DirtWindow(_signed64(r.offset), r.chunk, r.mask, bytes(r.bytes).hex())
+                for r in d.records[:d.nrecords]]
+        return cls(d.nonzero_bytes, d.dirty_windows, d.first_offset, d.last_offset, d.va_base, d.ms_locate,
+                   d.located, d.truncated, recs)
+
+    @classmethod
+    def from_json(cls, d: dict) -> "DirtReport":
+        return cls(**{**d, "records": [DirtWindow(**r) for r in d["records"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    @property
+    def chunks(self) -> List[int]:
+        return sorted({r.chunk for r in self.records})
+
+    def summary(self, first: int = 4) -> str:
+        """One line for an operator: extent, window count, chunks involved and the first few windows."""
+        more = " (records truncated)" if self.truncated else ""
+        recs = "; ".join(r.describe() for r in self.records[:first])
+        return (f"non-zero bytes at offsets {self.first_offset:#x}..{self.last_offset:#x} of va {self.va_base:#x}, "
+                f"{self.nonzero_bytes} bytes in {self.dirty_windows} dirty 16-byte windows{more}, "
+                f"chunks {self.chunks}; first windows: {recs}")
+
+
+def last_dirt(cuda_ordinal: int) -> "Optional[DirtReport]":
+    """The dirt report of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_dirt);
+    None when it cannot be read."""
+    d = N.DirtReport()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_dirt(cuda_ordinal, C.byref(d)) != N.OK:
+        return None
+    return DirtReport.from_native(d)
 
 
 @dataclass
@@ -68,6 +145,9 @@ class ScrubReport:
     mismatch_bytes: int = 0          # bytes that did not hold their tag
     ms_tag: float = 0.0              # tag-fill kernels
     ms_check: float = 0.0            # check-and-zero kernels
+    # Where the dirt is (a DirtReport), set for every report with nonzero_bytes != 0.  Not a dataclass field,
+    # so positional construction, the field list and the JSON of a clean report stay as they were.
+    dirt = None
 
     @property
     def clean(self) -> bool:
@@ -103,12 +183,25 @@ class ScrubReport:
         return rep
 
     def as_json(self) -> dict:
-        """The report as the scrub workers print it: the tagged-gate fields only for a tagged call."""
+        """The report as the scrub workers print it: the tagged-gate fields only for a tagged call, "dirt" only
+        when there is a dirt report."""
         d = dataclasses.asdict(self)
         if self.check == "zero":
             for name in TAG_FIELDS:
                 del d[name]
+        if self.dirt is not None:
+            d["dirt"] = self.dirt.as_json()
         return d
+
+    @classmethod
+    def from_json(cls, d: dict) -> "ScrubReport":
+        """Inverse of as_json."""
+        d = dict(d)
+        dirt = d.pop("dirt", None)
+        rep = cls(**d)
+        if dirt is not None:
+            rep.dirt = DirtReport.from_json(dirt)
+        return rep
 
 
 # ScrubReport fields that only a tagged call reports
@@ -181,17 +274,23 @@ class NvidiaDevice:
         (include/ccm.h: ccm_scrub_verify_tagged).
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
-        if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.
+        if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
+        found non-zero bytes, the report (or the GpuError, as `.dirt`) carries where they are.
         """
-        res = N.ScrubResult()
+        res, tag = N.ScrubResult(), None
         if _check_mode(check):
             tag = N.TagResult()
             rc = N.lib().ccm_scrub_verify_tagged(self.index, nbytes, C.byref(tag), C.byref(res))
-            _check(rc, "scrub_and_verify", self.bdf)
-            return ScrubReport.from_native(self.bdf, res, tag)
-        rc = N.lib().ccm_scrub_verify(self.index, nbytes, C.byref(res))
-        _check(rc, "scrub_and_verify", self.bdf)
-        return ScrubReport.from_native(self.bdf, res)
+        else:
+            rc = N.lib().ccm_scrub_verify(self.index, nbytes, C.byref(res))
+        err = _error(rc, "scrub_and_verify", self.bdf)   # the library's error text, before anything else runs
+        rep = ScrubReport.from_native(self.bdf, res, tag)
+        if rep.nonzero_bytes:
+            rep.dirt = last_dirt(self.cuda_ordinal)
+        if err is not None:
+            err.dirt = rep.dirt
+            raise err
+        return rep
 
     def wait_scrub_released(self) -> Tuple[float, float]:
         """Blocks until the HBM of the last scrub_and_verify() is back with the driver (libccm
@@ -247,12 +346,16 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
     idx = (C.c_int * n)(*[d.index for d in devices])
     res = (N.ScrubResult * n)()
     wall = C.c_double(0.0)
+    tags = (N.TagResult * n)() if tagged else None
     if tagged:
-        tags = (N.TagResult * n)()
         N.lib().ccm_scrub_verify_many_tagged(n, idx, nbytes, tags, res, C.byref(wall))
-        return [ScrubReport.from_native(d.bdf, res[i], tags[i]) for i, d in enumerate(devices)], wall.value
-    N.lib().ccm_scrub_verify_many(n, idx, nbytes, res, C.byref(wall))
-    return [ScrubReport.from_native(d.bdf, res[i]) for i, d in enumerate(devices)], wall.value
+    else:
+        N.lib().ccm_scrub_verify_many(n, idx, nbytes, res, C.byref(wall))
+    reports = [ScrubReport.from_native(d.bdf, res[i], tags[i] if tagged else None) for i, d in enumerate(devices)]
+    for rep, d in zip(reports, devices):
+        if rep.nonzero_bytes:
+            rep.dirt = last_dirt(d.cuda_ordinal)
+    return reports, wall.value
 
 
 def release_cuda_contexts(devices: Sequence[NvidiaDevice]) -> float:

@@ -531,7 +531,7 @@ class CCManager:
         if proc.returncode not in (0, 3) or not lines:
             raise ScrubFailure(f"scrub worker failed (exit {proc.returncode}): {proc.stderr.strip()[-500:]}")
         payload = _json.loads(lines[-1])
-        return [_devices.ScrubReport(**r) for r in payload["reports"]]
+        return [_devices.ScrubReport.from_json(r) for r in payload["reports"]]
 
     def _scrub_checked(self, gpu):
         """The tagged gate on one device.  A device that cannot run it fails the gate: it is never
@@ -546,6 +546,13 @@ class CCManager:
             raise ScrubFailure(f"device {gpu.bdf} returned a {getattr(rep, 'check', 'zero')} scrub report for "
                                f"CC_SCRUB_CHECK={self.scrub_check}; refusing to release it")
         return rep
+
+    def _note_dirt(self, bdf: str, dirt) -> None:
+        """Logs where a failed read-back found its non-zero bytes and keeps the report in
+        last_transition["scrub_dirt"][bdf]: the gate hands the memory back right afterwards, so this is
+        the only look anyone gets at it."""
+        self.last_transition.setdefault("scrub_dirt", {})[bdf] = dirt
+        logger.error("HBM dirt on %s: %s", bdf, dirt.summary())
 
     def _run_scrub(self, gpus: list) -> None:
         started = time.perf_counter()
@@ -565,13 +572,21 @@ class CCManager:
             def one(gpu):
                 if not hasattr(gpu, "scrub_and_verify"):
                     raise ScrubFailure(f"device {gpu.bdf} offers no HBM scrub; refusing to release it")
-                if self.scrub_check == "zero":
-                    return gpu.scrub_and_verify(self.scrub_bytes)   # the call every scrubbing device takes
-                return self._scrub_checked(gpu)
+                try:
+                    if self.scrub_check == "zero":
+                        return gpu.scrub_and_verify(self.scrub_bytes)   # the call every scrubbing device takes
+                    return self._scrub_checked(gpu)
+                except GpuError as exc:
+                    if getattr(exc, "dirt", None) is not None:
+                        self._note_dirt(gpu.bdf, exc.dirt)
+                    raise
             reports = self._fan_out(gpus, one, "scrub")
         elapsed = time.perf_counter() - started
         self.last_transition.setdefault("phase_seconds", {})["scrub"] = elapsed
         self.last_transition["scrub"] = reports
+        for rep in reports:
+            if getattr(rep, "dirt", None) is not None:
+                self._note_dirt(rep.bdf, rep.dirt)
         for rep in reports:
             mismatch = getattr(rep, "mismatch_bytes", 0)
             if rep.status != 0 or rep.nonzero_bytes != 0 or mismatch != 0:
