@@ -289,6 +289,70 @@ int ccm_scrub_last_dirt(int cuda_ordinal, ccm_dirt_report* out);
  * writes nothing into it; located == 1 and every record's chunk is 0. */
 int ccm_region_locate(int cuda_ordinal, const void* dptr, uint64_t bytes, void* stream, ccm_dirt_report* out);
 
+/* ---- where the tags were wrong: the report of a failed tagged check ----------------------------
+ * The tagged check-and-zero kernel books, in the same pass that counts mismatch_bytes, every 16-byte, 16-aligned
+ * window that differs from its tags; a check that finds nothing costs nothing more (no launch, memset or copy).
+ * When a tagged product call counts tag->mismatch_bytes != 0, it copies that book once after its last kernel and
+ * keeps it, classified, as the engine's mismatch report.  Every product call on the device replaces the report.
+ * The verdict, its precedence and the dirt report do not change.
+ *
+ * EXACT: mismatch_bytes, mismatch_windows, zero_windows, first_offset, last_offset.  The split of the other
+ * windows between ALIAS, PARTIAL and FOREIGN is known for the records only (telling them apart needs the
+ * decode below, which is not in the kernel's loop); with more than CCM_DIRT_RECORDS mismatched windows the records
+ * are some CCM_DIRT_RECORDS of them, not necessarily the lowest.
+ *
+ * Each record gets the first kind that fits, in this order:
+ *   CCM_MISMATCH_ZERO     every byte of the window inside the region reads 0 (the fill never reached it, or
+ *                         something zeroed it afterwards: e.g. the check of a second view got there first);
+ *   CCM_MISMATCH_ALIAS    the bytes are exactly this call's tags of a DIFFERENT 16-aligned window inside what the
+ *                         call mapped (the region, for ccm_region_tag_check_locate): two virtual views of one
+ *                         physical range.  source_offset / source_chunk name that window.  The decode: the tag is
+ *                         a bijection of the address within each 16 GiB window, so one whole 4-byte word of the
+ *                         window is inverted for every 16 GiB window the mapping spans, and a candidate is kept
+ *                         only if every byte of the window equals its tag.  A window with no whole word inside
+ *                         the region is never ALIAS;
+ *   CCM_MISMATCH_PARTIAL  some byte still holds its own tag: flipped or overwritten bytes in a tagged window;
+ *   CCM_MISMATCH_FOREIGN  anything else: data this call did not write (another writer, a stale mapping). */
+typedef enum ccm_mismatch_kind {
+  CCM_MISMATCH_ZERO = 1,
+  CCM_MISMATCH_ALIAS = 2,
+  CCM_MISMATCH_PARTIAL = 3,
+  CCM_MISMATCH_FOREIGN = 4
+} ccm_mismatch_kind;
+
+typedef struct ccm_mismatch_record {
+  uint64_t offset;         /* first byte of the window - va_base (as ccm_dirt_record.offset) */
+  uint32_t chunk;          /* physical allocation behind the window (as ccm_dirt_record.chunk) */
+  uint16_t mask;           /* bit i: byte i of the window differs from its tag (bytes outside the region: 0) */
+  uint16_t kind;           /* ccm_mismatch_kind */
+  uint64_t source_offset;  /* ALIAS: the window whose tags these are, - va_base; otherwise 0 */
+  uint32_t source_chunk;   /* ALIAS: the physical allocation behind it; otherwise 0 */
+  uint32_t reserved;
+  uint8_t bytes[16];       /* the window as the check read it, before it zeroed it */
+} ccm_mismatch_record;     /* 48 B */
+
+typedef struct ccm_mismatch_report {
+  uint64_t mismatch_bytes;    /* bytes that did not hold their tag (== ccm_tag_result.mismatch_bytes) */
+  uint64_t mismatch_windows;  /* windows with at least one such byte */
+  uint64_t zero_windows;      /* of those, windows whose bytes inside the region all read 0 */
+  uint64_t first_offset;      /* first / last mismatched byte, from va_base */
+  uint64_t last_offset;
+  uint64_t va_base;           /* as ccm_dirt_report.va_base */
+  uint32_t seed;              /* the tags' seed */
+  int32_t located;            /* 1: the report describes a failed check; 0: the last call's check was clean */
+  int32_t nrecords;           /* min(mismatch_windows, CCM_DIRT_RECORDS), distinct windows sorted by signed offset */
+  int32_t truncated;          /* mismatch_windows > CCM_DIRT_RECORDS */
+  ccm_mismatch_record records[CCM_DIRT_RECORDS];
+} ccm_mismatch_report;
+
+/* The mismatch report of the last product call on the CUDA device `cuda_ordinal` (located == 0 when its tagged
+ * check was clean, or it was not tagged).  CCM_ERR_NO_CUDA when there is no such CUDA device. */
+int ccm_scrub_last_mismatch(int cuda_ordinal, ccm_mismatch_report* out);
+/* ccm_region_tag_check_zero on caller-owned memory that also fills `out` (synchronises; any alignment, any
+ * length).  located == 1, every record's chunk is 0 and the ALIAS search is limited to the region. */
+int ccm_region_tag_check_locate(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream,
+                                ccm_mismatch_report* out);
+
 /* -- arena: the device-resident region, held across calls (bench / tests) -- */
 typedef struct ccm_arena_info {
   uint64_t bytes;              /* total bytes held                              */

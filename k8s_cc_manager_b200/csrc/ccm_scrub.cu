@@ -22,6 +22,7 @@
 #include <cuda_runtime.h>
 
 #include "ccm_internal.h"
+#include "ccm_mismatch.h"
 #include "scrub_kernels.cuh"
 
 namespace ccm {
@@ -92,12 +93,16 @@ static constexpr int kMaxPipeChunks = 32;
 //   [48]/[56] grab + done of tag_fill_kernel              [64]/[72] grab + done of tag_check_zero_kernel
 //   [80] mismatched byte count of the current tag check
 //   [96]/[104] grab + done of locate_dirt_kernel           [112] .. [152] its six result words (LocateOut)
+//   [160] .. [200] the six words of tag_check_zero_kernel's window book (LocateOut): zero before and after
+//                  every call, because a check that finds nothing never writes them and the host re-zeroes
+//                  them after a check that did (or that an error cut short)
 // The default kernels hand their pair back zeroed (GrabCtl), so they never share words with the
 // generic kernels, whose counter is memset by the host before every launch.
-static constexpr int kCtlWords = 160;
+static constexpr int kBookWords = 48;   // LocateOut word k at <first word> + 8k
 static constexpr int kNonzero = 0, kGenericGrab = 8, kScrubGrab = 16, kVerifyGrab = 32, kTagFillGrab = 48,
-                     kTagCheckGrab = 64, kMismatch = 80, kLocateGrab = 96, kLocateOut = 112;
-static constexpr int kLocateWords = kCtlWords - kLocateOut;  // LocateOut word k at kLocateOut + 8k
+                     kTagCheckGrab = 64, kMismatch = 80, kLocateGrab = 96, kLocateOut = 112, kCheckOut = 160;
+static constexpr int kCtlWords = kCheckOut + kBookWords;
+static constexpr int kLocateWords = kBookWords;
 
 // What a locate pass leaves for the host: its result words and records, copied back in one go.
 struct LocateHost {
@@ -107,6 +112,15 @@ struct LocateHost {
 static_assert(sizeof(DirtRecord) == sizeof(ccm_dirt_record) && offsetof(ccm_dirt_record, bytes) == 16 &&
               offsetof(ccm_dirt_record, mask) == 12 && kDirtRecords == CCM_DIRT_RECORDS,
               "DirtRecord must match ccm_dirt_record");
+static_assert(sizeof(ccm_mismatch_record) == 48 && offsetof(ccm_mismatch_record, mask) == offsetof(DirtRecord, mask) &&
+              offsetof(ccm_mismatch_record, chunk) == offsetof(DirtRecord, chunk) &&
+              offsetof(ccm_mismatch_record, source_offset) == 16 && offsetof(ccm_mismatch_record, bytes) == 32 &&
+              sizeof(ccm_mismatch_report) == 64 + 48 * CCM_DIRT_RECORDS,
+              "ccm_mismatch_record must keep its 48-byte layout");
+static_assert(ccm_mismatch::kK1 == kTagK1 && ccm_mismatch::kK2 == kTagK2, "host and device tags must agree");
+static_assert(ccm_mismatch::kZero == CCM_MISMATCH_ZERO && ccm_mismatch::kAlias == CCM_MISMATCH_ALIAS &&
+              ccm_mismatch::kPartial == CCM_MISMATCH_PARTIAL && ccm_mismatch::kForeign == CCM_MISMATCH_FOREIGN,
+              "ccm_mismatch.h kinds must match ccm_mismatch_kind");
 
 // One contiguous virtual range backed by VMM chunks (cuMemCreate / cuMemMap).
 struct VmmMapping {
@@ -132,6 +146,9 @@ struct ScrubEngine {
   DirtRecord* d_records = nullptr;          // the locate pass's records
   LocateHost* h_locate = nullptr;           // pinned
   ccm_dirt_report dirt{};                   // report of the last product call (ccm_scrub_last_dirt)
+  DirtRecord* d_check_records = nullptr;    // the tag check's records
+  LocateHost* h_check = nullptr;            // pinned
+  ccm_mismatch_report mismatch{};           // report of the last product call (ccm_scrub_last_mismatch)
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -149,6 +166,10 @@ struct ScrubEngine {
   LocateOut locate_out() const {
     unsigned long long* w = d_counter + kLocateOut;
     return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, d_records};
+  }
+  LocateOut check_out() const {
+    unsigned long long* w = d_counter + kCheckOut;
+    return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, d_check_records};
   }
   // Waits for the background release of the previous gate (no-op when none is pending).
   double join_reaper() {
@@ -204,6 +225,8 @@ int ScrubEngine::init() {
   // The locate pass runs with all HBM mapped: its records and their host copy are set aside now.
   CCM_CUDA(cudaMalloc(&d_records, kDirtRecords * sizeof(DirtRecord)));
   CCM_CUDA(cudaHostAlloc(&h_locate, sizeof(LocateHost), cudaHostAllocDefault));
+  CCM_CUDA(cudaMalloc(&d_check_records, kDirtRecords * sizeof(DirtRecord)));
+  CCM_CUDA(cudaHostAlloc(&h_check, sizeof(LocateHost), cudaHostAllocDefault));
   // The product call maps HBM down to the last granule; CUDA loads kernel code lazily at the
   // first launch and that needs device memory — make the default kernels resident now.
   cudaFuncAttributes fa;
@@ -283,10 +306,14 @@ int engine_teardown(int ordinal) {
   if (e->h_counter) cudaFreeHost(e->h_counter);
   if (e->d_records) cudaFree(e->d_records);
   if (e->h_locate) cudaFreeHost(e->h_locate);
+  if (e->d_check_records) cudaFree(e->d_check_records);
+  if (e->h_check) cudaFreeHost(e->h_check);
   e->d_counter = nullptr;
   e->h_counter = nullptr;
   e->d_records = nullptr;
   e->h_locate = nullptr;
+  e->d_check_records = nullptr;
+  e->h_check = nullptr;
   if (e->stream) cudaStreamDestroy(e->stream);
   e->stream = nullptr;
   e->ready = false;
@@ -573,11 +600,12 @@ static int tag_fill_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cu
 }
 
 // Check one range against the tags of `seed` and zero it (no sync); the mismatch count accumulates
-// into d_counter[kMismatch].
-static int tag_check_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cudaStream_t st) {
+// into d_counter[kMismatch], and the windows that differ into the check's book with offsets p - base
+// (every launch of one call passes the same base, or one that makes the offsets continue across its ranges).
+static int tag_check_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cudaStream_t st, uint64_t base) {
   if (n == 0) return CCM_OK;
   const cudaError_t err = launch_fast(CCM_TAG_CHECK, kTagThreads, kTagPer, e, kTagCheckGrab, st, split_region(p, n, 16, 128),
-                                      seed, e->d_counter + kMismatch);
+                                      seed, e->d_counter + kMismatch, e->check_out(), base);
   g_launches++;
   if (err != cudaSuccess) { set_error("tag check launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
   return CCM_OK;
@@ -750,6 +778,83 @@ static void finish_dirt(ccm_dirt_report* rep) {
     return (int64_t)a.offset < (int64_t)b.offset;
   });
   rep->truncated = rep->dirty_windows > (uint64_t)CCM_DIRT_RECORDS;
+}
+
+// ------------------------------------------------------------------ where the tags were wrong
+// One contiguous piece of what a tagged call checked: `bytes` at device address `addr`, which lie `offset` bytes into
+// what the report describes (the mapping, the concatenated segments, or the region).
+struct CheckSpan { uint64_t addr, bytes, offset; };
+
+// Zeroes the tag check's book for the next check and waits.  Needed only after a check that booked something (or
+// that an error may have cut short): a check that finds nothing never writes the book.
+static int clear_check_book(ScrubEngine* e, cudaStream_t st) {
+  CCM_CUDA(cudaMemsetAsync(e->d_counter + kCheckOut, 0, kBookWords * sizeof(unsigned long long), st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  return CCM_OK;
+}
+
+// After checks that counted mismatch_bytes != 0 (and finished): copies the book, zeroes it for the next check and
+// fills `rep`.  Offsets are as the kernels booked them; every record is classified (ccm_mismatch.h) against `spans`
+// (the ALIAS search covers exactly them) and gets chunk_of(offset).
+template <typename ChunkOf>
+static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_bytes, uint32_t seed, uint64_t va_base,
+                         const std::vector<CheckSpan>& spans, ccm_mismatch_report* rep, ChunkOf&& chunk_of) {
+  memset(rep, 0, sizeof *rep);
+  rep->located = 1;
+  rep->seed = seed;
+  rep->va_base = va_base;
+  rep->mismatch_bytes = mismatch_bytes;
+  LocateHost& h = *e->h_check;
+  CCM_CUDA(cudaMemcpyAsync(h.words, e->d_counter + kCheckOut, sizeof h.words, cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaMemcpyAsync(h.records, e->d_check_records, sizeof h.records, cudaMemcpyDeviceToHost, st));
+  if (int rc = clear_check_book(e, st)) return rc;
+  rep->zero_windows = h.words[0];
+  rep->mismatch_windows = h.words[8];
+  if (rep->mismatch_windows == 0) return CCM_OK;
+  rep->first_offset = ~h.words[16];
+  rep->last_offset = h.words[24];
+  const uint64_t claimed = h.words[32] < (uint64_t)kDirtRecords ? h.words[32] : (uint64_t)kDirtRecords;
+  std::vector<ccm_mismatch::Range> ranges;
+  for (const CheckSpan& sp : spans) ranges.push_back({sp.addr, sp.addr + sp.bytes});
+  // the span a booked offset belongs to: the last one that starts at or before it (a head window may start before
+  // the first)
+  auto span_at = [&](uint64_t o) -> const CheckSpan& {
+    size_t j = 0;
+    for (size_t k = 0; k < spans.size(); ++k)
+      if ((int64_t)spans[k].offset <= (int64_t)o) j = k;
+    return spans[j];
+  };
+  auto span_holding = [&](uint64_t a) -> const CheckSpan* {
+    for (const CheckSpan& sp : spans)
+      if (a >= sp.addr && a < sp.addr + sp.bytes) return &sp;
+    return nullptr;
+  };
+  for (uint64_t i = 0; i < claimed; ++i) {
+    const DirtRecord& d = h.records[i];
+    ccm_mismatch_record& r = rep->records[rep->nrecords++];
+    r.offset = d.offset;
+    r.chunk = chunk_of(d.offset);
+    r.mask = d.mask;
+    memcpy(r.bytes, &d.bytes, sizeof r.bytes);
+    const CheckSpan& sp = span_at(d.offset);
+    const uint64_t w = sp.addr + (d.offset - sp.offset);
+    uint32_t present = 0;
+    for (int b = 0; b < 16; ++b)
+      if (w + b >= sp.addr && w + b < sp.addr + sp.bytes) present |= 1u << b;
+    const ccm_mismatch::Verdict v = ccm_mismatch::classify(seed, w, r.bytes, present, ranges.data(), ranges.size());
+    r.kind = (uint16_t)v.kind;
+    if (v.kind == ccm_mismatch::kAlias) {
+      // offsets follow the span of the source's first present byte (a head window's source may start before it)
+      const CheckSpan* src = span_holding(v.source + (uint64_t)(__builtin_ctz(present)));
+      r.source_offset = src ? src->offset + (v.source - src->addr) : 0;
+      r.source_chunk = chunk_of(r.source_offset);
+    }
+  }
+  std::sort(rep->records, rep->records + rep->nrecords, [](const ccm_mismatch_record& a, const ccm_mismatch_record& b) {
+    return (int64_t)a.offset < (int64_t)b.offset;
+  });
+  rep->truncated = rep->mismatch_windows > (uint64_t)CCM_DIRT_RECORDS;
+  return CCM_OK;
 }
 
 int engine_arena_scrub(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, void* stream, float* ms) {
@@ -942,13 +1047,20 @@ static int arena_drill(ScrubEngine* e, int fill, uint64_t inject) {
 }
 
 // Tagged pass of the product call's fallback path: tag every segment, then (after the "tag_inject"
-// drill) check and zero every segment.  Fills tag->mismatch_bytes, ->ms_tag, ->ms_check, ->va_base.
+// drill) check and zero every segment.  Fills tag->mismatch_bytes, ->ms_tag, ->ms_check, ->va_base, and after
+// mismatches the engine's mismatch report (offsets into the concatenated segments, chunk = segment index).
 static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inject) {
   std::lock_guard<std::mutex> g(e->mu);
   CCM_ENSURE_READY(e);
   int rc = need_arena(e); if (rc) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->stream;
+  std::vector<CheckSpan> spans;
+  uint64_t shift = 0;
+  for (auto& s : e->segs) {
+    spans.push_back({(uint64_t)(uintptr_t)s.ptr, s.bytes, shift});
+    shift += s.bytes;
+  }
   // fills between ev[0] and ev[2], the drill, checks between ev[3] and ev[1]
   rc = run_counted(e, st, kMismatch, &tag->mismatch_bytes, nullptr, [&]() -> int {
     for (auto& s : e->segs) if (int rc2 = tag_fill_range(e, s.ptr, s.bytes, tag->seed, st)) return rc2;
@@ -956,16 +1068,28 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
     for (auto& s : e->segs)
       if (tag_inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &tag_inject, st, true));
     CCM_CUDA(cudaEventRecord(e->ev[3], st));
-    for (auto& s : e->segs) if (int rc2 = tag_check_range(e, s.ptr, s.bytes, tag->seed, st)) return rc2;
+    // base = segment address - its offset: the offsets continue from one segment into the next
+    for (const CheckSpan& sp : spans)
+      if (int rc2 = tag_check_range(e, (void*)(uintptr_t)sp.addr, sp.bytes, tag->seed, st, sp.addr - sp.offset)) return rc2;
     return CCM_OK;
   });
-  if (rc) return rc;
+  if (rc) { clear_check_book(e, st); return rc; }
   float a = 0, b = 0;
   CCM_CUDA(cudaEventElapsedTime(&a, e->ev[0], e->ev[2]));
   CCM_CUDA(cudaEventElapsedTime(&b, e->ev[3], e->ev[1]));
   tag->ms_tag = a;
   tag->ms_check = b;
   tag->va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
+  if (tag->mismatch_bytes != 0) {   // a failure of the report leaves it empty; it never changes the verdict
+    ccm_mismatch_report rep;
+    auto chunk_of = [&](uint64_t o) {
+      uint32_t i = 0;
+      for (size_t k = 0; k < spans.size(); ++k)
+        if ((int64_t)spans[k].offset <= (int64_t)o) i = (uint32_t)k;
+      return i;
+    };
+    if (take_mismatch(e, st, tag->mismatch_bytes, tag->seed, tag->va_base, spans, &rep, chunk_of) == CCM_OK) e->mismatch = rep;
+  }
   return CCM_OK;
 }
 
@@ -1118,6 +1242,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   int tag_timed = 0;
   std::vector<std::pair<uint64_t, uint64_t>> deferred;  // tagged: main-zone ranges, checked after the last mapping
   std::vector<std::pair<uint64_t, uint32_t>> pieces;    // (offset, handle index) of every mapped piece, ascending
+  bool checked = false;                                 // tagged: a check was enqueued (its book may be non-zero)
   auto tag_fill = [&](uint64_t off, uint64_t n) -> int {
     cudaEvent_t* evs = tag_timed < kMaxPipeChunks ? e->tag_ev[tag_timed] : nullptr;
     if (evs) cudaEventRecord(evs[0], st);
@@ -1135,7 +1260,8 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     }
     cudaEvent_t* evs = timed < kMaxPipeChunks ? e->pipe_ev[timed] : nullptr;
     if (evs) cudaEventRecord(evs[0], st);
-    int rc2 = tag ? tag_check_range(e, (void*)(m.base + off), n, tag->seed, st)
+    checked |= tag != nullptr;
+    int rc2 = tag ? tag_check_range(e, (void*)(m.base + off), n, tag->seed, st, (uint64_t)m.base)
                   : scrub_range(e, (void*)(m.base + off), n, CCM_SCRUB_AUTO, nullptr, st);
     if (evs) cudaEventRecord(evs[1], st);
     // fault drills: dirt the read-back of this range MUST find
@@ -1262,16 +1388,25 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
       tag->va_base = mapped ? (uint64_t)m.base : 0;
     }
   }
+  auto chunk_of = [&](uint64_t o) {
+    auto it = std::upper_bound(pieces.begin(), pieces.end(), o,
+                               [](uint64_t v, const std::pair<uint64_t, uint32_t>& pc) { return v < pc.first; });
+    return it == pieces.begin() ? 0u : std::prev(it)->second;
+  };
+  // ---- a failed tagged check: where were the tags wrong?  The checks booked it; one copy, no launch ---------
+  if (checked && rc == CCM_OK && tag->mismatch_bytes != 0) {
+    ccm_mismatch_report rep;
+    const std::vector<CheckSpan> spans{{(uint64_t)m.base, mapped, 0}};
+    if (take_mismatch(e, st, tag->mismatch_bytes, tag->seed, (uint64_t)m.base, spans, &rep, chunk_of) == CCM_OK)
+      e->mismatch = rep;   // never changes the verdict
+  } else if (checked && rc != CCM_OK) {
+    clear_check_book(e, st);
+  }
   // ---- a failed read-back: where is the dirt?  One more launch, before the mapping goes back -------------
   if (rc == CCM_OK && r->nonzero_bytes != 0) {
     ccm_dirt_report rep;
     memset(&rep, 0, sizeof rep);
     rep.va_base = (uint64_t)m.base;
-    auto chunk_of = [&](uint64_t o) {
-      auto it = std::upper_bound(pieces.begin(), pieces.end(), o,
-                                 [](uint64_t v, const std::pair<uint64_t, uint32_t>& pc) { return v < pc.first; });
-      return it == pieces.begin() ? 0u : std::prev(it)->second;
-    };
     if (locate_range(e, (const void*)m.base, mapped, 0, st, &rep, chunk_of) == CCM_OK) {  // never changes the verdict
       finish_dirt(&rep);
       e->dirt = rep;
@@ -1310,7 +1445,8 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   ccm_tag_result* tag = current_tag_call();
   {
     std::lock_guard<std::mutex> g(e->mu);
-    memset(&e->dirt, 0, sizeof e->dirt);  // every call replaces the report of the last one
+    memset(&e->dirt, 0, sizeof e->dirt);  // every call replaces the reports of the last one
+    memset(&e->mismatch, 0, sizeof e->mismatch);
   }
   ccm_scrub_result r;
   memset(&r, 0, sizeof r);
@@ -1454,7 +1590,55 @@ extern "C" int ccm_region_tag_check_zero(int cuda_ordinal, void* dptr, uint64_t 
   CCM_ENSURE_READY(e);
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->pick(stream);
-  return run_counted(e, st, kMismatch, mismatch, ms, [&] { return tag_check_range(e, dptr, bytes, seed, st); });
+  uint64_t count = 0;
+  const uint64_t base = (uint64_t)(uintptr_t)dptr;
+  int rc = run_counted(e, st, kMismatch, &count, ms, [&] { return tag_check_range(e, dptr, bytes, seed, st, base); });
+  if (rc == CCM_OK && count != 0) rc = clear_check_book(e, st);   // the next check starts from an empty book
+  else if (rc != CCM_OK) clear_check_book(e, st);
+  if (mismatch) *mismatch = count;
+  return rc;
+}
+
+extern "C" int ccm_region_tag_check_locate(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream,
+                                           ccm_mismatch_report* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  ScrubEngine* e = engine_for(cuda_ordinal);
+  if (!e) return CCM_ERR_NO_CUDA;
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  cudaStream_t st = e->pick(stream);
+  uint64_t count = 0;
+  const uint64_t base = (uint64_t)(uintptr_t)dptr;
+  int rc = run_counted(e, st, kMismatch, &count, nullptr, [&] { return tag_check_range(e, dptr, bytes, seed, st, base); });
+  if (rc != CCM_OK) { clear_check_book(e, st); return rc; }
+  ccm_mismatch_report rep;
+  memset(&rep, 0, sizeof rep);
+  rep.located = 1;
+  rep.seed = seed;
+  rep.va_base = base;
+  if (count != 0) {
+    const std::vector<CheckSpan> spans{{base, bytes, 0}};
+    if ((rc = take_mismatch(e, st, count, seed, base, spans, &rep, [](uint64_t) { return 0u; }))) return rc;
+  }
+  *out = rep;
+  return CCM_OK;
+}
+
+// ------------------------------------------------------------------------- mismatch report
+extern "C" int ccm_scrub_last_mismatch(int cuda_ordinal, ccm_mismatch_report* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  *out = e->mismatch;
+  return CCM_OK;
 }
 
 // ------------------------------------------------------------------------- dirt report

@@ -5,7 +5,8 @@
 // Runs the concurrent gate (ccm_scrub_verify_many, or ccm_scrub_verify_many_tagged with --check tagged)
 // and prints ONE JSON line with the same fields as k8s_cc_manager_b200.devices.ScrubReport (the
 // tagged-gate fields only with --check tagged, "dirt" only for a GPU whose read-back found non-zero bytes: where
-// they are, as ccm_scrub_last_dirt reports it).  Exit 0: every GPU clean; 3: gate failed;
+// they are, as ccm_scrub_last_dirt reports it; "mismatch" only for a GPU whose tagged check found bytes off their
+// tags, as ccm_scrub_last_mismatch reports it).  Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
 // post-reset step.
@@ -27,6 +28,26 @@ static void print_dirt(const ccm_dirt_report& d) {
     const ccm_dirt_record& w = d.records[k];
     printf("%s{\"offset\": %lld, \"chunk\": %u, \"mask\": %u, \"bytes\": \"", k ? ", " : "", (long long)w.offset,
            w.chunk, (unsigned)w.mask);
+    for (int b = 0; b < 16; ++b) printf("%02x", w.bytes[b]);
+    printf("\"}");
+  }
+  printf("]}");
+}
+
+// The "mismatch" object: the fields of k8s_cc_manager_b200.devices.MismatchReport, kinds by name.
+static void print_mismatch(const ccm_mismatch_report& m) {
+  static const char* const kinds[] = {"?", "zero", "alias", "partial", "foreign"};
+  printf(", \"mismatch\": {\"mismatch_bytes\": %llu, \"mismatch_windows\": %llu, \"zero_windows\": %llu, "
+         "\"first_offset\": %llu, \"last_offset\": %llu, \"va_base\": %llu, \"seed\": %u, \"located\": %d, "
+         "\"truncated\": %d, \"records\": [",
+         (unsigned long long)m.mismatch_bytes, (unsigned long long)m.mismatch_windows, (unsigned long long)m.zero_windows,
+         (unsigned long long)m.first_offset, (unsigned long long)m.last_offset, (unsigned long long)m.va_base, m.seed,
+         m.located, m.truncated);
+  for (int k = 0; k < m.nrecords; ++k) {
+    const ccm_mismatch_record& w = m.records[k];
+    printf("%s{\"offset\": %lld, \"chunk\": %u, \"mask\": %u, \"kind\": \"%s\", \"source_offset\": %lld, "
+           "\"source_chunk\": %u, \"bytes\": \"", k ? ", " : "", (long long)w.offset, w.chunk, (unsigned)w.mask,
+           kinds[w.kind <= 4 ? w.kind : 0], (long long)w.source_offset, w.source_chunk);
     for (int b = 0; b < 16; ++b) printf("%02x", w.bytes[b]);
     printf("\"}");
   }
@@ -112,6 +133,8 @@ int main(int argc, char** argv) {
     }
     ccm_dirt_report d;
     if (r.nonzero_bytes != 0 && ccm_scrub_last_dirt(ordinals[i], &d) == CCM_OK) print_dirt(d);
+    ccm_mismatch_report m;
+    if (tagged && tags[i].mismatch_bytes != 0 && ccm_scrub_last_mismatch(ordinals[i], &m) == CCM_OK) print_mismatch(m);
     printf("}");
   }
   printf("]}\n");

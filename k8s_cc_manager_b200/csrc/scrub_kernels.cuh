@@ -593,80 +593,30 @@ tag_fill_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed) {
   default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
 }
 
-// Counts the bytes that differ from the tags into cnt and stores zero over them.
-// The exact per-byte count is computed for every batch, branch-free, and the loaded words die before the
-// stores: on H100 this runs at 0.97x of a same-run device-to-device copy, where counting only batches whose
-// XOR is non-zero (verify_ld128_fast_kernel's trick) keeps the loaded words live across the stores and
-// runs at 0.75x (one H100 80GB HBM3, 700 W, 32 GiB region).
-struct TagCheckZeroOp {
-  uint32_t seed;
-  uint64_t cnt = 0;
-  template <int THREADS, int PER_THREAD>
-  __device__ __forceinline__ void chunk(uint8_t* p) {
-    uint4 v[PER_THREAD];
-#pragma unroll
-    for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16_cs(p + (uint32_t)u * THREADS * 16u);  // all loads first
-    uint32_t n = 0;
-#pragma unroll
-    for (int u = 0; u < PER_THREAD; ++u) {
-      const uint4 t = tag_vec(seed, addr(p + (uint32_t)u * THREADS * 16u));
-      n += nonzero_bytes_in_word(v[u].x ^ t.x) + nonzero_bytes_in_word(v[u].y ^ t.y) +
-           nonzero_bytes_in_word(v[u].z ^ t.z) + nonzero_bytes_in_word(v[u].w ^ t.w);
-    }
-#pragma unroll
-    for (int u = 0; u < PER_THREAD; ++u) st16(p + (uint32_t)u * THREADS * 16u, make_uint4(0, 0, 0, 0));
-    cnt += n;
-  }
-  __device__ __forceinline__ void vec(uint8_t* q) {
-    uint4 v = ld16_cs(q);
-    const uint4 t = tag_vec(seed, addr(q));
-    st16(q, make_uint4(0, 0, 0, 0));
-    cnt += nonzero_bytes_in_word(v.x ^ t.x) + nonzero_bytes_in_word(v.y ^ t.y) + nonzero_bytes_in_word(v.z ^ t.z) +
-           nonzero_bytes_in_word(v.w ^ t.w);
-  }
-  __device__ __forceinline__ void byte(uint8_t* x) {
-    cnt += *x != tag_byte(seed, addr(x));
-    *x = 0;
-  }
-};
-
-// Reads the tags back, counts every byte that differs from them (exact, u64, one atomic per CTA into
-// *mismatch) and stores zero over the same addresses.  All PER_THREAD loads are in flight before any use.
-// Chunks are taken in ascending order, so the last stretch this kernel writes is the first one the
-// descending zero read-back reads.
-template <int THREADS, int PER_THREAD>
-__global__ void __launch_bounds__(THREADS)
-tag_check_zero_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed, unsigned long long* mismatch) {
-  TagCheckZeroOp op{seed};
-  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
-  block_accumulate(op.cnt, mismatch);
-}
-
 // Fault drill "tag_inject": flips bits of single bytes (XOR, so the byte can never keep its tag).
 __global__ void xor_byte_kernel(uint8_t* p) { *p ^= 0xA5; }
 
-// ------------------------------------------------------------ locate the dirt
-// When the zero read-back counted dirt, this pass says where it is.  A dirty WINDOW is a 16-byte, 16-aligned address
-// window holding at least one non-zero byte of the region; in the body a window is one vector.  Results: the exact
-// number of non-zero bytes and of dirty windows, the offsets (from the region base) of the first and the last
-// non-zero byte, and up to kDirtRecords records of (window offset, mask of its non-zero bytes, its 16 bytes).
+// ---------------------------------------------------------------- window books
+// The locate pass and the tag check say WHERE they found what they count, in 16-byte, 16-aligned address windows
+// (in the body a window is one vector).  Both keep the same book: exact window count and first / last byte in
+// registers, one atomic per result word per CTA, and up to kDirtRecords records of (window offset, mask, 16 bytes).
 constexpr int kDirtRecords = 64;
 
 struct DirtRecord {       // layout of ccm_dirt_record (include/ccm.h); `chunk` is filled in by the host
   uint64_t offset;        // window address - region base (negative, two's complement, for the head window of a
                           // region that does not start 16-aligned)
   uint32_t chunk;
-  uint16_t mask;          // bit i: byte i of the window is non-zero (bytes outside the region read as 0)
+  uint16_t mask;          // bit i: byte i of the window is booked (locate: non-zero; check: differs from its tag)
   uint16_t reserved;
   uint4 bytes;
 };
 
 // Result words of one pass, each on its own line of the engine's control block; zero before the launch.
 struct LocateOut {
-  unsigned long long* nonzero;    // += non-zero bytes
-  unsigned long long* windows;    // += dirty windows
-  unsigned long long* first_inv;  // max of ~offset of the first non-zero byte (0: none)
-  unsigned long long* last;       // max of the offset of the last non-zero byte
+  unsigned long long* count;      // += the op's own count: non-zero bytes (locate), all-zero windows (tag check)
+  unsigned long long* windows;    // += windows booked
+  unsigned long long* first_inv;  // max of ~offset of the first booked byte (0: none)
+  unsigned long long* last;       // max of the offset of the last booked byte
   unsigned long long* slots;      // record slots claimed (may run past kDirtRecords)
   unsigned long long* full;       // set once kDirtRecords slots are taken
   DirtRecord* records;
@@ -690,14 +640,11 @@ __device__ __forceinline__ uint32_t nonzero_mask16(const Vec16& v) {
 
 // Counts, first / last offset and window count stay in registers; only records go through memory.  A record slot
 // is claimed with an atomicAdd only while the "records full" word is clear, and a thread that has seen it set (or
-// drew the last slot or a later one) never reads it again: a region that is dirty everywhere would otherwise serialise one
-// atomic per vector on a single address, about 5e9 of them at whole HBM.  The ragged head and tail are not taken
-// byte by byte (byte() does nothing): locate_dirt_kernel takes them window by window, so no window is counted or
-// recorded twice.
-struct LocateOp {
+// drew the last slot or a later one) never reads it again: a region that is booked everywhere would otherwise
+// serialise one atomic per vector on a single address, about 5e9 of them at whole HBM.
+struct WindowBook {
   LocateOut out;
-  const uint8_t* base;
-  uint64_t bytes = 0, windows = 0, first_inv = 0, last = 0;
+  uint64_t count = 0, windows = 0, first_inv = 0, last = 0;   // count: the op's own (out.count)
   bool full_seen = false;
 
   // A record slot (>= kDirtRecords: none left).
@@ -708,9 +655,8 @@ struct LocateOp {
     return slot;
   }
 
-  // Books one window at offset `off` whose non-zero bytes are `mask` (!= 0).
+  // Counts one window at offset `off` whose booked bytes are `mask` (!= 0).
   __device__ __forceinline__ void tally(uint64_t off, uint32_t mask) {
-    bytes += __popc(mask);
     windows += 1;
     const uint64_t lo = off + (uint64_t)(__ffs(mask) - 1), hi = off + (uint64_t)(31 - __clz(mask));
     first_inv = max(first_inv, (uint64_t)~lo);
@@ -727,62 +673,18 @@ struct LocateOp {
     out.records[slot] = r;
   }
 
-  template <int THREADS, int PER_THREAD>
-  __device__ __forceinline__ void chunk(const uint8_t* p) {
-    Vec16 v[PER_THREAD];
-#pragma unroll
-    for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16<kPolStreaming>(p + (uint32_t)u * THREADS * 16u, 0);  // all loads first
-    uint32_t any = 0;
-#pragma unroll
-    for (int u = 0; u < PER_THREAD; ++u)
-#pragma unroll
-      for (int k = 0; k < 4; ++k) any |= v[u].w[k];
-    if (any != 0) {  // rare except in a flood
-      const uint64_t off0 = (uint64_t)(p - base);
-#pragma unroll
-      for (int u = 0; u < PER_THREAD; ++u) window(off0 + (uint32_t)u * THREADS * 16u, nonzero_mask16(v[u]), v[u]);
-    }
-  }
-
-  // One window given as its aligned vector (a body vector, or a head / tail window from ragged_windows).
-  __device__ __forceinline__ void window(uint64_t off, uint32_t mask, const Vec16& v) {
-    if (mask == 0) return;
+  // Counts one window (mask != 0) and records it while slots last.
+  __device__ __forceinline__ void book(uint64_t off, uint32_t mask, const Vec16& v) {
     tally(off, mask);
     if (full_seen) return;
     const uint64_t slot = claim();
     if (slot < (uint64_t)kDirtRecords) record(slot, off, mask, v);
   }
 
-  __device__ __forceinline__ void vec(const uint8_t* p) {
-    const Vec16 v = ld16<kPolStreaming>(p, 0);
-    window((uint64_t)(p - base), nonzero_mask16(v), v);
-  }
-
-  __device__ __forceinline__ void byte(const uint8_t*) {}
-
-  // CTA 0: the windows of the ragged head and tail, one thread per window, bytes outside the region as 0.
-  __device__ __forceinline__ void ragged_windows(const RegionSplit& s) {
-    if (blockIdx.x != 0) return;
-    const uint64_t a0 = addr(s.base);
-    const uint64_t head_end = a0 + s.head, tail_start = head_end + s.body_vecs * 16, end = tail_start + s.tail;
-    const uint64_t first_win = a0 & ~15ull;
-    const uint64_t nhead = s.head ? (head_end - first_win + 15) / 16 : 0;   // at most 8
-    const uint64_t t = threadIdx.x;
-    uint64_t w0 = 0, lo = 0, hi = 0;
-    if (t < nhead) { w0 = first_win + 16 * t; lo = max(w0, a0); hi = min(w0 + 16, head_end); }
-    else if (t == nhead && s.tail) { w0 = tail_start; lo = tail_start; hi = end; }
-    else return;
-    Vec16 v = {{0, 0, 0, 0}};
-#pragma unroll
-    for (int i = 0; i < 16; ++i)
-      if (w0 + i >= lo && w0 + i < hi) v.w[i >> 2] |= (uint32_t)*(const uint8_t*)(uintptr_t)(w0 + i) << (8 * (i & 3));
-    window(w0 - a0, nonzero_mask16(v), v);
-  }
-
-  // One atomic per result word per CTA (skipped when the CTA found nothing), after a block reduction.
+  // One atomic per result word per CTA (skipped when the CTA booked nothing), after a block reduction.
   __device__ __forceinline__ void flush() {
     __shared__ uint64_t part[4][32];
-    uint64_t a = bytes, b = windows, c = first_inv, d = last;
+    uint64_t a = count, b = windows, c = first_inv, d = last;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       a += __shfl_xor_sync(0xffffffffu, a, o);
@@ -807,12 +709,185 @@ struct LocateOp {
         d = max(d, __shfl_xor_sync(0xffffffffu, d, o));
       }
       if (lane == 0 && b != 0) {
-        atomicAdd(out.nonzero, (unsigned long long)a);
+        atomicAdd(out.count, (unsigned long long)a);
         atomicAdd(out.windows, (unsigned long long)b);
         atomicMax(out.first_inv, (unsigned long long)c);
         atomicMax(out.last, (unsigned long long)d);
       }
     }
+  }
+};
+
+// CTA 0, one thread per window of the ragged head and tail: false for every other thread, otherwise true with the
+// window's address w0 and the part [lo, hi) of it that lies inside the region.
+__device__ __forceinline__ bool ragged_window(const RegionSplit& s, uint64_t& w0, uint64_t& lo, uint64_t& hi) {
+  if (blockIdx.x != 0) return false;
+  const uint64_t a0 = addr(s.base);
+  const uint64_t head_end = a0 + s.head, tail_start = head_end + s.body_vecs * 16, end = tail_start + s.tail;
+  const uint64_t first_win = a0 & ~15ull;
+  const uint64_t nhead = s.head ? (head_end - first_win + 15) / 16 : 0;   // at most 8
+  const uint64_t t = threadIdx.x;
+  if (t < nhead) { w0 = first_win + 16 * t; lo = max(w0, a0); hi = min(w0 + 16, head_end); return true; }
+  if (t == nhead && s.tail) { w0 = tail_start; lo = tail_start; hi = end; return true; }
+  return false;
+}
+
+// Counts the bytes that differ from the tags into cnt and stores zero over them.
+// The exact per-byte count is computed for every batch, branch-free, and the loaded words die before the
+// stores: on H100 this runs at 0.97x of a same-run device-to-device copy, where counting only batches whose
+// XOR is non-zero (verify_ld128_fast_kernel's trick) keeps the loaded words live across the stores and
+// runs at 0.75x (one H100 80GB HBM3, 700 W, 32 GiB region).
+//
+// Where the mismatches are: only a batch whose exact count is non-zero takes the rare branch, and it sits BEFORE
+// the stores, so the loaded words still die there.  It books every window of the batch that differs from its
+// tags (WindowBook: mask = the bytes that differ, the 16 bytes as read) and counts the booked windows whose bytes
+// inside the region all read 0 into book.count.  Offsets are addresses - `base`, so every launch of one call
+// books into the same words.  The ragged head and tail are not taken byte by byte (byte() does nothing):
+// tag_check_zero_kernel takes them window by window, so no window is counted or recorded twice.
+struct TagCheckZeroOp {
+  uint32_t seed;
+  WindowBook book;
+  uint64_t base;
+  uint64_t cnt = 0;
+
+  // One window given as what was read (bytes outside the region as 0) and its mask of bytes that differ.
+  __device__ __forceinline__ void window(uint64_t off, uint32_t mask, const Vec16& v) {
+    if (mask == 0) return;
+    book.count += (v.w[0] | v.w[1] | v.w[2] | v.w[3]) == 0;
+    book.book(off, mask, v);
+  }
+
+  __device__ __forceinline__ static uint32_t diff_mask(const uint4& v, const uint4& t) {
+    const Vec16 x = {{v.x ^ t.x, v.y ^ t.y, v.z ^ t.z, v.w ^ t.w}};
+    return nonzero_mask16(x);
+  }
+
+  template <int THREADS, int PER_THREAD>
+  __device__ __forceinline__ void chunk(uint8_t* p) {
+    uint4 v[PER_THREAD];
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16_cs(p + (uint32_t)u * THREADS * 16u);  // all loads first
+    uint32_t n = 0;
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) {
+      const uint4 t = tag_vec(seed, addr(p + (uint32_t)u * THREADS * 16u));
+      n += nonzero_bytes_in_word(v[u].x ^ t.x) + nonzero_bytes_in_word(v[u].y ^ t.y) +
+           nonzero_bytes_in_word(v[u].z ^ t.z) + nonzero_bytes_in_word(v[u].w ^ t.w);
+    }
+    if (n != 0) {  // rare except in a flood: book the batch's windows, before the stores
+      // The branch reads the batch's vectors again, four at a time: they come from L2 (this thread loaded them a
+      // moment ago) and nothing has stored over them yet.  Keeping the loaded words live into the branch instead
+      // would need more registers than a 512-thread CTA leaves a thread (128: ptxas spills).  Unless something
+      // else writes the range during the check (two views of one range checked in one launch), the branch reads
+      // exactly the bytes counted above.
+      const uint64_t off0 = addr(p) - base;
+#pragma unroll 4
+      for (uint32_t u = 0; u < (uint32_t)PER_THREAD; ++u) {
+        uint8_t* q = p + u * THREADS * 16u;
+        const uint4 x = ld16_cs(q);
+        window(off0 + u * THREADS * 16u, diff_mask(x, tag_vec(seed, addr(q))), Vec16{{x.x, x.y, x.z, x.w}});
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) st16(p + (uint32_t)u * THREADS * 16u, make_uint4(0, 0, 0, 0));
+    cnt += n;
+  }
+  __device__ __forceinline__ void vec(uint8_t* q) {
+    uint4 v = ld16_cs(q);
+    const uint32_t mask = diff_mask(v, tag_vec(seed, addr(q)));
+    window(addr(q) - base, mask, Vec16{{v.x, v.y, v.z, v.w}});
+    st16(q, make_uint4(0, 0, 0, 0));
+    cnt += __popc(mask);
+  }
+  __device__ __forceinline__ void byte(uint8_t*) {}
+
+  // CTA 0: the windows of the ragged head and tail, one thread per window.  Only bytes inside the region are
+  // compared and zeroed; the others count as 0 that holds its tag.
+  __device__ __forceinline__ void ragged_windows(const RegionSplit& s) {
+    uint64_t w0 = 0, lo = 0, hi = 0;
+    if (!ragged_window(s, w0, lo, hi)) return;
+    Vec16 v = {{0, 0, 0, 0}}, x = {{0, 0, 0, 0}};
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+      if (w0 + i >= lo && w0 + i < hi) {
+        uint8_t* b = (uint8_t*)(uintptr_t)(w0 + i);
+        const uint32_t got = *b;
+        v.w[i >> 2] |= got << (8 * (i & 3));
+        x.w[i >> 2] |= (uint32_t)(uint8_t)(got ^ tag_byte(seed, w0 + i)) << (8 * (i & 3));
+        *b = 0;
+      }
+    const uint32_t mask = nonzero_mask16(x);
+    window(w0 - base, mask, v);
+    cnt += __popc(mask);
+  }
+};
+
+// Reads the tags back, counts every byte that differs from them (exact, u64, one atomic per CTA into
+// *mismatch) and stores zero over the same addresses.  All PER_THREAD loads are in flight before any use.
+// Chunks are taken in ascending order, so the last stretch this kernel writes is the first one the
+// descending zero read-back reads.  The windows that differ are booked into `out` with offsets from `base`
+// (TagCheckZeroOp); a check that finds nothing writes none of those words.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS)
+tag_check_zero_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed, unsigned long long* mismatch,
+                      LocateOut out, uint64_t base) {
+  TagCheckZeroOp op{seed, {out}, base};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
+  op.ragged_windows(s);
+  op.book.flush();
+  block_accumulate(op.cnt, mismatch);
+}
+
+// ------------------------------------------------------------ locate the dirt
+// When the zero read-back counted dirt, this pass says where it is.  A dirty WINDOW holds at least one non-zero
+// byte of the region.  Results: the exact number of non-zero bytes (book.count) and of dirty windows, the offsets
+// (from the region base) of the first and the last non-zero byte, and up to kDirtRecords records of (window offset,
+// mask of its non-zero bytes, its 16 bytes).  The ragged head and tail are not taken byte by byte (byte() does
+// nothing): locate_dirt_kernel takes them window by window, so no window is counted or recorded twice.
+struct LocateOp {
+  WindowBook book;
+  const uint8_t* base;
+
+  template <int THREADS, int PER_THREAD>
+  __device__ __forceinline__ void chunk(const uint8_t* p) {
+    Vec16 v[PER_THREAD];
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16<kPolStreaming>(p + (uint32_t)u * THREADS * 16u, 0);  // all loads first
+    uint32_t any = 0;
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) any |= v[u].w[k];
+    if (any != 0) {  // rare except in a flood
+      const uint64_t off0 = (uint64_t)(p - base);
+#pragma unroll
+      for (int u = 0; u < PER_THREAD; ++u) window(off0 + (uint32_t)u * THREADS * 16u, nonzero_mask16(v[u]), v[u]);
+    }
+  }
+
+  // One window given as its aligned vector (a body vector, or a head / tail window from ragged_windows).
+  __device__ __forceinline__ void window(uint64_t off, uint32_t mask, const Vec16& v) {
+    if (mask == 0) return;
+    book.count += __popc(mask);
+    book.book(off, mask, v);
+  }
+
+  __device__ __forceinline__ void vec(const uint8_t* p) {
+    const Vec16 v = ld16<kPolStreaming>(p, 0);
+    window((uint64_t)(p - base), nonzero_mask16(v), v);
+  }
+
+  __device__ __forceinline__ void byte(const uint8_t*) {}
+
+  // CTA 0: the windows of the ragged head and tail, one thread per window, bytes outside the region as 0.
+  __device__ __forceinline__ void ragged_windows(const RegionSplit& s) {
+    uint64_t w0 = 0, lo = 0, hi = 0;
+    if (!ragged_window(s, w0, lo, hi)) return;
+    Vec16 v = {{0, 0, 0, 0}};
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+      if (w0 + i >= lo && w0 + i < hi) v.w[i >> 2] |= (uint32_t)*(const uint8_t*)(uintptr_t)(w0 + i) << (8 * (i & 3));
+    window(w0 - addr(s.base), nonzero_mask16(v), v);
   }
 };
 
@@ -823,10 +898,10 @@ struct LocateOp {
 template <int THREADS, int PER_THREAD>
 __global__ void __launch_bounds__(THREADS, 1)
 locate_dirt_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, LocateOut out) {
-  LocateOp op{out, s.base};
+  LocateOp op{{out}, s.base};
   default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
   op.ragged_windows(s);
-  op.flush();
+  op.book.flush();
 }
 
 // ------------------------------------------------------------ test scaffolding

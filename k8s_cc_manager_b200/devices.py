@@ -29,12 +29,14 @@ from . import _native as N
 
 class GpuError(Exception):
     """Raised for any failed device operation (reference: gpu.GpuError).  A scrub that read back dirt
-    carries its DirtReport as `.dirt`."""
+    carries its DirtReport as `.dirt`; a tagged scrub whose check found bytes off their tags carries its
+    MismatchReport as `.mismatch`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
         self.status = status
         self.dirt: "Optional[DirtReport]" = None
+        self.mismatch: "Optional[MismatchReport]" = None
 
 
 def _error(rc: int, what: str, bdf: str = "") -> "Optional[GpuError]":
@@ -120,6 +122,97 @@ def last_dirt(cuda_ordinal: int) -> "Optional[DirtReport]":
 
 
 @dataclass
+class MismatchWindow:
+    """One 16-byte, 16-aligned window that did not hold its tags (include/ccm.h: ccm_mismatch_record)."""
+    offset: int          # from the report's va_base (negative only for the head window of an unaligned raw region)
+    chunk: int           # physical allocation behind it, in creation order (fallback: segment index)
+    mask: int            # bit i: byte i differs from its tag
+    kind: str            # "zero" | "alias" | "partial" | "foreign" (include/ccm.h: ccm_mismatch_kind)
+    source_offset: int   # alias: the window whose tags these are; otherwise 0
+    source_chunk: int    # alias: the allocation behind that window; otherwise 0
+    bytes: str           # the 16 bytes as the check read them, hex
+
+    def describe(self) -> str:
+        return f"+{self.offset:#x} chunk {self.chunk} mask {self.mask:04x} [{self.bytes}]"
+
+
+@dataclass
+class MismatchReport:
+    """Where a failed tagged check found bytes that did not hold their tags (include/ccm.h: ccm_mismatch_report).
+    mismatch_bytes, mismatch_windows, zero_windows, first_offset and last_offset are exact.  The split between
+    alias, partial and foreign windows is known for the records only; records are distinct windows sorted by
+    offset, all of them unless `truncated`."""
+    mismatch_bytes: int
+    mismatch_windows: int
+    zero_windows: int        # mismatched windows whose bytes all read 0
+    first_offset: int        # first / last mismatched byte, from va_base
+    last_offset: int
+    va_base: int
+    seed: int
+    located: int             # 0: the last call's tagged check was clean (or it was not tagged)
+    truncated: int
+    records: List[MismatchWindow] = field(default_factory=list)
+
+    @classmethod
+    def from_native(cls, m: N.MismatchReport) -> "MismatchReport":
+        recs = [MismatchWindow(_signed64(r.offset), r.chunk, r.mask, N.MISMATCH_KINDS.get(r.kind, str(r.kind)),
+                               _signed64(r.source_offset), r.source_chunk, bytes(r.bytes).hex())
+                for r in m.records[:m.nrecords]]
+        return cls(m.mismatch_bytes, m.mismatch_windows, m.zero_windows, m.first_offset, m.last_offset, m.va_base,
+                   m.seed, m.located, m.truncated, recs)
+
+    @classmethod
+    def from_json(cls, d: dict) -> "MismatchReport":
+        return cls(**{**d, "records": [MismatchWindow(**r) for r in d["records"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    def by_kind(self) -> dict:
+        out: dict = {}
+        for r in self.records:
+            out.setdefault(r.kind, []).append(r)
+        return out
+
+    def summary(self, first: int = 2) -> str:
+        """One line for an operator: extent, exact window counts, then the records grouped by kind.  Alias records
+        are given as the distinct source - offset deltas with the chunk pairs (chunk <- source chunk)."""
+        more = " (records truncated)" if self.truncated else ""
+        parts = []
+        groups = self.by_kind()
+        for kind in ("alias", "zero", "partial", "foreign"):
+            recs = groups.get(kind, [])
+            if not recs:
+                continue
+            if kind == "alias":
+                deltas: dict = {}
+                for r in recs:
+                    deltas.setdefault(r.source_offset - r.offset, []).append(r)
+                for delta, rs in sorted(deltas.items()):
+                    lo, hi = min(r.offset for r in rs), max(r.offset for r in rs)
+                    pairs = ", ".join(f"chunk {c} \u2190 chunk {s}" for c, s in sorted({(r.chunk, r.source_chunk) for r in rs}))
+                    sign = "-" if delta < 0 else ""
+                    parts.append(f"alias: +{lo:#x}..+{hi:#x} hold the tags of +{lo + delta:#x}.. "
+                                 f"(delta {sign}{abs(delta):#x}, {pairs}; {len(rs)} records)")
+            else:
+                chunks = sorted({r.chunk for r in recs})
+                parts.append(f"{kind}: {len(recs)} records, chunks {chunks}; "
+                             + "; ".join(r.describe() for r in recs[:first]))
+        return (f"bytes off their tags at offsets {self.first_offset:#x}..{self.last_offset:#x} of va {self.va_base:#x}, "
+                f"{self.mismatch_bytes} bytes in {self.mismatch_windows} 16-byte windows, {self.zero_windows} of them "
+                f"all zero{more}; " + " | ".join(parts))
+
+
+def last_mismatch(cuda_ordinal: int) -> "Optional[MismatchReport]":
+    """The mismatch report of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_mismatch);
+    None when it cannot be read."""
+    m = N.MismatchReport()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_mismatch(cuda_ordinal, C.byref(m)) != N.OK:
+        return None
+    return MismatchReport.from_native(m)
+
+
+@dataclass
 class ScrubReport:
     """Outcome of one GPU's HBM scrub-and-verify (include/ccm.h: ccm_scrub_result)."""
     bdf: str
@@ -148,6 +241,9 @@ class ScrubReport:
     # Where the dirt is (a DirtReport), set for every report with nonzero_bytes != 0.  Not a dataclass field,
     # so positional construction, the field list and the JSON of a clean report stay as they were.
     dirt = None
+    # Where the tags were wrong (a MismatchReport), set for every report with mismatch_bytes != 0.  Not a dataclass
+    # field either, for the same reason.
+    mismatch = None
 
     @property
     def clean(self) -> bool:
@@ -191,6 +287,8 @@ class ScrubReport:
                 del d[name]
         if self.dirt is not None:
             d["dirt"] = self.dirt.as_json()
+        if self.mismatch is not None:
+            d["mismatch"] = self.mismatch.as_json()
         return d
 
     @classmethod
@@ -198,9 +296,12 @@ class ScrubReport:
         """Inverse of as_json."""
         d = dict(d)
         dirt = d.pop("dirt", None)
+        mismatch = d.pop("mismatch", None)
         rep = cls(**d)
         if dirt is not None:
             rep.dirt = DirtReport.from_json(dirt)
+        if mismatch is not None:
+            rep.mismatch = MismatchReport.from_json(mismatch)
         return rep
 
 
@@ -275,7 +376,8 @@ class NvidiaDevice:
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
         if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
-        found non-zero bytes, the report (or the GpuError, as `.dirt`) carries where they are.
+        found non-zero bytes, the report (or the GpuError, as `.dirt`) carries where they are; when the tagged check
+        found bytes off their tags, it carries where those are as `.mismatch`.
         """
         res, tag = N.ScrubResult(), None
         if _check_mode(check):
@@ -287,8 +389,10 @@ class NvidiaDevice:
         rep = ScrubReport.from_native(self.bdf, res, tag)
         if rep.nonzero_bytes:
             rep.dirt = last_dirt(self.cuda_ordinal)
+        if rep.mismatch_bytes:
+            rep.mismatch = last_mismatch(self.cuda_ordinal)
         if err is not None:
-            err.dirt = rep.dirt
+            err.dirt, err.mismatch = rep.dirt, rep.mismatch
             raise err
         return rep
 
@@ -355,6 +459,8 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
     for rep, d in zip(reports, devices):
         if rep.nonzero_bytes:
             rep.dirt = last_dirt(d.cuda_ordinal)
+        if rep.mismatch_bytes:
+            rep.mismatch = last_mismatch(d.cuda_ordinal)
     return reports, wall.value
 
 

@@ -554,6 +554,12 @@ class CCManager:
         self.last_transition.setdefault("scrub_dirt", {})[bdf] = dirt
         logger.error("HBM dirt on %s: %s", bdf, dirt.summary())
 
+    def _note_mismatch(self, bdf: str, mismatch) -> None:
+        """Logs where a failed tagged check found bytes off their tags (and whose tags they hold) and keeps the
+        report in last_transition["scrub_mismatch"][bdf], for the same reason as _note_dirt."""
+        self.last_transition.setdefault("scrub_mismatch", {})[bdf] = mismatch
+        logger.error("HBM tag mismatch on %s: %s", bdf, mismatch.summary())
+
     def _run_scrub(self, gpus: list) -> None:
         started = time.perf_counter()
         if self.scrub_isolation == "process":
@@ -579,6 +585,8 @@ class CCManager:
                 except GpuError as exc:
                     if getattr(exc, "dirt", None) is not None:
                         self._note_dirt(gpu.bdf, exc.dirt)
+                    if getattr(exc, "mismatch", None) is not None:
+                        self._note_mismatch(gpu.bdf, exc.mismatch)
                     raise
             reports = self._fan_out(gpus, one, "scrub")
         elapsed = time.perf_counter() - started
@@ -587,6 +595,8 @@ class CCManager:
         for rep in reports:
             if getattr(rep, "dirt", None) is not None:
                 self._note_dirt(rep.bdf, rep.dirt)
+            if getattr(rep, "mismatch", None) is not None:
+                self._note_mismatch(rep.bdf, rep.mismatch)
         for rep in reports:
             mismatch = getattr(rep, "mismatch_bytes", 0)
             if rep.status != 0 or rep.nonzero_bytes != 0 or mismatch != 0:
