@@ -272,6 +272,8 @@ static thread_local ScrubDrill t_scrub_drill;  // set for the duration of one sc
 const ScrubDrill& current_scrub_drill() { return t_scrub_drill; }
 static thread_local ccm_tag_result* t_tag_call = nullptr;  // likewise; nullptr = zero-only call
 ccm_tag_result* current_tag_call() { return t_tag_call; }
+static thread_local ccm_residue_report* t_residue_call = nullptr;  // likewise; nullptr = no census
+ccm_residue_report* current_residue_call() { return t_residue_call; }
 
 int sim_scrub_hook(int dev, ScrubDrill* drill) {
   return with_dev(dev, [&](Device& d) {
@@ -490,8 +492,11 @@ static ScrubEngine* engine_of_ordinal(int ordinal, int* rc) {
 }
 
 // tag: nullptr for the zero-only gate; otherwise the tagged gate runs, with tag->seed drawn here when 0.
-static int scrub_verify_one(int dev, uint64_t bytes, bool node_fanout, ccm_tag_result* tag, ccm_scrub_result* out) {
+// residue: nullptr, or the census report this call fills.
+static int scrub_verify_one(int dev, uint64_t bytes, bool node_fanout, ccm_tag_result* tag, ccm_scrub_result* out,
+                            ccm_residue_report* residue = nullptr) {
   if (out) { memset(out, 0, sizeof *out); out->bytes_requested = bytes; }
+  if (residue) memset(residue, 0, sizeof *residue);
   if (tag) {
     const uint32_t seed = tag->seed;
     memset(tag, 0, sizeof *tag);
@@ -507,7 +512,9 @@ static int scrub_verify_one(int dev, uint64_t bytes, bool node_fanout, ccm_tag_r
   if (!e) { if (out) out->status = rc; return rc; }
   t_scrub_drill = drill;
   t_tag_call = tag;
+  t_residue_call = residue;
   rc = engine_scrub_verify(e, bytes, drill.inject, node_fanout, out);
+  t_residue_call = nullptr;
   t_tag_call = nullptr;
   t_scrub_drill = ScrubDrill();
   return rc;
@@ -532,7 +539,7 @@ int ccm_scrub_release_wait(int dev, double* ms_release, double* ms_waited) {
 }
 
 static int scrub_verify_many(int n, const int* devs, uint64_t bytes, ccm_tag_result* tag, ccm_scrub_result* out,
-                             double* wall_ms) {
+                             double* wall_ms, ccm_residue_report* residue = nullptr) {
   if (n < 0 || (n > 0 && (!devs || !out))) return CCM_ERR_INVALID;
   const auto t0 = Clock::now();
   std::vector<std::thread> th;
@@ -540,7 +547,7 @@ static int scrub_verify_many(int n, const int* devs, uint64_t bytes, ccm_tag_res
   th.reserve(n);
   for (int i = 0; i < n; ++i)
     th.emplace_back([&, i] {
-      int rc = scrub_verify_one(devs[i], bytes, n > 1, tag ? &tag[i] : nullptr, &out[i]);
+      int rc = scrub_verify_one(devs[i], bytes, n > 1, tag ? &tag[i] : nullptr, &out[i], residue ? &residue[i] : nullptr);
       if (rc) errs[i] = last_error();
     });
   for (auto& t : th) t.join();
@@ -558,6 +565,18 @@ int ccm_scrub_verify_many_tagged(int n, const int* devs, uint64_t bytes, ccm_tag
                                  double* wall_ms) {
   if (n > 0 && !tag) return CCM_ERR_INVALID;
   return scrub_verify_many(n, devs, bytes, tag, out, wall_ms);
+}
+
+int ccm_scrub_verify_residue(int dev, uint64_t bytes, ccm_tag_result* tag, ccm_residue_report* residue,
+                             ccm_scrub_result* out) {
+  if (!residue) return CCM_ERR_INVALID;
+  return scrub_verify_one(dev, bytes, false, tag, out, residue);
+}
+
+int ccm_scrub_verify_many_residue(int n, const int* devs, uint64_t bytes, ccm_tag_result* tag,
+                                  ccm_residue_report* residue, ccm_scrub_result* out, double* wall_ms) {
+  if (n > 0 && !residue) return CCM_ERR_INVALID;
+  return scrub_verify_many(n, devs, bytes, tag, out, wall_ms, residue);
 }
 
 int ccm_arena_acquire(int dev, uint64_t bytes, ccm_arena_info* out) {
@@ -676,6 +695,7 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
   else if (k == "scrub_inject") d.drill.inject = v < 0 ? 0 : (uint64_t)v;
   else if (k == "tag_inject") d.drill.tag_inject = v < 0 ? 0 : (uint64_t)v;
   else if (k == "scrub_alias") d.drill.alias = v != 0;
+  else if (k == "scrub_residue") d.drill.residue = v < 0 ? 0 : (uint64_t)v;
   else if (k == "scrub_poison" || k == "scrub_flood") {
     if (v < 0 || v > 255) { set_error("sim key '%s' takes a byte value (0 = off), not %lld", k.c_str(), (long long)v); return CCM_ERR_INVALID; }
     (k == "scrub_poison" ? d.drill.poison : d.drill.flood) = (int)v;
@@ -720,6 +740,7 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "scrub_flood") *value = d.drill.flood;
     else if (k == "tag_inject") *value = (int64_t)d.drill.tag_inject;
     else if (k == "scrub_alias") *value = d.drill.alias;
+    else if (k == "scrub_residue") *value = (int64_t)d.drill.residue;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

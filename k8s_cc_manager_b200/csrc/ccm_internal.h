@@ -46,12 +46,16 @@ int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, b
 // Drills of the tagged call (sim keys "tag_inject", "scrub_alias"; ccm.h):
 //   tag_inject: that many bytes are XORed between the tag fill and the check, same candidates as inject;
 //   alias:      the second main-zone chunk starts with a second view of the first chunk (VMM path only).
+// Drill of the residue census (sim key "scrub_residue"; ccm.h):
+//   residue:    every mapping (arena path: segment) is zero-filled right after it is mapped (after poison), then
+//               that many bytes are set to 0xA5, same candidates as inject but per mapping.
 struct ScrubDrill {
   uint64_t inject = 0;
   int poison = 0;
   int flood = 0;
   uint64_t tag_inject = 0;
   int alias = 0;
+  uint64_t residue = 0;
 };
 // inject: the call's "scrub_inject" budget.  Its poison and flood drills are those current_scrub_drill()
 // returns on the calling thread.  (The engine entry points keep the signatures that host-only builds of
@@ -83,5 +87,8 @@ const ScrubDrill& current_scrub_drill();
 // The tag block of the tagged product call running on this thread (its seed already drawn), or nullptr
 // for the zero-only call.  The engine writes the call's mismatch count and kernel times into it.
 ccm_tag_result* current_tag_call();
+// The residue report of the census call running on this thread, or nullptr for a call without the census.  The
+// engine fills it.
+ccm_residue_report* current_residue_call();
 
 }  // namespace ccm

@@ -96,12 +96,15 @@ static constexpr int kMaxPipeChunks = 32;
 //   [160] .. [200] the six words of tag_check_zero_kernel's window book (LocateOut): zero before and after
 //                  every call, because a check that finds nothing never writes them and the host re-zeroes
 //                  them after a check that did (or that an error cut short)
+//   [208]/[216] grab + done of census_zero_kernel and census_tag_fill_kernel (one call runs one of them)
+//   [224] .. [264] the six words of the census's window book: zero before and after every call, as the check's
 // The default kernels hand their pair back zeroed (GrabCtl), so they never share words with the
 // generic kernels, whose counter is memset by the host before every launch.
 static constexpr int kBookWords = 48;   // LocateOut word k at <first word> + 8k
 static constexpr int kNonzero = 0, kGenericGrab = 8, kScrubGrab = 16, kVerifyGrab = 32, kTagFillGrab = 48,
-                     kTagCheckGrab = 64, kMismatch = 80, kLocateGrab = 96, kLocateOut = 112, kCheckOut = 160;
-static constexpr int kCtlWords = kCheckOut + kBookWords;
+                     kTagCheckGrab = 64, kMismatch = 80, kLocateGrab = 96, kLocateOut = 112, kCheckOut = 160,
+                     kCensusGrab = 208, kCensusOut = 224;
+static constexpr int kCtlWords = kCensusOut + kBookWords;
 static constexpr int kLocateWords = kBookWords;
 
 // What a locate pass leaves for the host: its result words and records, copied back in one go.
@@ -109,6 +112,16 @@ struct LocateHost {
   unsigned long long words[kLocateWords];
   DirtRecord records[kDirtRecords];
 };
+// What a census leaves for the host: its book words, and (only when it found something) its records.
+struct CensusHost {
+  unsigned long long words[kBookWords];
+  MaskRecord records[kDirtRecords];
+};
+static_assert(sizeof(MaskRecord) == sizeof(ccm_residue_record) && sizeof(ccm_residue_record) == 16 &&
+              offsetof(ccm_residue_record, chunk) == offsetof(MaskRecord, chunk) &&
+              offsetof(ccm_residue_record, mask) == offsetof(MaskRecord, mask) &&
+              sizeof(ccm_residue_report) == 64 + 16 * CCM_DIRT_RECORDS,
+              "MaskRecord must match ccm_residue_record");
 static_assert(sizeof(DirtRecord) == sizeof(ccm_dirt_record) && offsetof(ccm_dirt_record, bytes) == 16 &&
               offsetof(ccm_dirt_record, mask) == 12 && kDirtRecords == CCM_DIRT_RECORDS,
               "DirtRecord must match ccm_dirt_record");
@@ -149,6 +162,8 @@ struct ScrubEngine {
   DirtRecord* d_check_records = nullptr;    // the tag check's records
   LocateHost* h_check = nullptr;            // pinned
   ccm_mismatch_report mismatch{};           // report of the last product call (ccm_scrub_last_mismatch)
+  MaskRecord* d_census_records = nullptr;   // the census's records
+  CensusHost* h_census = nullptr;           // pinned
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -170,6 +185,10 @@ struct ScrubEngine {
   LocateOut check_out() const {
     unsigned long long* w = d_counter + kCheckOut;
     return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, d_check_records};
+  }
+  LocateOut census_out() const {   // the census records into d_census_records (MaskRecord), not here
+    unsigned long long* w = d_counter + kCensusOut;
+    return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, nullptr};
   }
   // Waits for the background release of the previous gate (no-op when none is pending).
   double join_reaper() {
@@ -193,6 +212,10 @@ static constexpr int kTagThreads = 512, kTagPer = 16;
 // The locate pass after a failed read-back: 128 KiB per grab, one persistent 512-thread CTA per SM.
 static constexpr int kLocateThreads = 512, kLocatePer = 16;
 #define CCM_LOCATE locate_dirt_kernel<kLocateThreads, kLocatePer>
+// The census that replaces a call's first pass: 128 KiB per grab, one persistent 512-thread CTA per SM.
+static constexpr int kCensusThreads = 512, kCensusPer = 16;
+#define CCM_CENSUS_ZERO census_zero_kernel<kCensusThreads, kCensusPer>
+#define CCM_CENSUS_TAG census_tag_fill_kernel<kCensusThreads, kCensusPer>
 
 const char* default_kernel_names() {
   static const std::string names = [] {
@@ -227,6 +250,8 @@ int ScrubEngine::init() {
   CCM_CUDA(cudaHostAlloc(&h_locate, sizeof(LocateHost), cudaHostAllocDefault));
   CCM_CUDA(cudaMalloc(&d_check_records, kDirtRecords * sizeof(DirtRecord)));
   CCM_CUDA(cudaHostAlloc(&h_check, sizeof(LocateHost), cudaHostAllocDefault));
+  CCM_CUDA(cudaMalloc(&d_census_records, kDirtRecords * sizeof(MaskRecord)));
+  CCM_CUDA(cudaHostAlloc(&h_census, sizeof(CensusHost), cudaHostAllocDefault));
   // The product call maps HBM down to the last granule; CUDA loads kernel code lazily at the
   // first launch and that needs device memory — make the default kernels resident now.
   cudaFuncAttributes fa;
@@ -235,6 +260,8 @@ int ScrubEngine::init() {
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_TAG_FILL));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_TAG_CHECK));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_LOCATE));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_CENSUS_ZERO));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_CENSUS_TAG));
   CCM_CUDA(cudaFuncGetAttributes(&fa, xor_byte_kernel));
   size_t fr = 0;
   CCM_CUDA(cudaMemGetInfo(&fr, &total_bytes));
@@ -308,6 +335,10 @@ int engine_teardown(int ordinal) {
   if (e->h_locate) cudaFreeHost(e->h_locate);
   if (e->d_check_records) cudaFree(e->d_check_records);
   if (e->h_check) cudaFreeHost(e->h_check);
+  if (e->d_census_records) cudaFree(e->d_census_records);
+  if (e->h_census) cudaFreeHost(e->h_census);
+  e->d_census_records = nullptr;
+  e->h_census = nullptr;
   e->d_counter = nullptr;
   e->h_counter = nullptr;
   e->d_records = nullptr;
@@ -611,6 +642,21 @@ static int tag_check_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, c
   return CCM_OK;
 }
 
+// The census of one range on `st` (no sync): books what the range holds into the census's book with offsets
+// p - base (as tag_check_range), then stores zero over it, or (tags) the tags of `seed`.
+static int census_range(ScrubEngine* e, void* p, uint64_t n, bool tags, uint32_t seed, cudaStream_t st, uint64_t base) {
+  if (n == 0) return CCM_OK;
+  const RegionSplit s = split_region(p, n, 16, 128);
+  const cudaError_t err =
+      tags ? launch_fast(CCM_CENSUS_TAG, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, seed, e->census_out(),
+                         e->d_census_records, base)
+           : launch_fast(CCM_CENSUS_ZERO, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, e->census_out(),
+                         e->d_census_records, base);
+  g_launches++;
+  if (err != cudaSuccess) { set_error("census launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
+  return CCM_OK;
+}
+
 // ----------------------------------------------------------------------- arena
 static constexpr uint64_t kMiB = 1ull << 20;
 
@@ -857,6 +903,50 @@ static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_byte
   return CCM_OK;
 }
 
+// ------------------------------------------------------------------ what the first pass erased
+// Zeroes the census's book for the next call and waits: after a census that booked something, or that an error may
+// have cut short (a census that finds nothing never writes the book).
+static int clear_census_book(ScrubEngine* e, cudaStream_t st) {
+  CCM_CUDA(cudaMemsetAsync(e->d_counter + kCensusOut, 0, kBookWords * sizeof(unsigned long long), st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  return CCM_OK;
+}
+
+// After the census launches of one call have finished: copies the book (and, only when it is not empty, the records),
+// zeroes it for the next call and fills `rep` (located = 1).  Offsets are as the kernels booked them; every record
+// gets chunk_of(offset).
+template <typename ChunkOf>
+static int take_residue(ScrubEngine* e, cudaStream_t st, uint64_t va_base, uint64_t examined, ccm_residue_report* rep,
+                        ChunkOf&& chunk_of) {
+  memset(rep, 0, sizeof *rep);
+  CensusHost& h = *e->h_census;
+  CCM_CUDA(cudaMemcpyAsync(h.words, e->d_counter + kCensusOut, sizeof h.words, cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  rep->located = 1;
+  rep->va_base = va_base;
+  rep->bytes_examined = examined;
+  rep->residue_bytes = h.words[0];
+  rep->residue_windows = h.words[8];
+  if (rep->residue_windows == 0) return CCM_OK;
+  CCM_CUDA(cudaMemcpyAsync(h.records, e->d_census_records, sizeof h.records, cudaMemcpyDeviceToHost, st));
+  if (int rc = clear_census_book(e, st)) return rc;
+  rep->first_offset = ~h.words[16];
+  rep->last_offset = h.words[24];
+  const uint64_t claimed = h.words[32] < (uint64_t)kDirtRecords ? h.words[32] : (uint64_t)kDirtRecords;
+  for (uint64_t i = 0; i < claimed; ++i) {
+    ccm_residue_record& r = rep->records[rep->nrecords++];
+    r.offset = h.records[i].offset;
+    r.chunk = chunk_of(r.offset);
+    r.mask = h.records[i].mask;
+    r.reserved = 0;
+  }
+  std::sort(rep->records, rep->records + rep->nrecords, [](const ccm_residue_record& a, const ccm_residue_record& b) {
+    return (int64_t)a.offset < (int64_t)b.offset;
+  });
+  rep->truncated = rep->residue_windows > (uint64_t)CCM_DIRT_RECORDS;
+  return CCM_OK;
+}
+
 int engine_arena_scrub(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, void* stream, float* ms) {
   std::lock_guard<std::mutex> g(e->mu);
   CCM_ENSURE_READY(e);
@@ -1031,25 +1121,66 @@ static cudaError_t inject_dirt(uint8_t* p, uint64_t n, uint64_t* budget, cudaStr
   return cudaSuccess;
 }
 
+// Drill "scrub_residue" on one mapping (or segment) [p, p+n): zero-filled, then its inject_dirt candidates set to
+// 0xA5 while *budget lasts.
+static cudaError_t residue_drill(uint8_t* p, uint64_t n, uint64_t* budget, cudaStream_t st) {
+  const cudaError_t err = cudaMemsetAsync(p, 0, n, st);
+  return err == cudaSuccess ? inject_dirt(p, n, budget, st) : err;
+}
+
 // Fault drills on the segments of the arena the product call's fallback path holds: every segment is
-// filled with `fill` (0 = no fill), then up to `inject` bytes are dirtied, 4 candidates per segment.
-static int arena_drill(ScrubEngine* e, int fill, uint64_t inject) {
-  if (!fill && !inject) return CCM_OK;
+// filled with `fill` (0 = no fill), then (residue != 0) drilled with "scrub_residue", then up to `inject` bytes are
+// dirtied, 4 candidates per segment.
+static int arena_drill(ScrubEngine* e, int fill, uint64_t inject, uint64_t residue = 0) {
+  if (!fill && !inject && !residue) return CCM_OK;
   std::lock_guard<std::mutex> g(e->mu);
   CCM_ENSURE_READY(e);
   int rc = need_arena(e); if (rc) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
+  const bool drill_residue = residue != 0;
   for (auto& s : e->segs) {
     if (fill) CCM_CUDA(cudaMemsetAsync(s.ptr, fill, s.bytes, e->stream));
+    if (drill_residue) CCM_CUDA(residue_drill(s.ptr, s.bytes, &residue, e->stream));
     if (inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &inject, e->stream));
   }
   return CCM_OK;
 }
 
+// The segment a fallback offset (into the concatenated segments) lies in: the last one that starts at or before it.
+static uint32_t segment_of(const std::vector<Segment>& segs, uint64_t o) {
+  uint32_t i = 0;
+  uint64_t start = 0;
+  for (size_t k = 0; k < segs.size(); start += segs[k].bytes, ++k)
+    if ((int64_t)start <= (int64_t)o) i = (uint32_t)k;
+  return i;
+}
+
+// The zero gate's first pass on the fallback path, with the census: one census launch per segment (timed as the
+// scrub, *ms), offsets into the concatenated segments, chunk = segment index.
+static int arena_census(ScrubEngine* e, ccm_residue_report* res, float* ms) {
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  int rc = need_arena(e); if (rc) return rc;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  cudaStream_t st = e->stream;
+  rc = run_timed(e, st, ms, [&]() -> int {
+    uint64_t shift = 0;
+    for (auto& s : e->segs) {
+      if (int rc2 = census_range(e, s.ptr, s.bytes, false, 0, st, (uint64_t)(uintptr_t)s.ptr - shift)) return rc2;
+      shift += s.bytes;
+    }
+    return CCM_OK;
+  });
+  if (rc) { clear_census_book(e, st); return rc; }
+  return take_residue(e, st, (uint64_t)(uintptr_t)e->segs.front().ptr, e->arena_bytes, res,
+                      [&](uint64_t o) { return segment_of(e->segs, o); });
+}
+
 // Tagged pass of the product call's fallback path: tag every segment, then (after the "tag_inject"
 // drill) check and zero every segment.  Fills tag->mismatch_bytes, ->ms_tag, ->ms_check, ->va_base, and after
 // mismatches the engine's mismatch report (offsets into the concatenated segments, chunk = segment index).
-static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inject) {
+// res (census call): the fills are census fills, and `res` gets what they found.
+static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inject, ccm_residue_report* res) {
   std::lock_guard<std::mutex> g(e->mu);
   CCM_ENSURE_READY(e);
   int rc = need_arena(e); if (rc) return rc;
@@ -1063,7 +1194,12 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
   }
   // fills between ev[0] and ev[2], the drill, checks between ev[3] and ev[1]
   rc = run_counted(e, st, kMismatch, &tag->mismatch_bytes, nullptr, [&]() -> int {
-    for (auto& s : e->segs) if (int rc2 = tag_fill_range(e, s.ptr, s.bytes, tag->seed, st)) return rc2;
+    for (const CheckSpan& sp : spans) {
+      void* p = (void*)(uintptr_t)sp.addr;
+      if (int rc2 = res ? census_range(e, p, sp.bytes, true, tag->seed, st, sp.addr - sp.offset)
+                        : tag_fill_range(e, p, sp.bytes, tag->seed, st))
+        return rc2;
+    }
     CCM_CUDA(cudaEventRecord(e->ev[2], st));
     for (auto& s : e->segs)
       if (tag_inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &tag_inject, st, true));
@@ -1073,7 +1209,11 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
       if (int rc2 = tag_check_range(e, (void*)(uintptr_t)sp.addr, sp.bytes, tag->seed, st, sp.addr - sp.offset)) return rc2;
     return CCM_OK;
   });
-  if (rc) { clear_check_book(e, st); return rc; }
+  if (rc) {
+    clear_check_book(e, st);
+    if (res) clear_census_book(e, st);
+    return rc;
+  }
   float a = 0, b = 0;
   CCM_CUDA(cudaEventElapsedTime(&a, e->ev[0], e->ev[2]));
   CCM_CUDA(cudaEventElapsedTime(&b, e->ev[3], e->ev[1]));
@@ -1090,6 +1230,7 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
     };
     if (take_mismatch(e, st, tag->mismatch_bytes, tag->seed, tag->va_base, spans, &rep, chunk_of) == CCM_OK) e->mismatch = rep;
   }
+  if (res) return take_residue(e, st, tag->va_base, e->arena_bytes, res, [&](uint64_t o) { return segment_of(e->segs, o); });
   return CCM_OK;
 }
 
@@ -1243,10 +1384,14 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   std::vector<std::pair<uint64_t, uint64_t>> deferred;  // tagged: main-zone ranges, checked after the last mapping
   std::vector<std::pair<uint64_t, uint32_t>> pieces;    // (offset, handle index) of every mapped piece, ascending
   bool checked = false;                                 // tagged: a check was enqueued (its book may be non-zero)
+  // Census call: the first pass over each mapping (the scrub, or the tag fill) is the census of the same range.
+  ccm_residue_report* res = current_residue_call();
+  uint64_t residue = drill.residue;                     // "scrub_residue" budget, spent in mapping order
   auto tag_fill = [&](uint64_t off, uint64_t n) -> int {
     cudaEvent_t* evs = tag_timed < kMaxPipeChunks ? e->tag_ev[tag_timed] : nullptr;
     if (evs) cudaEventRecord(evs[0], st);
-    const int rc2 = tag_fill_range(e, (void*)(m.base + off), n, tag->seed, st);
+    const int rc2 = res ? census_range(e, (void*)(m.base + off), n, true, tag->seed, st, (uint64_t)m.base)
+                        : tag_fill_range(e, (void*)(m.base + off), n, tag->seed, st);
     if (evs) { cudaEventRecord(evs[1], st); ++tag_timed; }
     return rc2;
   };
@@ -1262,6 +1407,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     if (evs) cudaEventRecord(evs[0], st);
     checked |= tag != nullptr;
     int rc2 = tag ? tag_check_range(e, (void*)(m.base + off), n, tag->seed, st, (uint64_t)m.base)
+            : res ? census_range(e, (void*)(m.base + off), n, false, 0, st, (uint64_t)m.base)
                   : scrub_range(e, (void*)(m.base + off), n, CCM_SCRUB_AUTO, nullptr, st);
     if (evs) cudaEventRecord(evs[1], st);
     // fault drills: dirt the read-back of this range MUST find
@@ -1326,6 +1472,10 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     if (drill.poison) {
       cudaError_t perr = cudaMemsetAsync((void*)(m.base + off), drill.poison, n, st);
       if (perr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(perr)); rc = CCM_ERR_CUDA; break; }
+    }
+    if (drill.residue) {   // fault drill: a known residue, whatever the driver handed back
+      cudaError_t rerr = residue_drill((uint8_t*)(m.base + off), n, &residue, st);
+      if (rerr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(rerr)); rc = CCM_ERR_CUDA; break; }
     }
     if (tag) rc = tag_fill(off, n);
     // tail-zone granules are scrubbed with ONE launch pair once the zone is mapped
@@ -1402,6 +1552,12 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   } else if (checked && rc != CCM_OK) {
     clear_check_book(e, st);
   }
+  // ---- census call: what the first pass found.  The censuses booked it; one copy, no launch ----------------
+  if (res && rc == CCM_OK) {
+    if (take_residue(e, st, (uint64_t)m.base, mapped, res, chunk_of) != CCM_OK) memset(res, 0, sizeof *res);
+  } else if (res) {
+    clear_census_book(e, st);
+  }
   // ---- a failed read-back: where is the dirt?  One more launch, before the mapping goes back -------------
   if (rc == CCM_OK && r->nonzero_bytes != 0) {
     ccm_dirt_report rep;
@@ -1443,6 +1599,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   ScrubDrill drill = current_scrub_drill();
   drill.inject = inject;
   ccm_tag_result* tag = current_tag_call();
+  ccm_residue_report* res = current_residue_call();
   {
     std::lock_guard<std::mutex> g(e->mu);
     memset(&e->dirt, 0, sizeof e->dirt);  // every call replaces the reports of the last one
@@ -1452,7 +1609,8 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   memset(&r, 0, sizeof r);
   r.bytes_requested = bytes;
   r.sm_count = e->sm_count;
-  r.scrub_variant = resolve_scrub_variant(CCM_SCRUB_AUTO);
+  // a census call always runs the census kernel: the shape and stores of the default st128 scrub, whatever is pinned
+  r.scrub_variant = res ? CCM_SCRUB_ST128 : resolve_scrub_variant(CCM_SCRUB_AUTO);
   r.verify_variant = resolve_verify_variant(CCM_VERIFY_AUTO);
   int rc = CCM_ERR_UNSUPPORTED;
   if (env_u64("CCM_PIPELINE", 1) != 0) rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r);
@@ -1470,10 +1628,12 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       r.segments = ai.segments;
       float ms_s = 0, ms_v = 0;
       uint64_t nz = 0;
-      rc = arena_drill(e, drill.poison, 0);
+      rc = arena_drill(e, drill.poison, 0, drill.residue);
       if (rc == CCM_OK && tag) {
-        rc = arena_tag_check(e, tag, drill.tag_inject);
+        rc = arena_tag_check(e, tag, drill.tag_inject, res);
         ms_s = (float)tag->ms_check;
+      } else if (rc == CCM_OK && res) {
+        rc = arena_census(e, res, &ms_s);
       } else if (rc == CCM_OK) {
         rc = engine_arena_scrub(e, CCM_SCRUB_AUTO, nullptr, nullptr, &ms_s);
       }
@@ -1624,6 +1784,22 @@ extern "C" int ccm_region_tag_check_locate(int cuda_ordinal, void* dptr, uint64_
   }
   *out = rep;
   return CCM_OK;
+}
+
+// ------------------------------------------------------------------------- residue census
+extern "C" int ccm_region_census(int cuda_ordinal, void* dptr, uint64_t bytes, int store_tags, uint32_t seed, void* stream,
+                                 ccm_residue_report* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  ScrubEngine* e = engine_for(cuda_ordinal);
+  if (!e) return CCM_ERR_NO_CUDA;
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  cudaStream_t st = e->pick(stream);
+  const uint64_t base = (uint64_t)(uintptr_t)dptr;
+  if (int rc = census_range(e, dptr, bytes, store_tags != 0, seed, st, base)) { clear_census_book(e, st); return rc; }
+  return take_residue(e, st, base, bytes, out, [](uint64_t) { return 0u; });
 }
 
 // ------------------------------------------------------------------------- mismatch report

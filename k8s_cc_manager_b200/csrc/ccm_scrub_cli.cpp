@@ -1,12 +1,13 @@
 // ccm-scrub — native command-line front end of the HBM scrub gate (links libccm.so).
 //
-//   ccm-scrub [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] (--all | --bdf <pci address> ...)
+//   ccm-scrub [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] (--all | --bdf <pci address> ...)
 //
 // Runs the concurrent gate (ccm_scrub_verify_many, or ccm_scrub_verify_many_tagged with --check tagged)
 // and prints ONE JSON line with the same fields as k8s_cc_manager_b200.devices.ScrubReport (the
 // tagged-gate fields only with --check tagged, "dirt" only for a GPU whose read-back found non-zero bytes: where
 // they are, as ccm_scrub_last_dirt reports it; "mismatch" only for a GPU whose tagged check found bytes off their
-// tags, as ccm_scrub_last_mismatch reports it).  Exit 0: every GPU clean; 3: gate failed;
+// tags, as ccm_scrub_last_mismatch reports it; "residue" for every GPU with --residue, which runs the census
+// calls, ccm_scrub_verify_many_residue).  Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
 // post-reset step.
@@ -54,19 +55,36 @@ static void print_mismatch(const ccm_mismatch_report& m) {
   printf("]}");
 }
 
+// The "residue" object: the fields of k8s_cc_manager_b200.devices.ResidueReport (no bytes: there are none).
+static void print_residue(const ccm_residue_report& r) {
+  printf(", \"residue\": {\"residue_bytes\": %llu, \"residue_windows\": %llu, \"first_offset\": %llu, "
+         "\"last_offset\": %llu, \"bytes_examined\": %llu, \"va_base\": %llu, \"located\": %d, \"truncated\": %d, "
+         "\"records\": [",
+         (unsigned long long)r.residue_bytes, (unsigned long long)r.residue_windows, (unsigned long long)r.first_offset,
+         (unsigned long long)r.last_offset, (unsigned long long)r.bytes_examined, (unsigned long long)r.va_base,
+         r.located, r.truncated);
+  for (int k = 0; k < r.nrecords; ++k) {
+    const ccm_residue_record& w = r.records[k];
+    printf("%s{\"offset\": %lld, \"chunk\": %u, \"mask\": %u}", k ? ", " : "", (long long)w.offset, w.chunk,
+           (unsigned)w.mask);
+  }
+  printf("]}");
+}
+
 static int usage(const char* argv0) {
-  fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] (--all | --bdf <bdf> ...)\n",
-          argv0);
+  fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] "
+          "(--all | --bdf <bdf> ...)\n", argv0);
   return 2;
 }
 
 int main(int argc, char** argv) {
   std::vector<std::string> bdfs;
   unsigned long long bytes = 0;
-  bool all = false, tagged = false;
+  bool all = false, tagged = false, residue = false;
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     if (a == "--all") all = true;
+    else if (a == "--residue") residue = true;
     else if (a == "--bdf" && i + 1 < argc) bdfs.emplace_back(argv[++i]);
     else if (a == "--bytes" && i + 1 < argc) bytes = strtoull(argv[++i], nullptr, 10);
     else if (a == "--check" && i + 1 < argc) {
@@ -109,8 +127,12 @@ int main(int argc, char** argv) {
   }
   std::vector<ccm_scrub_result> res(devs.size() ? devs.size() : 1);
   std::vector<ccm_tag_result> tags(res.size());
+  std::vector<ccm_residue_report> census(residue ? res.size() : 0);
   double wall_ms = 0;
-  if (tagged) ccm_scrub_verify_many_tagged((int)devs.size(), devs.data(), bytes, tags.data(), res.data(), &wall_ms);
+  if (residue)
+    ccm_scrub_verify_many_residue((int)devs.size(), devs.data(), bytes, tagged ? tags.data() : nullptr, census.data(),
+                                  res.data(), &wall_ms);
+  else if (tagged) ccm_scrub_verify_many_tagged((int)devs.size(), devs.data(), bytes, tags.data(), res.data(), &wall_ms);
   else ccm_scrub_verify_many((int)devs.size(), devs.data(), bytes, res.data(), &wall_ms);
   bool clean = true;
   printf("{\"wall_ms\": %.3f, \"reports\": [", wall_ms);
@@ -135,6 +157,7 @@ int main(int argc, char** argv) {
     if (r.nonzero_bytes != 0 && ccm_scrub_last_dirt(ordinals[i], &d) == CCM_OK) print_dirt(d);
     ccm_mismatch_report m;
     if (tagged && tags[i].mismatch_bytes != 0 && ccm_scrub_last_mismatch(ordinals[i], &m) == CCM_OK) print_mismatch(m);
+    if (residue) print_residue(census[i]);
     printf("}");
   }
   printf("]}\n");

@@ -29,6 +29,7 @@
 //   scrub_tma_kernel                                     cp.async.bulk stores from one zero tile
 //   tag_fill_kernel / tag_check_zero_kernel              the tagged gate's known-answer pass
 //   locate_dirt_kernel                                   where the dirt is, after a failed read-back
+//   census_zero_kernel / census_tag_fill_kernel          what the first pass found before it erased it
 //   fill_pattern_kernel                                  seeded test pattern (tests only)
 // The grab loop (grab_chunks) and the epilogue after the last whole chunk or tile (finish_region,
 // ragged_bytes) are written once.  The five compile-time-shape kernels are one frame (default_kernel)
@@ -597,9 +598,10 @@ tag_fill_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed) {
 __global__ void xor_byte_kernel(uint8_t* p) { *p ^= 0xA5; }
 
 // ---------------------------------------------------------------- window books
-// The locate pass and the tag check say WHERE they found what they count, in 16-byte, 16-aligned address windows
-// (in the body a window is one vector).  Both keep the same book: exact window count and first / last byte in
-// registers, one atomic per result word per CTA, and up to kDirtRecords records of (window offset, mask, 16 bytes).
+// The locate pass, the tag check and the census say WHERE they found what they count, in 16-byte, 16-aligned address
+// windows (in the body a window is one vector).  All keep the same book: exact window count and first / last byte in
+// registers, one atomic per result word per CTA, and up to kDirtRecords records of (window offset, mask, 16 bytes);
+// the census records no bytes (MaskRecord).
 constexpr int kDirtRecords = 64;
 
 struct DirtRecord {       // layout of ccm_dirt_record (include/ccm.h); `chunk` is filled in by the host
@@ -609,6 +611,13 @@ struct DirtRecord {       // layout of ccm_dirt_record (include/ccm.h); `chunk` 
   uint16_t mask;          // bit i: byte i of the window is booked (locate: non-zero; check: differs from its tag)
   uint16_t reserved;
   uint4 bytes;
+};
+
+struct MaskRecord {       // layout of ccm_residue_record (include/ccm.h): a window without its bytes
+  uint64_t offset;        // as DirtRecord::offset
+  uint32_t chunk;         // filled in by the host
+  uint16_t mask;          // bit i: byte i of the window is non-zero
+  uint16_t reserved;
 };
 
 // Result words of one pass, each on its own line of the engine's control block; zero before the launch.
@@ -661,6 +670,22 @@ struct WindowBook {
     const uint64_t lo = off + (uint64_t)(__ffs(mask) - 1), hi = off + (uint64_t)(31 - __clz(mask));
     first_inv = max(first_inv, (uint64_t)~lo);
     last = max(last, hi);
+  }
+
+  // Counts n windows (n may be 0: then nothing changes) whose booked bytes run from off + lo to off + hi, without a
+  // branch.
+  __device__ __forceinline__ void tally_span(uint64_t off, uint32_t lo, uint32_t hi, uint32_t n) {
+    windows += n;
+    first_inv = max(first_inv, n ? (uint64_t)~(off + lo) : (uint64_t)0);
+    last = max(last, n ? off + hi : (uint64_t)0);
+  }
+
+  // Records a window (mask != 0) by offset and mask only, into `recs`, while slots last: for a pass whose bytes must
+  // not leave the device.  The window is tallied by the caller.
+  __device__ __forceinline__ void record_mask(MaskRecord* recs, uint64_t off, uint32_t mask) {
+    if (full_seen) return;
+    const uint64_t slot = claim();
+    if (slot < (uint64_t)kDirtRecords) recs[slot] = MaskRecord{off, 0u, (uint16_t)mask, (uint16_t)0};
   }
 
   __device__ __forceinline__ void record(uint64_t slot, uint64_t off, uint32_t mask, const Vec16& v) {
@@ -899,6 +924,121 @@ template <int THREADS, int PER_THREAD>
 __global__ void __launch_bounds__(THREADS, 1)
 locate_dirt_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, LocateOut out) {
   LocateOp op{{out}, s.base};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
+  op.ragged_windows(s);
+  op.book.flush();
+}
+
+// ------------------------------------------------------- census of what the gate erases
+// The first pass of a census call reads every vector before it writes it, and books what was there: the exact
+// number of non-zero bytes (book.count) and of non-zero windows, the first and last non-zero byte, and up to
+// kDirtRecords records of (window offset, mask of its non-zero bytes).  What it reads is the previous tenant's data,
+// so no byte of it is recorded: only counts, offsets and masks leave the registers.
+//
+// Residue may be everywhere (memory nobody cleared), so the dense case must stay cheap: each vector's mask is
+// computed while its words are live, the window is tallied branch-free, and the only branch claims a record slot
+// while the book is not full.  The loaded words die before the stores.  Then it stores zero, or (TAGS) the tags of
+// `seed`, over the same addresses.  Offsets are addresses - `base`, so every launch of one call books into the
+// same words.  The ragged head and tail are taken window by window by CTA 0 (byte() does nothing).
+template <bool TAGS>
+struct CensusOp {
+  uint32_t seed;
+  WindowBook book;
+  MaskRecord* records;
+  uint64_t base;
+
+  __device__ __forceinline__ void store(uint8_t* q) {
+    if constexpr (TAGS) st16(q, tag_vec(seed, addr(q)));
+    else st16(q, make_uint4(0, 0, 0, 0));
+  }
+
+  // One window outside the batches (a leftover vector, a ragged window).
+  __device__ __forceinline__ void window(uint64_t off, uint32_t mask) {
+    if (mask == 0) return;
+    book.count += __popc(mask);
+    book.tally(off, mask);
+    book.record_mask(records, off, mask);
+  }
+
+  // The batch's tally runs on offsets relative to its first vector (< 2^32), and the branch that claims record slots
+  // depends on every mask: all PER_THREAD loads are in flight before the first branch.
+  template <int THREADS, int PER_THREAD>
+  __device__ __forceinline__ void chunk(uint8_t* p) {
+    constexpr uint32_t kStride = THREADS * 16u;
+    uint32_t mask[PER_THREAD];
+    {
+      uint4 v[PER_THREAD];
+#pragma unroll
+      for (int u = 0; u < PER_THREAD; ++u) v[u] = ld16_cs(p + (uint32_t)u * kStride);  // all loads first
+#pragma unroll
+      for (int u = 0; u < PER_THREAD; ++u) mask[u] = nonzero_mask16(Vec16{{v[u].x, v[u].y, v[u].z, v[u].w}});
+    }
+    uint32_t any = 0, n = 0, nwin = 0, lo = 0xFFFFFFFFu, hi = 0;
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) {
+      const uint32_t m = mask[u], at = (uint32_t)u * kStride;
+      any |= m;
+      n += __popc(m);
+      nwin += m != 0;
+      lo = min(lo, m ? at + (uint32_t)(__ffs(m) - 1) : 0xFFFFFFFFu);
+      hi = max(hi, m ? at + (uint32_t)(31 - __clz(m)) : 0u);
+    }
+    const uint64_t off0 = addr(p) - base;
+    book.count += n;
+    book.tally_span(off0, lo, hi, nwin);
+    if (any != 0 && !book.full_seen) {  // only until the book is full, however dense the residue
+#pragma unroll
+      for (int u = 0; u < PER_THREAD; ++u)
+        if (mask[u] != 0) book.record_mask(records, off0 + (uint32_t)u * kStride, mask[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < PER_THREAD; ++u) store(p + (uint32_t)u * kStride);
+  }
+
+  __device__ __forceinline__ void vec(uint8_t* q) {
+    const uint4 v = ld16_cs(q);
+    window(addr(q) - base, nonzero_mask16(Vec16{{v.x, v.y, v.z, v.w}}));
+    store(q);
+  }
+
+  __device__ __forceinline__ void byte(uint8_t*) {}
+
+  // CTA 0: the windows of the ragged head and tail, one thread per window.  Only bytes inside the region are read
+  // and written; the others count as 0.
+  __device__ __forceinline__ void ragged_windows(const RegionSplit& s) {
+    uint64_t w0 = 0, lo = 0, hi = 0;
+    if (!ragged_window(s, w0, lo, hi)) return;
+    uint32_t mask = 0;
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+      if (w0 + i >= lo && w0 + i < hi) {
+        uint8_t* b = (uint8_t*)(uintptr_t)(w0 + i);
+        mask |= (uint32_t)(*b != 0) << i;
+        *b = TAGS ? tag_byte(seed, w0 + i) : (uint8_t)0;
+      }
+    window(w0 - base, mask);
+  }
+};
+
+// The zero gate's first pass with a census: books what each vector held (CensusOp), then zeroes it.  Frame of
+// scrub_st128_fast_kernel: persistent CTAs, one THREADS * PER_THREAD * 16-byte chunk per grab in ascending order,
+// self-resetting GrabCtl.  A census that finds nothing writes none of `out`'s words.  Minimum one CTA per SM in the
+// launch bounds, as locate_dirt_kernel: ptxas then keeps more of the batch's loads in flight before the first mask.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS, 1)
+census_zero_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, LocateOut out, MaskRecord* records, uint64_t base) {
+  CensusOp<false> op{0, {out}, records, base};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
+  op.ragged_windows(s);
+  op.book.flush();
+}
+
+// The tagged gate's fill with a census: books what each vector held, then writes the tags of `seed` (tag_fill_kernel).
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS, 1)
+census_tag_fill_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed, LocateOut out, MaskRecord* records,
+                       uint64_t base) {
+  CensusOp<true> op{seed, {out}, records, base};
   default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
   op.ragged_windows(s);
   op.book.flush();

@@ -37,6 +37,7 @@ class GpuError(Exception):
         self.status = status
         self.dirt: "Optional[DirtReport]" = None
         self.mismatch: "Optional[MismatchReport]" = None
+        self.residue: "Optional[ResidueReport]" = None   # a census call's report (what the first pass erased)
 
 
 def _error(rc: int, what: str, bdf: str = "") -> "Optional[GpuError]":
@@ -213,6 +214,63 @@ def last_mismatch(cuda_ordinal: int) -> "Optional[MismatchReport]":
 
 
 @dataclass
+class ResidueWindow:
+    """One 16-byte, 16-aligned window that held non-zero bytes when the census read it (include/ccm.h:
+    ccm_residue_record).  It carries no bytes: they were the previous tenant's data."""
+    offset: int      # from the report's va_base (negative only for the head window of an unaligned raw region)
+    chunk: int       # physical allocation behind it, in creation order (fallback: segment index)
+    mask: int        # bit i: byte i was non-zero
+
+    def describe(self) -> str:
+        return f"+{self.offset:#x} chunk {self.chunk} mask {self.mask:04x}"
+
+
+@dataclass
+class ResidueReport:
+    """What a census call's first pass found in the memory it mapped, before it erased it (include/ccm.h:
+    ccm_residue_report).  residue_bytes, residue_windows, first_offset and last_offset are exact; records are distinct
+    windows sorted by offset, all of them unless `truncated`."""
+    residue_bytes: int
+    residue_windows: int
+    first_offset: int        # first / last non-zero byte, from va_base (0 when there is none)
+    last_offset: int
+    bytes_examined: int      # == bytes_scrubbed
+    va_base: int
+    located: int             # 1: a census ran over everything the call mapped
+    truncated: int
+    records: List[ResidueWindow] = field(default_factory=list)
+
+    @classmethod
+    def from_native(cls, r: N.ResidueReport) -> "ResidueReport":
+        recs = [ResidueWindow(_signed64(w.offset), w.chunk, w.mask) for w in r.records[:r.nrecords]]
+        return cls(r.residue_bytes, r.residue_windows, r.first_offset, r.last_offset, r.bytes_examined, r.va_base,
+                   r.located, r.truncated, recs)
+
+    @classmethod
+    def from_json(cls, d: dict) -> "ResidueReport":
+        return cls(**{**d, "records": [ResidueWindow(**r) for r in d["records"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    @property
+    def chunks(self) -> List[int]:
+        return sorted({r.chunk for r in self.records})
+
+    def summary(self, first: int = 4) -> str:
+        """One line for an operator: "none", or the count, extent, chunks and first windows."""
+        if not self.located:
+            return "no census ran"
+        if self.residue_bytes == 0:
+            return f"none: all {self.bytes_examined} bytes examined were zero at first touch"
+        more = " (records truncated)" if self.truncated else ""
+        recs = "; ".join(r.describe() for r in self.records[:first])
+        return (f"{self.residue_bytes} of {self.bytes_examined} bytes were non-zero at first touch, in "
+                f"{self.residue_windows} 16-byte windows at offsets {self.first_offset:#x}..{self.last_offset:#x} of va "
+                f"{self.va_base:#x}{more}, chunks {self.chunks}; first windows: {recs}")
+
+
+@dataclass
 class ScrubReport:
     """Outcome of one GPU's HBM scrub-and-verify (include/ccm.h: ccm_scrub_result)."""
     bdf: str
@@ -244,6 +302,9 @@ class ScrubReport:
     # Where the tags were wrong (a MismatchReport), set for every report with mismatch_bytes != 0.  Not a dataclass
     # field either, for the same reason.
     mismatch = None
+    # What the first pass found before it erased it (a ResidueReport), set for every report of a census call
+    # (residue=True).  Not a dataclass field either.
+    residue = None
 
     @property
     def clean(self) -> bool:
@@ -289,6 +350,8 @@ class ScrubReport:
             d["dirt"] = self.dirt.as_json()
         if self.mismatch is not None:
             d["mismatch"] = self.mismatch.as_json()
+        if self.residue is not None:
+            d["residue"] = self.residue.as_json()
         return d
 
     @classmethod
@@ -297,11 +360,14 @@ class ScrubReport:
         d = dict(d)
         dirt = d.pop("dirt", None)
         mismatch = d.pop("mismatch", None)
+        residue = d.pop("residue", None)
         rep = cls(**d)
         if dirt is not None:
             rep.dirt = DirtReport.from_json(dirt)
         if mismatch is not None:
             rep.mismatch = MismatchReport.from_json(mismatch)
+        if residue is not None:
+            rep.residue = ResidueReport.from_json(residue)
         return rep
 
 
@@ -369,30 +435,38 @@ class NvidiaDevice:
         _check(N.lib().ccm_wait_for_boot(self.index, timeout_ms), "wait_for_boot", self.bdf)
 
     # -- NEW: HBM scrub-and-verify ---------------------------------------------
-    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero") -> ScrubReport:
+    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False) -> ScrubReport:
         """Zero-fills and reads back this GPU's HBM (nbytes=0: all the context can map).
         check="tagged" first writes and checks an address-tagged known answer
-        (include/ccm.h: ccm_scrub_verify_tagged).
+        (include/ccm.h: ccm_scrub_verify_tagged).  residue=True runs the census in the first pass and attaches what
+        it found as `.residue` (include/ccm.h: ccm_scrub_verify_residue); it never changes the verdict.
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
         if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
         found non-zero bytes, the report (or the GpuError, as `.dirt`) carries where they are; when the tagged check
         found bytes off their tags, it carries where those are as `.mismatch`.
         """
-        res, tag = N.ScrubResult(), None
+        res, tag, census = N.ScrubResult(), None, None
         if _check_mode(check):
             tag = N.TagResult()
+        if residue:
+            census = N.ResidueReport()
+            rc = N.lib().ccm_scrub_verify_residue(self.index, nbytes, C.byref(tag) if tag is not None else None,
+                                                  C.byref(census), C.byref(res))
+        elif tag is not None:
             rc = N.lib().ccm_scrub_verify_tagged(self.index, nbytes, C.byref(tag), C.byref(res))
         else:
             rc = N.lib().ccm_scrub_verify(self.index, nbytes, C.byref(res))
         err = _error(rc, "scrub_and_verify", self.bdf)   # the library's error text, before anything else runs
         rep = ScrubReport.from_native(self.bdf, res, tag)
+        if census is not None:
+            rep.residue = ResidueReport.from_native(census)
         if rep.nonzero_bytes:
             rep.dirt = last_dirt(self.cuda_ordinal)
         if rep.mismatch_bytes:
             rep.mismatch = last_mismatch(self.cuda_ordinal)
         if err is not None:
-            err.dirt, err.mismatch = rep.dirt, rep.mismatch
+            err.dirt, err.mismatch, err.residue = rep.dirt, rep.mismatch, rep.residue
             raise err
         return rep
 
@@ -437,10 +511,11 @@ def find_gpus() -> Tuple[List[NvidiaDevice], int]:
 
 
 def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
-                          check: str = "zero") -> Tuple[List[ScrubReport], float]:
+                          check: str = "zero", residue: bool = False) -> Tuple[List[ScrubReport], float]:
     """Concurrent multi-context scrub of several GPUs through ONE native call
     (ccm_scrub_verify_many: one host thread + primary context + stream per GPU, no
-    peer access, no collective; check="tagged": ccm_scrub_verify_many_tagged).  Returns
+    peer access, no collective; check="tagged": ccm_scrub_verify_many_tagged; residue=True:
+    ccm_scrub_verify_many_residue, each report with its `.residue`).  Returns
     (reports, wall_ms); never raises for a per-device failure — inspect report.status /
     report.clean."""
     tagged = _check_mode(check)
@@ -451,11 +526,17 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
     res = (N.ScrubResult * n)()
     wall = C.c_double(0.0)
     tags = (N.TagResult * n)() if tagged else None
-    if tagged:
+    census = (N.ResidueReport * n)() if residue else None
+    if residue:
+        N.lib().ccm_scrub_verify_many_residue(n, idx, nbytes, tags, census, res, C.byref(wall))
+    elif tagged:
         N.lib().ccm_scrub_verify_many_tagged(n, idx, nbytes, tags, res, C.byref(wall))
     else:
         N.lib().ccm_scrub_verify_many(n, idx, nbytes, res, C.byref(wall))
     reports = [ScrubReport.from_native(d.bdf, res[i], tags[i] if tagged else None) for i, d in enumerate(devices)]
+    if residue:
+        for i, rep in enumerate(reports):
+            rep.residue = ResidueReport.from_native(census[i])
     for rep, d in zip(reports, devices):
         if rep.nonzero_bytes:
             rep.dirt = last_dirt(d.cuda_ordinal)
@@ -512,10 +593,12 @@ class ScrubbingProxy:
         native = object.__getattribute__(self, "_native")
         return native.wait_scrub_released() if native is not None else (0.0, 0.0)
 
-    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero") -> ScrubReport:
+    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False) -> ScrubReport:
         native = object.__getattribute__(self, "_native")
         if native is None:
             raise GpuError(f"no CUDA device with PCI address {self._foreign.bdf}: HBM scrub cannot run", N.ERR_NO_CUDA)
+        if residue:
+            return native.scrub_and_verify(nbytes, check=check, residue=True)
         if check == "zero":
             return native.scrub_and_verify(nbytes)   # exactly the call a zero-only device takes
         return native.scrub_and_verify(nbytes, check=check)

@@ -61,6 +61,7 @@ CC_MODE_CONFIG_LABEL = "nvidia.com/cc.mode"
 READINESS_FILE = os.environ.get("CC_READINESS_FILE", "/run/nvidia/validations/.cc-manager-ctr-ready")
 VALID_MODES = ("on", "off", "devtools", "ppcie")
 SCRUB_SKIPPED_ANNOTATION = "nvidia.com/cc-manager.scrub-skipped"
+RESIDUE_MODES = ("off", "report")   # CC_SCRUB_RESIDUE
 
 WATCH_TIMEOUT_SECONDS = 300
 RECONNECT_DELAY_SECONDS = 5
@@ -102,7 +103,8 @@ class CCManager:
                  kubeconfig: str = "", v1=None,
                  device_source: Optional[Callable[[], tuple]] = None,
                  scrub_mode: Optional[str] = None, scrub_bytes: Optional[int] = None,
-                 max_parallel: Optional[int] = None, scrub_check: Optional[str] = None):
+                 max_parallel: Optional[int] = None, scrub_check: Optional[str] = None,
+                 scrub_residue: Optional[str] = None):
         env = os.environ
         self.operator_namespace = env.get("OPERATOR_NAMESPACE", "gpu-operator")
         self.evict_operator_components = env.get("EVICT_OPERATOR_COMPONENTS", "true").lower() == "true"
@@ -137,6 +139,13 @@ class CCManager:
         self.scrub_check = (scrub_check or env.get("CC_SCRUB_CHECK", "zero")).lower()
         if self.scrub_check not in _devices.CHECKS:
             raise ValueError(f"CC_SCRUB_CHECK must be 'zero' or 'tagged', not {self.scrub_check!r}")
+        # off:    the gate says nothing about what it erased.
+        # report: the gate's first pass also counts and locates what the memory held before it erased it (a census:
+        #         one more read of the mapping, no more launches).  Logged and kept in
+        #         last_transition["scrub_residue"]; it is a report, never a reason to fail the gate.
+        self.scrub_residue = (scrub_residue or env.get("CC_SCRUB_RESIDUE", "off")).lower()
+        if self.scrub_residue not in RESIDUE_MODES:
+            raise ValueError(f"CC_SCRUB_RESIDUE must be 'off' or 'report', not {self.scrub_residue!r}")
         self.max_parallel = int(max_parallel if max_parallel is not None else env.get("CC_MAX_PARALLEL", "0"))
         # "full-HBM" is enforced, not assumed: when scrubbing everything (scrub_bytes == 0) a GPU on
         # which less than this fraction of DEVICE memory was zeroed and read back fails the gate
@@ -520,6 +529,8 @@ class CCManager:
             cmd = [sys.executable, "-m", "k8s_cc_manager_b200.scrub_worker", "--bytes", str(self.scrub_bytes)]
         if self.scrub_check != "zero":
             cmd += ["--check", self.scrub_check]
+        if self.census:
+            cmd += ["--residue"]
         for gpu in gpus:
             cmd += ["--bdf", gpu.bdf]
         env = dict(os.environ)
@@ -547,6 +558,34 @@ class CCManager:
                                f"CC_SCRUB_CHECK={self.scrub_check}; refusing to release it")
         return rep
 
+    @property
+    def census(self) -> bool:
+        return self.scrub_residue == "report"
+
+    def _scrub_with_residue(self, gpu):
+        """The census call on one device.  A device whose scrub_and_verify cannot take `residue` is scrubbed exactly
+        as without the census, with a warning: the census is a report, and its absence never holds a GPU back."""
+        try:
+            inspect.signature(gpu.scrub_and_verify).bind(self.scrub_bytes, check=self.scrub_check, residue=True)
+        except (TypeError, ValueError):
+            logger.warning("Device %s cannot report HBM residue (CC_SCRUB_RESIDUE=report): its gate runs without "
+                           "the census", gpu.bdf)
+            return self._scrub_one(gpu, census=False)
+        return gpu.scrub_and_verify(self.scrub_bytes, check=self.scrub_check, residue=True)
+
+    def _scrub_one(self, gpu, census: bool):
+        if census:
+            return self._scrub_with_residue(gpu)
+        if self.scrub_check == "zero":
+            return gpu.scrub_and_verify(self.scrub_bytes)   # the call every scrubbing device takes
+        return self._scrub_checked(gpu)
+
+    def _note_residue(self, bdf: str, residue) -> None:
+        """Logs what the census found before the gate erased it ("none" included) and keeps the report in
+        last_transition["scrub_residue"][bdf]."""
+        self.last_transition.setdefault("scrub_residue", {})[bdf] = residue
+        logger.info("HBM residue on %s: %s", bdf, residue.summary())
+
     def _note_dirt(self, bdf: str, dirt) -> None:
         """Logs where a failed read-back found its non-zero bytes and keeps the report in
         last_transition["scrub_dirt"][bdf]: the gate hands the memory back right afterwards, so this is
@@ -568,7 +607,10 @@ class CCManager:
             # ONE native call for the whole node (maps first, then launches: DESIGN.md §6) — also when the
             # register work belongs to a foreign library and libccm only scrubs (ScrubbingProxy)
             natives = [self._native_of(g) for g in gpus]
-            if self.scrub_check == "zero":
+            if self.census:
+                reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes, check=self.scrub_check,
+                                                            residue=True)
+            elif self.scrub_check == "zero":
                 reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes)
             else:
                 reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes, check=self.scrub_check)
@@ -579,10 +621,10 @@ class CCManager:
                 if not hasattr(gpu, "scrub_and_verify"):
                     raise ScrubFailure(f"device {gpu.bdf} offers no HBM scrub; refusing to release it")
                 try:
-                    if self.scrub_check == "zero":
-                        return gpu.scrub_and_verify(self.scrub_bytes)   # the call every scrubbing device takes
-                    return self._scrub_checked(gpu)
+                    return self._scrub_one(gpu, self.census)
                 except GpuError as exc:
+                    if getattr(exc, "residue", None) is not None:
+                        self._note_residue(gpu.bdf, exc.residue)
                     if getattr(exc, "dirt", None) is not None:
                         self._note_dirt(gpu.bdf, exc.dirt)
                     if getattr(exc, "mismatch", None) is not None:
@@ -593,6 +635,8 @@ class CCManager:
         self.last_transition.setdefault("phase_seconds", {})["scrub"] = elapsed
         self.last_transition["scrub"] = reports
         for rep in reports:
+            if getattr(rep, "residue", None) is not None:
+                self._note_residue(rep.bdf, rep.residue)
             if getattr(rep, "dirt", None) is not None:
                 self._note_dirt(rep.bdf, rep.dirt)
             if getattr(rep, "mismatch", None) is not None:
@@ -860,6 +904,9 @@ def build_arg_parser() -> argparse.ArgumentParser:
     parser.add_argument("--scrub-check", default=None, choices=("zero", "tagged"),
                         help="what the scrub gate checks: zero read-back, or an address-tagged known answer "
                              "before it (default: $CC_SCRUB_CHECK or zero)")
+    parser.add_argument("--scrub-residue", default=None, choices=RESIDUE_MODES,
+                        help="report what the scrub gate found in HBM before it erased it (never fails the gate; "
+                             "default: $CC_SCRUB_RESIDUE or off)")
     return parser
 
 
@@ -884,6 +931,7 @@ def main(argv: Optional[List[str]] = None) -> None:
     try:
         CCManager(node_name=args.node_name, default_mode=default_mode, host_cc=host_cc,
                   kubeconfig=args.kubeconfig, scrub_mode=args.scrub_mode, scrub_check=args.scrub_check,
+                  scrub_residue=args.scrub_residue,
                   device_source=_device_source_from_env()).run()
     except KeyboardInterrupt:
         logger.info("Shutting down...")

@@ -8,7 +8,7 @@ concurrent gate (ccm_scrub_verify_many: one host thread + context + stream per G
 short-lived process and reads ONE JSON line back; the process exit returns every CUDA resource.
 
 Output (stdout, last line):  {"wall_ms": ..., "reports": [ {ScrubReport fields}, ... ]}
-(the tagged-gate fields only with --check tagged).
+(the tagged-gate fields only with --check tagged; "residue" only with --residue).
 Exit code: 0 if every GPU is clean, 3 if the gate failed, 2 on usage errors.
 """
 from __future__ import annotations
@@ -22,12 +22,16 @@ from . import _native as N
 from . import devices as D
 
 
-def run(bdfs: List[str], nbytes: int, check: str = "zero") -> dict:
+def run(bdfs: List[str], nbytes: int, check: str = "zero", residue: bool = False) -> dict:
     by_bdf = {d.bdf: d for d in D.find_gpus()[0] if d.is_gpu()}
     missing = [b for b in bdfs if b not in by_bdf]
     if missing:
         raise SystemExit(f"unknown GPU(s): {', '.join(missing)} (known: {', '.join(sorted(by_bdf))})")
-    reports, wall_ms = D.scrub_and_verify_many([by_bdf[b] for b in bdfs], nbytes, check=check)
+    devs = [by_bdf[b] for b in bdfs]
+    if residue:
+        reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check, residue=True)
+    else:
+        reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check)
     return {"wall_ms": wall_ms, "reports": [r.as_json() for r in reports]}
 
 
@@ -38,12 +42,14 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap.add_argument("--backend", choices=sorted(N.BACKENDS), default=None)
     ap.add_argument("--check", choices=D.CHECKS, default="zero",
                     help="zero: zero-fill + read-back; tagged: an address-tagged known answer first")
+    ap.add_argument("--residue", action="store_true",
+                    help="report what the first pass found in the memory before it erased it (never fails the gate)")
     args = ap.parse_args(argv)
     if not args.bdf:
         ap.error("at least one --bdf is required")
     if args.backend:
         D.select_backend(args.backend)
-    out = run([b.lower() for b in args.bdf], args.bytes, args.check)
+    out = run([b.lower() for b in args.bdf], args.bytes, args.check, args.residue)
     print(json.dumps(out), flush=True)
     return 0 if all(r["status"] == 0 and r["nonzero_bytes"] == 0 and r.get("mismatch_bytes", 0) == 0
                     for r in out["reports"]) else 3
