@@ -92,12 +92,13 @@ static constexpr int kMaxPipeChunks = 32;
 //   [16]/[24] grab + done of scrub_st128_fast_kernel      [32]/[40] grab + done of verify_ld128_fast_kernel
 //   [48]/[56] grab + done of tag_fill_kernel              [64]/[72] grab + done of tag_check_zero_kernel
 //   [80] mismatched byte count of the current tag check
-//   [96]/[104] grab + done of locate_dirt_kernel           [112] .. [152] its six result words (LocateOut)
-//   [160] .. [200] the six words of tag_check_zero_kernel's window book (LocateOut): zero before and after
-//                  every call, because a check that finds nothing never writes them and the host re-zeroes
-//                  them after a check that did (or that an error cut short)
+//   [96]/[104] grab + done of locate_dirt_kernel           [112] .. [152] its window book (the dirt book)
+//   [160] .. [200] the window book of tag_check_zero_kernel (the check book)
 //   [208]/[216] grab + done of census_zero_kernel and census_tag_fill_kernel (one call runs one of them)
-//   [224] .. [264] the six words of the census's window book: zero before and after every call, as the check's
+//   [224] .. [264] the window book of the census (the census book)
+// A window book is the six result words of one pass (LocateOut).  All three are zero between calls: a pass that
+// books nothing never writes them, and the host re-zeroes a book after reading one that is not empty
+// (read_book) and after a pass that an error may have cut short (drop_book).
 // The default kernels hand their pair back zeroed (GrabCtl), so they never share words with the
 // generic kernels, whose counter is memset by the host before every launch.
 static constexpr int kBookWords = 48;   // LocateOut word k at <first word> + 8k
@@ -105,17 +106,17 @@ static constexpr int kNonzero = 0, kGenericGrab = 8, kScrubGrab = 16, kVerifyGra
                      kTagCheckGrab = 64, kMismatch = 80, kLocateGrab = 96, kLocateOut = 112, kCheckOut = 160,
                      kCensusGrab = 208, kCensusOut = 224;
 static constexpr int kCtlWords = kCensusOut + kBookWords;
-static constexpr int kLocateWords = kBookWords;
 
-// What a locate pass leaves for the host: its result words and records, copied back in one go.
-struct LocateHost {
-  unsigned long long words[kLocateWords];
-  DirtRecord records[kDirtRecords];
-};
-// What a census leaves for the host: its book words, and (only when it found something) its records.
-struct CensusHost {
+enum Book { kDirtBook, kCheckBook, kCensusBook, kBooks };
+static constexpr int kBookOut[kBooks] = {kLocateOut, kCheckOut, kCensusOut};   // each book's first word
+
+// The host copy of one book: its words, and (only when it booked something) its records.  One at a time, under e->mu.
+struct BookHost {
   unsigned long long words[kBookWords];
-  MaskRecord records[kDirtRecords];
+  union {
+    DirtRecord dirt[kDirtRecords];   // dirt and check books
+    MaskRecord mask[kDirtRecords];   // census book
+  };
 };
 static_assert(sizeof(MaskRecord) == sizeof(ccm_residue_record) && sizeof(ccm_residue_record) == 16 &&
               offsetof(ccm_residue_record, chunk) == offsetof(MaskRecord, chunk) &&
@@ -156,14 +157,10 @@ struct ScrubEngine {
   int step_count = 0;
   unsigned long long* d_counter = nullptr;
   unsigned long long* h_counter = nullptr;  // pinned
-  DirtRecord* d_records = nullptr;          // the locate pass's records
-  LocateHost* h_locate = nullptr;           // pinned
+  DirtRecord* d_records = nullptr;          // kDirtRecords records per book, in Book order
+  BookHost* h_book = nullptr;               // pinned
   ccm_dirt_report dirt{};                   // report of the last product call (ccm_scrub_last_dirt)
-  DirtRecord* d_check_records = nullptr;    // the tag check's records
-  LocateHost* h_check = nullptr;            // pinned
   ccm_mismatch_report mismatch{};           // report of the last product call (ccm_scrub_last_mismatch)
-  MaskRecord* d_census_records = nullptr;   // the census's records
-  CensusHost* h_census = nullptr;           // pinned
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -178,17 +175,11 @@ struct ScrubEngine {
   cudaStream_t pick(void* s) const { return s ? (cudaStream_t)s : stream; }
   // the grab word of a default kernel and its done word, one line further on
   GrabCtl ctl(int grab) const { return GrabCtl{d_counter + grab, d_counter + grab + 8}; }
-  LocateOut locate_out() const {
-    unsigned long long* w = d_counter + kLocateOut;
-    return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, d_records};
-  }
-  LocateOut check_out() const {
-    unsigned long long* w = d_counter + kCheckOut;
-    return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, d_check_records};
-  }
-  LocateOut census_out() const {   // the census records into d_census_records (MaskRecord), not here
-    unsigned long long* w = d_counter + kCensusOut;
-    return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, nullptr};
+  DirtRecord* book_records(Book b) const { return d_records + b * kDirtRecords; }
+  // The census records into book_records(kCensusBook) as MaskRecord, passed to it apart from its LocateOut.
+  LocateOut book_out(Book b) const {
+    unsigned long long* w = d_counter + kBookOut[b];
+    return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, b == kCensusBook ? nullptr : book_records(b)};
   }
   // Waits for the background release of the previous gate (no-op when none is pending).
   double join_reaper() {
@@ -245,13 +236,9 @@ int ScrubEngine::init() {
   CCM_CUDA(cudaMalloc(&d_counter, kCtlWords * sizeof(unsigned long long)));
   CCM_CUDA(cudaMemset(d_counter, 0, kCtlWords * sizeof(unsigned long long)));
   CCM_CUDA(cudaHostAlloc(&h_counter, 64, cudaHostAllocDefault));
-  // The locate pass runs with all HBM mapped: its records and their host copy are set aside now.
-  CCM_CUDA(cudaMalloc(&d_records, kDirtRecords * sizeof(DirtRecord)));
-  CCM_CUDA(cudaHostAlloc(&h_locate, sizeof(LocateHost), cudaHostAllocDefault));
-  CCM_CUDA(cudaMalloc(&d_check_records, kDirtRecords * sizeof(DirtRecord)));
-  CCM_CUDA(cudaHostAlloc(&h_check, sizeof(LocateHost), cudaHostAllocDefault));
-  CCM_CUDA(cudaMalloc(&d_census_records, kDirtRecords * sizeof(MaskRecord)));
-  CCM_CUDA(cudaHostAlloc(&h_census, sizeof(CensusHost), cudaHostAllocDefault));
+  // The books' passes run with all HBM mapped: their records and the host copy are set aside now.
+  CCM_CUDA(cudaMalloc(&d_records, kBooks * kDirtRecords * sizeof(DirtRecord)));
+  CCM_CUDA(cudaHostAlloc(&h_book, sizeof(BookHost), cudaHostAllocDefault));
   // The product call maps HBM down to the last granule; CUDA loads kernel code lazily at the
   // first launch and that needs device memory — make the default kernels resident now.
   cudaFuncAttributes fa;
@@ -332,19 +319,11 @@ int engine_teardown(int ordinal) {
   if (e->d_counter) cudaFree(e->d_counter);
   if (e->h_counter) cudaFreeHost(e->h_counter);
   if (e->d_records) cudaFree(e->d_records);
-  if (e->h_locate) cudaFreeHost(e->h_locate);
-  if (e->d_check_records) cudaFree(e->d_check_records);
-  if (e->h_check) cudaFreeHost(e->h_check);
-  if (e->d_census_records) cudaFree(e->d_census_records);
-  if (e->h_census) cudaFreeHost(e->h_census);
-  e->d_census_records = nullptr;
-  e->h_census = nullptr;
+  if (e->h_book) cudaFreeHost(e->h_book);
   e->d_counter = nullptr;
   e->h_counter = nullptr;
   e->d_records = nullptr;
-  e->h_locate = nullptr;
-  e->d_check_records = nullptr;
-  e->h_check = nullptr;
+  e->h_book = nullptr;
   if (e->stream) cudaStreamDestroy(e->stream);
   e->stream = nullptr;
   e->ready = false;
@@ -636,7 +615,7 @@ static int tag_fill_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cu
 static int tag_check_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cudaStream_t st, uint64_t base) {
   if (n == 0) return CCM_OK;
   const cudaError_t err = launch_fast(CCM_TAG_CHECK, kTagThreads, kTagPer, e, kTagCheckGrab, st, split_region(p, n, 16, 128),
-                                      seed, e->d_counter + kMismatch, e->check_out(), base);
+                                      seed, e->d_counter + kMismatch, e->book_out(kCheckBook), base);
   g_launches++;
   if (err != cudaSuccess) { set_error("tag check launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
   return CCM_OK;
@@ -647,11 +626,12 @@ static int tag_check_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, c
 static int census_range(ScrubEngine* e, void* p, uint64_t n, bool tags, uint32_t seed, cudaStream_t st, uint64_t base) {
   if (n == 0) return CCM_OK;
   const RegionSplit s = split_region(p, n, 16, 128);
+  MaskRecord* recs = (MaskRecord*)e->book_records(kCensusBook);
   const cudaError_t err =
-      tags ? launch_fast(CCM_CENSUS_TAG, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, seed, e->census_out(),
-                         e->d_census_records, base)
-           : launch_fast(CCM_CENSUS_ZERO, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, e->census_out(),
-                         e->d_census_records, base);
+      tags ? launch_fast(CCM_CENSUS_TAG, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, seed,
+                         e->book_out(kCensusBook), recs, base)
+           : launch_fast(CCM_CENSUS_ZERO, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, e->book_out(kCensusBook),
+                         recs, base);
   g_launches++;
   if (err != cudaSuccess) { set_error("census launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
   return CCM_OK;
@@ -778,52 +758,76 @@ static int run_counted(ScrubEngine* e, cudaStream_t st, int word, uint64_t* coun
   return CCM_OK;
 }
 
+// ------------------------------------------------------------------ window books
+// What a book holds, decoded: the pass's own count, the windows booked, the first and last booked byte (meaningful
+// only when windows != 0) and how many records e->h_book holds.
+struct BookHead { uint64_t count, windows, first, last, nrecords; };
+
+// Zeroes book `b` for the next pass and waits: after a pass that an error may have cut short, or whose book is not
+// read.
+static int drop_book(ScrubEngine* e, Book b, cudaStream_t st) {
+  CCM_CUDA(cudaMemsetAsync(e->d_counter + kBookOut[b], 0, kBookWords * sizeof(unsigned long long), st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  return CCM_OK;
+}
+
+// After the passes that book into `b` (the caller holds e->mu): copies the book's words, waits and decodes them into
+// *head.  Only a book that is not empty costs more: its records are copied to e->h_book, and it is zeroed for the
+// next pass.
+static int read_book(ScrubEngine* e, Book b, cudaStream_t st, BookHead* head) {
+  BookHost& h = *e->h_book;
+  CCM_CUDA(cudaMemcpyAsync(h.words, e->d_counter + kBookOut[b], sizeof h.words, cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  *head = BookHead{h.words[0], h.words[8], ~h.words[16], h.words[24], std::min<uint64_t>(h.words[32], kDirtRecords)};
+  if (head->windows == 0) return CCM_OK;
+  CCM_CUDA(cudaMemcpyAsync(h.dirt, e->book_records(b), b == kCensusBook ? sizeof h.mask : sizeof h.dirt,
+                           cudaMemcpyDeviceToHost, st));
+  return drop_book(e, b, st);
+}
+
+// Sorts a report's records by offset (signed: a head window that starts before the region comes first) and sets
+// truncated: `windows` were booked, more than the records hold.
+template <typename Report>
+static void sort_records(Report* rep, uint64_t windows) {
+  std::sort(rep->records, rep->records + rep->nrecords,
+            [](const auto& a, const auto& b) { return (int64_t)a.offset < (int64_t)b.offset; });
+  rep->truncated = windows > (uint64_t)CCM_DIRT_RECORDS;
+}
+
 // ------------------------------------------------------------------ locate the dirt
 // One locate pass over [p, p+n) on `st` (synchronises; the caller holds e->mu).  What it found is added to `rep`
 // with its offsets moved by `shift` (the range's offset in what `rep` describes), and each new record gets the chunk
-// chunk_of(offset).  Records are kept while `rep` has room; finish_dirt() sorts them.
+// chunk_of(offset).  Records are kept while `rep` has room; sort_records() sorts them.
 template <typename ChunkOf>
 static int locate_range(ScrubEngine* e, const void* p, uint64_t n, uint64_t shift, cudaStream_t st,
                         ccm_dirt_report* rep, ChunkOf&& chunk_of) {
   rep->located = 1;
   if (n == 0) return CCM_OK;
-  CCM_CUDA(cudaMemsetAsync(e->d_counter + kLocateOut, 0, kLocateWords * sizeof(unsigned long long), st));
   float ms = 0;
   int rc = run_timed(e, st, &ms, [&]() -> int {
     const cudaError_t err = launch_fast(CCM_LOCATE, kLocateThreads, kLocatePer, e, kLocateGrab, st,
-                                        split_region(p, n, 16, 128), e->locate_out());
+                                        split_region(p, n, 16, 128), e->book_out(kDirtBook));
     g_launches++;
     if (err != cudaSuccess) { set_error("locate launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
     return CCM_OK;
   });
-  if (rc) return rc;
-  LocateHost& h = *e->h_locate;
-  CCM_CUDA(cudaMemcpyAsync(h.words, e->d_counter + kLocateOut, sizeof h.words, cudaMemcpyDeviceToHost, st));
-  CCM_CUDA(cudaMemcpyAsync(h.records, e->d_records, sizeof h.records, cudaMemcpyDeviceToHost, st));
-  CCM_CUDA(cudaStreamSynchronize(st));
-  const uint64_t nonzero = h.words[0], windows = h.words[8], first = ~h.words[16] + shift, last = h.words[24] + shift;
-  const uint64_t claimed = h.words[32] < (uint64_t)kDirtRecords ? h.words[32] : (uint64_t)kDirtRecords;
+  if (rc) { drop_book(e, kDirtBook, st); return rc; }
+  BookHead bk;
+  if ((rc = read_book(e, kDirtBook, st, &bk))) return rc;
   rep->ms_locate += ms;
-  if (windows == 0) return CCM_OK;
+  if (bk.windows == 0) return CCM_OK;
+  const uint64_t first = bk.first + shift, last = bk.last + shift;
   if (rep->dirty_windows == 0 || first < rep->first_offset) rep->first_offset = first;
   if (rep->dirty_windows == 0 || last > rep->last_offset) rep->last_offset = last;
-  rep->nonzero_bytes += nonzero;
-  rep->dirty_windows += windows;
-  for (uint64_t i = 0; i < claimed && rep->nrecords < CCM_DIRT_RECORDS; ++i) {
+  rep->nonzero_bytes += bk.count;
+  rep->dirty_windows += bk.windows;
+  for (uint64_t i = 0; i < bk.nrecords && rep->nrecords < CCM_DIRT_RECORDS; ++i) {
     ccm_dirt_record& r = rep->records[rep->nrecords++];
-    memcpy(&r, &h.records[i], sizeof r);
+    memcpy(&r, &e->h_book->dirt[i], sizeof r);
     r.offset += shift;
     r.chunk = chunk_of(r.offset);
   }
   return CCM_OK;
-}
-
-// Sorts the records by offset (signed: a head window that starts before the region comes first) and sets truncated.
-static void finish_dirt(ccm_dirt_report* rep) {
-  std::sort(rep->records, rep->records + rep->nrecords, [](const ccm_dirt_record& a, const ccm_dirt_record& b) {
-    return (int64_t)a.offset < (int64_t)b.offset;
-  });
-  rep->truncated = rep->dirty_windows > (uint64_t)CCM_DIRT_RECORDS;
 }
 
 // ------------------------------------------------------------------ where the tags were wrong
@@ -831,17 +835,9 @@ static void finish_dirt(ccm_dirt_report* rep) {
 // what the report describes (the mapping, the concatenated segments, or the region).
 struct CheckSpan { uint64_t addr, bytes, offset; };
 
-// Zeroes the tag check's book for the next check and waits.  Needed only after a check that booked something (or
-// that an error may have cut short): a check that finds nothing never writes the book.
-static int clear_check_book(ScrubEngine* e, cudaStream_t st) {
-  CCM_CUDA(cudaMemsetAsync(e->d_counter + kCheckOut, 0, kBookWords * sizeof(unsigned long long), st));
-  CCM_CUDA(cudaStreamSynchronize(st));
-  return CCM_OK;
-}
-
-// After checks that counted mismatch_bytes != 0 (and finished): copies the book, zeroes it for the next check and
-// fills `rep`.  Offsets are as the kernels booked them; every record is classified (ccm_mismatch.h) against `spans`
-// (the ALIAS search covers exactly them) and gets chunk_of(offset).
+// After checks that counted mismatch_bytes != 0 (and finished): reads the check book and fills `rep`.  Offsets are as
+// the kernels booked them; every record is classified (ccm_mismatch.h) against `spans` (the ALIAS search covers
+// exactly them) and gets chunk_of(offset).
 template <typename ChunkOf>
 static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_bytes, uint32_t seed, uint64_t va_base,
                          const std::vector<CheckSpan>& spans, ccm_mismatch_report* rep, ChunkOf&& chunk_of) {
@@ -850,16 +846,13 @@ static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_byte
   rep->seed = seed;
   rep->va_base = va_base;
   rep->mismatch_bytes = mismatch_bytes;
-  LocateHost& h = *e->h_check;
-  CCM_CUDA(cudaMemcpyAsync(h.words, e->d_counter + kCheckOut, sizeof h.words, cudaMemcpyDeviceToHost, st));
-  CCM_CUDA(cudaMemcpyAsync(h.records, e->d_check_records, sizeof h.records, cudaMemcpyDeviceToHost, st));
-  if (int rc = clear_check_book(e, st)) return rc;
-  rep->zero_windows = h.words[0];
-  rep->mismatch_windows = h.words[8];
-  if (rep->mismatch_windows == 0) return CCM_OK;
-  rep->first_offset = ~h.words[16];
-  rep->last_offset = h.words[24];
-  const uint64_t claimed = h.words[32] < (uint64_t)kDirtRecords ? h.words[32] : (uint64_t)kDirtRecords;
+  BookHead bk;
+  if (int rc = read_book(e, kCheckBook, st, &bk)) return rc;
+  rep->zero_windows = bk.count;
+  rep->mismatch_windows = bk.windows;
+  if (bk.windows == 0) return CCM_OK;
+  rep->first_offset = bk.first;
+  rep->last_offset = bk.last;
   std::vector<ccm_mismatch::Range> ranges;
   for (const CheckSpan& sp : spans) ranges.push_back({sp.addr, sp.addr + sp.bytes});
   // the span a booked offset belongs to: the last one that starts at or before it (a head window may start before
@@ -875,8 +868,8 @@ static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_byte
       if (a >= sp.addr && a < sp.addr + sp.bytes) return &sp;
     return nullptr;
   };
-  for (uint64_t i = 0; i < claimed; ++i) {
-    const DirtRecord& d = h.records[i];
+  for (uint64_t i = 0; i < bk.nrecords; ++i) {
+    const DirtRecord& d = e->h_book->dirt[i];
     ccm_mismatch_record& r = rep->records[rep->nrecords++];
     r.offset = d.offset;
     r.chunk = chunk_of(d.offset);
@@ -896,54 +889,36 @@ static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_byte
       r.source_chunk = chunk_of(r.source_offset);
     }
   }
-  std::sort(rep->records, rep->records + rep->nrecords, [](const ccm_mismatch_record& a, const ccm_mismatch_record& b) {
-    return (int64_t)a.offset < (int64_t)b.offset;
-  });
-  rep->truncated = rep->mismatch_windows > (uint64_t)CCM_DIRT_RECORDS;
+  sort_records(rep, bk.windows);
   return CCM_OK;
 }
 
 // ------------------------------------------------------------------ what the first pass erased
-// Zeroes the census's book for the next call and waits: after a census that booked something, or that an error may
-// have cut short (a census that finds nothing never writes the book).
-static int clear_census_book(ScrubEngine* e, cudaStream_t st) {
-  CCM_CUDA(cudaMemsetAsync(e->d_counter + kCensusOut, 0, kBookWords * sizeof(unsigned long long), st));
-  CCM_CUDA(cudaStreamSynchronize(st));
-  return CCM_OK;
-}
-
-// After the census launches of one call have finished: copies the book (and, only when it is not empty, the records),
-// zeroes it for the next call and fills `rep` (located = 1).  Offsets are as the kernels booked them; every record
-// gets chunk_of(offset).
+// After the census launches of one call have finished: reads the census book and fills `rep` (located = 1).  Offsets
+// are as the kernels booked them; every record gets chunk_of(offset).
 template <typename ChunkOf>
 static int take_residue(ScrubEngine* e, cudaStream_t st, uint64_t va_base, uint64_t examined, ccm_residue_report* rep,
                         ChunkOf&& chunk_of) {
   memset(rep, 0, sizeof *rep);
-  CensusHost& h = *e->h_census;
-  CCM_CUDA(cudaMemcpyAsync(h.words, e->d_counter + kCensusOut, sizeof h.words, cudaMemcpyDeviceToHost, st));
-  CCM_CUDA(cudaStreamSynchronize(st));
+  BookHead bk;
+  if (int rc = read_book(e, kCensusBook, st, &bk)) return rc;
   rep->located = 1;
   rep->va_base = va_base;
   rep->bytes_examined = examined;
-  rep->residue_bytes = h.words[0];
-  rep->residue_windows = h.words[8];
-  if (rep->residue_windows == 0) return CCM_OK;
-  CCM_CUDA(cudaMemcpyAsync(h.records, e->d_census_records, sizeof h.records, cudaMemcpyDeviceToHost, st));
-  if (int rc = clear_census_book(e, st)) return rc;
-  rep->first_offset = ~h.words[16];
-  rep->last_offset = h.words[24];
-  const uint64_t claimed = h.words[32] < (uint64_t)kDirtRecords ? h.words[32] : (uint64_t)kDirtRecords;
-  for (uint64_t i = 0; i < claimed; ++i) {
+  rep->residue_bytes = bk.count;
+  rep->residue_windows = bk.windows;
+  if (bk.windows == 0) return CCM_OK;
+  rep->first_offset = bk.first;
+  rep->last_offset = bk.last;
+  for (uint64_t i = 0; i < bk.nrecords; ++i) {
+    const MaskRecord& m = e->h_book->mask[i];
     ccm_residue_record& r = rep->records[rep->nrecords++];
-    r.offset = h.records[i].offset;
+    r.offset = m.offset;
     r.chunk = chunk_of(r.offset);
-    r.mask = h.records[i].mask;
+    r.mask = m.mask;
     r.reserved = 0;
   }
-  std::sort(rep->records, rep->records + rep->nrecords, [](const ccm_residue_record& a, const ccm_residue_record& b) {
-    return (int64_t)a.offset < (int64_t)b.offset;
-  });
-  rep->truncated = rep->residue_windows > (uint64_t)CCM_DIRT_RECORDS;
+  sort_records(rep, bk.windows);
   return CCM_OK;
 }
 
@@ -1171,7 +1146,7 @@ static int arena_census(ScrubEngine* e, ccm_residue_report* res, float* ms) {
     }
     return CCM_OK;
   });
-  if (rc) { clear_census_book(e, st); return rc; }
+  if (rc) { drop_book(e, kCensusBook, st); return rc; }
   return take_residue(e, st, (uint64_t)(uintptr_t)e->segs.front().ptr, e->arena_bytes, res,
                       [&](uint64_t o) { return segment_of(e->segs, o); });
 }
@@ -1186,6 +1161,7 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
   int rc = need_arena(e); if (rc) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->stream;
+  auto chunk_of = [&](uint64_t o) { return segment_of(e->segs, o); };
   std::vector<CheckSpan> spans;
   uint64_t shift = 0;
   for (auto& s : e->segs) {
@@ -1210,8 +1186,8 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
     return CCM_OK;
   });
   if (rc) {
-    clear_check_book(e, st);
-    if (res) clear_census_book(e, st);
+    drop_book(e, kCheckBook, st);
+    if (res) drop_book(e, kCensusBook, st);
     return rc;
   }
   float a = 0, b = 0;
@@ -1222,15 +1198,9 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
   tag->va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
   if (tag->mismatch_bytes != 0) {   // a failure of the report leaves it empty; it never changes the verdict
     ccm_mismatch_report rep;
-    auto chunk_of = [&](uint64_t o) {
-      uint32_t i = 0;
-      for (size_t k = 0; k < spans.size(); ++k)
-        if ((int64_t)spans[k].offset <= (int64_t)o) i = (uint32_t)k;
-      return i;
-    };
     if (take_mismatch(e, st, tag->mismatch_bytes, tag->seed, tag->va_base, spans, &rep, chunk_of) == CCM_OK) e->mismatch = rep;
   }
-  if (res) return take_residue(e, st, tag->va_base, e->arena_bytes, res, [&](uint64_t o) { return segment_of(e->segs, o); });
+  if (res) return take_residue(e, st, tag->va_base, e->arena_bytes, res, chunk_of);
   return CCM_OK;
 }
 
@@ -1248,7 +1218,7 @@ static void arena_locate(ScrubEngine* e) {
       return;
     shift += e->segs[i].bytes;
   }
-  finish_dirt(&rep);
+  sort_records(&rep, rep.dirty_windows);
   e->dirt = rep;
 }
 
@@ -1550,13 +1520,13 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     if (take_mismatch(e, st, tag->mismatch_bytes, tag->seed, (uint64_t)m.base, spans, &rep, chunk_of) == CCM_OK)
       e->mismatch = rep;   // never changes the verdict
   } else if (checked && rc != CCM_OK) {
-    clear_check_book(e, st);
+    drop_book(e, kCheckBook, st);
   }
   // ---- census call: what the first pass found.  The censuses booked it; one copy, no launch ----------------
   if (res && rc == CCM_OK) {
     if (take_residue(e, st, (uint64_t)m.base, mapped, res, chunk_of) != CCM_OK) memset(res, 0, sizeof *res);
   } else if (res) {
-    clear_census_book(e, st);
+    drop_book(e, kCensusBook, st);
   }
   // ---- a failed read-back: where is the dirt?  One more launch, before the mapping goes back -------------
   if (rc == CCM_OK && r->nonzero_bytes != 0) {
@@ -1564,7 +1534,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     memset(&rep, 0, sizeof rep);
     rep.va_base = (uint64_t)m.base;
     if (locate_range(e, (const void*)m.base, mapped, 0, st, &rep, chunk_of) == CCM_OK) {  // never changes the verdict
-      finish_dirt(&rep);
+      sort_records(&rep, rep.dirty_windows);
       e->dirt = rep;
     }
   }
@@ -1753,8 +1723,10 @@ extern "C" int ccm_region_tag_check_zero(int cuda_ordinal, void* dptr, uint64_t 
   uint64_t count = 0;
   const uint64_t base = (uint64_t)(uintptr_t)dptr;
   int rc = run_counted(e, st, kMismatch, &count, ms, [&] { return tag_check_range(e, dptr, bytes, seed, st, base); });
-  if (rc == CCM_OK && count != 0) rc = clear_check_book(e, st);   // the next check starts from an empty book
-  else if (rc != CCM_OK) clear_check_book(e, st);
+  if (rc != CCM_OK || count != 0) {   // the next check starts from an empty book
+    const int rc2 = drop_book(e, kCheckBook, st);
+    if (rc == CCM_OK) rc = rc2;
+  }
   if (mismatch) *mismatch = count;
   return rc;
 }
@@ -1772,7 +1744,7 @@ extern "C" int ccm_region_tag_check_locate(int cuda_ordinal, void* dptr, uint64_
   uint64_t count = 0;
   const uint64_t base = (uint64_t)(uintptr_t)dptr;
   int rc = run_counted(e, st, kMismatch, &count, nullptr, [&] { return tag_check_range(e, dptr, bytes, seed, st, base); });
-  if (rc != CCM_OK) { clear_check_book(e, st); return rc; }
+  if (rc != CCM_OK) { drop_book(e, kCheckBook, st); return rc; }
   ccm_mismatch_report rep;
   memset(&rep, 0, sizeof rep);
   rep.located = 1;
@@ -1798,7 +1770,7 @@ extern "C" int ccm_region_census(int cuda_ordinal, void* dptr, uint64_t bytes, i
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->pick(stream);
   const uint64_t base = (uint64_t)(uintptr_t)dptr;
-  if (int rc = census_range(e, dptr, bytes, store_tags != 0, seed, st, base)) { clear_census_book(e, st); return rc; }
+  if (int rc = census_range(e, dptr, bytes, store_tags != 0, seed, st, base)) { drop_book(e, kCensusBook, st); return rc; }
   return take_residue(e, st, base, bytes, out, [](uint64_t) { return 0u; });
 }
 
@@ -1844,7 +1816,7 @@ extern "C" int ccm_region_locate(int cuda_ordinal, const void* dptr, uint64_t by
   memset(&rep, 0, sizeof rep);
   rep.va_base = (uint64_t)(uintptr_t)dptr;
   if (int rc = locate_range(e, dptr, bytes, 0, e->pick(stream), &rep, [](uint64_t) { return 0u; })) return rc;
-  finish_dirt(&rep);
+  sort_records(&rep, rep.dirty_windows);
   *out = rep;
   return CCM_OK;
 }

@@ -30,14 +30,14 @@ from . import _native as N
 class GpuError(Exception):
     """Raised for any failed device operation (reference: gpu.GpuError).  A scrub that read back dirt
     carries its DirtReport as `.dirt`; a tagged scrub whose check found bytes off their tags carries its
-    MismatchReport as `.mismatch`."""
+    MismatchReport as `.mismatch`; a census call carries its ResidueReport (what the first pass erased) as
+    `.residue`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
         self.status = status
-        self.dirt: "Optional[DirtReport]" = None
-        self.mismatch: "Optional[MismatchReport]" = None
-        self.residue: "Optional[ResidueReport]" = None   # a census call's report (what the first pass erased)
+        for attr, _ in _REPORTS:
+            setattr(self, attr, None)
 
 
 def _error(rc: int, what: str, bdf: str = "") -> "Optional[GpuError]":
@@ -58,6 +58,32 @@ def _signed64(x: int) -> int:
     return x - (1 << 64) if x >= 1 << 63 else x
 
 
+class _WindowReport:
+    """What the three window reports share: their JSON and the chunks their records lie in.  Each report is a
+    dataclass with a `records` field of its WINDOW type."""
+    WINDOW: type
+
+    @classmethod
+    def from_json(cls, d: dict):
+        return cls(**{**d, "records": [cls.WINDOW(**r) for r in d["records"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    @property
+    def chunks(self) -> List[int]:
+        return sorted({r.chunk for r in self.records})
+
+
+def _last_report(cuda_ordinal: int, getter: str, native: type, report: type):
+    """The report `getter` (ccm_scrub_last_dirt / ccm_scrub_last_mismatch) gives for the last product call on a CUDA
+    device; None when it cannot be read."""
+    out = native()
+    if cuda_ordinal < 0 or getattr(N.lib(), getter)(cuda_ordinal, C.byref(out)) != N.OK:
+        return None
+    return report.from_native(out)
+
+
 @dataclass
 class DirtWindow:
     """One dirty 16-byte, 16-aligned window (include/ccm.h: ccm_dirt_record)."""
@@ -72,10 +98,11 @@ class DirtWindow:
 
 
 @dataclass
-class DirtReport:
+class DirtReport(_WindowReport):
     """Where the read-back of a failed scrub found its non-zero bytes (include/ccm.h: ccm_dirt_report).
     Every field but the choice of `records` is exact; records are distinct windows sorted by offset, all of
     them unless `truncated`."""
+    WINDOW = DirtWindow
     nonzero_bytes: int       # the locate pass's own recount
     dirty_windows: int
     first_offset: int        # first / last non-zero byte, from va_base
@@ -93,17 +120,6 @@ class DirtReport:
         return cls(d.nonzero_bytes, d.dirty_windows, d.first_offset, d.last_offset, d.va_base, d.ms_locate,
                    d.located, d.truncated, recs)
 
-    @classmethod
-    def from_json(cls, d: dict) -> "DirtReport":
-        return cls(**{**d, "records": [DirtWindow(**r) for r in d["records"]]})
-
-    def as_json(self) -> dict:
-        return dataclasses.asdict(self)
-
-    @property
-    def chunks(self) -> List[int]:
-        return sorted({r.chunk for r in self.records})
-
     def summary(self, first: int = 4) -> str:
         """One line for an operator: extent, window count, chunks involved and the first few windows."""
         more = " (records truncated)" if self.truncated else ""
@@ -116,10 +132,7 @@ class DirtReport:
 def last_dirt(cuda_ordinal: int) -> "Optional[DirtReport]":
     """The dirt report of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_dirt);
     None when it cannot be read."""
-    d = N.DirtReport()
-    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_dirt(cuda_ordinal, C.byref(d)) != N.OK:
-        return None
-    return DirtReport.from_native(d)
+    return _last_report(cuda_ordinal, "ccm_scrub_last_dirt", N.DirtReport, DirtReport)
 
 
 @dataclass
@@ -138,11 +151,12 @@ class MismatchWindow:
 
 
 @dataclass
-class MismatchReport:
+class MismatchReport(_WindowReport):
     """Where a failed tagged check found bytes that did not hold their tags (include/ccm.h: ccm_mismatch_report).
     mismatch_bytes, mismatch_windows, zero_windows, first_offset and last_offset are exact.  The split between
     alias, partial and foreign windows is known for the records only; records are distinct windows sorted by
     offset, all of them unless `truncated`."""
+    WINDOW = MismatchWindow
     mismatch_bytes: int
     mismatch_windows: int
     zero_windows: int        # mismatched windows whose bytes all read 0
@@ -161,13 +175,6 @@ class MismatchReport:
                 for r in m.records[:m.nrecords]]
         return cls(m.mismatch_bytes, m.mismatch_windows, m.zero_windows, m.first_offset, m.last_offset, m.va_base,
                    m.seed, m.located, m.truncated, recs)
-
-    @classmethod
-    def from_json(cls, d: dict) -> "MismatchReport":
-        return cls(**{**d, "records": [MismatchWindow(**r) for r in d["records"]]})
-
-    def as_json(self) -> dict:
-        return dataclasses.asdict(self)
 
     def by_kind(self) -> dict:
         out: dict = {}
@@ -207,10 +214,7 @@ class MismatchReport:
 def last_mismatch(cuda_ordinal: int) -> "Optional[MismatchReport]":
     """The mismatch report of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_mismatch);
     None when it cannot be read."""
-    m = N.MismatchReport()
-    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_mismatch(cuda_ordinal, C.byref(m)) != N.OK:
-        return None
-    return MismatchReport.from_native(m)
+    return _last_report(cuda_ordinal, "ccm_scrub_last_mismatch", N.MismatchReport, MismatchReport)
 
 
 @dataclass
@@ -226,10 +230,11 @@ class ResidueWindow:
 
 
 @dataclass
-class ResidueReport:
+class ResidueReport(_WindowReport):
     """What a census call's first pass found in the memory it mapped, before it erased it (include/ccm.h:
     ccm_residue_report).  residue_bytes, residue_windows, first_offset and last_offset are exact; records are distinct
     windows sorted by offset, all of them unless `truncated`."""
+    WINDOW = ResidueWindow
     residue_bytes: int
     residue_windows: int
     first_offset: int        # first / last non-zero byte, from va_base (0 when there is none)
@@ -246,17 +251,6 @@ class ResidueReport:
         return cls(r.residue_bytes, r.residue_windows, r.first_offset, r.last_offset, r.bytes_examined, r.va_base,
                    r.located, r.truncated, recs)
 
-    @classmethod
-    def from_json(cls, d: dict) -> "ResidueReport":
-        return cls(**{**d, "records": [ResidueWindow(**r) for r in d["records"]]})
-
-    def as_json(self) -> dict:
-        return dataclasses.asdict(self)
-
-    @property
-    def chunks(self) -> List[int]:
-        return sorted({r.chunk for r in self.records})
-
     def summary(self, first: int = 4) -> str:
         """One line for an operator: "none", or the count, extent, chunks and first windows."""
         if not self.located:
@@ -268,6 +262,10 @@ class ResidueReport:
         return (f"{self.residue_bytes} of {self.bytes_examined} bytes were non-zero at first touch, in "
                 f"{self.residue_windows} 16-byte windows at offsets {self.first_offset:#x}..{self.last_offset:#x} of va "
                 f"{self.va_base:#x}{more}, chunks {self.chunks}; first windows: {recs}")
+
+
+# The window reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
+_REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport))
 
 
 @dataclass
@@ -340,35 +338,38 @@ class ScrubReport:
         return rep
 
     def as_json(self) -> dict:
-        """The report as the scrub workers print it: the tagged-gate fields only for a tagged call, "dirt" only
-        when there is a dirt report."""
+        """The report as the scrub workers print it: the tagged-gate fields only for a tagged call, "dirt",
+        "mismatch" and "residue" only when that report is attached."""
         d = dataclasses.asdict(self)
         if self.check == "zero":
             for name in TAG_FIELDS:
                 del d[name]
-        if self.dirt is not None:
-            d["dirt"] = self.dirt.as_json()
-        if self.mismatch is not None:
-            d["mismatch"] = self.mismatch.as_json()
-        if self.residue is not None:
-            d["residue"] = self.residue.as_json()
+        for attr, _ in _REPORTS:
+            if getattr(self, attr) is not None:
+                d[attr] = getattr(self, attr).as_json()
         return d
 
     @classmethod
     def from_json(cls, d: dict) -> "ScrubReport":
         """Inverse of as_json."""
         d = dict(d)
-        dirt = d.pop("dirt", None)
-        mismatch = d.pop("mismatch", None)
-        residue = d.pop("residue", None)
+        found = [(attr, kind, d.pop(attr, None)) for attr, kind in _REPORTS]
         rep = cls(**d)
-        if dirt is not None:
-            rep.dirt = DirtReport.from_json(dirt)
-        if mismatch is not None:
-            rep.mismatch = MismatchReport.from_json(mismatch)
-        if residue is not None:
-            rep.residue = ResidueReport.from_json(residue)
+        for attr, kind, js in found:
+            if js is not None:
+                setattr(rep, attr, kind.from_json(js))
         return rep
+
+
+def _attach_reports(rep: ScrubReport, cuda_ordinal: int, census: "N.ResidueReport | None") -> None:
+    """Attaches to the report of a call what that call found: the census's report, and the device's last dirt /
+    mismatch report when the call counted non-zero / mismatched bytes."""
+    if census is not None:
+        rep.residue = ResidueReport.from_native(census)
+    if rep.nonzero_bytes:
+        rep.dirt = last_dirt(cuda_ordinal)
+    if rep.mismatch_bytes:
+        rep.mismatch = last_mismatch(cuda_ordinal)
 
 
 # ScrubReport fields that only a tagged call reports
@@ -459,14 +460,10 @@ class NvidiaDevice:
             rc = N.lib().ccm_scrub_verify(self.index, nbytes, C.byref(res))
         err = _error(rc, "scrub_and_verify", self.bdf)   # the library's error text, before anything else runs
         rep = ScrubReport.from_native(self.bdf, res, tag)
-        if census is not None:
-            rep.residue = ResidueReport.from_native(census)
-        if rep.nonzero_bytes:
-            rep.dirt = last_dirt(self.cuda_ordinal)
-        if rep.mismatch_bytes:
-            rep.mismatch = last_mismatch(self.cuda_ordinal)
+        _attach_reports(rep, self.cuda_ordinal, census)
         if err is not None:
-            err.dirt, err.mismatch, err.residue = rep.dirt, rep.mismatch, rep.residue
+            for attr, _ in _REPORTS:
+                setattr(err, attr, getattr(rep, attr))
             raise err
         return rep
 
@@ -534,14 +531,8 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
     else:
         N.lib().ccm_scrub_verify_many(n, idx, nbytes, res, C.byref(wall))
     reports = [ScrubReport.from_native(d.bdf, res[i], tags[i] if tagged else None) for i, d in enumerate(devices)]
-    if residue:
-        for i, rep in enumerate(reports):
-            rep.residue = ResidueReport.from_native(census[i])
-    for rep, d in zip(reports, devices):
-        if rep.nonzero_bytes:
-            rep.dirt = last_dirt(d.cuda_ordinal)
-        if rep.mismatch_bytes:
-            rep.mismatch = last_mismatch(d.cuda_ordinal)
+    for i, (rep, d) in enumerate(zip(reports, devices)):
+        _attach_reports(rep, d.cuda_ordinal, census[i] if residue else None)
     return reports, wall.value
 
 

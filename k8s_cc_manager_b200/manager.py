@@ -580,24 +580,24 @@ class CCManager:
             return gpu.scrub_and_verify(self.scrub_bytes)   # the call every scrubbing device takes
         return self._scrub_checked(gpu)
 
-    def _note_residue(self, bdf: str, residue) -> None:
-        """Logs what the census found before the gate erased it ("none" included) and keeps the report in
-        last_transition["scrub_residue"][bdf]."""
-        self.last_transition.setdefault("scrub_residue", {})[bdf] = residue
-        logger.info("HBM residue on %s: %s", bdf, residue.summary())
+    # The window reports a scrub report or GpuError may carry, in the order they are logged: (attribute, key of
+    # last_transition that keeps them by bdf, log level, log line).  Residue is what the census found before the gate
+    # erased it ("none" included); dirt is where a failed read-back found its non-zero bytes; mismatch is where a
+    # failed tagged check found bytes off their tags, and whose tags they hold.
+    _REPORT_NOTES = (
+        ("residue", "scrub_residue", logging.INFO, "HBM residue on %s: %s"),
+        ("dirt", "scrub_dirt", logging.ERROR, "HBM dirt on %s: %s"),
+        ("mismatch", "scrub_mismatch", logging.ERROR, "HBM tag mismatch on %s: %s"),
+    )
 
-    def _note_dirt(self, bdf: str, dirt) -> None:
-        """Logs where a failed read-back found its non-zero bytes and keeps the report in
-        last_transition["scrub_dirt"][bdf]: the gate hands the memory back right afterwards, so this is
-        the only look anyone gets at it."""
-        self.last_transition.setdefault("scrub_dirt", {})[bdf] = dirt
-        logger.error("HBM dirt on %s: %s", bdf, dirt.summary())
-
-    def _note_mismatch(self, bdf: str, mismatch) -> None:
-        """Logs where a failed tagged check found bytes off their tags (and whose tags they hold) and keeps the
-        report in last_transition["scrub_mismatch"][bdf], for the same reason as _note_dirt."""
-        self.last_transition.setdefault("scrub_mismatch", {})[bdf] = mismatch
-        logger.error("HBM tag mismatch on %s: %s", bdf, mismatch.summary())
+    def _note_reports(self, bdf: str, holder) -> None:
+        """Logs every window report `holder` carries and keeps it in last_transition: the gate hands the memory back
+        right after the verdict, so this is the only look anyone gets at it."""
+        for attr, key, level, line in self._REPORT_NOTES:
+            report = getattr(holder, attr, None)
+            if report is not None:
+                self.last_transition.setdefault(key, {})[bdf] = report
+                logger.log(level, line, bdf, report.summary())
 
     def _run_scrub(self, gpus: list) -> None:
         started = time.perf_counter()
@@ -623,24 +623,14 @@ class CCManager:
                 try:
                     return self._scrub_one(gpu, self.census)
                 except GpuError as exc:
-                    if getattr(exc, "residue", None) is not None:
-                        self._note_residue(gpu.bdf, exc.residue)
-                    if getattr(exc, "dirt", None) is not None:
-                        self._note_dirt(gpu.bdf, exc.dirt)
-                    if getattr(exc, "mismatch", None) is not None:
-                        self._note_mismatch(gpu.bdf, exc.mismatch)
+                    self._note_reports(gpu.bdf, exc)
                     raise
             reports = self._fan_out(gpus, one, "scrub")
         elapsed = time.perf_counter() - started
         self.last_transition.setdefault("phase_seconds", {})["scrub"] = elapsed
         self.last_transition["scrub"] = reports
         for rep in reports:
-            if getattr(rep, "residue", None) is not None:
-                self._note_residue(rep.bdf, rep.residue)
-            if getattr(rep, "dirt", None) is not None:
-                self._note_dirt(rep.bdf, rep.dirt)
-            if getattr(rep, "mismatch", None) is not None:
-                self._note_mismatch(rep.bdf, rep.mismatch)
+            self._note_reports(rep.bdf, rep)
         for rep in reports:
             mismatch = getattr(rep, "mismatch_bytes", 0)
             if rep.status != 0 or rep.nonzero_bytes != 0 or mismatch != 0:
