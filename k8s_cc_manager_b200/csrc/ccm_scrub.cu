@@ -96,9 +96,9 @@ static constexpr int kMaxPipeChunks = 32;
 //   [160] .. [200] the window book of tag_check_zero_kernel (the check book)
 //   [208]/[216] grab + done of census_zero_kernel and census_tag_fill_kernel (one call runs one of them)
 //   [224] .. [264] the window book of the census (the census book)
-// A window book is the six result words of one pass (LocateOut).  All three are zero between calls: a pass that
-// books nothing never writes them, and the host re-zeroes a book after reading one that is not empty
-// (read_book) and after a pass that an error may have cut short (drop_book).
+// A window book is the six result words of one pass (LocateOut), its records and its page map (d_pages).  All three
+// are zero between calls: a pass that books nothing never writes them, and the host re-zeroes a book after reading one
+// that is not empty (read_book) and after a pass that an error may have cut short (drop_book).
 // The default kernels hand their pair back zeroed (GrabCtl), so they never share words with the
 // generic kernels, whose counter is memset by the host before every launch.
 static constexpr int kBookWords = 48;   // LocateOut word k at <first word> + 8k
@@ -131,6 +131,11 @@ static_assert(sizeof(ccm_mismatch_record) == 48 && offsetof(ccm_mismatch_record,
               offsetof(ccm_mismatch_record, source_offset) == 16 && offsetof(ccm_mismatch_record, bytes) == 32 &&
               sizeof(ccm_mismatch_report) == 64 + 48 * CCM_DIRT_RECORDS,
               "ccm_mismatch_record must keep its 48-byte layout");
+static_assert(sizeof(ccm_page_entry) == 16 && offsetof(ccm_page_entry, bytes) == 8 &&
+              offsetof(ccm_page_entry, chunk) == 12 && CCM_PAGE_BYTES == kPageBytes,
+              "ccm_page_entry must keep its 16-byte layout, and the pages their size");
+static_assert(CCM_BOOK_DIRT == kDirtBook + 1 && CCM_BOOK_MISMATCH == kCheckBook + 1 &&
+              CCM_BOOK_RESIDUE == kCensusBook + 1, "ccm_book must name the books in Book order");
 static_assert(ccm_mismatch::kK1 == kTagK1 && ccm_mismatch::kK2 == kTagK2, "host and device tags must agree");
 static_assert(ccm_mismatch::kZero == CCM_MISMATCH_ZERO && ccm_mismatch::kAlias == CCM_MISMATCH_ALIAS &&
               ccm_mismatch::kPartial == CCM_MISMATCH_PARTIAL && ccm_mismatch::kForeign == CCM_MISMATCH_FOREIGN,
@@ -159,6 +164,10 @@ struct ScrubEngine {
   unsigned long long* h_counter = nullptr;  // pinned
   DirtRecord* d_records = nullptr;          // kDirtRecords records per book, in Book order
   BookHost* h_book = nullptr;               // pinned
+  uint64_t npages = 0;                      // page words per book: ceil(device total / kPageBytes) + 1
+  uint32_t* d_pages = nullptr;              // npages page words per book, in Book order
+  uint32_t* h_pages = nullptr;              // pinned, npages words: the page range of one book at a time
+  std::vector<ccm_page_entry> pages[kBooks];   // the page map behind each book's last report (ccm_last_page_map)
   ccm_dirt_report dirt{};                   // report of the last product call (ccm_scrub_last_dirt)
   ccm_mismatch_report mismatch{};           // report of the last product call (ccm_scrub_last_mismatch)
   std::vector<Segment> segs;
@@ -176,10 +185,12 @@ struct ScrubEngine {
   // the grab word of a default kernel and its done word, one line further on
   GrabCtl ctl(int grab) const { return GrabCtl{d_counter + grab, d_counter + grab + 8}; }
   DirtRecord* book_records(Book b) const { return d_records + b * kDirtRecords; }
+  uint32_t* book_pages(Book b) const { return d_pages + b * npages; }
   // The census records into book_records(kCensusBook) as MaskRecord, passed to it apart from its LocateOut.
   LocateOut book_out(Book b) const {
     unsigned long long* w = d_counter + kBookOut[b];
-    return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, b == kCensusBook ? nullptr : book_records(b)};
+    return LocateOut{w, w + 8, w + 16, w + 24, w + 32, w + 40, b == kCensusBook ? nullptr : book_records(b),
+                     book_pages(b)};
   }
   // Waits for the background release of the previous gate (no-op when none is pending).
   double join_reaper() {
@@ -236,9 +247,16 @@ int ScrubEngine::init() {
   CCM_CUDA(cudaMalloc(&d_counter, kCtlWords * sizeof(unsigned long long)));
   CCM_CUDA(cudaMemset(d_counter, 0, kCtlWords * sizeof(unsigned long long)));
   CCM_CUDA(cudaHostAlloc(&h_counter, 64, cudaHostAllocDefault));
-  // The books' passes run with all HBM mapped: their records and the host copy are set aside now.
+  // The books' passes run with all HBM mapped: their records, page maps and host copies are set aside now.  A page
+  // map has a word for every 2 MiB page of the device, and one more (a region that is not page-aligned).
+  size_t fr = 0;
+  CCM_CUDA(cudaMemGetInfo(&fr, &total_bytes));
+  npages = (total_bytes + kPageBytes - 1) / kPageBytes + 1;
   CCM_CUDA(cudaMalloc(&d_records, kBooks * kDirtRecords * sizeof(DirtRecord)));
   CCM_CUDA(cudaHostAlloc(&h_book, sizeof(BookHost), cudaHostAllocDefault));
+  CCM_CUDA(cudaMalloc(&d_pages, kBooks * npages * sizeof(uint32_t)));
+  CCM_CUDA(cudaMemset(d_pages, 0, kBooks * npages * sizeof(uint32_t)));
+  CCM_CUDA(cudaHostAlloc(&h_pages, npages * sizeof(uint32_t), cudaHostAllocDefault));
   // The product call maps HBM down to the last granule; CUDA loads kernel code lazily at the
   // first launch and that needs device memory — make the default kernels resident now.
   cudaFuncAttributes fa;
@@ -250,8 +268,6 @@ int ScrubEngine::init() {
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_CENSUS_ZERO));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_CENSUS_TAG));
   CCM_CUDA(cudaFuncGetAttributes(&fa, xor_byte_kernel));
-  size_t fr = 0;
-  CCM_CUDA(cudaMemGetInfo(&fr, &total_bytes));
   ready = true;
   return CCM_OK;
 }
@@ -320,10 +336,14 @@ int engine_teardown(int ordinal) {
   if (e->h_counter) cudaFreeHost(e->h_counter);
   if (e->d_records) cudaFree(e->d_records);
   if (e->h_book) cudaFreeHost(e->h_book);
+  if (e->d_pages) cudaFree(e->d_pages);
+  if (e->h_pages) cudaFreeHost(e->h_pages);
   e->d_counter = nullptr;
   e->h_counter = nullptr;
   e->d_records = nullptr;
   e->h_book = nullptr;
+  e->d_pages = nullptr;
+  e->h_pages = nullptr;
   if (e->stream) cudaStreamDestroy(e->stream);
   e->stream = nullptr;
   e->ready = false;
@@ -767,22 +787,50 @@ struct BookHead { uint64_t count, windows, first, last, nrecords; };
 // read.
 static int drop_book(ScrubEngine* e, Book b, cudaStream_t st) {
   CCM_CUDA(cudaMemsetAsync(e->d_counter + kBookOut[b], 0, kBookWords * sizeof(unsigned long long), st));
+  CCM_CUDA(cudaMemsetAsync(e->book_pages(b), 0, e->npages * sizeof(uint32_t), st));
   CCM_CUDA(cudaStreamSynchronize(st));
   return CCM_OK;
 }
 
 // After the passes that book into `b` (the caller holds e->mu): copies the book's words, waits and decodes them into
-// *head.  Only a book that is not empty costs more: its records are copied to e->h_book, and it is zeroed for the
-// next pass.
+// *head.  Only a book that is not empty costs more: its records are copied to e->h_book, the pages its windows can lie
+// on to e->pages[b] (appended: the caller clears the list when a report begins, and finish_pages() completes it), and
+// the book is zeroed for the next pass.
 static int read_book(ScrubEngine* e, Book b, cudaStream_t st, BookHead* head) {
   BookHost& h = *e->h_book;
   CCM_CUDA(cudaMemcpyAsync(h.words, e->d_counter + kBookOut[b], sizeof h.words, cudaMemcpyDeviceToHost, st));
   CCM_CUDA(cudaStreamSynchronize(st));
   *head = BookHead{h.words[0], h.words[8], ~h.words[16], h.words[24], std::min<uint64_t>(h.words[32], kDirtRecords)};
   if (head->windows == 0) return CCM_OK;
+  // A window starts at most 15 bytes before its first booked byte: the pages from that of first - 15 to that of last.
+  const uint64_t lo = head->first < 15 ? 0 : (head->first - 15) >> kPageShift;
+  const uint64_t hi = std::min<uint64_t>(head->last >> kPageShift, e->npages - 1);
+  const uint64_t np = hi >= lo ? hi - lo + 1 : 0;
+  uint32_t* pages = e->book_pages(b) + lo;
   CCM_CUDA(cudaMemcpyAsync(h.dirt, e->book_records(b), b == kCensusBook ? sizeof h.mask : sizeof h.dirt,
                            cudaMemcpyDeviceToHost, st));
-  return drop_book(e, b, st);
+  CCM_CUDA(cudaMemcpyAsync(e->h_pages, pages, np * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaMemsetAsync(e->d_counter + kBookOut[b], 0, kBookWords * sizeof(unsigned long long), st));
+  CCM_CUDA(cudaMemsetAsync(pages, 0, np * sizeof(uint32_t), st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  for (uint64_t i = 0; i < np; ++i)
+    if (e->h_pages[i]) e->pages[b].push_back(ccm_page_entry{lo + i, e->h_pages[i], 0});
+  return CCM_OK;
+}
+
+// Completes the page map read_book() gathered for book `b`: ascending, one entry per page (a page that two fallback
+// segments share was read twice), each with the chunk of its first byte, chunk_of(page offset).
+template <typename ChunkOf>
+static void finish_pages(ScrubEngine* e, Book b, ChunkOf&& chunk_of) {
+  std::vector<ccm_page_entry>& v = e->pages[b];
+  std::sort(v.begin(), v.end(), [](const ccm_page_entry& x, const ccm_page_entry& y) { return x.page < y.page; });
+  size_t k = 0;
+  for (size_t i = 0; i < v.size(); ++i) {
+    if (k && v[k - 1].page == v[i].page) v[k - 1].bytes += v[i].bytes;
+    else v[k++] = v[i];
+  }
+  v.resize(k);
+  for (ccm_page_entry& p : v) p.chunk = chunk_of(p.page * (uint64_t)kPageBytes);
 }
 
 // Sorts a report's records by offset (signed: a head window that starts before the region comes first) and sets
@@ -795,9 +843,10 @@ static void sort_records(Report* rep, uint64_t windows) {
 }
 
 // ------------------------------------------------------------------ locate the dirt
-// One locate pass over [p, p+n) on `st` (synchronises; the caller holds e->mu).  What it found is added to `rep`
-// with its offsets moved by `shift` (the range's offset in what `rep` describes), and each new record gets the chunk
-// chunk_of(offset).  Records are kept while `rep` has room; sort_records() sorts them.
+// One locate pass over [p, p+n) on `st` (synchronises; the caller holds e->mu).  The kernel books offsets from
+// p - shift (`shift`: the range's offset in what `rep` describes), and what it found is added to `rep`: each new record
+// gets the chunk chunk_of(offset), and its pages are appended to the dirt book's page map (read_book).  Records are
+// kept while `rep` has room; sort_records() sorts them.
 template <typename ChunkOf>
 static int locate_range(ScrubEngine* e, const void* p, uint64_t n, uint64_t shift, cudaStream_t st,
                         ccm_dirt_report* rep, ChunkOf&& chunk_of) {
@@ -806,7 +855,8 @@ static int locate_range(ScrubEngine* e, const void* p, uint64_t n, uint64_t shif
   float ms = 0;
   int rc = run_timed(e, st, &ms, [&]() -> int {
     const cudaError_t err = launch_fast(CCM_LOCATE, kLocateThreads, kLocatePer, e, kLocateGrab, st,
-                                        split_region(p, n, 16, 128), e->book_out(kDirtBook));
+                                        split_region(p, n, 16, 128), e->book_out(kDirtBook),
+                                        (uint64_t)(uintptr_t)p - shift);
     g_launches++;
     if (err != cudaSuccess) { set_error("locate launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
     return CCM_OK;
@@ -816,15 +866,13 @@ static int locate_range(ScrubEngine* e, const void* p, uint64_t n, uint64_t shif
   if ((rc = read_book(e, kDirtBook, st, &bk))) return rc;
   rep->ms_locate += ms;
   if (bk.windows == 0) return CCM_OK;
-  const uint64_t first = bk.first + shift, last = bk.last + shift;
-  if (rep->dirty_windows == 0 || first < rep->first_offset) rep->first_offset = first;
-  if (rep->dirty_windows == 0 || last > rep->last_offset) rep->last_offset = last;
+  if (rep->dirty_windows == 0 || bk.first < rep->first_offset) rep->first_offset = bk.first;
+  if (rep->dirty_windows == 0 || bk.last > rep->last_offset) rep->last_offset = bk.last;
   rep->nonzero_bytes += bk.count;
   rep->dirty_windows += bk.windows;
   for (uint64_t i = 0; i < bk.nrecords && rep->nrecords < CCM_DIRT_RECORDS; ++i) {
     ccm_dirt_record& r = rep->records[rep->nrecords++];
     memcpy(&r, &e->h_book->dirt[i], sizeof r);
-    r.offset += shift;
     r.chunk = chunk_of(r.offset);
   }
   return CCM_OK;
@@ -847,7 +895,9 @@ static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_byte
   rep->va_base = va_base;
   rep->mismatch_bytes = mismatch_bytes;
   BookHead bk;
+  e->pages[kCheckBook].clear();
   if (int rc = read_book(e, kCheckBook, st, &bk)) return rc;
+  finish_pages(e, kCheckBook, chunk_of);
   rep->zero_windows = bk.count;
   rep->mismatch_windows = bk.windows;
   if (bk.windows == 0) return CCM_OK;
@@ -901,7 +951,9 @@ static int take_residue(ScrubEngine* e, cudaStream_t st, uint64_t va_base, uint6
                         ChunkOf&& chunk_of) {
   memset(rep, 0, sizeof *rep);
   BookHead bk;
+  e->pages[kCensusBook].clear();
   if (int rc = read_book(e, kCensusBook, st, &bk)) return rc;
+  finish_pages(e, kCensusBook, chunk_of);
   rep->located = 1;
   rep->va_base = va_base;
   rep->bytes_examined = examined;
@@ -1212,13 +1264,17 @@ static void arena_locate(ScrubEngine* e) {
   ccm_dirt_report rep;
   memset(&rep, 0, sizeof rep);
   rep.va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
+  e->pages[kDirtBook].clear();
   uint64_t shift = 0;
   for (size_t i = 0; i < e->segs.size(); ++i) {
-    if (locate_range(e, e->segs[i].ptr, e->segs[i].bytes, shift, e->stream, &rep, [i](uint64_t) { return (uint32_t)i; }))
+    if (locate_range(e, e->segs[i].ptr, e->segs[i].bytes, shift, e->stream, &rep, [i](uint64_t) { return (uint32_t)i; })) {
+      e->pages[kDirtBook].clear();
       return;
+    }
     shift += e->segs[i].bytes;
   }
   sort_records(&rep, rep.dirty_windows);
+  finish_pages(e, kDirtBook, [&](uint64_t o) { return segment_of(e->segs, o); });
   e->dirt = rep;
 }
 
@@ -1533,9 +1589,13 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     ccm_dirt_report rep;
     memset(&rep, 0, sizeof rep);
     rep.va_base = (uint64_t)m.base;
+    e->pages[kDirtBook].clear();
     if (locate_range(e, (const void*)m.base, mapped, 0, st, &rep, chunk_of) == CCM_OK) {  // never changes the verdict
       sort_records(&rep, rep.dirty_windows);
+      finish_pages(e, kDirtBook, chunk_of);
       e->dirt = rep;
+    } else {
+      e->pages[kDirtBook].clear();
     }
   }
   // ---- give the HBM back: on the reaper (default) or right here -----------------------
@@ -1574,6 +1634,9 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     std::lock_guard<std::mutex> g(e->mu);
     memset(&e->dirt, 0, sizeof e->dirt);  // every call replaces the reports of the last one
     memset(&e->mismatch, 0, sizeof e->mismatch);
+    e->pages[kDirtBook].clear();          // and their page maps (a census call: the residue's too)
+    e->pages[kCheckBook].clear();
+    if (res) e->pages[kCensusBook].clear();
   }
   ccm_scrub_result r;
   memset(&r, 0, sizeof r);
@@ -1743,6 +1806,7 @@ extern "C" int ccm_region_tag_check_locate(int cuda_ordinal, void* dptr, uint64_
   cudaStream_t st = e->pick(stream);
   uint64_t count = 0;
   const uint64_t base = (uint64_t)(uintptr_t)dptr;
+  e->pages[kCheckBook].clear();
   int rc = run_counted(e, st, kMismatch, &count, nullptr, [&] { return tag_check_range(e, dptr, bytes, seed, st, base); });
   if (rc != CCM_OK) { drop_book(e, kCheckBook, st); return rc; }
   ccm_mismatch_report rep;
@@ -1815,8 +1879,33 @@ extern "C" int ccm_region_locate(int cuda_ordinal, const void* dptr, uint64_t by
   ccm_dirt_report rep;
   memset(&rep, 0, sizeof rep);
   rep.va_base = (uint64_t)(uintptr_t)dptr;
-  if (int rc = locate_range(e, dptr, bytes, 0, e->pick(stream), &rep, [](uint64_t) { return 0u; })) return rc;
+  e->pages[kDirtBook].clear();
+  if (int rc = locate_range(e, dptr, bytes, 0, e->pick(stream), &rep, [](uint64_t) { return 0u; })) {
+    e->pages[kDirtBook].clear();
+    return rc;
+  }
   sort_records(&rep, rep.dirty_windows);
+  finish_pages(e, kDirtBook, [](uint64_t) { return 0u; });
   *out = rep;
+  return CCM_OK;
+}
+
+// ------------------------------------------------------------------------- page maps
+extern "C" int ccm_last_page_map(int cuda_ordinal, int book, ccm_page_entry* out, uint64_t cap, uint64_t* n) {
+  if (!n || (cap && !out) || book < CCM_BOOK_DIRT || book > CCM_BOOK_RESIDUE) {
+    set_error("ccm_last_page_map: book %d, cap %llu (needs n, and out when cap > 0)", book, (unsigned long long)cap);
+    return CCM_ERR_INVALID;
+  }
+  *n = 0;
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no call ever reported anything (and none is started here)
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  const std::vector<ccm_page_entry>& v = e->pages[book - CCM_BOOK_DIRT];
+  *n = v.size();
+  if (cap) memcpy(out, v.data(), std::min<uint64_t>(cap, v.size()) * sizeof(ccm_page_entry));
   return CCM_OK;
 }

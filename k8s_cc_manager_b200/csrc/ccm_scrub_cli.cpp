@@ -7,20 +7,63 @@
 // tagged-gate fields only with --check tagged, "dirt" only for a GPU whose read-back found non-zero bytes: where
 // they are, as ccm_scrub_last_dirt reports it; "mismatch" only for a GPU whose tagged check found bytes off their
 // tags, as ccm_scrub_last_mismatch reports it; "residue" for every GPU with --residue, which runs the census
-// calls, ccm_scrub_verify_many_residue).  Exit 0: every GPU clean; 3: gate failed;
+// calls, ccm_scrub_verify_many_residue; each of the three with a "pages" member, the digest of its page map from
+// ccm_last_page_map).  Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
 // post-reset step.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <string>
 #include <vector>
 
 #include "ccm.h"
 
+// The value of a report's "pages" member: null when it booked no window, else the fields of
+// k8s_cc_manager_b200.devices.PageDigest, from ccm_last_page_map: page count, exact bytes and pages per chunk, and the
+// first 64 runs of consecutive pages in one chunk.
+static void print_pages(int ordinal, int book, uint64_t windows) {
+  uint64_t n = 0;
+  std::vector<ccm_page_entry> v;
+  if (windows == 0 || ccm_last_page_map(ordinal, book, nullptr, 0, &n) != CCM_OK) { printf("null"); return; }
+  v.resize(n);
+  if (n && ccm_last_page_map(ordinal, book, v.data(), n, &n) != CCM_OK) { printf("null"); return; }
+  struct Run { uint64_t first, pages, bytes; uint32_t chunk; };
+  std::vector<Run> runs;
+  std::map<uint32_t, std::pair<uint64_t, uint64_t>> chunks;   // chunk -> (pages, bytes)
+  uint64_t bytes = 0;
+  for (const ccm_page_entry& p : v) {
+    bytes += p.bytes;
+    chunks[p.chunk].first += 1;
+    chunks[p.chunk].second += p.bytes;
+    if (!runs.empty() && runs.back().chunk == p.chunk && runs.back().first + runs.back().pages == p.page) {
+      runs.back().pages += 1;
+      runs.back().bytes += p.bytes;
+    } else {
+      runs.push_back({p.page, 1, p.bytes, p.chunk});
+    }
+  }
+  const size_t keep = 64;   // k8s_cc_manager_b200.devices.PAGE_RUNS
+  printf("{\"pages\": %llu, \"bytes\": %llu, \"nruns\": %llu, \"runs_truncated\": %d, \"by_chunk\": [",
+         (unsigned long long)v.size(), (unsigned long long)bytes, (unsigned long long)runs.size(), runs.size() > keep);
+  bool sep = false;
+  for (const auto& c : chunks) {
+    printf("%s{\"chunk\": %u, \"pages\": %llu, \"bytes\": %llu}", sep ? ", " : "", c.first,
+           (unsigned long long)c.second.first, (unsigned long long)c.second.second);
+    sep = true;
+  }
+  printf("], \"runs\": [");
+  for (size_t k = 0; k < runs.size() && k < keep; ++k)
+    printf("%s{\"first_page\": %llu, \"pages\": %llu, \"chunk\": %u, \"bytes\": %llu}", k ? ", " : "",
+           (unsigned long long)runs[k].first, (unsigned long long)runs[k].pages, runs[k].chunk,
+           (unsigned long long)runs[k].bytes);
+  printf("]}");
+}
+
 // The "dirt" object: the fields of k8s_cc_manager_b200.devices.DirtReport, records with their bytes in hex.
-static void print_dirt(const ccm_dirt_report& d) {
+static void print_dirt(const ccm_dirt_report& d, int ordinal) {
   printf(", \"dirt\": {\"nonzero_bytes\": %llu, \"dirty_windows\": %llu, \"first_offset\": %llu, \"last_offset\": %llu, "
          "\"va_base\": %llu, \"ms_locate\": %.3f, \"located\": %d, \"truncated\": %d, \"records\": [",
          (unsigned long long)d.nonzero_bytes, (unsigned long long)d.dirty_windows, (unsigned long long)d.first_offset,
@@ -32,11 +75,13 @@ static void print_dirt(const ccm_dirt_report& d) {
     for (int b = 0; b < 16; ++b) printf("%02x", w.bytes[b]);
     printf("\"}");
   }
-  printf("]}");
+  printf("], \"pages\": ");
+  print_pages(ordinal, CCM_BOOK_DIRT, d.dirty_windows);
+  printf("}");
 }
 
 // The "mismatch" object: the fields of k8s_cc_manager_b200.devices.MismatchReport, kinds by name.
-static void print_mismatch(const ccm_mismatch_report& m) {
+static void print_mismatch(const ccm_mismatch_report& m, int ordinal) {
   static const char* const kinds[] = {"?", "zero", "alias", "partial", "foreign"};
   printf(", \"mismatch\": {\"mismatch_bytes\": %llu, \"mismatch_windows\": %llu, \"zero_windows\": %llu, "
          "\"first_offset\": %llu, \"last_offset\": %llu, \"va_base\": %llu, \"seed\": %u, \"located\": %d, "
@@ -52,11 +97,13 @@ static void print_mismatch(const ccm_mismatch_report& m) {
     for (int b = 0; b < 16; ++b) printf("%02x", w.bytes[b]);
     printf("\"}");
   }
-  printf("]}");
+  printf("], \"pages\": ");
+  print_pages(ordinal, CCM_BOOK_MISMATCH, m.mismatch_windows);
+  printf("}");
 }
 
 // The "residue" object: the fields of k8s_cc_manager_b200.devices.ResidueReport (no bytes: there are none).
-static void print_residue(const ccm_residue_report& r) {
+static void print_residue(const ccm_residue_report& r, int ordinal) {
   printf(", \"residue\": {\"residue_bytes\": %llu, \"residue_windows\": %llu, \"first_offset\": %llu, "
          "\"last_offset\": %llu, \"bytes_examined\": %llu, \"va_base\": %llu, \"located\": %d, \"truncated\": %d, "
          "\"records\": [",
@@ -68,7 +115,9 @@ static void print_residue(const ccm_residue_report& r) {
     printf("%s{\"offset\": %lld, \"chunk\": %u, \"mask\": %u}", k ? ", " : "", (long long)w.offset, w.chunk,
            (unsigned)w.mask);
   }
-  printf("]}");
+  printf("], \"pages\": ");
+  print_pages(ordinal, CCM_BOOK_RESIDUE, r.residue_windows);
+  printf("}");
 }
 
 static int usage(const char* argv0) {
@@ -154,10 +203,10 @@ int main(int argc, char** argv) {
              t.seed, (unsigned long long)t.mismatch_bytes, t.ms_tag, t.ms_check);
     }
     ccm_dirt_report d;
-    if (r.nonzero_bytes != 0 && ccm_scrub_last_dirt(ordinals[i], &d) == CCM_OK) print_dirt(d);
+    if (r.nonzero_bytes != 0 && ccm_scrub_last_dirt(ordinals[i], &d) == CCM_OK) print_dirt(d, ordinals[i]);
     ccm_mismatch_report m;
-    if (tagged && tags[i].mismatch_bytes != 0 && ccm_scrub_last_mismatch(ordinals[i], &m) == CCM_OK) print_mismatch(m);
-    if (residue) print_residue(census[i]);
+    if (tagged && tags[i].mismatch_bytes != 0 && ccm_scrub_last_mismatch(ordinals[i], &m) == CCM_OK) print_mismatch(m, ordinals[i]);
+    if (residue) print_residue(census[i], ordinals[i]);
     printf("}");
   }
   printf("]}\n");

@@ -601,7 +601,9 @@ __global__ void xor_byte_kernel(uint8_t* p) { *p ^= 0xA5; }
 // The locate pass, the tag check and the census say WHERE they found what they count, in 16-byte, 16-aligned address
 // windows (in the body a window is one vector).  All keep the same book: exact window count and first / last byte in
 // registers, one atomic per result word per CTA, and up to kDirtRecords records of (window offset, mask, 16 bytes);
-// the census records no bytes (MaskRecord).
+// the census records no bytes (MaskRecord).  Each also counts its booked bytes per 2 MiB page (LocateOut::pages): a
+// batch's bytes add up over the active lanes of the warp, one atomic per page per warp per batch, and only in the
+// branch that books.
 constexpr int kDirtRecords = 64;
 
 struct DirtRecord {       // layout of ccm_dirt_record (include/ccm.h); `chunk` is filled in by the host
@@ -620,6 +622,12 @@ struct MaskRecord {       // layout of ccm_residue_record (include/ccm.h): a win
   uint16_t reserved;
 };
 
+// The page map: booked bytes per 2 MiB page (the VMM granule: every chunk the product call maps is a whole number of
+// pages).  A window belongs to the page of its offset, offset >> kPageShift; the head window of a region that does
+// not start 16-aligned, whose offset is negative, belongs to page 0.
+constexpr int kPageShift = 21;
+constexpr uint32_t kPageBytes = 1u << kPageShift;
+
 // Result words of one pass, each on its own line of the engine's control block; zero before the launch.
 struct LocateOut {
   unsigned long long* count;      // += the op's own count: non-zero bytes (locate), all-zero windows (tag check)
@@ -629,6 +637,7 @@ struct LocateOut {
   unsigned long long* slots;      // record slots claimed (may run past kDirtRecords)
   unsigned long long* full;       // set once kDirtRecords slots are taken
   DirtRecord* records;
+  uint32_t* pages;                // += booked bytes of each page (zero before the launch, like the words)
 };
 
 // Bit 7 of each byte of the result is set iff that byte of w is non-zero (as in nonzero_bytes_in_word).
@@ -704,6 +713,53 @@ struct WindowBook {
     if (full_seen) return;
     const uint64_t slot = claim();
     if (slot < (uint64_t)kDirtRecords) record(slot, off, mask, v);
+  }
+
+  __device__ __forceinline__ static uint32_t page_of(uint64_t off) {
+    return (int64_t)off < 0 ? 0u : (uint32_t)(off >> kPageShift);
+  }
+
+  // Bytes from a chunk's first byte (offset c0, never negative: every caller's base lies at or before its body) to
+  // the next page boundary.  A chunk (128 KiB) is shorter than a page, so its vectors lie on c0's page (chunk-relative
+  // offset < the room) or the next one.
+  __device__ __forceinline__ static uint32_t page_room(uint64_t c0) {
+    return kPageBytes - ((uint32_t)c0 & (kPageBytes - 1));
+  }
+
+  // Pages of one batch: lo booked bytes on the page of the chunk offset c0, hi on the next (only when the chunk
+  // `crosses` a page boundary, which a 2 MiB-aligned body never does; the same for every lane of the chunk).  Every
+  // active lane is in the same chunk, so they add up over the active lanes and one lane issues one atomic per non-zero
+  // page.
+  // (Before sm_80 there is no __reduce_add_sync: every lane adds its own bytes.  The library builds for sm_90a only;
+  // the fallback keeps this header compiling for any architecture.)
+  __device__ __forceinline__ void pages_batch(uint64_t c0, uint32_t lo, uint32_t hi, bool crosses) {
+#if defined(__CUDA_ARCH__) && __CUDA_ARCH__ < 800
+    if (lo) atomicAdd(out.pages + page_of(c0), lo);
+    if (crosses && hi) atomicAdd(out.pages + page_of(c0) + 1, hi);
+#else
+    const uint32_t active = __activemask();
+    lo = __reduce_add_sync(active, lo);
+    if (crosses) hi = __reduce_add_sync(active, hi);
+    if ((threadIdx.x & 31u) == (uint32_t)(__ffs(active) - 1)) {
+      const uint32_t page = page_of(c0);
+      if (lo) atomicAdd(out.pages + page, lo);
+      if (crosses && hi) atomicAdd(out.pages + page + 1, hi);
+    }
+#endif
+  }
+
+  // Pages of one window outside the batches (a leftover vector, a ragged window) with `bytes` != 0 booked: the active
+  // lanes that book into one page add up, and one of them issues the atomic.
+  __device__ __forceinline__ void pages_window(uint64_t off, uint32_t bytes) {
+#if defined(__CUDA_ARCH__) && __CUDA_ARCH__ < 800
+    atomicAdd(out.pages + page_of(off), bytes);
+#else
+    const uint32_t active = __activemask();
+    const uint32_t page = page_of(off);
+    const uint32_t peers = __match_any_sync(active, page);
+    bytes = __reduce_add_sync(peers, bytes);
+    if ((threadIdx.x & 31u) == (uint32_t)(__ffs(peers) - 1)) atomicAdd(out.pages + page, bytes);
+#endif
   }
 
   // One atomic per result word per CTA (skipped when the CTA booked nothing), after a block reduction.
@@ -782,6 +838,13 @@ struct TagCheckZeroOp {
     book.book(off, mask, v);
   }
 
+  // A window outside the batches: booked, and its bytes added to its page.
+  __device__ __forceinline__ void single(uint64_t off, uint32_t mask, const Vec16& v) {
+    if (mask == 0) return;
+    window(off, mask, v);
+    book.pages_window(off, __popc(mask));
+  }
+
   __device__ __forceinline__ static uint32_t diff_mask(const uint4& v, const uint4& t) {
     const Vec16 x = {{v.x ^ t.x, v.y ^ t.y, v.z ^ t.z, v.w ^ t.w}};
     return nonzero_mask16(x);
@@ -806,12 +869,20 @@ struct TagCheckZeroOp {
       // else writes the range during the check (two views of one range checked in one launch), the branch reads
       // exactly the bytes counted above.
       const uint64_t off0 = addr(p) - base;
+      const uint32_t room = WindowBook::page_room(off0 - threadIdx.x * 16u);
+      const bool crosses = room < (uint32_t)THREADS * PER_THREAD * 16u;
+      uint32_t hi = 0;   // bytes on the page after the chunk's first (n - hi on its own)
 #pragma unroll 4
       for (uint32_t u = 0; u < (uint32_t)PER_THREAD; ++u) {
         uint8_t* q = p + u * THREADS * 16u;
         const uint4 x = ld16_cs(q);
-        window(off0 + u * THREADS * 16u, diff_mask(x, tag_vec(seed, addr(q))), Vec16{{x.x, x.y, x.z, x.w}});
+        const uint32_t mask = diff_mask(x, tag_vec(seed, addr(q)));
+        window(off0 + u * THREADS * 16u, mask, Vec16{{x.x, x.y, x.z, x.w}});
+        if (crosses) hi += threadIdx.x * 16u + u * THREADS * 16u >= room ? __popc(mask) : 0u;
       }
+      // The pages add up to n, the count the verdict takes, also when a second view changed the batch in between.
+      hi = min(hi, n);
+      book.pages_batch(off0 - threadIdx.x * 16u, n - hi, hi, crosses);
     }
 #pragma unroll
     for (int u = 0; u < PER_THREAD; ++u) st16(p + (uint32_t)u * THREADS * 16u, make_uint4(0, 0, 0, 0));
@@ -820,7 +891,7 @@ struct TagCheckZeroOp {
   __device__ __forceinline__ void vec(uint8_t* q) {
     uint4 v = ld16_cs(q);
     const uint32_t mask = diff_mask(v, tag_vec(seed, addr(q)));
-    window(addr(q) - base, mask, Vec16{{v.x, v.y, v.z, v.w}});
+    single(addr(q) - base, mask, Vec16{{v.x, v.y, v.z, v.w}});
     st16(q, make_uint4(0, 0, 0, 0));
     cnt += __popc(mask);
   }
@@ -842,7 +913,7 @@ struct TagCheckZeroOp {
         *b = 0;
       }
     const uint32_t mask = nonzero_mask16(x);
-    window(w0 - base, mask, v);
+    single(w0 - base, mask, v);
     cnt += __popc(mask);
   }
 };
@@ -871,7 +942,7 @@ tag_check_zero_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t see
 // nothing): locate_dirt_kernel takes them window by window, so no window is counted or recorded twice.
 struct LocateOp {
   WindowBook book;
-  const uint8_t* base;
+  uint64_t base;
 
   template <int THREADS, int PER_THREAD>
   __device__ __forceinline__ void chunk(const uint8_t* p) {
@@ -884,9 +955,24 @@ struct LocateOp {
 #pragma unroll
       for (int k = 0; k < 4; ++k) any |= v[u].w[k];
     if (any != 0) {  // rare except in a flood
-      const uint64_t off0 = (uint64_t)(p - base);
+      const uint64_t off0 = addr(p) - base;
+      uint32_t n = 0;
 #pragma unroll
-      for (int u = 0; u < PER_THREAD; ++u) window(off0 + (uint32_t)u * THREADS * 16u, nonzero_mask16(v[u]), v[u]);
+      for (int u = 0; u < PER_THREAD; ++u) {
+        const uint32_t mask = nonzero_mask16(v[u]);
+        window(off0 + (uint32_t)u * THREADS * 16u, mask, v[u]);
+        n += __popc(mask);
+      }
+      // the pages: the bytes past the page boundary inside the chunk, if there is one, go on the next page
+      const uint32_t room = WindowBook::page_room(off0 - threadIdx.x * 16u);
+      const bool crosses = room < (uint32_t)THREADS * PER_THREAD * 16u;
+      uint32_t hi = 0;
+      if (crosses) {
+#pragma unroll
+        for (int u = 0; u < PER_THREAD; ++u)
+          hi += threadIdx.x * 16u + (uint32_t)u * THREADS * 16u >= room ? __popc(nonzero_mask16(v[u])) : 0u;
+      }
+      book.pages_batch(off0 - threadIdx.x * 16u, n - hi, hi, crosses);
     }
   }
 
@@ -897,9 +983,16 @@ struct LocateOp {
     book.book(off, mask, v);
   }
 
+  // A window outside the batches: booked, and its bytes added to its page.
+  __device__ __forceinline__ void single(uint64_t off, uint32_t mask, const Vec16& v) {
+    if (mask == 0) return;
+    window(off, mask, v);
+    book.pages_window(off, __popc(mask));
+  }
+
   __device__ __forceinline__ void vec(const uint8_t* p) {
     const Vec16 v = ld16<kPolStreaming>(p, 0);
-    window((uint64_t)(p - base), nonzero_mask16(v), v);
+    single(addr(p) - base, nonzero_mask16(v), v);
   }
 
   __device__ __forceinline__ void byte(const uint8_t*) {}
@@ -912,18 +1005,19 @@ struct LocateOp {
 #pragma unroll
     for (int i = 0; i < 16; ++i)
       if (w0 + i >= lo && w0 + i < hi) v.w[i >> 2] |= (uint32_t)*(const uint8_t*)(uintptr_t)(w0 + i) << (8 * (i & 3));
-    window(w0 - addr(s.base), nonzero_mask16(v), v);
+    single(w0 - base, nonzero_mask16(v), v);
   }
 };
 
 // Reads the region (writes nothing into it) and reports where its non-zero bytes are.  Frame, loads and batching of
 // verify_ld128_fast_kernel: persistent CTAs, one THREADS * PER_THREAD * 16-byte chunk per grab in ascending order, all
 // PER_THREAD loads in flight, then OR; only batches whose OR is non-zero do more work.  Minimum one CTA per SM in the
-// launch bounds: the compiler may then use the registers the flood path needs instead of spilling it.
+// launch bounds: the compiler may then use the registers the flood path needs instead of spilling it.  Offsets are
+// addresses - `base` (as the tag check's), so every launch of one call books into the same words and page map.
 template <int THREADS, int PER_THREAD>
 __global__ void __launch_bounds__(THREADS, 1)
-locate_dirt_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, LocateOut out) {
-  LocateOp op{{out}, s.base};
+locate_dirt_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, LocateOut out, uint64_t base) {
+  LocateOp op{{out}, base};
   default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
   op.ragged_windows(s);
   op.book.flush();
@@ -958,6 +1052,7 @@ struct CensusOp {
     book.count += __popc(mask);
     book.tally(off, mask);
     book.record_mask(records, off, mask);
+    book.pages_window(off, __popc(mask));
   }
 
   // The batch's tally runs on offsets relative to its first vector (< 2^32), and the branch that claims record slots
@@ -986,6 +1081,16 @@ struct CensusOp {
     const uint64_t off0 = addr(p) - base;
     book.count += n;
     book.tally_span(off0, lo, hi, nwin);
+    if (n != 0) {   // the pages: bytes on the chunk's first page and (past a boundary inside the chunk) on the next
+      const uint32_t room = WindowBook::page_room(off0 - threadIdx.x * 16u);
+      const bool crosses = room < (uint32_t)PER_THREAD * kStride;
+      uint32_t up = 0;
+      if (crosses) {
+#pragma unroll
+        for (int u = 0; u < PER_THREAD; ++u) up += threadIdx.x * 16u + (uint32_t)u * kStride >= room ? __popc(mask[u]) : 0u;
+      }
+      book.pages_batch(off0 - threadIdx.x * 16u, n - up, up, crosses);
+    }
     if (any != 0 && !book.full_seen) {  // only until the book is full, however dense the residue
 #pragma unroll
       for (int u = 0; u < PER_THREAD; ++u)

@@ -58,14 +58,122 @@ def _signed64(x: int) -> int:
     return x - (1 << 64) if x >= 1 << 63 else x
 
 
+PAGE_BYTES = N.PAGE_BYTES
+PAGE_RUNS = 64      # runs a PageDigest keeps
+
+
+@dataclass(frozen=True)
+class PageRun:
+    """A maximal stretch of consecutive 2 MiB pages in one chunk that all hold booked bytes."""
+    first_page: int      # offset of its first byte from the report's va_base = first_page * PAGE_BYTES
+    pages: int
+    chunk: int
+    bytes: int
+
+    def describe(self) -> str:
+        lo, hi = self.first_page * PAGE_BYTES, (self.first_page + self.pages) * PAGE_BYTES - 1
+        return f"+{lo:#x}..+{hi:#x} chunk {self.chunk} {self.bytes} B"
+
+
+@dataclass(frozen=True)
+class ChunkPages:
+    """The booked bytes of one chunk (physical allocation), and on how many of its pages they lie."""
+    chunk: int
+    pages: int
+    bytes: int
+
+
+@dataclass
+class PageDigest:
+    """What a report carries of its page map (its `pages` field, and its JSON): the page count, exact totals per chunk,
+    and the first PAGE_RUNS runs."""
+    pages: int                   # pages holding at least one booked byte
+    bytes: int                   # booked bytes on them: the report's exact count
+    nruns: int                   # runs of consecutive pages in one chunk (all of them)
+    runs_truncated: int          # nruns > len(runs)
+    by_chunk: List[ChunkPages] = field(default_factory=list)   # ascending chunk
+    runs: List[PageRun] = field(default_factory=list)          # ascending, the first PAGE_RUNS
+
+    @classmethod
+    def from_json(cls, d: dict) -> "PageDigest":
+        return cls(**{**d, "by_chunk": [ChunkPages(**c) for c in d["by_chunk"]],
+                      "runs": [PageRun(**r) for r in d["runs"]]})
+
+    def summary(self, first: int = 4) -> str:
+        """One line for an operator: how many pages, the bytes of each chunk, and the first few runs."""
+        chunks = ", ".join(f"chunk {c.chunk}: {c.bytes} B on {c.pages} pages" for c in self.by_chunk)
+        more = f" (+{self.nruns - first} more)" if self.nruns > first else ""
+        return (f"{self.bytes} bytes on {self.pages} 2 MiB pages in {self.nruns} runs; {chunks}; runs: "
+                + "; ".join(r.describe() for r in self.runs[:first]) + more)
+
+
+class PageMap:
+    """The booked bytes of every 2 MiB page behind one report (include/ccm.h: ccm_last_page_map), ascending."""
+
+    def __init__(self, entries):
+        """entries: (page, bytes, chunk) tuples or ccm_page_entry structures."""
+        rows = [(e.page, e.bytes, e.chunk) if hasattr(e, "page") else tuple(e) for e in entries]
+        self.entries: List[Tuple[int, int, int]] = sorted((int(p), int(b), int(c)) for p, b, c in rows)
+
+    def __len__(self) -> int:
+        return len(self.entries)
+
+    @property
+    def bytes(self) -> int:
+        return sum(b for _, b, _ in self.entries)
+
+    def by_chunk(self) -> dict:
+        """{chunk: booked bytes}: exact, per physical allocation."""
+        out: dict = {}
+        for _, b, c in self.entries:
+            out[c] = out.get(c, 0) + b
+        return dict(sorted(out.items()))
+
+    def runs(self) -> List[PageRun]:
+        """Maximal stretches of consecutive pages in one chunk, with their bytes, ascending."""
+        runs: List[PageRun] = []
+        for p, b, c in self.entries:
+            last = runs[-1] if runs else None
+            if last is not None and last.chunk == c and last.first_page + last.pages == p:
+                runs[-1] = PageRun(last.first_page, last.pages + 1, c, last.bytes + b)
+            else:
+                runs.append(PageRun(p, 1, c, b))
+        return runs
+
+    def digest(self, keep: int = PAGE_RUNS) -> PageDigest:
+        runs = self.runs()
+        pages: dict = {}
+        for _, _, c in self.entries:
+            pages[c] = pages.get(c, 0) + 1
+        chunks = [ChunkPages(c, pages[c], b) for c, b in self.by_chunk().items()]
+        return PageDigest(len(self.entries), self.bytes, len(runs), int(len(runs) > keep), chunks, runs[:keep])
+
+    def summary(self) -> str:
+        return self.digest().summary()
+
+
+def last_page_map(cuda_ordinal: int, book: int) -> "Optional[PageMap]":
+    """The page map behind the last report of `book` (N.BOOK_DIRT / BOOK_MISMATCH / BOOK_RESIDUE) on a CUDA device
+    (include/ccm.h: ccm_last_page_map); None when it cannot be read."""
+    n = C.c_uint64(0)
+    if cuda_ordinal < 0 or N.lib().ccm_last_page_map(cuda_ordinal, book, None, 0, C.byref(n)) != N.OK:
+        return None
+    buf = (N.PageEntry * max(1, n.value))()
+    if N.lib().ccm_last_page_map(cuda_ordinal, book, buf, n.value, C.byref(n)) != N.OK:
+        return None
+    return PageMap(buf[:n.value])
+
+
 class _WindowReport:
     """What the three window reports share: their JSON and the chunks their records lie in.  Each report is a
-    dataclass with a `records` field of its WINDOW type."""
+    dataclass with a `records` field of its WINDOW type and, last, a `pages` field (a PageDigest, or None)."""
     WINDOW: type
 
     @classmethod
     def from_json(cls, d: dict):
-        return cls(**{**d, "records": [cls.WINDOW(**r) for r in d["records"]]})
+        pages = d.get("pages")
+        return cls(**{**d, "records": [cls.WINDOW(**r) for r in d["records"]],
+                      "pages": PageDigest.from_json(pages) if pages is not None else None})
 
     def as_json(self) -> dict:
         return dataclasses.asdict(self)
@@ -103,6 +211,7 @@ class DirtReport(_WindowReport):
     Every field but the choice of `records` is exact; records are distinct windows sorted by offset, all of
     them unless `truncated`."""
     WINDOW = DirtWindow
+    BOOK, WINDOWS = N.BOOK_DIRT, "dirty_windows"
     nonzero_bytes: int       # the locate pass's own recount
     dirty_windows: int
     first_offset: int        # first / last non-zero byte, from va_base
@@ -112,6 +221,7 @@ class DirtReport(_WindowReport):
     located: int             # 0: no locate pass ran (the call read back clean)
     truncated: int
     records: List[DirtWindow] = field(default_factory=list)
+    pages: Optional[PageDigest] = None   # its page map, when it booked a window (last_page_map)
 
     @classmethod
     def from_native(cls, d: N.DirtReport) -> "DirtReport":
@@ -157,6 +267,7 @@ class MismatchReport(_WindowReport):
     alias, partial and foreign windows is known for the records only; records are distinct windows sorted by
     offset, all of them unless `truncated`."""
     WINDOW = MismatchWindow
+    BOOK, WINDOWS = N.BOOK_MISMATCH, "mismatch_windows"
     mismatch_bytes: int
     mismatch_windows: int
     zero_windows: int        # mismatched windows whose bytes all read 0
@@ -167,6 +278,7 @@ class MismatchReport(_WindowReport):
     located: int             # 0: the last call's tagged check was clean (or it was not tagged)
     truncated: int
     records: List[MismatchWindow] = field(default_factory=list)
+    pages: Optional[PageDigest] = None   # its page map, when it booked a window (last_page_map)
 
     @classmethod
     def from_native(cls, m: N.MismatchReport) -> "MismatchReport":
@@ -235,6 +347,7 @@ class ResidueReport(_WindowReport):
     ccm_residue_report).  residue_bytes, residue_windows, first_offset and last_offset are exact; records are distinct
     windows sorted by offset, all of them unless `truncated`."""
     WINDOW = ResidueWindow
+    BOOK, WINDOWS = N.BOOK_RESIDUE, "residue_windows"
     residue_bytes: int
     residue_windows: int
     first_offset: int        # first / last non-zero byte, from va_base (0 when there is none)
@@ -244,6 +357,7 @@ class ResidueReport(_WindowReport):
     located: int             # 1: a census ran over everything the call mapped
     truncated: int
     records: List[ResidueWindow] = field(default_factory=list)
+    pages: Optional[PageDigest] = None   # its page map, when it booked a window (last_page_map)
 
     @classmethod
     def from_native(cls, r: N.ResidueReport) -> "ResidueReport":
@@ -363,13 +477,19 @@ class ScrubReport:
 
 def _attach_reports(rep: ScrubReport, cuda_ordinal: int, census: "N.ResidueReport | None") -> None:
     """Attaches to the report of a call what that call found: the census's report, and the device's last dirt /
-    mismatch report when the call counted non-zero / mismatched bytes."""
+    mismatch report when the call counted non-zero / mismatched bytes; each report that booked a window with its page
+    map's digest."""
     if census is not None:
         rep.residue = ResidueReport.from_native(census)
     if rep.nonzero_bytes:
         rep.dirt = last_dirt(cuda_ordinal)
     if rep.mismatch_bytes:
         rep.mismatch = last_mismatch(cuda_ordinal)
+    for attr, _ in _REPORTS:
+        report = getattr(rep, attr)
+        if report is not None and getattr(report, report.WINDOWS):
+            pages = last_page_map(cuda_ordinal, report.BOOK)
+            report.pages = pages.digest() if pages is not None else None
 
 
 # ScrubReport fields that only a tagged call reports
