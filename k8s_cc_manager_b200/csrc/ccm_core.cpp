@@ -696,6 +696,8 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
   else if (k == "tag_inject") d.drill.tag_inject = v < 0 ? 0 : (uint64_t)v;
   else if (k == "scrub_alias") d.drill.alias = v != 0;
   else if (k == "scrub_residue") d.drill.residue = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "triage_stay") d.drill.triage_stay = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "triage_return") d.drill.triage_return = v < 0 ? 0 : (uint64_t)v;
   else if (k == "scrub_poison" || k == "scrub_flood") {
     if (v < 0 || v > 255) { set_error("sim key '%s' takes a byte value (0 = off), not %lld", k.c_str(), (long long)v); return CCM_ERR_INVALID; }
     (k == "scrub_poison" ? d.drill.poison : d.drill.flood) = (int)v;
@@ -741,6 +743,8 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "tag_inject") *value = (int64_t)d.drill.tag_inject;
     else if (k == "scrub_alias") *value = d.drill.alias;
     else if (k == "scrub_residue") *value = (int64_t)d.drill.residue;
+    else if (k == "triage_stay") *value = (int64_t)d.drill.triage_stay;
+    else if (k == "triage_return") *value = (int64_t)d.drill.triage_return;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

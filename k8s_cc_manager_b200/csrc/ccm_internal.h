@@ -49,6 +49,10 @@ int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, b
 // Drill of the residue census (sim key "scrub_residue"; ccm.h):
 //   residue:    every mapping (arena path: segment) is zero-filled right after it is mapped (after poison), then
 //               that many bytes are set to 0xA5, same candidates as inject but per mapping.
+// Drills of the dirt triage (sim keys "triage_stay", "triage_return"; ccm.h), only in a call that triages:
+//   triage_stay:   the first byte of each of the first that many dirt pages is XORed between the re-zero and the
+//                  first re-read;
+//   triage_return: the same bytes, between the first and the second re-read.
 struct ScrubDrill {
   uint64_t inject = 0;
   int poison = 0;
@@ -56,6 +60,8 @@ struct ScrubDrill {
   uint64_t tag_inject = 0;
   int alias = 0;
   uint64_t residue = 0;
+  uint64_t triage_stay = 0;
+  uint64_t triage_return = 0;
 };
 // inject: the call's "scrub_inject" budget.  Its poison and flood drills are those current_scrub_drill()
 // returns on the calling thread.  (The engine entry points keep the signatures that host-only builds of

@@ -170,6 +170,9 @@ struct ScrubEngine {
   std::vector<ccm_page_entry> pages[kBooks];   // the page map behind each book's last report (ccm_last_page_map)
   ccm_dirt_report dirt{};                   // report of the last product call (ccm_scrub_last_dirt)
   ccm_mismatch_report mismatch{};           // report of the last product call (ccm_scrub_last_mismatch)
+  uint32_t triage_hold_ms = 0;              // the dirt triage's hold when armed (ccm_scrub_triage); 0 = disarmed
+  ccm_triage_report triage{};               // report of the last product call (ccm_scrub_last_triage)
+  std::vector<ccm_triage_page> triage_pages;   // and its pages (ccm_last_triage_pages)
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -794,9 +797,9 @@ static int drop_book(ScrubEngine* e, Book b, cudaStream_t st) {
 
 // After the passes that book into `b` (the caller holds e->mu): copies the book's words, waits and decodes them into
 // *head.  Only a book that is not empty costs more: its records are copied to e->h_book, the pages its windows can lie
-// on to e->pages[b] (appended: the caller clears the list when a report begins, and finish_pages() completes it), and
-// the book is zeroed for the next pass.
-static int read_book(ScrubEngine* e, Book b, cudaStream_t st, BookHead* head) {
+// on to e->pages[b] (appended: the caller clears the list when a report begins, and finish_pages() completes it), or to
+// *into, and the book is zeroed for the next pass.
+static int read_book(ScrubEngine* e, Book b, cudaStream_t st, BookHead* head, std::vector<ccm_page_entry>* into = nullptr) {
   BookHost& h = *e->h_book;
   CCM_CUDA(cudaMemcpyAsync(h.words, e->d_counter + kBookOut[b], sizeof h.words, cudaMemcpyDeviceToHost, st));
   CCM_CUDA(cudaStreamSynchronize(st));
@@ -813,8 +816,9 @@ static int read_book(ScrubEngine* e, Book b, cudaStream_t st, BookHead* head) {
   CCM_CUDA(cudaMemsetAsync(e->d_counter + kBookOut[b], 0, kBookWords * sizeof(unsigned long long), st));
   CCM_CUDA(cudaMemsetAsync(pages, 0, np * sizeof(uint32_t), st));
   CCM_CUDA(cudaStreamSynchronize(st));
+  std::vector<ccm_page_entry>& out = into ? *into : e->pages[b];
   for (uint64_t i = 0; i < np; ++i)
-    if (e->h_pages[i]) e->pages[b].push_back(ccm_page_entry{lo + i, e->h_pages[i], 0});
+    if (e->h_pages[i]) out.push_back(ccm_page_entry{lo + i, e->h_pages[i], 0});
   return CCM_OK;
 }
 
@@ -843,6 +847,15 @@ static void sort_records(Report* rep, uint64_t windows) {
 }
 
 // ------------------------------------------------------------------ locate the dirt
+// One locate launch over [p, p+n) on `st` (no sync) into the dirt book, with offsets from `base`.
+static int locate_launch(ScrubEngine* e, const void* p, uint64_t n, uint64_t base, cudaStream_t st) {
+  const cudaError_t err = launch_fast(CCM_LOCATE, kLocateThreads, kLocatePer, e, kLocateGrab, st,
+                                      split_region(p, n, 16, 128), e->book_out(kDirtBook), base);
+  g_launches++;
+  if (err != cudaSuccess) { set_error("locate launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
+  return CCM_OK;
+}
+
 // One locate pass over [p, p+n) on `st` (synchronises; the caller holds e->mu).  The kernel books offsets from
 // p - shift (`shift`: the range's offset in what `rep` describes), and what it found is added to `rep`: each new record
 // gets the chunk chunk_of(offset), and its pages are appended to the dirt book's page map (read_book).  Records are
@@ -853,14 +866,7 @@ static int locate_range(ScrubEngine* e, const void* p, uint64_t n, uint64_t shif
   rep->located = 1;
   if (n == 0) return CCM_OK;
   float ms = 0;
-  int rc = run_timed(e, st, &ms, [&]() -> int {
-    const cudaError_t err = launch_fast(CCM_LOCATE, kLocateThreads, kLocatePer, e, kLocateGrab, st,
-                                        split_region(p, n, 16, 128), e->book_out(kDirtBook),
-                                        (uint64_t)(uintptr_t)p - shift);
-    g_launches++;
-    if (err != cudaSuccess) { set_error("locate launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
-    return CCM_OK;
-  });
+  int rc = run_timed(e, st, &ms, [&] { return locate_launch(e, p, n, (uint64_t)(uintptr_t)p - shift, st); });
   if (rc) { drop_book(e, kDirtBook, st); return rc; }
   BookHead bk;
   if ((rc = read_book(e, kDirtBook, st, &bk))) return rc;
@@ -972,6 +978,112 @@ static int take_residue(ScrubEngine* e, cudaStream_t st, uint64_t va_base, uint6
   }
   sort_records(rep, bk.windows);
   return CCM_OK;
+}
+
+// ------------------------------------------------------------------ what kind of dirt
+// One contiguous piece of the dirty memory the triage re-zeroes and re-reads: `bytes` at device address `addr`,
+// `offset` bytes from the dirt report's va_base, inside span `span` of what the call mapped.
+struct TriageRun { uint64_t addr, bytes, offset; size_t span; };
+
+// The runs of a dirt page map (ascending pages): each page intersected with every span of what the call mapped
+// (ascending, as CheckSpan), adjacent pieces inside one span merged.
+static std::vector<TriageRun> triage_runs(const std::vector<ccm_page_entry>& pages, const std::vector<CheckSpan>& spans) {
+  std::vector<TriageRun> runs;
+  size_t j = 0;
+  for (const ccm_page_entry& p : pages) {
+    const uint64_t lo = p.page * (uint64_t)kPageBytes, hi = lo + kPageBytes;
+    while (j < spans.size() && spans[j].offset + spans[j].bytes <= lo) ++j;
+    for (size_t k = j; k < spans.size() && spans[k].offset < hi; ++k) {
+      const uint64_t a = std::max(lo, spans[k].offset), b = std::min(hi, spans[k].offset + spans[k].bytes);
+      if (a >= b) continue;
+      if (!runs.empty() && runs.back().span == k && runs.back().offset + runs.back().bytes == a) runs.back().bytes += b - a;
+      else runs.push_back({spans[k].addr + (a - spans[k].offset), b - a, a, k});
+    }
+  }
+  return runs;
+}
+
+// The triage of a failed read-back (ccm.h: ccm_scrub_triage).  Runs when the device is armed, after the locate pass
+// filled e->dirt and e->pages[kDirtBook], while the call still holds what it mapped (`spans`, offsets from the dirt
+// report's va_base; the caller holds e->mu).  Re-zeroes every run (T1), re-reads it (T2), waits the hold and re-reads
+// it again (T3), and fills e->triage and e->triage_pages.  T2 and T3 book into the dirt book, which read_book() left
+// zero, through read_book() into their own page maps, and leave it zero.  Never changes the verdict or another report:
+// after an error the triage report stays empty.
+static void triage_dirt(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& spans, const ScrubDrill& drill) {
+  if (e->triage_hold_ms == 0 || !e->dirt.located || e->pages[kDirtBook].empty()) return;
+  const double t0 = now_ms();
+  const std::vector<ccm_page_entry>& dirt = e->pages[kDirtBook];
+  const std::vector<TriageRun> runs = triage_runs(dirt, spans);
+  // drills: the first byte of each of the first k dirt pages, which lies in the run holding its offset
+  auto xor_pages = [&](uint64_t k) -> int {
+    for (size_t i = 0; i < dirt.size() && i < k; ++i) {
+      const uint64_t o = dirt[i].page * (uint64_t)kPageBytes;
+      auto it = std::upper_bound(runs.begin(), runs.end(), o, [](uint64_t v, const TriageRun& r) { return v < r.offset; });
+      if (it == runs.begin() || o >= std::prev(it)->offset + std::prev(it)->bytes) continue;
+      xor_byte_kernel<<<1, 1, 0, st>>>((uint8_t*)(uintptr_t)(std::prev(it)->addr + (o - std::prev(it)->offset)));
+      g_launches++;
+      CCM_CUDA(cudaGetLastError());
+    }
+    return CCM_OK;
+  };
+  // one re-read of every run, booked and read back: its head and its page map
+  auto reread = [&](BookHead* head, std::vector<ccm_page_entry>* map) -> int {
+    for (const TriageRun& r : runs)
+      if (int rc = locate_launch(e, (const void*)(uintptr_t)r.addr, r.bytes, r.addr - r.offset, st)) return rc;
+    return read_book(e, kDirtBook, st, head, map);
+  };
+  BookHead t2{}, t3{};
+  std::vector<ccm_page_entry> map2, map3;
+  double ms_hold = 0;
+  int rc = CCM_OK;
+  for (const TriageRun& r : runs)
+    if (rc == CCM_OK) rc = scrub_range(e, (void*)(uintptr_t)r.addr, r.bytes, CCM_SCRUB_ST128, nullptr, st);   // T1
+  if (rc == CCM_OK) rc = xor_pages(drill.triage_stay);
+  if (rc == CCM_OK) rc = reread(&t2, &map2);                                                                   // T2
+  if (rc == CCM_OK) rc = xor_pages(drill.triage_return);
+  if (rc == CCM_OK) {
+    const double h0 = now_ms();
+    std::this_thread::sleep_for(std::chrono::milliseconds(e->triage_hold_ms));
+    ms_hold = now_ms() - h0;
+    rc = reread(&t3, &map3);                                                                                   // T3
+  }
+  if (rc != CCM_OK) { drop_book(e, kDirtBook, st); return; }
+
+  ccm_triage_report t;
+  memset(&t, 0, sizeof t);
+  t.triaged = 1;
+  t.hold_ms = e->triage_hold_ms;
+  t.runs = (int32_t)runs.size();
+  t.va_base = e->dirt.va_base;
+  t.pages_examined = dirt.size();
+  for (const TriageRun& r : runs) t.bytes_examined += r.bytes;
+  t.t2_bytes = t2.count;
+  t.t3_bytes = t3.count;
+  if (t2.windows) { t.t2_first_offset = t2.first; t.t2_last_offset = t2.last; }
+  if (t3.windows) { t.t3_first_offset = t3.first; t.t3_last_offset = t3.last; }
+  // one entry per dirt page; the re-reads' maps are ascending and lie on dirt pages
+  std::vector<ccm_triage_page> out;
+  out.reserve(dirt.size());
+  size_t i2 = 0, i3 = 0;
+  for (const ccm_page_entry& p : dirt) {
+    while (i2 < map2.size() && map2[i2].page < p.page) ++i2;
+    while (i3 < map3.size() && map3[i3].page < p.page) ++i3;
+    ccm_triage_page tp;
+    memset(&tp, 0, sizeof tp);
+    tp.page = p.page;
+    tp.chunk = p.chunk;
+    tp.dirt_bytes = p.bytes;
+    tp.t2_bytes = i2 < map2.size() && map2[i2].page == p.page ? map2[i2].bytes : 0;
+    tp.t3_bytes = i3 < map3.size() && map3[i3].page == p.page ? map3[i3].bytes : 0;
+    if (tp.t2_bytes) { tp.cls = CCM_TRIAGE_STAYS; t.stay_pages++; t.stay_bytes += p.bytes; }
+    else if (tp.t3_bytes) { tp.cls = CCM_TRIAGE_RETURNS; t.return_pages++; t.return_bytes += p.bytes; }
+    else { tp.cls = CCM_TRIAGE_CLEARS; t.clear_pages++; t.clear_bytes += p.bytes; }
+    out.push_back(tp);
+  }
+  t.ms_hold = ms_hold;
+  t.ms_triage = now_ms() - t0;
+  e->triage = t;
+  e->triage_pages.swap(out);
 }
 
 int engine_arena_scrub(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, void* stream, float* ms) {
@@ -1257,8 +1369,9 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
 }
 
 // The dirt report of the fallback path: one locate pass per segment, offsets into the concatenated segments,
-// chunk = segment index.  A failure of the pass leaves the report empty; it never changes the verdict.
-static void arena_locate(ScrubEngine* e) {
+// chunk = segment index.  A failure of the pass leaves the report empty; it never changes the verdict.  Then, when the
+// device is armed, the triage of the dirt, segment by segment (`drill`: the call's drills).
+static void arena_locate(ScrubEngine* e, const ScrubDrill& drill) {
   std::lock_guard<std::mutex> g(e->mu);
   if (!e->ready || e->segs.empty() || cudaSetDevice(e->ordinal) != cudaSuccess) return;
   ccm_dirt_report rep;
@@ -1276,6 +1389,13 @@ static void arena_locate(ScrubEngine* e) {
   sort_records(&rep, rep.dirty_windows);
   finish_pages(e, kDirtBook, [&](uint64_t o) { return segment_of(e->segs, o); });
   e->dirt = rep;
+  std::vector<CheckSpan> spans;
+  shift = 0;
+  for (const Segment& s : e->segs) {
+    spans.push_back({(uint64_t)(uintptr_t)s.ptr, s.bytes, shift});
+    shift += s.bytes;
+  }
+  triage_dirt(e, e->stream, spans, drill);
 }
 
 // ------------------------------------------------------- VMM (driver API, lazy)
@@ -1594,6 +1714,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
       sort_records(&rep, rep.dirty_windows);
       finish_pages(e, kDirtBook, chunk_of);
       e->dirt = rep;
+      triage_dirt(e, st, {{(uint64_t)m.base, mapped, 0}}, drill);   // armed: what kind of dirt, while it is mapped
     } else {
       e->pages[kDirtBook].clear();
     }
@@ -1634,6 +1755,8 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     std::lock_guard<std::mutex> g(e->mu);
     memset(&e->dirt, 0, sizeof e->dirt);  // every call replaces the reports of the last one
     memset(&e->mismatch, 0, sizeof e->mismatch);
+    memset(&e->triage, 0, sizeof e->triage);
+    e->triage_pages.clear();
     e->pages[kDirtBook].clear();          // and their page maps (a census call: the residue's too)
     e->pages[kCheckBook].clear();
     if (res) e->pages[kCensusBook].clear();
@@ -1672,7 +1795,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       }
       if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
       if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
-      if (rc == CCM_OK && nz != 0) arena_locate(e);
+      if (rc == CCM_OK && nz != 0) arena_locate(e, drill);
       r.ms_scrub = ms_s;
       r.ms_verify = ms_v;
       r.nonzero_bytes = nz;
@@ -1907,5 +2030,57 @@ extern "C" int ccm_last_page_map(int cuda_ordinal, int book, ccm_page_entry* out
   const std::vector<ccm_page_entry>& v = e->pages[book - CCM_BOOK_DIRT];
   *n = v.size();
   if (cap) memcpy(out, v.data(), std::min<uint64_t>(cap, v.size()) * sizeof(ccm_page_entry));
+  return CCM_OK;
+}
+
+// ------------------------------------------------------------------------- dirt triage
+static_assert(sizeof(ccm_triage_page) == 32 && sizeof(ccm_triage_report) == 152, "triage structs keep their layout");
+
+extern "C" int ccm_scrub_triage(int cuda_ordinal, uint32_t hold_ms) {
+  if (hold_ms > CCM_TRIAGE_MAX_HOLD_MS) {
+    set_error("ccm_scrub_triage: hold of %u ms is longer than %u ms", hold_ms, CCM_TRIAGE_MAX_HOLD_MS);
+    return CCM_ERR_INVALID;
+  }
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  // disarming an engine that was never created leaves nothing armed (and starts no context)
+  ScrubEngine* e = hold_ms ? engine_for(cuda_ordinal) : engine_lookup(cuda_ordinal);
+  if (!e) return hold_ms ? CCM_ERR_NO_CUDA : CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  e->triage_hold_ms = hold_ms;
+  return CCM_OK;
+}
+
+extern "C" int ccm_scrub_last_triage(int cuda_ordinal, ccm_triage_report* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  *out = e->triage;
+  return CCM_OK;
+}
+
+extern "C" int ccm_last_triage_pages(int cuda_ordinal, ccm_triage_page* out, uint64_t cap, uint64_t* n) {
+  if (!n || (cap && !out)) {
+    set_error("ccm_last_triage_pages: cap %llu (needs n, and out when cap > 0)", (unsigned long long)cap);
+    return CCM_ERR_INVALID;
+  }
+  *n = 0;
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  *n = e->triage_pages.size();
+  if (cap) memcpy(out, e->triage_pages.data(), std::min<uint64_t>(cap, *n) * sizeof(ccm_triage_page));
   return CCM_OK;
 }

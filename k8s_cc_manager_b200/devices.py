@@ -31,7 +31,7 @@ class GpuError(Exception):
     """Raised for any failed device operation (reference: gpu.GpuError).  A scrub that read back dirt
     carries its DirtReport as `.dirt`; a tagged scrub whose check found bytes off their tags carries its
     MismatchReport as `.mismatch`; a census call carries its ResidueReport (what the first pass erased) as
-    `.residue`."""
+    `.residue`; a triage call that read back dirt carries its TriageReport (what kind of dirt) as `.triage`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
@@ -378,8 +378,113 @@ class ResidueReport(_WindowReport):
                 f"{self.va_base:#x}{more}, chunks {self.chunks}; first windows: {recs}")
 
 
-# The window reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
-_REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport))
+TRIAGE_PAGES = 64       # pages that did not clear a TriageReport keeps
+TRIAGE_HOLD_MS = 100    # default hold between the triage's two re-reads
+
+
+@dataclass(frozen=True)
+class TriagePage:
+    """The class of one page of the dirt page map after the triage (include/ccm.h: ccm_triage_page)."""
+    page: int            # offset of the page from the report's va_base = page * PAGE_BYTES
+    chunk: int           # physical allocation behind its first byte (as PageEntry.chunk)
+    cls: str             # "stays" | "returns" | "clears"
+    dirt_bytes: int      # the dirt page map's bytes on it
+    t2_bytes: int        # non-zero bytes the re-read right after the re-zero found on it
+    t3_bytes: int        # non-zero bytes the re-read after the hold found on it
+
+    def describe(self) -> str:
+        return (f"+{self.page * PAGE_BYTES:#x} chunk {self.chunk} {self.cls} ({self.dirt_bytes} B dirt, "
+                f"{self.t2_bytes} B at once, {self.t3_bytes} B after the hold)")
+
+
+def last_triage_pages(cuda_ordinal: int) -> "Optional[List[TriagePage]]":
+    """The pages of the last triage on a CUDA device (include/ccm.h: ccm_last_triage_pages), ascending; None when they
+    cannot be read."""
+    n = C.c_uint64(0)
+    if cuda_ordinal < 0 or N.lib().ccm_last_triage_pages(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
+        return None
+    buf = (N.TriagePage * max(1, n.value))()
+    if N.lib().ccm_last_triage_pages(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
+        return None
+    return [TriagePage(p.page, p.chunk, N.TRIAGE_CLASSES.get(p.cls, str(p.cls)), p.dirt_bytes, p.t2_bytes, p.t3_bytes)
+            for p in buf[:n.value]]
+
+
+@dataclass
+class TriageReport:
+    """What kind of dirt a failed read-back found (include/ccm.h: ccm_triage_report): the dirty pages re-zeroed and
+    re-read at once and after a hold.  A page "stays" when zero stored over it does not read back as zero, "returns"
+    when it reads back zero at once but not after the hold (something is still writing this GPU's memory), and
+    "clears" otherwise.  Every count is exact; `suspect_pages` are the first TRIAGE_PAGES pages that did not clear."""
+    pages_examined: int
+    bytes_examined: int
+    stay_pages: int
+    stay_bytes: int          # the dirt report's bytes on the pages of each class
+    return_pages: int
+    return_bytes: int
+    clear_pages: int
+    clear_bytes: int
+    t2_bytes: int            # non-zero bytes found at once (T2) and after the hold (T3)
+    t3_bytes: int
+    t2_first_offset: int     # first / last of them, from va_base (0 when there is none)
+    t2_last_offset: int
+    t3_first_offset: int
+    t3_last_offset: int
+    va_base: int
+    ms_hold: float           # the hold actually waited
+    ms_triage: float
+    hold_ms: int             # the hold asked for
+    runs: int                # contiguous runs the dirty pages make
+    triaged: int
+    suspect_pages: List[TriagePage] = field(default_factory=list)
+    suspect_truncated: int = 0
+
+    @classmethod
+    def from_native(cls, t: N.TriageReport, pages: "Optional[List[TriagePage]]" = None) -> "TriageReport":
+        suspect = [p for p in pages or () if p.cls != "clears"]
+        return cls(*(getattr(t, name) for name, _ in N.TriageReport._fields_ if name != "reserved"),
+                   suspect_pages=suspect[:TRIAGE_PAGES], suspect_truncated=int(len(suspect) > TRIAGE_PAGES))
+
+    @classmethod
+    def from_json(cls, d: dict) -> "TriageReport":
+        return cls(**{**d, "suspect_pages": [TriagePage(**p) for p in d["suspect_pages"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    def summary(self, first: int = 4) -> str:
+        """One line for an operator: pages and runs, the count of each class, the hold, and the first few pages that
+        did not clear."""
+        line = (f"{self.pages_examined} pages in {self.runs} runs: {self.stay_pages} stay, {self.return_pages} return, "
+                f"{self.clear_pages} clear (hold {self.hold_ms} ms)")
+        if self.suspect_pages:
+            more = " (+more)" if self.suspect_truncated or len(self.suspect_pages) > first else ""
+            line += "; " + "; ".join(p.describe() for p in self.suspect_pages[:first]) + more
+        return line
+
+
+def last_triage(cuda_ordinal: int) -> "Optional[TriageReport]":
+    """The triage report of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_triage), with the
+    pages that did not clear; None when it cannot be read."""
+    out = N.TriageReport()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_triage(cuda_ordinal, C.byref(out)) != N.OK:
+        return None
+    return TriageReport.from_native(out, last_triage_pages(cuda_ordinal) if out.triaged else None)
+
+
+def _arm_triage(cuda_ordinal: int, hold_ms: int) -> bool:
+    """Arms (hold_ms > 0) or disarms (0) the triage on a CUDA device; False when the library refused."""
+    return cuda_ordinal >= 0 and N.lib().ccm_scrub_triage(cuda_ordinal, hold_ms) == N.OK
+
+
+def _triage_hold(hold_ms: int) -> int:
+    if not 0 < hold_ms <= N.TRIAGE_MAX_HOLD_MS:
+        raise ValueError(f"triage hold must be 1..{N.TRIAGE_MAX_HOLD_MS} ms, not {hold_ms}")
+    return int(hold_ms)
+
+
+# The reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
+_REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport))
 
 
 @dataclass
@@ -417,6 +522,9 @@ class ScrubReport:
     # What the first pass found before it erased it (a ResidueReport), set for every report of a census call
     # (residue=True).  Not a dataclass field either.
     residue = None
+    # What kind of dirt it is (a TriageReport), set for every report of a triage call (triage=True) that triaged: one
+    # whose read-back found non-zero bytes.  Not a dataclass field either.
+    triage = None
 
     @property
     def clean(self) -> bool:
@@ -453,7 +561,7 @@ class ScrubReport:
 
     def as_json(self) -> dict:
         """The report as the scrub workers print it: the tagged-gate fields only for a tagged call, "dirt",
-        "mismatch" and "residue" only when that report is attached."""
+        "mismatch", "residue" and "triage" only when that report is attached."""
         d = dataclasses.asdict(self)
         if self.check == "zero":
             for name in TAG_FIELDS:
@@ -475,19 +583,23 @@ class ScrubReport:
         return rep
 
 
-def _attach_reports(rep: ScrubReport, cuda_ordinal: int, census: "N.ResidueReport | None") -> None:
+def _attach_reports(rep: ScrubReport, cuda_ordinal: int, census: "N.ResidueReport | None",
+                    triage: bool = False) -> None:
     """Attaches to the report of a call what that call found: the census's report, and the device's last dirt /
     mismatch report when the call counted non-zero / mismatched bytes; each report that booked a window with its page
-    map's digest."""
+    map's digest; and for a triage call whose read-back found non-zero bytes, the triage report when it ran."""
     if census is not None:
         rep.residue = ResidueReport.from_native(census)
     if rep.nonzero_bytes:
         rep.dirt = last_dirt(cuda_ordinal)
     if rep.mismatch_bytes:
         rep.mismatch = last_mismatch(cuda_ordinal)
+    if triage and rep.nonzero_bytes:
+        report = last_triage(cuda_ordinal)
+        rep.triage = report if report is not None and report.triaged else None
     for attr, _ in _REPORTS:
         report = getattr(rep, attr)
-        if report is not None and getattr(report, report.WINDOWS):
+        if isinstance(report, _WindowReport) and getattr(report, report.WINDOWS):
             pages = last_page_map(cuda_ordinal, report.BOOK)
             report.pages = pages.digest() if pages is not None else None
 
@@ -556,11 +668,15 @@ class NvidiaDevice:
         _check(N.lib().ccm_wait_for_boot(self.index, timeout_ms), "wait_for_boot", self.bdf)
 
     # -- NEW: HBM scrub-and-verify ---------------------------------------------
-    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False) -> ScrubReport:
+    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
+                         triage_hold_ms: int = TRIAGE_HOLD_MS) -> ScrubReport:
         """Zero-fills and reads back this GPU's HBM (nbytes=0: all the context can map).
         check="tagged" first writes and checks an address-tagged known answer
         (include/ccm.h: ccm_scrub_verify_tagged).  residue=True runs the census in the first pass and attaches what
         it found as `.residue` (include/ccm.h: ccm_scrub_verify_residue); it never changes the verdict.
+        triage=True arms the dirt triage for this call (include/ccm.h: ccm_scrub_triage): when the read-back finds
+        non-zero bytes, the dirty pages are re-zeroed and re-read at once and after `triage_hold_ms`, and what
+        kind of dirt it is comes attached as `.triage`; it never changes the verdict either.
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
         if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
@@ -570,17 +686,22 @@ class NvidiaDevice:
         res, tag, census = N.ScrubResult(), None, None
         if _check_mode(check):
             tag = N.TagResult()
-        if residue:
-            census = N.ResidueReport()
-            rc = N.lib().ccm_scrub_verify_residue(self.index, nbytes, C.byref(tag) if tag is not None else None,
-                                                  C.byref(census), C.byref(res))
-        elif tag is not None:
-            rc = N.lib().ccm_scrub_verify_tagged(self.index, nbytes, C.byref(tag), C.byref(res))
-        else:
-            rc = N.lib().ccm_scrub_verify(self.index, nbytes, C.byref(res))
-        err = _error(rc, "scrub_and_verify", self.bdf)   # the library's error text, before anything else runs
+        armed = triage and _arm_triage(self.cuda_ordinal, _triage_hold(triage_hold_ms))
+        try:
+            if residue:
+                census = N.ResidueReport()
+                rc = N.lib().ccm_scrub_verify_residue(self.index, nbytes, C.byref(tag) if tag is not None else None,
+                                                      C.byref(census), C.byref(res))
+            elif tag is not None:
+                rc = N.lib().ccm_scrub_verify_tagged(self.index, nbytes, C.byref(tag), C.byref(res))
+            else:
+                rc = N.lib().ccm_scrub_verify(self.index, nbytes, C.byref(res))
+            err = _error(rc, "scrub_and_verify", self.bdf)   # the library's error text, before anything else runs
+        finally:
+            if armed:
+                _arm_triage(self.cuda_ordinal, 0)
         rep = ScrubReport.from_native(self.bdf, res, tag)
-        _attach_reports(rep, self.cuda_ordinal, census)
+        _attach_reports(rep, self.cuda_ordinal, census, armed)
         if err is not None:
             for attr, _ in _REPORTS:
                 setattr(err, attr, getattr(rep, attr))
@@ -628,31 +749,39 @@ def find_gpus() -> Tuple[List[NvidiaDevice], int]:
 
 
 def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
-                          check: str = "zero", residue: bool = False) -> Tuple[List[ScrubReport], float]:
+                          check: str = "zero", residue: bool = False, triage: bool = False,
+                          triage_hold_ms: int = TRIAGE_HOLD_MS) -> Tuple[List[ScrubReport], float]:
     """Concurrent multi-context scrub of several GPUs through ONE native call
     (ccm_scrub_verify_many: one host thread + primary context + stream per GPU, no
     peer access, no collective; check="tagged": ccm_scrub_verify_many_tagged; residue=True:
-    ccm_scrub_verify_many_residue, each report with its `.residue`).  Returns
+    ccm_scrub_verify_many_residue, each report with its `.residue`; triage=True: every GPU armed for the dirt
+    triage, as in NvidiaDevice.scrub_and_verify).  Returns
     (reports, wall_ms); never raises for a per-device failure — inspect report.status /
     report.clean."""
     tagged = _check_mode(check)
     n = len(devices)
     if n == 0:
         return [], 0.0
+    hold = _triage_hold(triage_hold_ms) if triage else 0
     idx = (C.c_int * n)(*[d.index for d in devices])
     res = (N.ScrubResult * n)()
     wall = C.c_double(0.0)
     tags = (N.TagResult * n)() if tagged else None
     census = (N.ResidueReport * n)() if residue else None
-    if residue:
-        N.lib().ccm_scrub_verify_many_residue(n, idx, nbytes, tags, census, res, C.byref(wall))
-    elif tagged:
-        N.lib().ccm_scrub_verify_many_tagged(n, idx, nbytes, tags, res, C.byref(wall))
-    else:
-        N.lib().ccm_scrub_verify_many(n, idx, nbytes, res, C.byref(wall))
+    armed = {d.cuda_ordinal for d in devices if triage and _arm_triage(d.cuda_ordinal, hold)}
+    try:
+        if residue:
+            N.lib().ccm_scrub_verify_many_residue(n, idx, nbytes, tags, census, res, C.byref(wall))
+        elif tagged:
+            N.lib().ccm_scrub_verify_many_tagged(n, idx, nbytes, tags, res, C.byref(wall))
+        else:
+            N.lib().ccm_scrub_verify_many(n, idx, nbytes, res, C.byref(wall))
+    finally:
+        for ordinal in armed:
+            _arm_triage(ordinal, 0)
     reports = [ScrubReport.from_native(d.bdf, res[i], tags[i] if tagged else None) for i, d in enumerate(devices)]
     for i, (rep, d) in enumerate(zip(reports, devices)):
-        _attach_reports(rep, d.cuda_ordinal, census[i] if residue else None)
+        _attach_reports(rep, d.cuda_ordinal, census[i] if residue else None, d.cuda_ordinal in armed)
     return reports, wall.value
 
 
@@ -704,10 +833,14 @@ class ScrubbingProxy:
         native = object.__getattribute__(self, "_native")
         return native.wait_scrub_released() if native is not None else (0.0, 0.0)
 
-    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False) -> ScrubReport:
+    def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
+                         triage_hold_ms: int = TRIAGE_HOLD_MS) -> ScrubReport:
         native = object.__getattribute__(self, "_native")
         if native is None:
             raise GpuError(f"no CUDA device with PCI address {self._foreign.bdf}: HBM scrub cannot run", N.ERR_NO_CUDA)
+        if triage:
+            return native.scrub_and_verify(nbytes, check=check, residue=residue, triage=True,
+                                           triage_hold_ms=triage_hold_ms)
         if residue:
             return native.scrub_and_verify(nbytes, check=check, residue=True)
         if check == "zero":

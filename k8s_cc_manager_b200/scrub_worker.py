@@ -8,7 +8,8 @@ concurrent gate (ccm_scrub_verify_many: one host thread + context + stream per G
 short-lived process and reads ONE JSON line back; the process exit returns every CUDA resource.
 
 Output (stdout, last line):  {"wall_ms": ..., "reports": [ {ScrubReport fields}, ... ]}
-(the tagged-gate fields only with --check tagged; "residue" only with --residue).
+(the tagged-gate fields only with --check tagged; "residue" only with --residue; "triage" only with --triage, for a
+GPU whose read-back found non-zero bytes).
 Exit code: 0 if every GPU is clean, 3 if the gate failed, 2 on usage errors.
 """
 from __future__ import annotations
@@ -22,13 +23,17 @@ from . import _native as N
 from . import devices as D
 
 
-def run(bdfs: List[str], nbytes: int, check: str = "zero", residue: bool = False) -> dict:
+def run(bdfs: List[str], nbytes: int, check: str = "zero", residue: bool = False, triage_hold_ms: int = 0) -> dict:
+    """triage_hold_ms > 0 arms the dirt triage with that hold."""
     by_bdf = {d.bdf: d for d in D.find_gpus()[0] if d.is_gpu()}
     missing = [b for b in bdfs if b not in by_bdf]
     if missing:
         raise SystemExit(f"unknown GPU(s): {', '.join(missing)} (known: {', '.join(sorted(by_bdf))})")
     devs = [by_bdf[b] for b in bdfs]
-    if residue:
+    if triage_hold_ms:
+        reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check, residue=residue, triage=True,
+                                                   triage_hold_ms=triage_hold_ms)
+    elif residue:
         reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check, residue=True)
     else:
         reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check)
@@ -44,12 +49,18 @@ def main(argv: Optional[List[str]] = None) -> int:
                     help="zero: zero-fill + read-back; tagged: an address-tagged known answer first")
     ap.add_argument("--residue", action="store_true",
                     help="report what the first pass found in the memory before it erased it (never fails the gate)")
+    ap.add_argument("--triage", action="store_true",
+                    help="after a failed read-back, re-zero and re-read the dirty pages: does the dirt stay, return or "
+                         "clear (never fails the gate)")
+    ap.add_argument("--triage-hold-ms", type=int, default=D.TRIAGE_HOLD_MS,
+                    help="the triage's hold between its two re-reads (default %(default)s)")
     args = ap.parse_args(argv)
     if not args.bdf:
         ap.error("at least one --bdf is required")
     if args.backend:
         D.select_backend(args.backend)
-    out = run([b.lower() for b in args.bdf], args.bytes, args.check, args.residue)
+    out = run([b.lower() for b in args.bdf], args.bytes, args.check, args.residue,
+              args.triage_hold_ms if args.triage else 0)
     print(json.dumps(out), flush=True)
     return 0 if all(r["status"] == 0 and r["nonzero_bytes"] == 0 and r.get("mismatch_bytes", 0) == 0
                     for r in out["reports"]) else 3
