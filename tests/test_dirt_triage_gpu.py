@@ -159,7 +159,11 @@ def test_triage_of_injected_dirt(lib, path):
 @pytest.mark.parametrize("env", [{}, {"CCM_PIPELINE": "0"}], ids=["vmm", "fallback"])
 def test_flood_examines_every_mapped_page(lib, env):
     nbytes = 0 if not env else 4 * GiB
-    out = call(lib, "zero", env, {"scrub_flood": PP.FLOOD}, nbytes, hold=HOLD_MS)
+    assert_flood(call(lib, "zero", env, {"scrub_flood": PP.FLOOD}, nbytes, hold=HOLD_MS), env, nbytes)
+
+
+def assert_flood(out: dict, env: dict, nbytes: int):
+    """An armed flooded call: every mapped page examined in one run per mapped range, and every page clears."""
     res, t = out["res"], out["triage"]
     assert out["rc"] == N.ERR_DIRTY and res.nonzero_bytes == res.bytes_scrubbed
     assert t.pages_examined == -(-res.bytes_scrubbed // PAGE) and t.bytes_examined == res.bytes_scrubbed

@@ -295,8 +295,14 @@ DRILL_CALLS = {                       # drill -> (call, sim drills, book of the 
 
 
 def check_product(lib, drill: str, env: dict, nbytes: int = 0, many: bool = False):
-    call, drills, book = DRILL_CALLS[drill]
-    rc, res, tag, rr, dirt, mm, maps = product(lib, call, env, drills, nbytes, many)
+    call, drills, _ = DRILL_CALLS[drill]
+    return assert_product(drill, env, nbytes, many, product(lib, call, env, drills, nbytes, many))
+
+
+def assert_product(drill: str, env: dict, nbytes: int, many: bool, out):
+    """What one product() call under `drill` left: its report and page maps against product_plan."""
+    _, _, book = DRILL_CALLS[drill]
+    rc, res, tag, rr, dirt, mm, maps = out
     what = (drill, env, nbytes, many)
     chunks, ranges = layout(env, res, nbytes, many)
     if drill == "scrub_inject":
@@ -347,8 +353,11 @@ def test_product_call_pages_through_the_fan_out(lib, drill):
 def test_scrub_alias_pages(lib, mf):
     """Two views of one physical range: the pages lie in the first chunk's offsets or the aliased view's, and every
     page carries the chunk its records carry."""
-    rc, res, tag, rr, dirt, mm, maps = product(lib, "tagged", {"CCM_MAP_FIRST": str(mf)}, {"scrub_alias": 1},
-                                                nbytes=4 * GiB)
+    assert_alias(mf, product(lib, "tagged", {"CCM_MAP_FIRST": str(mf)}, {"scrub_alias": 1}, nbytes=4 * GiB))
+
+
+def assert_alias(mf: int, out):
+    rc, res, tag, rr, dirt, mm, maps = out
     assert rc == N.ERR_MISMATCH and mm.located
     pages = {p: b for p, b, _ in maps[N.BOOK_MISMATCH]}
     assert_report_invariants(mm, pages, ("alias", mf))
