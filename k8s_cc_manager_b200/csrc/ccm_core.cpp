@@ -698,9 +698,9 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
   else if (k == "scrub_residue") d.drill.residue = v < 0 ? 0 : (uint64_t)v;
   else if (k == "triage_stay") d.drill.triage_stay = v < 0 ? 0 : (uint64_t)v;
   else if (k == "triage_return") d.drill.triage_return = v < 0 ? 0 : (uint64_t)v;
-  else if (k == "scrub_poison" || k == "scrub_flood") {
+  else if (k == "scrub_poison" || k == "scrub_flood" || k == "tag_flood") {
     if (v < 0 || v > 255) { set_error("sim key '%s' takes a byte value (0 = off), not %lld", k.c_str(), (long long)v); return CCM_ERR_INVALID; }
-    (k == "scrub_poison" ? d.drill.poison : d.drill.flood) = (int)v;
+    (k == "scrub_poison" ? d.drill.poison : k == "scrub_flood" ? d.drill.flood : d.drill.tag_flood) = (int)v;
   }
   else { set_error("unknown sim key '%s'", k.c_str()); return CCM_ERR_INVALID; }
   return CCM_OK;
@@ -745,6 +745,7 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "scrub_residue") *value = (int64_t)d.drill.residue;
     else if (k == "triage_stay") *value = (int64_t)d.drill.triage_stay;
     else if (k == "triage_return") *value = (int64_t)d.drill.triage_return;
+    else if (k == "tag_flood") *value = d.drill.tag_flood;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

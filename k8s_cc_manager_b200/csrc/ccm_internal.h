@@ -45,14 +45,16 @@ int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, b
 //           and its read-back; the verdict must be DIRTY with nonzero_bytes == bytes_scrubbed.
 // Drills of the tagged call (sim keys "tag_inject", "scrub_alias"; ccm.h):
 //   tag_inject: that many bytes are XORed between the tag fill and the check, same candidates as inject;
-//   alias:      the second main-zone chunk starts with a second view of the first chunk (VMM path only).
+//   alias:      the second main-zone chunk starts with a second view of the first chunk (VMM path only);
+//   tag_flood:  every range tag_inject acts on is filled with this byte between the tag fill and the check.
 // Drill of the residue census (sim key "scrub_residue"; ccm.h):
 //   residue:    every mapping (arena path: segment) is zero-filled right after it is mapped (after poison), then
 //               that many bytes are set to 0xA5, same candidates as inject but per mapping.
-// Drills of the dirt triage (sim keys "triage_stay", "triage_return"; ccm.h), only in a call that triages:
-//   triage_stay:   the first byte of each of the first that many dirt pages is XORed between the re-zero and the
-//                  first re-read;
-//   triage_return: the same bytes, between the first and the second re-read.
+// Drills of the dirt and mismatch triages (sim keys "triage_stay", "triage_return"; ccm.h), only in a call that
+// triages; each triage acts on the pages of its own page map:
+//   triage_stay:   the first byte of each of the first that many pages is XORed between the triage's first step (the
+//                  re-zero, or the re-tag) and its second (the first re-read, or the check-and-zero);
+//   triage_return: the same bytes, between its second and third step.
 struct ScrubDrill {
   uint64_t inject = 0;
   int poison = 0;
@@ -62,6 +64,7 @@ struct ScrubDrill {
   uint64_t residue = 0;
   uint64_t triage_stay = 0;
   uint64_t triage_return = 0;
+  int tag_flood = 0;
 };
 // inject: the call's "scrub_inject" budget.  Its poison and flood drills are those current_scrub_drill()
 // returns on the calling thread.  (The engine entry points keep the signatures that host-only builds of

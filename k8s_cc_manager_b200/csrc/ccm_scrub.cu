@@ -12,6 +12,7 @@
 #include <chrono>
 #include <cstddef>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -173,6 +174,9 @@ struct ScrubEngine {
   uint32_t triage_hold_ms = 0;              // the dirt triage's hold when armed (ccm_scrub_triage); 0 = disarmed
   ccm_triage_report triage{};               // report of the last product call (ccm_scrub_last_triage)
   std::vector<ccm_triage_page> triage_pages;   // and its pages (ccm_last_triage_pages)
+  uint32_t mtriage_hold_ms = 0;             // the mismatch triage's hold when armed (ccm_scrub_mismatch_triage)
+  ccm_triage_report mtriage{};              // report of the last product call (ccm_scrub_last_mismatch_triage)
+  std::vector<ccm_triage_page> mtriage_pages;  // and its pages (ccm_last_mismatch_triage_pages)
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -1003,21 +1007,28 @@ static std::vector<TriageRun> triage_runs(const std::vector<ccm_page_entry>& pag
   return runs;
 }
 
-// The triage of a failed read-back (ccm.h: ccm_scrub_triage).  Runs when the device is armed, after the locate pass
-// filled e->dirt and e->pages[kDirtBook], while the call still holds what it mapped (`spans`, offsets from the dirt
-// report's va_base; the caller holds e->mu).  Re-zeroes every run (T1), re-reads it (T2), waits the hold and re-reads
-// it again (T3), and fills e->triage and e->triage_pages.  T2 and T3 book into the dirt book, which read_book() left
-// zero, through read_book() into their own page maps, and leave it zero.  Never changes the verdict or another report:
-// after an error the triage report stays empty.
-static void triage_dirt(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& spans, const ScrubDrill& drill) {
-  if (e->triage_hold_ms == 0 || !e->dirt.located || e->pages[kDirtBook].empty()) return;
+// The steps of one triage: each enqueues one launch over one run on the triage's stream (no sync).  T2 and T3 book
+// into b2 and b3, which the triage reads back into page maps of its own.
+struct TriageSteps {
+  std::function<int(const TriageRun&)> t1, t2, t3;
+  Book b2, b3;
+};
+
+// A triage (ccm.h: ccm_scrub_triage, ccm_scrub_mismatch_triage), while the call still holds what it mapped (`spans`,
+// offsets from `va_base`; the caller holds e->mu): over every run of the page map `map`, T1, then T2 (booked), the hold
+// of `hold_ms`, then T3 (booked).  The drills XOR the first byte of each of the first "triage_stay" pages of `map`
+// between T1 and T2, and of the first "triage_return" pages between T2 and T3.  A page is STAYS when T2 booked bytes
+// on it, RETURNS when only T3 did, CLEARS otherwise; fills *report and *pages.  b2 and b3 must be zero when it starts
+// (read_book() left them so) and are zero when it ends.  After an error it drops them and leaves *report empty.
+static void run_triage(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& spans, const ScrubDrill& drill,
+                       const std::vector<ccm_page_entry>& map, uint64_t va_base, uint32_t hold_ms,
+                       const TriageSteps& steps, ccm_triage_report* report, std::vector<ccm_triage_page>* pages) {
   const double t0 = now_ms();
-  const std::vector<ccm_page_entry>& dirt = e->pages[kDirtBook];
-  const std::vector<TriageRun> runs = triage_runs(dirt, spans);
-  // drills: the first byte of each of the first k dirt pages, which lies in the run holding its offset
+  const std::vector<TriageRun> runs = triage_runs(map, spans);
+  // drills: the first byte of each of the first k pages, which lies in the run holding its offset
   auto xor_pages = [&](uint64_t k) -> int {
-    for (size_t i = 0; i < dirt.size() && i < k; ++i) {
-      const uint64_t o = dirt[i].page * (uint64_t)kPageBytes;
+    for (size_t i = 0; i < map.size() && i < k; ++i) {
+      const uint64_t o = map[i].page * (uint64_t)kPageBytes;
       auto it = std::upper_bound(runs.begin(), runs.end(), o, [](uint64_t v, const TriageRun& r) { return v < r.offset; });
       if (it == runs.begin() || o >= std::prev(it)->offset + std::prev(it)->bytes) continue;
       xor_byte_kernel<<<1, 1, 0, st>>>((uint8_t*)(uintptr_t)(std::prev(it)->addr + (o - std::prev(it)->offset)));
@@ -1026,46 +1037,51 @@ static void triage_dirt(ScrubEngine* e, cudaStream_t st, const std::vector<Check
     }
     return CCM_OK;
   };
-  // one re-read of every run, booked and read back: its head and its page map
-  auto reread = [&](BookHead* head, std::vector<ccm_page_entry>* map) -> int {
+  // one step over every run: each launch, then (booked) its book read back into its head and page map
+  auto step = [&](const std::function<int(const TriageRun&)>& launch, Book b, BookHead* head,
+                  std::vector<ccm_page_entry>* into) -> int {
     for (const TriageRun& r : runs)
-      if (int rc = locate_launch(e, (const void*)(uintptr_t)r.addr, r.bytes, r.addr - r.offset, st)) return rc;
-    return read_book(e, kDirtBook, st, head, map);
+      if (int rc = launch(r)) return rc;
+    return head ? read_book(e, b, st, head, into) : CCM_OK;
   };
   BookHead t2{}, t3{};
   std::vector<ccm_page_entry> map2, map3;
   double ms_hold = 0;
-  int rc = CCM_OK;
-  for (const TriageRun& r : runs)
-    if (rc == CCM_OK) rc = scrub_range(e, (void*)(uintptr_t)r.addr, r.bytes, CCM_SCRUB_ST128, nullptr, st);   // T1
+  int rc = step(steps.t1, kBooks, nullptr, nullptr);                                                           // T1
   if (rc == CCM_OK) rc = xor_pages(drill.triage_stay);
-  if (rc == CCM_OK) rc = reread(&t2, &map2);                                                                   // T2
+  if (rc == CCM_OK) rc = step(steps.t2, steps.b2, &t2, &map2);                                                 // T2
   if (rc == CCM_OK) rc = xor_pages(drill.triage_return);
   if (rc == CCM_OK) {
     const double h0 = now_ms();
-    std::this_thread::sleep_for(std::chrono::milliseconds(e->triage_hold_ms));
+    std::this_thread::sleep_for(std::chrono::milliseconds(hold_ms));
     ms_hold = now_ms() - h0;
-    rc = reread(&t3, &map3);                                                                                   // T3
+    rc = step(steps.t3, steps.b3, &t3, &map3);                                                                 // T3
   }
-  if (rc != CCM_OK) { drop_book(e, kDirtBook, st); return; }
+  if (rc != CCM_OK) {
+    drop_book(e, steps.b2, st);
+    if (steps.b3 != steps.b2) drop_book(e, steps.b3, st);
+    return;
+  }
 
   ccm_triage_report t;
   memset(&t, 0, sizeof t);
   t.triaged = 1;
-  t.hold_ms = e->triage_hold_ms;
+  t.hold_ms = hold_ms;
   t.runs = (int32_t)runs.size();
-  t.va_base = e->dirt.va_base;
-  t.pages_examined = dirt.size();
+  t.va_base = va_base;
+  t.pages_examined = map.size();
   for (const TriageRun& r : runs) t.bytes_examined += r.bytes;
-  t.t2_bytes = t2.count;
-  t.t3_bytes = t3.count;
+  // bytes from the page maps: every book maps exactly the bytes it counts, and the check book's count word is not
+  // its byte count
+  for (const ccm_page_entry& p : map2) t.t2_bytes += p.bytes;
+  for (const ccm_page_entry& p : map3) t.t3_bytes += p.bytes;
   if (t2.windows) { t.t2_first_offset = t2.first; t.t2_last_offset = t2.last; }
   if (t3.windows) { t.t3_first_offset = t3.first; t.t3_last_offset = t3.last; }
-  // one entry per dirt page; the re-reads' maps are ascending and lie on dirt pages
+  // one entry per page of the map; T2's and T3's maps are ascending and lie on its pages
   std::vector<ccm_triage_page> out;
-  out.reserve(dirt.size());
+  out.reserve(map.size());
   size_t i2 = 0, i3 = 0;
-  for (const ccm_page_entry& p : dirt) {
+  for (const ccm_page_entry& p : map) {
     while (i2 < map2.size() && map2[i2].page < p.page) ++i2;
     while (i3 < map3.size() && map3[i3].page < p.page) ++i3;
     ccm_triage_page tp;
@@ -1082,8 +1098,48 @@ static void triage_dirt(ScrubEngine* e, cudaStream_t st, const std::vector<Check
   }
   t.ms_hold = ms_hold;
   t.ms_triage = now_ms() - t0;
-  e->triage = t;
-  e->triage_pages.swap(out);
+  *report = t;
+  pages->swap(out);
+}
+
+// The triage of a failed read-back (ccm.h: ccm_scrub_triage).  Runs when the device is armed, after the locate pass
+// filled e->dirt and e->pages[kDirtBook], while the call still holds what it mapped (`spans`, offsets from the dirt
+// report's va_base; the caller holds e->mu).  Re-zeroes every run with the default scrub (T1), re-reads it with the
+// locate kernel (T2), waits the hold and re-reads it again (T3); T2 and T3 book into the dirt book.  Fills e->triage
+// and e->triage_pages.  Never changes the verdict or another report.
+static void triage_dirt(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& spans, const ScrubDrill& drill) {
+  if (e->triage_hold_ms == 0 || !e->dirt.located || e->pages[kDirtBook].empty()) return;
+  auto locate = [&](const TriageRun& r) {
+    return locate_launch(e, (const void*)(uintptr_t)r.addr, r.bytes, r.addr - r.offset, st);
+  };
+  const TriageSteps steps{
+      [&](const TriageRun& r) { return scrub_range(e, (void*)(uintptr_t)r.addr, r.bytes, CCM_SCRUB_ST128, nullptr, st); },
+      locate, locate, kDirtBook, kDirtBook};
+  run_triage(e, st, spans, drill, e->pages[kDirtBook], e->dirt.va_base, e->triage_hold_ms, steps, &e->triage,
+             &e->triage_pages);
+}
+
+// The triage of a failed tagged check (ccm.h: ccm_scrub_mismatch_triage).  Runs when the device is armed, after
+// take_mismatch() filled e->mismatch and e->pages[kCheckBook] (and after the dirt triage, when the call runs it), while
+// the call still holds what it mapped (`spans`, offsets from the mismatch report's va_base; the caller holds e->mu).
+// Writes the tags of `seed` over every run again (T1), checks and zeroes it (T2, into the check book, with the base the
+// gate's check used, so its offsets and pages are the mismatch report's own), waits the hold and reads it for zeros
+// (T3, into the dirt book).  T2 leaves the runs zero, so no tag outlives the call.  Fills e->mtriage and
+// e->mtriage_pages.  Never changes the verdict or another report.
+static void triage_mismatch(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& spans,
+                            const ScrubDrill& drill, uint32_t seed) {
+  if (e->mtriage_hold_ms == 0 || !e->mismatch.located || e->pages[kCheckBook].empty()) return;
+  const TriageSteps steps{
+      [&](const TriageRun& r) { return tag_fill_range(e, (void*)(uintptr_t)r.addr, r.bytes, seed, st); },
+      [&](const TriageRun& r) {
+        return tag_check_range(e, (void*)(uintptr_t)r.addr, r.bytes, seed, st, r.addr - r.offset);
+      },
+      [&](const TriageRun& r) {
+        return locate_launch(e, (const void*)(uintptr_t)r.addr, r.bytes, r.addr - r.offset, st);
+      },
+      kCheckBook, kDirtBook};
+  run_triage(e, st, spans, drill, e->pages[kCheckBook], e->mismatch.va_base, e->mtriage_hold_ms, steps, &e->mtriage,
+             &e->mtriage_pages);
 }
 
 int engine_arena_scrub(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, void* stream, float* ms) {
@@ -1315,23 +1371,31 @@ static int arena_census(ScrubEngine* e, ccm_residue_report* res, float* ms) {
                       [&](uint64_t o) { return segment_of(e->segs, o); });
 }
 
-// Tagged pass of the product call's fallback path: tag every segment, then (after the "tag_inject"
-// drill) check and zero every segment.  Fills tag->mismatch_bytes, ->ms_tag, ->ms_check, ->va_base, and after
+// What the fallback path holds, as the spans of its checks and triages: every segment, with its offset into the
+// concatenated segments.
+static std::vector<CheckSpan> arena_spans(const std::vector<Segment>& segs) {
+  std::vector<CheckSpan> spans;
+  uint64_t shift = 0;
+  for (const Segment& s : segs) {
+    spans.push_back({(uint64_t)(uintptr_t)s.ptr, s.bytes, shift});
+    shift += s.bytes;
+  }
+  return spans;
+}
+
+// Tagged pass of the product call's fallback path: tag every segment, then (after the "tag_flood" and "tag_inject"
+// drills) check and zero every segment.  Fills tag->mismatch_bytes, ->ms_tag, ->ms_check, ->va_base, and after
 // mismatches the engine's mismatch report (offsets into the concatenated segments, chunk = segment index).
 // res (census call): the fills are census fills, and `res` gets what they found.
-static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inject, ccm_residue_report* res) {
+static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inject, int tag_flood,
+                           ccm_residue_report* res) {
   std::lock_guard<std::mutex> g(e->mu);
   CCM_ENSURE_READY(e);
   int rc = need_arena(e); if (rc) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->stream;
   auto chunk_of = [&](uint64_t o) { return segment_of(e->segs, o); };
-  std::vector<CheckSpan> spans;
-  uint64_t shift = 0;
-  for (auto& s : e->segs) {
-    spans.push_back({(uint64_t)(uintptr_t)s.ptr, s.bytes, shift});
-    shift += s.bytes;
-  }
+  const std::vector<CheckSpan> spans = arena_spans(e->segs);
   // fills between ev[0] and ev[2], the drill, checks between ev[3] and ev[1]
   rc = run_counted(e, st, kMismatch, &tag->mismatch_bytes, nullptr, [&]() -> int {
     for (const CheckSpan& sp : spans) {
@@ -1341,8 +1405,10 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
         return rc2;
     }
     CCM_CUDA(cudaEventRecord(e->ev[2], st));
-    for (auto& s : e->segs)
+    for (auto& s : e->segs) {
+      if (tag_flood) CCM_CUDA(cudaMemsetAsync(s.ptr, tag_flood, s.bytes, st));
       if (tag_inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &tag_inject, st, true));
+    }
     CCM_CUDA(cudaEventRecord(e->ev[3], st));
     // base = segment address - its offset: the offsets continue from one segment into the next
     for (const CheckSpan& sp : spans)
@@ -1389,13 +1455,15 @@ static void arena_locate(ScrubEngine* e, const ScrubDrill& drill) {
   sort_records(&rep, rep.dirty_windows);
   finish_pages(e, kDirtBook, [&](uint64_t o) { return segment_of(e->segs, o); });
   e->dirt = rep;
-  std::vector<CheckSpan> spans;
-  shift = 0;
-  for (const Segment& s : e->segs) {
-    spans.push_back({(uint64_t)(uintptr_t)s.ptr, s.bytes, shift});
-    shift += s.bytes;
-  }
-  triage_dirt(e, e->stream, spans, drill);
+  triage_dirt(e, e->stream, arena_spans(e->segs), drill);
+}
+
+// The mismatch triage of the fallback path, when the device is armed: segment by segment, with the offsets of the
+// mismatch report (into the concatenated segments).
+static void arena_triage_mismatch(ScrubEngine* e, uint32_t seed, const ScrubDrill& drill) {
+  std::lock_guard<std::mutex> g(e->mu);
+  if (!e->ready || e->segs.empty() || cudaSetDevice(e->ordinal) != cudaSuccess) return;
+  triage_mismatch(e, e->stream, arena_spans(e->segs), drill, seed);
 }
 
 // ------------------------------------------------------- VMM (driver API, lazy)
@@ -1545,8 +1613,9 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   // enqueue scrub (+ read-back) of [off, off+n) with CUDA events around each kernel; in the tagged gate the
   // scrub is the check-and-zero pass
   auto enqueue = [&](uint64_t off, uint64_t n) -> int {
-    if (tag && tag_inject) {
-      const cudaError_t ierr = inject_dirt((uint8_t*)(m.base + off), n, &tag_inject, st, true);
+    if (tag && (drill.tag_flood || tag_inject)) {
+      cudaError_t ierr = drill.tag_flood ? cudaMemsetAsync((void*)(m.base + off), drill.tag_flood, n, st) : cudaSuccess;
+      if (ierr == cudaSuccess && tag_inject) ierr = inject_dirt((uint8_t*)(m.base + off), n, &tag_inject, st, true);
       if (ierr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(ierr)); return CCM_ERR_CUDA; }
     }
     cudaEvent_t* evs = timed < kMaxPipeChunks ? e->pipe_ev[timed] : nullptr;
@@ -1719,6 +1788,9 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
       e->pages[kDirtBook].clear();
     }
   }
+  // ---- a failed tagged check, armed: what kind of mismatch, while it is mapped ----------------------------
+  if (checked && rc == CCM_OK && tag->mismatch_bytes != 0)
+    triage_mismatch(e, st, {{(uint64_t)m.base, mapped, 0}}, drill, tag->seed);
   // ---- give the HBM back: on the reaper (default) or right here -----------------------
   if (rc == CCM_OK && async_release_enabled()) {
     r->release_deferred = 1;
@@ -1757,6 +1829,8 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     memset(&e->mismatch, 0, sizeof e->mismatch);
     memset(&e->triage, 0, sizeof e->triage);
     e->triage_pages.clear();
+    memset(&e->mtriage, 0, sizeof e->mtriage);
+    e->mtriage_pages.clear();
     e->pages[kDirtBook].clear();          // and their page maps (a census call: the residue's too)
     e->pages[kCheckBook].clear();
     if (res) e->pages[kCensusBook].clear();
@@ -1786,7 +1860,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       uint64_t nz = 0;
       rc = arena_drill(e, drill.poison, 0, drill.residue);
       if (rc == CCM_OK && tag) {
-        rc = arena_tag_check(e, tag, drill.tag_inject, res);
+        rc = arena_tag_check(e, tag, drill.tag_inject, drill.tag_flood, res);
         ms_s = (float)tag->ms_check;
       } else if (rc == CCM_OK && res) {
         rc = arena_census(e, res, &ms_s);
@@ -1796,6 +1870,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
       if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
       if (rc == CCM_OK && nz != 0) arena_locate(e, drill);
+      if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) arena_triage_mismatch(e, tag->seed, drill);
       r.ms_scrub = ms_s;
       r.ms_verify = ms_v;
       r.nonzero_bytes = nz;
@@ -2033,12 +2108,13 @@ extern "C" int ccm_last_page_map(int cuda_ordinal, int book, ccm_page_entry* out
   return CCM_OK;
 }
 
-// ------------------------------------------------------------------------- dirt triage
+// ------------------------------------------------------------------------- dirt and mismatch triages
 static_assert(sizeof(ccm_triage_page) == 32 && sizeof(ccm_triage_report) == 152, "triage structs keep their layout");
 
-extern "C" int ccm_scrub_triage(int cuda_ordinal, uint32_t hold_ms) {
+// Arms or disarms one triage (`hold`: the engine's hold of that triage) on a CUDA device.
+static int arm_triage(const char* fn, int cuda_ordinal, uint32_t hold_ms, uint32_t ScrubEngine::*hold) {
   if (hold_ms > CCM_TRIAGE_MAX_HOLD_MS) {
-    set_error("ccm_scrub_triage: hold of %u ms is longer than %u ms", hold_ms, CCM_TRIAGE_MAX_HOLD_MS);
+    set_error("%s: hold of %u ms is longer than %u ms", fn, hold_ms, CCM_TRIAGE_MAX_HOLD_MS);
     return CCM_ERR_INVALID;
   }
   if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
@@ -2049,11 +2125,12 @@ extern "C" int ccm_scrub_triage(int cuda_ordinal, uint32_t hold_ms) {
   ScrubEngine* e = hold_ms ? engine_for(cuda_ordinal) : engine_lookup(cuda_ordinal);
   if (!e) return hold_ms ? CCM_ERR_NO_CUDA : CCM_OK;
   std::lock_guard<std::mutex> g(e->mu);
-  e->triage_hold_ms = hold_ms;
+  e->*hold = hold_ms;
   return CCM_OK;
 }
 
-extern "C" int ccm_scrub_last_triage(int cuda_ordinal, ccm_triage_report* out) {
+// The last report of one triage (`rep`) on a CUDA device.
+static int last_triage(int cuda_ordinal, ccm_triage_report* out, ccm_triage_report ScrubEngine::*rep) {
   if (!out) return CCM_ERR_INVALID;
   memset(out, 0, sizeof *out);
   if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
@@ -2063,13 +2140,15 @@ extern "C" int ccm_scrub_last_triage(int cuda_ordinal, ccm_triage_report* out) {
   ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
   if (!e) return CCM_OK;
   std::lock_guard<std::mutex> g(e->mu);
-  *out = e->triage;
+  *out = e->*rep;
   return CCM_OK;
 }
 
-extern "C" int ccm_last_triage_pages(int cuda_ordinal, ccm_triage_page* out, uint64_t cap, uint64_t* n) {
+// The pages of that report (`pages`).
+static int last_triage_pages(const char* fn, int cuda_ordinal, ccm_triage_page* out, uint64_t cap, uint64_t* n,
+                             std::vector<ccm_triage_page> ScrubEngine::*pages) {
   if (!n || (cap && !out)) {
-    set_error("ccm_last_triage_pages: cap %llu (needs n, and out when cap > 0)", (unsigned long long)cap);
+    set_error("%s: cap %llu (needs n, and out when cap > 0)", fn, (unsigned long long)cap);
     return CCM_ERR_INVALID;
   }
   *n = 0;
@@ -2080,7 +2159,32 @@ extern "C" int ccm_last_triage_pages(int cuda_ordinal, ccm_triage_page* out, uin
   ScrubEngine* e = engine_lookup(cuda_ordinal);
   if (!e) return CCM_OK;
   std::lock_guard<std::mutex> g(e->mu);
-  *n = e->triage_pages.size();
-  if (cap) memcpy(out, e->triage_pages.data(), std::min<uint64_t>(cap, *n) * sizeof(ccm_triage_page));
+  const std::vector<ccm_triage_page>& v = e->*pages;
+  *n = v.size();
+  if (cap) memcpy(out, v.data(), std::min<uint64_t>(cap, *n) * sizeof(ccm_triage_page));
   return CCM_OK;
+}
+
+extern "C" int ccm_scrub_triage(int cuda_ordinal, uint32_t hold_ms) {
+  return arm_triage("ccm_scrub_triage", cuda_ordinal, hold_ms, &ScrubEngine::triage_hold_ms);
+}
+
+extern "C" int ccm_scrub_last_triage(int cuda_ordinal, ccm_triage_report* out) {
+  return last_triage(cuda_ordinal, out, &ScrubEngine::triage);
+}
+
+extern "C" int ccm_last_triage_pages(int cuda_ordinal, ccm_triage_page* out, uint64_t cap, uint64_t* n) {
+  return last_triage_pages("ccm_last_triage_pages", cuda_ordinal, out, cap, n, &ScrubEngine::triage_pages);
+}
+
+extern "C" int ccm_scrub_mismatch_triage(int cuda_ordinal, uint32_t hold_ms) {
+  return arm_triage("ccm_scrub_mismatch_triage", cuda_ordinal, hold_ms, &ScrubEngine::mtriage_hold_ms);
+}
+
+extern "C" int ccm_scrub_last_mismatch_triage(int cuda_ordinal, ccm_triage_report* out) {
+  return last_triage(cuda_ordinal, out, &ScrubEngine::mtriage);
+}
+
+extern "C" int ccm_last_mismatch_triage_pages(int cuda_ordinal, ccm_triage_page* out, uint64_t cap, uint64_t* n) {
+  return last_triage_pages("ccm_last_mismatch_triage_pages", cuda_ordinal, out, cap, n, &ScrubEngine::mtriage_pages);
 }

@@ -1,7 +1,7 @@
 // ccm-scrub — native command-line front end of the HBM scrub gate (links libccm.so).
 //
-//   ccm-scrub [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] [--triage [--triage-hold-ms MS]]
-//             (--all | --bdf <pci address> ...)
+//   ccm-scrub [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] [--triage]
+//             [--mismatch-triage] [--triage-hold-ms MS] (--all | --bdf <pci address> ...)
 //
 // Runs the concurrent gate (ccm_scrub_verify_many, or ccm_scrub_verify_many_tagged with --check tagged)
 // and prints ONE JSON line with the same fields as k8s_cc_manager_b200.devices.ScrubReport (the
@@ -10,7 +10,10 @@
 // tags, as ccm_scrub_last_mismatch reports it; "residue" for every GPU with --residue, which runs the census
 // calls, ccm_scrub_verify_many_residue; each of the three with a "pages" member, the digest of its page map from
 // ccm_last_page_map; "triage" with --triage, which arms every GPU for the dirt triage (ccm_scrub_triage), for a GPU whose
-// read-back found non-zero bytes: what kind of dirt, as ccm_scrub_last_triage and ccm_last_triage_pages report it).
+// read-back found non-zero bytes: what kind of dirt, as ccm_scrub_last_triage and ccm_last_triage_pages report it;
+// "mismatch_triage" with --mismatch-triage, which needs --check tagged and arms every GPU for the mismatch triage
+// (ccm_scrub_mismatch_triage), for a GPU whose tagged check found bytes off their tags: what kind of mismatch, as
+// ccm_scrub_last_mismatch_triage and ccm_last_mismatch_triage_pages report it).
 // Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
@@ -156,22 +159,56 @@ static void print_residue(const ccm_residue_report& r, int ordinal) {
   printf("}");
 }
 
+// The "mismatch_triage" object: the fields of k8s_cc_manager_b200.devices.TriageReport for the mismatch page map, with
+// the first 64 pages that did not clear (devices.TRIAGE_PAGES).
+static void print_mismatch_triage(const ccm_triage_report& t, int ordinal) {
+  static const char* const classes[] = {"?", "stays", "returns", "clears"};
+  printf(", \"mismatch_triage\": {\"pages_examined\": %llu, \"bytes_examined\": %llu, \"stay_pages\": %llu, "
+         "\"stay_bytes\": %llu, \"return_pages\": %llu, \"return_bytes\": %llu, \"clear_pages\": %llu, "
+         "\"clear_bytes\": %llu, \"t2_bytes\": %llu, \"t3_bytes\": %llu, \"t2_first_offset\": %llu, "
+         "\"t2_last_offset\": %llu, \"t3_first_offset\": %llu, \"t3_last_offset\": %llu, \"va_base\": %llu, "
+         "\"ms_hold\": %.3f, \"ms_triage\": %.3f, \"hold_ms\": %u, \"runs\": %d, \"triaged\": %d, \"suspect_pages\": [",
+         (unsigned long long)t.pages_examined, (unsigned long long)t.bytes_examined, (unsigned long long)t.stay_pages,
+         (unsigned long long)t.stay_bytes, (unsigned long long)t.return_pages, (unsigned long long)t.return_bytes,
+         (unsigned long long)t.clear_pages, (unsigned long long)t.clear_bytes, (unsigned long long)t.t2_bytes,
+         (unsigned long long)t.t3_bytes, (unsigned long long)t.t2_first_offset, (unsigned long long)t.t2_last_offset,
+         (unsigned long long)t.t3_first_offset, (unsigned long long)t.t3_last_offset, (unsigned long long)t.va_base,
+         t.ms_hold, t.ms_triage, t.hold_ms, t.runs, t.triaged);
+  uint64_t n = 0;
+  std::vector<ccm_triage_page> v;
+  if (ccm_last_mismatch_triage_pages(ordinal, nullptr, 0, &n) == CCM_OK) {
+    v.resize(n);
+    if (n && ccm_last_mismatch_triage_pages(ordinal, v.data(), n, &n) != CCM_OK) v.clear();
+  }
+  const size_t keep = 64;   // k8s_cc_manager_b200.devices.TRIAGE_PAGES
+  size_t shown = 0, suspect = 0;
+  for (const ccm_triage_page& p : v) {
+    if (p.cls == CCM_TRIAGE_CLEARS) continue;
+    if (suspect++ >= keep) continue;
+    printf("%s{\"page\": %llu, \"chunk\": %u, \"cls\": \"%s\", \"dirt_bytes\": %u, \"t2_bytes\": %u, \"t3_bytes\": %u}",
+           shown++ ? ", " : "", (unsigned long long)p.page, p.chunk, classes[p.cls <= 3 ? p.cls : 0], p.dirt_bytes,
+           p.t2_bytes, p.t3_bytes);
+  }
+  printf("], \"suspect_truncated\": %d}", suspect > keep);
+}
+
 static int usage(const char* argv0) {
   fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] "
-          "[--triage [--triage-hold-ms MS]] (--all | --bdf <bdf> ...)\n", argv0);
+          "[--triage] [--mismatch-triage] [--triage-hold-ms MS] (--all | --bdf <bdf> ...)\n", argv0);
   return 2;
 }
 
 int main(int argc, char** argv) {
   std::vector<std::string> bdfs;
   unsigned long long bytes = 0;
-  bool all = false, tagged = false, residue = false, triage = false;
+  bool all = false, tagged = false, residue = false, triage = false, mismatch_triage = false;
   unsigned long triage_hold_ms = 100;   // k8s_cc_manager_b200.devices.TRIAGE_HOLD_MS
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     if (a == "--all") all = true;
     else if (a == "--residue") residue = true;
     else if (a == "--triage") triage = true;
+    else if (a == "--mismatch-triage") mismatch_triage = true;
     else if (a == "--triage-hold-ms" && i + 1 < argc) {
       triage_hold_ms = strtoul(argv[++i], nullptr, 10);
       if (triage_hold_ms == 0 || triage_hold_ms > CCM_TRIAGE_MAX_HOLD_MS) return usage(argv[0]);
@@ -190,6 +227,10 @@ int main(int argc, char** argv) {
     } else return usage(argv[0]);
   }
   if (!all && bdfs.empty()) return usage(argv[0]);
+  if (mismatch_triage && !tagged) {
+    fprintf(stderr, "--mismatch-triage needs --check tagged\n");
+    return usage(argv[0]);
+  }
 
   int n = 0;
   ccm_enumerate(nullptr, 0, &n);
@@ -223,12 +264,17 @@ int main(int argc, char** argv) {
   std::vector<int> armed;   // ordinals armed for the triage, disarmed once the gate is done
   for (size_t i = 0; triage && i < ordinals.size(); ++i)
     if (ordinals[i] >= 0 && ccm_scrub_triage(ordinals[i], (uint32_t)triage_hold_ms) == CCM_OK) armed.push_back(ordinals[i]);
+  std::vector<int> marmed;   // and for the mismatch triage
+  for (size_t i = 0; mismatch_triage && i < ordinals.size(); ++i)
+    if (ordinals[i] >= 0 && ccm_scrub_mismatch_triage(ordinals[i], (uint32_t)triage_hold_ms) == CCM_OK)
+      marmed.push_back(ordinals[i]);
   if (residue)
     ccm_scrub_verify_many_residue((int)devs.size(), devs.data(), bytes, tagged ? tags.data() : nullptr, census.data(),
                                   res.data(), &wall_ms);
   else if (tagged) ccm_scrub_verify_many_tagged((int)devs.size(), devs.data(), bytes, tags.data(), res.data(), &wall_ms);
   else ccm_scrub_verify_many((int)devs.size(), devs.data(), bytes, res.data(), &wall_ms);
   for (int o : armed) ccm_scrub_triage(o, 0);
+  for (int o : marmed) ccm_scrub_mismatch_triage(o, 0);
   bool clean = true;
   printf("{\"wall_ms\": %.3f, \"reports\": [", wall_ms);
   for (size_t i = 0; i < devs.size(); ++i) {
@@ -256,6 +302,9 @@ int main(int argc, char** argv) {
     ccm_triage_report t;
     if (triage && r.nonzero_bytes != 0 && ccm_scrub_last_triage(ordinals[i], &t) == CCM_OK && t.triaged)
       print_triage(t, ordinals[i]);
+    if (mismatch_triage && tags[i].mismatch_bytes != 0 && ccm_scrub_last_mismatch_triage(ordinals[i], &t) == CCM_OK &&
+        t.triaged)
+      print_mismatch_triage(t, ordinals[i]);
     printf("}");
   }
   printf("]}\n");

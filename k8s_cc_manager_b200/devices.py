@@ -31,7 +31,8 @@ class GpuError(Exception):
     """Raised for any failed device operation (reference: gpu.GpuError).  A scrub that read back dirt
     carries its DirtReport as `.dirt`; a tagged scrub whose check found bytes off their tags carries its
     MismatchReport as `.mismatch`; a census call carries its ResidueReport (what the first pass erased) as
-    `.residue`; a triage call that read back dirt carries its TriageReport (what kind of dirt) as `.triage`."""
+    `.residue`; a triage call that read back dirt carries its TriageReport (what kind of dirt) as `.triage`; a mismatch
+    triage call whose tagged check failed carries its TriageReport (what kind of mismatch) as `.mismatch_triage`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
@@ -400,11 +401,22 @@ class TriagePage:
 def last_triage_pages(cuda_ordinal: int) -> "Optional[List[TriagePage]]":
     """The pages of the last triage on a CUDA device (include/ccm.h: ccm_last_triage_pages), ascending; None when they
     cannot be read."""
+    return _triage_pages(cuda_ordinal, "ccm_last_triage_pages")
+
+
+def last_mismatch_triage_pages(cuda_ordinal: int) -> "Optional[List[TriagePage]]":
+    """The pages of the last mismatch triage on a CUDA device (include/ccm.h: ccm_last_mismatch_triage_pages), one per
+    page of the mismatch page map, ascending (`dirt_bytes`: that map's bytes on the page); None when they cannot be
+    read."""
+    return _triage_pages(cuda_ordinal, "ccm_last_mismatch_triage_pages")
+
+
+def _triage_pages(cuda_ordinal: int, fn: str) -> "Optional[List[TriagePage]]":
     n = C.c_uint64(0)
-    if cuda_ordinal < 0 or N.lib().ccm_last_triage_pages(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
+    if cuda_ordinal < 0 or getattr(N.lib(), fn)(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
         return None
     buf = (N.TriagePage * max(1, n.value))()
-    if N.lib().ccm_last_triage_pages(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
+    if getattr(N.lib(), fn)(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
         return None
     return [TriagePage(p.page, p.chunk, N.TRIAGE_CLASSES.get(p.cls, str(p.cls)), p.dirt_bytes, p.t2_bytes, p.t3_bytes)
             for p in buf[:n.value]]
@@ -472,9 +484,30 @@ def last_triage(cuda_ordinal: int) -> "Optional[TriageReport]":
     return TriageReport.from_native(out, last_triage_pages(cuda_ordinal) if out.triaged else None)
 
 
+def last_mismatch_triage(cuda_ordinal: int) -> "Optional[TriageReport]":
+    """The mismatch triage report of the last product call on a CUDA device (include/ccm.h:
+    ccm_scrub_last_mismatch_triage), with the pages that did not clear; None when it cannot be read.  Its byte counts
+    are bytes of the mismatch page map, and its va_base is the mismatch report's."""
+    out = N.TriageReport()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_mismatch_triage(cuda_ordinal, C.byref(out)) != N.OK:
+        return None
+    return TriageReport.from_native(out, last_mismatch_triage_pages(cuda_ordinal) if out.triaged else None)
+
+
 def _arm_triage(cuda_ordinal: int, hold_ms: int) -> bool:
     """Arms (hold_ms > 0) or disarms (0) the triage on a CUDA device; False when the library refused."""
     return cuda_ordinal >= 0 and N.lib().ccm_scrub_triage(cuda_ordinal, hold_ms) == N.OK
+
+
+def _arm_mismatch_triage(cuda_ordinal: int, hold_ms: int) -> bool:
+    """Arms (hold_ms > 0) or disarms (0) the mismatch triage on a CUDA device; False when the library refused."""
+    return cuda_ordinal >= 0 and N.lib().ccm_scrub_mismatch_triage(cuda_ordinal, hold_ms) == N.OK
+
+
+def _mismatch_triage_check(mismatch_triage: bool, check: str) -> None:
+    """The mismatch triage triages what the tagged check found: it needs check="tagged"."""
+    if mismatch_triage and check != "tagged":
+        raise ValueError(f"mismatch_triage needs check='tagged', not {check!r}")
 
 
 def _triage_hold(hold_ms: int) -> int:
@@ -484,7 +517,8 @@ def _triage_hold(hold_ms: int) -> int:
 
 
 # The reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
-_REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport))
+_REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport),
+            ("mismatch_triage", TriageReport))
 
 
 @dataclass
@@ -525,6 +559,10 @@ class ScrubReport:
     # What kind of dirt it is (a TriageReport), set for every report of a triage call (triage=True) that triaged: one
     # whose read-back found non-zero bytes.  Not a dataclass field either.
     triage = None
+    # What kind of mismatch it is (a TriageReport of the mismatch page map), set for every report of a mismatch triage
+    # call (mismatch_triage=True) that triaged: one whose tagged check found bytes off their tags.  Not a dataclass
+    # field either.
+    mismatch_triage = None
 
     @property
     def clean(self) -> bool:
@@ -561,7 +599,7 @@ class ScrubReport:
 
     def as_json(self) -> dict:
         """The report as the scrub workers print it: the tagged-gate fields only for a tagged call, "dirt",
-        "mismatch", "residue" and "triage" only when that report is attached."""
+        "mismatch", "residue", "triage" and "mismatch_triage" only when that report is attached."""
         d = dataclasses.asdict(self)
         if self.check == "zero":
             for name in TAG_FIELDS:
@@ -584,10 +622,11 @@ class ScrubReport:
 
 
 def _attach_reports(rep: ScrubReport, cuda_ordinal: int, census: "N.ResidueReport | None",
-                    triage: bool = False) -> None:
+                    triage: bool = False, mismatch_triage: bool = False) -> None:
     """Attaches to the report of a call what that call found: the census's report, and the device's last dirt /
     mismatch report when the call counted non-zero / mismatched bytes; each report that booked a window with its page
-    map's digest; and for a triage call whose read-back found non-zero bytes, the triage report when it ran."""
+    map's digest; for a triage call whose read-back found non-zero bytes, the triage report when it ran; and for a
+    mismatch triage call whose tagged check found bytes off their tags, the mismatch triage report when it ran."""
     if census is not None:
         rep.residue = ResidueReport.from_native(census)
     if rep.nonzero_bytes:
@@ -597,6 +636,9 @@ def _attach_reports(rep: ScrubReport, cuda_ordinal: int, census: "N.ResidueRepor
     if triage and rep.nonzero_bytes:
         report = last_triage(cuda_ordinal)
         rep.triage = report if report is not None and report.triaged else None
+    if mismatch_triage and rep.mismatch_bytes:
+        report = last_mismatch_triage(cuda_ordinal)
+        rep.mismatch_triage = report if report is not None and report.triaged else None
     for attr, _ in _REPORTS:
         report = getattr(rep, attr)
         if isinstance(report, _WindowReport) and getattr(report, report.WINDOWS):
@@ -669,7 +711,7 @@ class NvidiaDevice:
 
     # -- NEW: HBM scrub-and-verify ---------------------------------------------
     def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
-                         triage_hold_ms: int = TRIAGE_HOLD_MS) -> ScrubReport:
+                         triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False) -> ScrubReport:
         """Zero-fills and reads back this GPU's HBM (nbytes=0: all the context can map).
         check="tagged" first writes and checks an address-tagged known answer
         (include/ccm.h: ccm_scrub_verify_tagged).  residue=True runs the census in the first pass and attaches what
@@ -677,6 +719,10 @@ class NvidiaDevice:
         triage=True arms the dirt triage for this call (include/ccm.h: ccm_scrub_triage): when the read-back finds
         non-zero bytes, the dirty pages are re-zeroed and re-read at once and after `triage_hold_ms`, and what
         kind of dirt it is comes attached as `.triage`; it never changes the verdict either.
+        mismatch_triage=True (check="tagged" only, else ValueError) arms the mismatch triage for this call
+        (include/ccm.h: ccm_scrub_mismatch_triage): when the tagged check finds bytes off their tags, those pages are
+        re-tagged, checked and zeroed, held for `triage_hold_ms` and read for zeros, and what kind of mismatch it is
+        comes attached as `.mismatch_triage`; it never changes the verdict either.
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
         if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
@@ -686,7 +732,10 @@ class NvidiaDevice:
         res, tag, census = N.ScrubResult(), None, None
         if _check_mode(check):
             tag = N.TagResult()
-        armed = triage and _arm_triage(self.cuda_ordinal, _triage_hold(triage_hold_ms))
+        _mismatch_triage_check(mismatch_triage, check)
+        hold = _triage_hold(triage_hold_ms) if triage or mismatch_triage else 0
+        armed = triage and _arm_triage(self.cuda_ordinal, hold)
+        marmed = mismatch_triage and _arm_mismatch_triage(self.cuda_ordinal, hold)
         try:
             if residue:
                 census = N.ResidueReport()
@@ -700,8 +749,10 @@ class NvidiaDevice:
         finally:
             if armed:
                 _arm_triage(self.cuda_ordinal, 0)
+            if marmed:
+                _arm_mismatch_triage(self.cuda_ordinal, 0)
         rep = ScrubReport.from_native(self.bdf, res, tag)
-        _attach_reports(rep, self.cuda_ordinal, census, armed)
+        _attach_reports(rep, self.cuda_ordinal, census, armed, marmed)
         if err is not None:
             for attr, _ in _REPORTS:
                 setattr(err, attr, getattr(rep, attr))
@@ -750,25 +801,29 @@ def find_gpus() -> Tuple[List[NvidiaDevice], int]:
 
 def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
                           check: str = "zero", residue: bool = False, triage: bool = False,
-                          triage_hold_ms: int = TRIAGE_HOLD_MS) -> Tuple[List[ScrubReport], float]:
+                          triage_hold_ms: int = TRIAGE_HOLD_MS,
+                          mismatch_triage: bool = False) -> Tuple[List[ScrubReport], float]:
     """Concurrent multi-context scrub of several GPUs through ONE native call
     (ccm_scrub_verify_many: one host thread + primary context + stream per GPU, no
     peer access, no collective; check="tagged": ccm_scrub_verify_many_tagged; residue=True:
     ccm_scrub_verify_many_residue, each report with its `.residue`; triage=True: every GPU armed for the dirt
-    triage, as in NvidiaDevice.scrub_and_verify).  Returns
+    triage, as in NvidiaDevice.scrub_and_verify; mismatch_triage=True: every GPU armed for the mismatch triage, as
+    there).  Returns
     (reports, wall_ms); never raises for a per-device failure — inspect report.status /
     report.clean."""
     tagged = _check_mode(check)
+    _mismatch_triage_check(mismatch_triage, check)
     n = len(devices)
     if n == 0:
         return [], 0.0
-    hold = _triage_hold(triage_hold_ms) if triage else 0
+    hold = _triage_hold(triage_hold_ms) if triage or mismatch_triage else 0
     idx = (C.c_int * n)(*[d.index for d in devices])
     res = (N.ScrubResult * n)()
     wall = C.c_double(0.0)
     tags = (N.TagResult * n)() if tagged else None
     census = (N.ResidueReport * n)() if residue else None
     armed = {d.cuda_ordinal for d in devices if triage and _arm_triage(d.cuda_ordinal, hold)}
+    marmed = {d.cuda_ordinal for d in devices if mismatch_triage and _arm_mismatch_triage(d.cuda_ordinal, hold)}
     try:
         if residue:
             N.lib().ccm_scrub_verify_many_residue(n, idx, nbytes, tags, census, res, C.byref(wall))
@@ -779,9 +834,12 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
     finally:
         for ordinal in armed:
             _arm_triage(ordinal, 0)
+        for ordinal in marmed:
+            _arm_mismatch_triage(ordinal, 0)
     reports = [ScrubReport.from_native(d.bdf, res[i], tags[i] if tagged else None) for i, d in enumerate(devices)]
     for i, (rep, d) in enumerate(zip(reports, devices)):
-        _attach_reports(rep, d.cuda_ordinal, census[i] if residue else None, d.cuda_ordinal in armed)
+        _attach_reports(rep, d.cuda_ordinal, census[i] if residue else None, d.cuda_ordinal in armed,
+                        d.cuda_ordinal in marmed)
     return reports, wall.value
 
 
@@ -834,10 +892,14 @@ class ScrubbingProxy:
         return native.wait_scrub_released() if native is not None else (0.0, 0.0)
 
     def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
-                         triage_hold_ms: int = TRIAGE_HOLD_MS) -> ScrubReport:
+                         triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False) -> ScrubReport:
         native = object.__getattribute__(self, "_native")
+        _mismatch_triage_check(mismatch_triage, check)
         if native is None:
             raise GpuError(f"no CUDA device with PCI address {self._foreign.bdf}: HBM scrub cannot run", N.ERR_NO_CUDA)
+        if mismatch_triage:
+            return native.scrub_and_verify(nbytes, check=check, residue=residue, triage=triage,
+                                           triage_hold_ms=triage_hold_ms, mismatch_triage=True)
         if triage:
             return native.scrub_and_verify(nbytes, check=check, residue=residue, triage=True,
                                            triage_hold_ms=triage_hold_ms)

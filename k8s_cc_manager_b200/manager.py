@@ -62,8 +62,8 @@ READINESS_FILE = os.environ.get("CC_READINESS_FILE", "/run/nvidia/validations/.c
 VALID_MODES = ("on", "off", "devtools", "ppcie")
 SCRUB_SKIPPED_ANNOTATION = "nvidia.com/cc-manager.scrub-skipped"
 RESIDUE_MODES = ("off", "report")   # CC_SCRUB_RESIDUE
-TRIAGE_MODES = ("off", "report")    # CC_SCRUB_TRIAGE
-# How long the dirt triage waits between re-reading the re-zeroed dirty pages at once and again: long enough for an
+TRIAGE_MODES = ("off", "report")    # CC_SCRUB_TRIAGE, CC_SCRUB_MISMATCH_TRIAGE
+# How long the dirt and mismatch triages wait before their last re-read of the pages they re-wrote: long enough for an
 # agent that still writes this GPU's memory to show itself, short against a transition.
 SCRUB_TRIAGE_HOLD_MS = 100
 
@@ -108,7 +108,8 @@ class CCManager:
                  device_source: Optional[Callable[[], tuple]] = None,
                  scrub_mode: Optional[str] = None, scrub_bytes: Optional[int] = None,
                  max_parallel: Optional[int] = None, scrub_check: Optional[str] = None,
-                 scrub_residue: Optional[str] = None, scrub_triage: Optional[str] = None):
+                 scrub_residue: Optional[str] = None, scrub_triage: Optional[str] = None,
+                 scrub_mismatch_triage: Optional[str] = None):
         env = os.environ
         self.operator_namespace = env.get("OPERATOR_NAMESPACE", "gpu-operator")
         self.evict_operator_components = env.get("EVICT_OPERATOR_COMPONENTS", "true").lower() == "true"
@@ -158,6 +159,17 @@ class CCManager:
         self.scrub_triage = (scrub_triage or env.get("CC_SCRUB_TRIAGE", "off")).lower()
         if self.scrub_triage not in TRIAGE_MODES:
             raise ValueError(f"CC_SCRUB_TRIAGE must be 'off' or 'report', not {self.scrub_triage!r}")
+        # off:    a failed tagged check reports where the tags were wrong.
+        # report: it also writes the tags over those pages again, checks and zeroes them, and reads them for zeros after
+        #         SCRUB_TRIAGE_HOLD_MS, and says whether the mismatch stays (hardware or a broken mapping), returns
+        #         (something still writes this GPU's memory) or clears (a one-time write).  Needs CC_SCRUB_CHECK=tagged.
+        #         Logged and kept in last_transition["scrub_mismatch_triage"]; it never changes the verdict.
+        self.scrub_mismatch_triage = (scrub_mismatch_triage or env.get("CC_SCRUB_MISMATCH_TRIAGE", "off")).lower()
+        if self.scrub_mismatch_triage not in TRIAGE_MODES:
+            raise ValueError(f"CC_SCRUB_MISMATCH_TRIAGE must be 'off' or 'report', not {self.scrub_mismatch_triage!r}")
+        if self.scrub_mismatch_triage == "report" and self.scrub_check != "tagged":
+            raise ValueError("CC_SCRUB_MISMATCH_TRIAGE=report triages what the tagged check finds: it needs "
+                             f"CC_SCRUB_CHECK=tagged, not {self.scrub_check!r}")
         self.max_parallel = int(max_parallel if max_parallel is not None else env.get("CC_MAX_PARALLEL", "0"))
         # "full-HBM" is enforced, not assumed: when scrubbing everything (scrub_bytes == 0) a GPU on
         # which less than this fraction of DEVICE memory was zeroed and read back fails the gate
@@ -545,6 +557,8 @@ class CCManager:
             cmd += ["--residue"]
         if self.triage:
             cmd += ["--triage", "--triage-hold-ms", str(SCRUB_TRIAGE_HOLD_MS)]
+        if self.mismatch_triage:
+            cmd += ["--mismatch-triage"] + ([] if self.triage else ["--triage-hold-ms", str(SCRUB_TRIAGE_HOLD_MS)])
         for gpu in gpus:
             cmd += ["--bdf", gpu.bdf]
         env = dict(os.environ)
@@ -610,6 +624,30 @@ class CCManager:
                                f"CC_SCRUB_CHECK={self.scrub_check}; refusing to release it")
         return rep
 
+    @property
+    def mismatch_triage(self) -> bool:
+        return self.scrub_mismatch_triage == "report"
+
+    def _scrub_with_mismatch_triage(self, gpu):
+        """The mismatch triage call on one device (with the dirt triage and the census when they are on).  A device
+        whose scrub_and_verify cannot take `mismatch_triage` is scrubbed exactly as without it, with a warning."""
+        kwargs = dict(check=self.scrub_check, triage_hold_ms=SCRUB_TRIAGE_HOLD_MS, mismatch_triage=True)
+        if self.triage:
+            kwargs["triage"] = True
+        if self.census:
+            kwargs["residue"] = True
+        try:
+            inspect.signature(gpu.scrub_and_verify).bind(self.scrub_bytes, **kwargs)
+        except (TypeError, ValueError):
+            logger.warning("Device %s cannot triage HBM tag mismatches (CC_SCRUB_MISMATCH_TRIAGE=report): its gate "
+                           "runs without the mismatch triage", gpu.bdf)
+            return self._scrub_with_triage(gpu, self.census) if self.triage else self._scrub_one(gpu, self.census)
+        rep = gpu.scrub_and_verify(self.scrub_bytes, **kwargs)
+        if getattr(rep, "check", "zero") != self.scrub_check:   # as _scrub_checked: never zero-only in its place
+            raise ScrubFailure(f"device {gpu.bdf} returned a {getattr(rep, 'check', 'zero')} scrub report for "
+                               f"CC_SCRUB_CHECK={self.scrub_check}; refusing to release it")
+        return rep
+
     def _scrub_one(self, gpu, census: bool):
         if census:
             return self._scrub_with_residue(gpu)
@@ -627,8 +665,10 @@ class CCManager:
         ("mismatch", "scrub_mismatch", logging.ERROR, "HBM tag mismatch on %s: %s"),
     )
     # Logged after them: whether that dirt stays, returns or clears when its pages are zeroed and read back once more
-    # (CC_SCRUB_TRIAGE=report).  It has no page line: it is itself a verdict per page.
-    _TRIAGE_NOTES = (("triage", "scrub_triage", logging.ERROR, "HBM dirt triage on %s: %s"),)
+    # (CC_SCRUB_TRIAGE=report), then whether that mismatch does when its pages are tagged and checked once more
+    # (CC_SCRUB_MISMATCH_TRIAGE=report).  They have no page line: each is itself a verdict per page.
+    _TRIAGE_NOTES = (("triage", "scrub_triage", logging.ERROR, "HBM dirt triage on %s: %s"),
+                     ("mismatch_triage", "scrub_mismatch_triage", logging.ERROR, "HBM mismatch triage on %s: %s"))
 
     # One more line per report that carries its page map: which 2 MiB pages, and so which allocations, hold its bytes.
     _PAGE_NOTES = {
@@ -657,7 +697,14 @@ class CCManager:
             # ONE native call for the whole node (maps first, then launches: DESIGN.md §6) — also when the
             # register work belongs to a foreign library and libccm only scrubs (ScrubbingProxy)
             natives = [self._native_of(g) for g in gpus]
-            if self.triage:
+            if self.mismatch_triage:
+                extra = {"residue": True} if self.census else {}
+                if self.triage:
+                    extra["triage"] = True
+                reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes, check=self.scrub_check,
+                                                            triage_hold_ms=SCRUB_TRIAGE_HOLD_MS, mismatch_triage=True,
+                                                            **extra)
+            elif self.triage:
                 extra = {"residue": True} if self.census else {}
                 reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes, check=self.scrub_check,
                                                             triage=True, triage_hold_ms=SCRUB_TRIAGE_HOLD_MS, **extra)
@@ -675,6 +722,8 @@ class CCManager:
                 if not hasattr(gpu, "scrub_and_verify"):
                     raise ScrubFailure(f"device {gpu.bdf} offers no HBM scrub; refusing to release it")
                 try:
+                    if self.mismatch_triage:
+                        return self._scrub_with_mismatch_triage(gpu)
                     if self.triage:
                         return self._scrub_with_triage(gpu, self.census)
                     return self._scrub_one(gpu, self.census)
@@ -956,6 +1005,10 @@ def build_arg_parser() -> argparse.ArgumentParser:
     parser.add_argument("--scrub-triage", default=None, choices=TRIAGE_MODES,
                         help="after a failed read-back, re-zero and re-read the dirty pages and report whether the dirt "
                              "stays, returns or clears (never changes the verdict; default: $CC_SCRUB_TRIAGE or off)")
+    parser.add_argument("--scrub-mismatch-triage", default=None, choices=TRIAGE_MODES,
+                        help="with --scrub-check tagged, after a failed check, re-tag, check and re-read the pages off "
+                             "their tags and report whether the mismatch stays, returns or clears (never changes the "
+                             "verdict; default: $CC_SCRUB_MISMATCH_TRIAGE or off)")
     return parser
 
 
@@ -981,6 +1034,7 @@ def main(argv: Optional[List[str]] = None) -> None:
         CCManager(node_name=args.node_name, default_mode=default_mode, host_cc=host_cc,
                   kubeconfig=args.kubeconfig, scrub_mode=args.scrub_mode, scrub_check=args.scrub_check,
                   scrub_residue=args.scrub_residue, scrub_triage=args.scrub_triage,
+                  scrub_mismatch_triage=args.scrub_mismatch_triage,
                   device_source=_device_source_from_env()).run()
     except KeyboardInterrupt:
         logger.info("Shutting down...")

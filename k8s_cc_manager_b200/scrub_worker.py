@@ -9,7 +9,8 @@ short-lived process and reads ONE JSON line back; the process exit returns every
 
 Output (stdout, last line):  {"wall_ms": ..., "reports": [ {ScrubReport fields}, ... ]}
 (the tagged-gate fields only with --check tagged; "residue" only with --residue; "triage" only with --triage, for a
-GPU whose read-back found non-zero bytes).
+GPU whose read-back found non-zero bytes; "mismatch_triage" only with --mismatch-triage, for a GPU whose tagged check
+found bytes off their tags).
 Exit code: 0 if every GPU is clean, 3 if the gate failed, 2 on usage errors.
 """
 from __future__ import annotations
@@ -23,14 +24,20 @@ from . import _native as N
 from . import devices as D
 
 
-def run(bdfs: List[str], nbytes: int, check: str = "zero", residue: bool = False, triage_hold_ms: int = 0) -> dict:
-    """triage_hold_ms > 0 arms the dirt triage with that hold."""
+def run(bdfs: List[str], nbytes: int, check: str = "zero", residue: bool = False, triage_hold_ms: int = 0,
+        mismatch_triage_hold_ms: int = 0) -> dict:
+    """triage_hold_ms > 0 arms the dirt triage with that hold, mismatch_triage_hold_ms > 0 the mismatch triage (with
+    the same hold when both are armed)."""
     by_bdf = {d.bdf: d for d in D.find_gpus()[0] if d.is_gpu()}
     missing = [b for b in bdfs if b not in by_bdf]
     if missing:
         raise SystemExit(f"unknown GPU(s): {', '.join(missing)} (known: {', '.join(sorted(by_bdf))})")
     devs = [by_bdf[b] for b in bdfs]
-    if triage_hold_ms:
+    if mismatch_triage_hold_ms:
+        reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check, residue=residue,
+                                                   triage=bool(triage_hold_ms),
+                                                   triage_hold_ms=mismatch_triage_hold_ms, mismatch_triage=True)
+    elif triage_hold_ms:
         reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check, residue=residue, triage=True,
                                                    triage_hold_ms=triage_hold_ms)
     elif residue:
@@ -52,15 +59,20 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap.add_argument("--triage", action="store_true",
                     help="after a failed read-back, re-zero and re-read the dirty pages: does the dirt stay, return or "
                          "clear (never fails the gate)")
+    ap.add_argument("--mismatch-triage", action="store_true",
+                    help="with --check tagged, after a failed check, re-tag, check and re-read the pages off their tags: "
+                         "does the mismatch stay, return or clear (never fails the gate)")
     ap.add_argument("--triage-hold-ms", type=int, default=D.TRIAGE_HOLD_MS,
-                    help="the triage's hold between its two re-reads (default %(default)s)")
+                    help="the triages' hold before their last re-read (default %(default)s)")
     args = ap.parse_args(argv)
     if not args.bdf:
         ap.error("at least one --bdf is required")
+    if args.mismatch_triage and args.check != "tagged":
+        ap.error("--mismatch-triage needs --check tagged")
     if args.backend:
         D.select_backend(args.backend)
     out = run([b.lower() for b in args.bdf], args.bytes, args.check, args.residue,
-              args.triage_hold_ms if args.triage else 0)
+              args.triage_hold_ms if args.triage else 0, args.triage_hold_ms if args.mismatch_triage else 0)
     print(json.dumps(out), flush=True)
     return 0 if all(r["status"] == 0 and r["nonzero_bytes"] == 0 and r.get("mismatch_bytes", 0) == 0
                     for r in out["reports"]) else 3
