@@ -433,6 +433,7 @@ const char* ccm_strerror(int status) {
     case CCM_ERR_FAULT: return "injected fault";
     case CCM_ERR_NOT_BOOTED: return "device not booted since its last reset";
     case CCM_ERR_MISMATCH: return "HBM bytes did not hold their address tag (tagged scrub gate)";
+    case CCM_ERR_UNCOVERED: return "a scrub gate pass did not walk every mapped byte exactly once (coverage proof)";
   }
   return "unknown ccm status";
 }
@@ -698,6 +699,11 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
   else if (k == "scrub_residue") d.drill.residue = v < 0 ? 0 : (uint64_t)v;
   else if (k == "triage_stay") d.drill.triage_stay = v < 0 ? 0 : (uint64_t)v;
   else if (k == "triage_return") d.drill.triage_return = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "cover_skip") d.drill.cover_skip = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "cover_pass") {
+    if (v < 0 || v > CCM_PASS_READBACK) { set_error("sim key 'cover_pass' takes 0..3, not %lld", (long long)v); return CCM_ERR_INVALID; }
+    d.drill.cover_pass = v == 0 ? (int)CCM_PASS_READBACK : (int)v;
+  }
   else if (k == "scrub_poison" || k == "scrub_flood" || k == "tag_flood") {
     if (v < 0 || v > 255) { set_error("sim key '%s' takes a byte value (0 = off), not %lld", k.c_str(), (long long)v); return CCM_ERR_INVALID; }
     (k == "scrub_poison" ? d.drill.poison : k == "scrub_flood" ? d.drill.flood : d.drill.tag_flood) = (int)v;
@@ -746,6 +752,8 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "triage_stay") *value = (int64_t)d.drill.triage_stay;
     else if (k == "triage_return") *value = (int64_t)d.drill.triage_return;
     else if (k == "tag_flood") *value = d.drill.tag_flood;
+    else if (k == "cover_skip") *value = (int64_t)d.drill.cover_skip;
+    else if (k == "cover_pass") *value = d.drill.cover_pass;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

@@ -55,6 +55,9 @@ int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, b
 //   triage_stay:   the first byte of each of the first that many pages is XORed between the triage's first step (the
 //                  re-zero, or the re-tag) and its second (the first re-read, or the check-and-zero);
 //   triage_return: the same bytes, between its second and third step.
+// Drill of the coverage proof (sim keys "cover_skip", "cover_pass"; ccm.h), armed or not:
+//   cover_skip:    that many is written into the grab word of the first default-frame launch of pass cover_pass
+//                  (CCM_PASS_*; the sim key's 0 is stored as CCM_PASS_READBACK), just before it on the stream.
 struct ScrubDrill {
   uint64_t inject = 0;
   int poison = 0;
@@ -65,6 +68,8 @@ struct ScrubDrill {
   uint64_t triage_stay = 0;
   uint64_t triage_return = 0;
   int tag_flood = 0;
+  uint64_t cover_skip = 0;
+  int cover_pass = CCM_PASS_READBACK;
 };
 // inject: the call's "scrub_inject" budget.  Its poison and flood drills are those current_scrub_drill()
 // returns on the calling thread.  (The engine entry points keep the signatures that host-only builds of

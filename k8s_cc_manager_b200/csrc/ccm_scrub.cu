@@ -149,6 +149,19 @@ struct VmmMapping {
   std::vector<CUmemGenericAllocationHandle> handles;
 };
 
+// The product call's passes while it enqueues them (ccm.h: ccm_scrub_prove, and the "cover_skip" drill).  Every range
+// launch of the scrub, census, tag fill, tag check and read-back asks it for its cover map (gate_launch); the locate pass
+// and the triages run after it is cleared.
+struct GatePasses {
+  bool active = false;   // the call's passes are being enqueued
+  bool prove = false;    // ... with the proving kernels, into the cover maps
+  struct Span { uint64_t addr, bytes, base; };
+  std::vector<Span> spans;   // what the call holds, and the address of page 0 of the pages its bytes lie on
+  int skip_pass = 0;     // drill "cover_skip": pending for the first launch of this pass (CCM_PASS_*; 0 = none)
+  uint64_t skip = 0;
+};
+static constexpr int kPasses = 3;   // CCM_PASS_FIRST, CHECK, READBACK
+
 struct ScrubEngine {
   int ordinal = -1;
   std::mutex mu;
@@ -177,6 +190,12 @@ struct ScrubEngine {
   uint32_t mtriage_hold_ms = 0;             // the mismatch triage's hold when armed (ccm_scrub_mismatch_triage)
   ccm_triage_report mtriage{};              // report of the last product call (ccm_scrub_last_mismatch_triage)
   std::vector<ccm_triage_page> mtriage_pages;  // and its pages (ccm_last_mismatch_triage_pages)
+  bool prove = false;                       // the coverage proof is armed (ccm_scrub_prove)
+  uint32_t* d_cover = nullptr;              // kPasses cover maps of npages words (the last: outside slot); zero between calls
+  uint32_t* h_cover = nullptr;              // pinned copy of all of them
+  GatePasses gate;                          // the product call's passes, while it enqueues them
+  ccm_cover_report cover{};                 // report of the last product call (ccm_scrub_last_cover)
+  std::vector<ccm_cover_page> cover_pages;  // and its inexact pages (ccm_last_cover_pages)
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -225,6 +244,13 @@ static constexpr int kLocateThreads = 512, kLocatePer = 16;
 static constexpr int kCensusThreads = 512, kCensusPer = 16;
 #define CCM_CENSUS_ZERO census_zero_kernel<kCensusThreads, kCensusPer>
 #define CCM_CENSUS_TAG census_tag_fill_kernel<kCensusThreads, kCensusPer>
+// The proving twins (coverage proof): the same shapes.
+#define CCM_COVER_ZERO cover_zero_pass<kFastScrubThreads, kFastScrubPer, kPolDefault>
+#define CCM_COVER_READ cover_read_pass<kFastVerifyThreads, kFastVerifyPer, kPolStreaming>
+#define CCM_COVER_TAG_FILL cover_tag_fill_pass<kTagThreads, kTagPer>
+#define CCM_COVER_TAG_CHECK cover_tag_check_pass<kTagThreads, kTagPer>
+#define CCM_COVER_CENSUS_ZERO cover_census_zero_pass<kCensusThreads, kCensusPer>
+#define CCM_COVER_CENSUS_TAG cover_census_tag_pass<kCensusThreads, kCensusPer>
 
 const char* default_kernel_names() {
   static const std::string names = [] {
@@ -345,6 +371,10 @@ int engine_teardown(int ordinal) {
   if (e->h_book) cudaFreeHost(e->h_book);
   if (e->d_pages) cudaFree(e->d_pages);
   if (e->h_pages) cudaFreeHost(e->h_pages);
+  if (e->d_cover) cudaFree(e->d_cover);
+  if (e->h_cover) cudaFreeHost(e->h_cover);
+  e->d_cover = nullptr;
+  e->h_cover = nullptr;
   e->d_counter = nullptr;
   e->h_counter = nullptr;
   e->d_records = nullptr;
@@ -510,12 +540,36 @@ static bool is_fast_scrub(int variant, const ccm_launch_cfg* cfg) {
   return cfg == nullptr && resolve_scrub_variant(variant) == CCM_SCRUB_ST128;
 }
 
+// Before a default-frame launch over [p, ...) that may belong to pass `pass` (CCM_PASS_*) of the product call, whose
+// GrabCtl pair is at word `grab`: *cover = the pass's cover map when the call proves (map == nullptr otherwise), and the
+// "cover_skip" drill, when it is pending for this pass, writes its count into the grab word first.
+static int gate_launch(ScrubEngine* e, int pass, const void* p, int grab, cudaStream_t st, CoverOut* cover) {
+  GatePasses& g = e->gate;
+  *cover = CoverOut{nullptr, 0, 0};
+  if (!g.active) return CCM_OK;
+  if (g.skip_pass == pass) {
+    e->h_counter[7] = g.skip;   // pinned and unchanged until the call ends: the copy runs in stream order
+    CCM_CUDA(cudaMemcpyAsync(e->d_counter + grab, e->h_counter + 7, sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
+    g.skip_pass = 0;
+  }
+  if (g.prove) {
+    const uint64_t a = (uint64_t)(uintptr_t)p;
+    // a launch outside what the call holds counts into the outside slot: its offsets all lie past the map
+    uint64_t base = a - (uint64_t)e->npages * kPageBytes;
+    for (const GatePasses::Span& sp : g.spans)
+      if (a >= sp.addr && a < sp.addr + sp.bytes) base = sp.base;
+    *cover = CoverOut{e->d_cover + (uint64_t)(pass - 1) * e->npages, base, (uint32_t)(e->npages - 1)};
+  }
+  return CCM_OK;
+}
+
 // Scrub one contiguous range on `st` (no sync).  zero_on_exit: see scrub_st128_fast_kernel
 // (honoured by the default kernel only — callers check is_fast_scrub()).
 static int scrub_range(ScrubEngine* e, void* p, uint64_t n, int variant, const ccm_launch_cfg* cfg,
                        cudaStream_t st, unsigned long long* zero_on_exit = nullptr) {
   if (n == 0) return CCM_OK;
   variant = resolve_scrub_variant(variant);
+  if (e->gate.prove && cfg == nullptr) variant = CCM_SCRUB_ST128;   // a proving call runs the proving twin
   Shape sh = scrub_shape(variant, cfg);
   sh.threads = clamp_threads(sh.threads);
   // the host computes the tile count, so it must use the UNROLL that is actually instantiated
@@ -531,7 +585,10 @@ static int scrub_range(ScrubEngine* e, void* p, uint64_t n, int variant, const c
       if (cfg == nullptr) {
         // library default: compile-time shape (one persistent 512-thread CTA per SM, 16 x STG.128 per
         // thread per 128 KiB grab) — scrub_st128_fast_kernel
-        err = launch_fast(CCM_FAST_SCRUB, kFastScrubThreads, kFastScrubPer, e, kScrubGrab, st, s, zero_on_exit);
+        CoverOut cv;
+        if (int rc = gate_launch(e, CCM_PASS_FIRST, p, kScrubGrab, st, &cv)) return rc;
+        err = cv.map ? launch_fast(CCM_COVER_ZERO, kFastScrubThreads, kFastScrubPer, e, kScrubGrab, st, s, zero_on_exit, cv)
+                     : launch_fast(CCM_FAST_SCRUB, kFastScrubThreads, kFastScrubPer, e, kScrubGrab, st, s, zero_on_exit);
         g_launches++;
         break;
       }
@@ -589,6 +646,7 @@ static int verify_range(ScrubEngine* e, const void* p, uint64_t n, int variant, 
                         cudaStream_t st) {
   if (n == 0) return CCM_OK;
   variant = resolve_verify_variant(variant);
+  if (e->gate.prove && cfg == nullptr) variant = CCM_VERIFY_LD128;
   Shape sh = verify_shape(cfg);
   sh.threads = clamp_threads(sh.threads);
   if (sh.unroll != 1 && sh.unroll != 2 && sh.unroll != 8) sh.unroll = 4;
@@ -600,7 +658,12 @@ static int verify_range(ScrubEngine* e, const void* p, uint64_t n, int variant, 
       if (cfg == nullptr) {
         // library default: one persistent 1024-thread CTA per SM, 8 x LDG.128 in flight per thread
         // per 128 KiB grab — verify_ld128_fast_kernel
-        err = launch_fast(CCM_FAST_VERIFY, kFastVerifyThreads, kFastVerifyPer, e, kVerifyGrab, st, s, e->d_counter + kNonzero);
+        CoverOut cv;
+        if (int rc = gate_launch(e, CCM_PASS_READBACK, p, kVerifyGrab, st, &cv)) return rc;
+        err = cv.map ? launch_fast(CCM_COVER_READ, kFastVerifyThreads, kFastVerifyPer, e, kVerifyGrab, st, s,
+                                   e->d_counter + kNonzero, cv)
+                     : launch_fast(CCM_FAST_VERIFY, kFastVerifyThreads, kFastVerifyPer, e, kVerifyGrab, st, s,
+                                   e->d_counter + kNonzero);
         break;
       }
       Sched sc;
@@ -630,7 +693,11 @@ static int verify_range(ScrubEngine* e, const void* p, uint64_t n, int variant, 
 // Write the tags of `seed` over one range on `st` (no sync).
 static int tag_fill_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cudaStream_t st) {
   if (n == 0) return CCM_OK;
-  const cudaError_t err = launch_fast(CCM_TAG_FILL, kTagThreads, kTagPer, e, kTagFillGrab, st, split_region(p, n, 16, 128), seed);
+  CoverOut cv;
+  if (int rc = gate_launch(e, CCM_PASS_FIRST, p, kTagFillGrab, st, &cv)) return rc;
+  const RegionSplit s = split_region(p, n, 16, 128);
+  const cudaError_t err = cv.map ? launch_fast(CCM_COVER_TAG_FILL, kTagThreads, kTagPer, e, kTagFillGrab, st, s, seed, cv)
+                                 : launch_fast(CCM_TAG_FILL, kTagThreads, kTagPer, e, kTagFillGrab, st, s, seed);
   g_launches++;
   if (err != cudaSuccess) { set_error("tag fill launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
   return CCM_OK;
@@ -641,8 +708,14 @@ static int tag_fill_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cu
 // (every launch of one call passes the same base, or one that makes the offsets continue across its ranges).
 static int tag_check_range(ScrubEngine* e, void* p, uint64_t n, uint32_t seed, cudaStream_t st, uint64_t base) {
   if (n == 0) return CCM_OK;
-  const cudaError_t err = launch_fast(CCM_TAG_CHECK, kTagThreads, kTagPer, e, kTagCheckGrab, st, split_region(p, n, 16, 128),
-                                      seed, e->d_counter + kMismatch, e->book_out(kCheckBook), base);
+  CoverOut cv;
+  if (int rc = gate_launch(e, CCM_PASS_CHECK, p, kTagCheckGrab, st, &cv)) return rc;
+  const RegionSplit s = split_region(p, n, 16, 128);
+  const cudaError_t err =
+      cv.map ? launch_fast(CCM_COVER_TAG_CHECK, kTagThreads, kTagPer, e, kTagCheckGrab, st, s, seed, e->d_counter + kMismatch,
+                           e->book_out(kCheckBook), base, cv)
+             : launch_fast(CCM_TAG_CHECK, kTagThreads, kTagPer, e, kTagCheckGrab, st, s, seed, e->d_counter + kMismatch,
+                           e->book_out(kCheckBook), base);
   g_launches++;
   if (err != cudaSuccess) { set_error("tag check launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
   return CCM_OK;
@@ -654,8 +727,14 @@ static int census_range(ScrubEngine* e, void* p, uint64_t n, bool tags, uint32_t
   if (n == 0) return CCM_OK;
   const RegionSplit s = split_region(p, n, 16, 128);
   MaskRecord* recs = (MaskRecord*)e->book_records(kCensusBook);
+  CoverOut cv;
+  if (int rc = gate_launch(e, CCM_PASS_FIRST, p, kCensusGrab, st, &cv)) return rc;
   const cudaError_t err =
-      tags ? launch_fast(CCM_CENSUS_TAG, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, seed,
+      cv.map ? (tags ? launch_fast(CCM_COVER_CENSUS_TAG, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, seed,
+                                   e->book_out(kCensusBook), recs, base, cv)
+                     : launch_fast(CCM_COVER_CENSUS_ZERO, kCensusThreads, kCensusPer, e, kCensusGrab, st, s,
+                                   e->book_out(kCensusBook), recs, base, cv))
+      : tags ? launch_fast(CCM_CENSUS_TAG, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, seed,
                          e->book_out(kCensusBook), recs, base)
            : launch_fast(CCM_CENSUS_ZERO, kCensusThreads, kCensusPer, e, kCensusGrab, st, s, e->book_out(kCensusBook),
                          recs, base);
@@ -982,6 +1061,122 @@ static int take_residue(ScrubEngine* e, cudaStream_t st, uint64_t va_base, uint6
   }
   sort_records(rep, bk.windows);
   return CCM_OK;
+}
+
+// ------------------------------------------------------------------ coverage proof
+// Sets aside the cover maps and their host copy, and makes the proving kernels resident (a whole-HBM call cannot load a
+// module once everything is mapped).  The caller holds e->mu.
+static int ensure_cover(ScrubEngine* e) {
+  if (e->d_cover) return CCM_OK;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  const size_t bytes = kPasses * e->npages * sizeof(uint32_t);
+  if (!e->h_cover) CCM_CUDA(cudaHostAlloc(&e->h_cover, bytes, cudaHostAllocDefault));
+  cudaFuncAttributes fa;
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_ZERO));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_READ));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_TAG_FILL));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_TAG_CHECK));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_CENSUS_ZERO));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_CENSUS_TAG));
+  uint32_t* d = nullptr;
+  CCM_CUDA(cudaMalloc(&d, bytes));
+  const cudaError_t err = cudaMemset(d, 0, bytes);
+  if (err != cudaSuccess) {
+    cudaFree(d);
+    set_error("cover map memset failed: %s", cudaGetErrorString(err));
+    return CCM_ERR_CUDA;
+  }
+  e->d_cover = d;
+  return CCM_OK;
+}
+
+// After the passes of a proving call have finished (the caller holds e->mu): copies the cover maps once, zeroes them
+// for the next call, and compares every pass that ran against what the call mapped, [0, mapped) from va_base.  Fills
+// e->cover (proved = 1) and e->cover_pages; each inexact page gets chunk_of(page offset).
+template <typename ChunkOf>
+static int take_cover(ScrubEngine* e, cudaStream_t st, uint64_t mapped, uint64_t va_base, bool tagged,
+                      ccm_cover_report* out, ChunkOf&& chunk_of) {
+  e->gate.prove = false;
+  const double t0 = now_ms();
+  const size_t bytes = kPasses * e->npages * sizeof(uint32_t);
+  CCM_CUDA(cudaMemcpyAsync(e->h_cover, e->d_cover, bytes, cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaMemsetAsync(e->d_cover, 0, bytes, st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  ccm_cover_report rep;
+  memset(&rep, 0, sizeof rep);
+  rep.bytes_mapped = mapped;
+  rep.pages_mapped = (mapped + kPageBytes - 1) / kPageBytes;
+  rep.va_base = va_base;
+  rep.proved = 1;
+  const bool ran[kPasses] = {true, tagged, true};
+  for (int k = 0; k < kPasses; ++k) rep.pass[k].ran = ran[k];
+  const uint64_t np = e->npages - 1;   // pages of a map; word np is its outside slot
+  std::vector<ccm_cover_page> pages;
+  for (uint64_t p = 0; p < np; ++p) {
+    const uint64_t lo = p * kPageBytes;
+    const uint32_t expected = lo < mapped ? (uint32_t)std::min<uint64_t>(kPageBytes, mapped - lo) : 0u;
+    ccm_cover_page cp;
+    memset(&cp, 0, sizeof cp);
+    cp.page = p;
+    cp.expected = expected;
+    bool exact = true;
+    for (int k = 0; k < kPasses; ++k) {
+      if (!ran[k]) continue;
+      const uint32_t c = e->h_cover[k * e->npages + p];
+      ccm_cover_pass& ps = rep.pass[k];
+      cp.count[k] = c;
+      ps.bytes_counted += c;
+      if (c < expected) {
+        if (ps.pages_short++ == 0) ps.first_short_page = p;
+        ps.bytes_missing += expected - c;
+      } else if (c > expected) {
+        ps.pages_over++;
+        ps.bytes_extra += c - expected;
+      }
+      exact &= c == expected;
+    }
+    if (!exact) {
+      cp.chunk = chunk_of(lo);
+      pages.push_back(cp);
+    }
+  }
+  rep.covered = 1;
+  for (int k = 0; k < kPasses; ++k) {
+    if (!ran[k]) continue;
+    ccm_cover_pass& ps = rep.pass[k];
+    ps.bytes_outside = e->h_cover[k * e->npages + np];
+    ps.bytes_counted += ps.bytes_outside;
+    ps.bytes_extra += ps.bytes_outside;
+    if (ps.bytes_missing || ps.bytes_extra) rep.covered = 0;
+  }
+  rep.ms_prove = now_ms() - t0;
+  e->cover = *out = rep;
+  e->cover_pages.swap(pages);
+  return CCM_OK;
+}
+
+// Starts the passes of one product call (the caller holds e->mu, before the call maps or launches anything): the
+// "cover_skip" drill pending, and when the device is armed, the cover maps set aside.  An armed call that cannot count
+// fails here: it never runs unproven.  The caller adds the spans of what it holds.
+static int begin_gate(ScrubEngine* e, const ScrubDrill& drill) {
+  e->gate = GatePasses();
+  e->gate.active = true;
+  if (drill.cover_skip) { e->gate.skip_pass = drill.cover_pass; e->gate.skip = drill.cover_skip; }
+  if (!e->prove) return CCM_OK;
+  if (int rc = ensure_cover(e)) { e->gate.active = false; return rc; }
+  e->gate.prove = true;
+  return CCM_OK;
+}
+
+// Ends them after every call, whatever it returned.  An armed call cut short by an error leaves partial counts: the
+// maps are zero again for the next one.
+static void end_gate(ScrubEngine* e) {
+  std::lock_guard<std::mutex> g(e->mu);
+  if (e->gate.prove && e->d_cover && e->ready && cudaSetDevice(e->ordinal) == cudaSuccess) {
+    cudaMemsetAsync(e->d_cover, 0, kPasses * e->npages * sizeof(uint32_t), e->stream);
+    cudaStreamSynchronize(e->stream);
+  }
+  e->gate = GatePasses();
 }
 
 // ------------------------------------------------------------------ what kind of dirt
@@ -1466,6 +1661,17 @@ static void arena_triage_mismatch(ScrubEngine* e, uint32_t seed, const ScrubDril
   triage_mismatch(e, e->stream, arena_spans(e->segs), drill, seed);
 }
 
+// The coverage proof of the fallback path, after its read-back: page offsets into the concatenated segments from the
+// first segment's address, chunk = segment index.
+static int arena_cover(ScrubEngine* e, bool tagged, ccm_cover_report* out) {
+  std::lock_guard<std::mutex> g(e->mu);
+  e->gate.active = false;
+  if (!e->gate.prove) return CCM_OK;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  return take_cover(e, e->stream, e->arena_bytes, (uint64_t)(uintptr_t)e->segs.front().ptr, tagged, out,
+                    [&](uint64_t o) { return segment_of(e->segs, o); });
+}
+
 // ------------------------------------------------------- VMM (driver API, lazy)
 // The product call maps HBM in chunks through the virtual-memory-management API so
 // that (a) the chunks sit in ONE contiguous virtual range (one verify launch) and (b)
@@ -1535,7 +1741,7 @@ static bool async_release_enabled() { return env_u64("CCM_ASYNC_RELEASE", 1) != 
 // * the verdict is returned as soon as the 8-byte count is on the host; cuMemUnmap/cuMemRelease
 //   (serialised node-wide by the driver) run on the engine's reaper thread.
 static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDrill& drill, bool node_fanout,
-                                  ccm_scrub_result* r) {
+                                  ccm_scrub_result* r, ccm_cover_report* cover) {
   const VmmApi& api = vmm();
   if (!api.ok) return CCM_ERR_UNSUPPORTED;
   std::lock_guard<std::mutex> g(e->mu);
@@ -1543,6 +1749,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   if (!e->segs.empty()) { set_error("arena already held on CUDA device %d", e->ordinal); return CCM_ERR_STATE; }
   r->ms_release_wait = e->join_reaper();
   CCM_CUDA(cudaSetDevice(e->ordinal));
+  if (int rc0 = begin_gate(e, drill)) return rc0;
   size_t fr = 0, tot = 0;
   CCM_CUDA(cudaMemGetInfo(&fr, &tot));
   r->device_total_bytes = tot;
@@ -1581,6 +1788,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   VmmMapping m;
   if (api.AddressReserve(&m.base, va_bytes, 0, 0, 0) != CUDA_SUCCESS) return CCM_ERR_UNSUPPORTED;
   m.va_bytes = va_bytes;
+  e->gate.spans = {{(uint64_t)m.base, va_bytes, (uint64_t)m.base}};
   cudaStream_t st = e->stream;
   CUmemAccessDesc acc;
   memset(&acc, 0, sizeof acc);
@@ -1718,6 +1926,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     rc = CCM_ERR_CUDA;
   cudaError_t serr = cudaStreamSynchronize(st);  // nothing may still touch the mapping below
   if (rc == CCM_OK && serr != cudaSuccess) { set_error("stream sync failed: %s", cudaGetErrorString(serr)); rc = CCM_ERR_CUDA; }
+  e->gate.active = false;   // the locate pass and the triages below are not the call's passes
 
   const uint64_t mapped = m.mapped;
   const int nchunks = (int)m.handles.size();
@@ -1758,6 +1967,8 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
                                [](uint64_t v, const std::pair<uint64_t, uint32_t>& pc) { return v < pc.first; });
     return it == pieces.begin() ? 0u : std::prev(it)->second;
   };
+  // ---- coverage proof: one copy of the cover maps, no launch ------------------------------------------------
+  if (rc == CCM_OK && e->gate.prove) rc = take_cover(e, st, mapped, (uint64_t)m.base, tag != nullptr, cover, chunk_of);
   // ---- a failed tagged check: where were the tags wrong?  The checks booked it; one copy, no launch ---------
   if (checked && rc == CCM_OK && tag->mismatch_bytes != 0) {
     ccm_mismatch_report rep;
@@ -1823,6 +2034,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   drill.inject = inject;
   ccm_tag_result* tag = current_tag_call();
   ccm_residue_report* res = current_residue_call();
+  bool prove = false;
   {
     std::lock_guard<std::mutex> g(e->mu);
     memset(&e->dirt, 0, sizeof e->dirt);  // every call replaces the reports of the last one
@@ -1834,22 +2046,33 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     e->pages[kDirtBook].clear();          // and their page maps (a census call: the residue's too)
     e->pages[kCheckBook].clear();
     if (res) e->pages[kCensusBook].clear();
+    memset(&e->cover, 0, sizeof e->cover);
+    e->cover_pages.clear();
+    prove = e->prove;
   }
   ccm_scrub_result r;
   memset(&r, 0, sizeof r);
   r.bytes_requested = bytes;
   r.sm_count = e->sm_count;
   // a census call always runs the census kernel: the shape and stores of the default st128 scrub, whatever is pinned
-  r.scrub_variant = res ? CCM_SCRUB_ST128 : resolve_scrub_variant(CCM_SCRUB_AUTO);
-  r.verify_variant = resolve_verify_variant(CCM_VERIFY_AUTO);
+  // and so does a proving call, with the proving twins of the default kernels
+  r.scrub_variant = res || prove ? CCM_SCRUB_ST128 : resolve_scrub_variant(CCM_SCRUB_AUTO);
+  r.verify_variant = prove ? CCM_VERIFY_LD128 : resolve_verify_variant(CCM_VERIFY_AUTO);
   int rc = CCM_ERR_UNSUPPORTED;
-  if (env_u64("CCM_PIPELINE", 1) != 0) rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r);
+  ccm_cover_report cover;   // this call's own copy of the coverage report
+  memset(&cover, 0, sizeof cover);
+  if (env_u64("CCM_PIPELINE", 1) != 0) rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r, &cover);
   if (rc == CCM_ERR_UNSUPPORTED) {
     // plain path: one cudaMalloc'ed arena, whole-arena scrub, whole-arena verify (the drills act per
     // segment: poison before the scrub, flood + inject between the scrub and the verify)
     ccm_arena_info ai;
     rc = engine_arena_acquire(e, bytes, &ai);
     if (rc == CCM_OK) {
+      {
+        std::lock_guard<std::mutex> g(e->mu);
+        rc = begin_gate(e, drill);
+        for (const CheckSpan& sp : arena_spans(e->segs)) e->gate.spans.push_back({sp.addr, sp.bytes, sp.addr - sp.offset});
+      }
       r.ms_acquire = ai.ms_acquire;
       r.bytes_scrubbed = ai.bytes;
       r.device_total_bytes = ai.device_total_bytes;
@@ -1858,7 +2081,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       r.segments = ai.segments;
       float ms_s = 0, ms_v = 0;
       uint64_t nz = 0;
-      rc = arena_drill(e, drill.poison, 0, drill.residue);
+      if (rc == CCM_OK) rc = arena_drill(e, drill.poison, 0, drill.residue);
       if (rc == CCM_OK && tag) {
         rc = arena_tag_check(e, tag, drill.tag_inject, drill.tag_flood, res);
         ms_s = (float)tag->ms_check;
@@ -1869,6 +2092,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       }
       if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
       if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
+      if (rc == CCM_OK) rc = arena_cover(e, tag != nullptr, &cover);
       if (rc == CCM_OK && nz != 0) arena_locate(e, drill);
       if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) arena_triage_mismatch(e, tag->seed, drill);
       r.ms_scrub = ms_s;
@@ -1878,7 +2102,20 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       if (rc == CCM_OK) rc = rc2;
     }
   }
-  if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) {
+  end_gate(e);
+  static const char* const kPassNames[kPasses] = {"first", "check", "read-back"};
+  int short_pass = -1;
+  for (int k = 0; k < kPasses && short_pass < 0; ++k)
+    if (cover.pass[k].ran && (cover.pass[k].bytes_missing || cover.pass[k].bytes_extra)) short_pass = k;
+  if (rc == CCM_OK && cover.proved && !cover.covered && short_pass >= 0) {
+    const ccm_cover_pass& ps = cover.pass[short_pass];
+    set_error("HBM coverage proof failed on CUDA device %d: the %s pass counted %llu of %llu mapped bytes (%llu missing, "
+              "%llu extra; %llu pages short, first short page %llu)", e->ordinal, kPassNames[short_pass],
+              (unsigned long long)ps.bytes_counted, (unsigned long long)cover.bytes_mapped,
+              (unsigned long long)ps.bytes_missing, (unsigned long long)ps.bytes_extra,
+              (unsigned long long)ps.pages_short, (unsigned long long)ps.first_short_page);
+    rc = CCM_ERR_UNCOVERED;
+  } else if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) {
     set_error("tagged scrub found %llu bytes that did not hold their tag (and %llu non-zero bytes after the zeroing) "
               "on CUDA device %d", (unsigned long long)tag->mismatch_bytes, (unsigned long long)r.nonzero_bytes, e->ordinal);
     rc = CCM_ERR_MISMATCH;
@@ -2187,4 +2424,57 @@ extern "C" int ccm_scrub_last_mismatch_triage(int cuda_ordinal, ccm_triage_repor
 
 extern "C" int ccm_last_mismatch_triage_pages(int cuda_ordinal, ccm_triage_page* out, uint64_t cap, uint64_t* n) {
   return last_triage_pages("ccm_last_mismatch_triage_pages", cuda_ordinal, out, cap, n, &ScrubEngine::mtriage_pages);
+}
+
+// ------------------------------------------------------------------------- coverage proof
+static_assert(sizeof(ccm_cover_pass) == 64 && sizeof(ccm_cover_report) == 232 && sizeof(ccm_cover_page) == 32 &&
+              offsetof(ccm_cover_report, pass) == 40, "cover structs keep their layout");
+
+extern "C" int ccm_scrub_prove(int cuda_ordinal, int on) {
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  // disarming an engine that was never created leaves nothing armed (and starts no context)
+  ScrubEngine* e = on ? engine_for(cuda_ordinal) : engine_lookup(cuda_ordinal);
+  if (!e) return on ? CCM_ERR_NO_CUDA : CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  if (on) {
+    CCM_ENSURE_READY(e);
+    if (int rc = ensure_cover(e)) return rc;
+  }
+  e->prove = on != 0;
+  return CCM_OK;
+}
+
+extern "C" int ccm_scrub_last_cover(int cuda_ordinal, ccm_cover_report* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  *out = e->cover;
+  return CCM_OK;
+}
+
+extern "C" int ccm_last_cover_pages(int cuda_ordinal, ccm_cover_page* out, uint64_t cap, uint64_t* n) {
+  if (!n || (cap && !out)) {
+    set_error("ccm_last_cover_pages: cap %llu (needs n, and out when cap > 0)", (unsigned long long)cap);
+    return CCM_ERR_INVALID;
+  }
+  *n = 0;
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  *n = e->cover_pages.size();
+  if (cap) memcpy(out, e->cover_pages.data(), std::min<uint64_t>(cap, *n) * sizeof(ccm_cover_page));
+  return CCM_OK;
 }

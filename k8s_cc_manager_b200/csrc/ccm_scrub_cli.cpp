@@ -1,7 +1,7 @@
 // ccm-scrub — native command-line front end of the HBM scrub gate (links libccm.so).
 //
 //   ccm-scrub [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] [--triage]
-//             [--mismatch-triage] [--triage-hold-ms MS] (--all | --bdf <pci address> ...)
+//             [--mismatch-triage] [--triage-hold-ms MS] [--prove] (--all | --bdf <pci address> ...)
 //
 // Runs the concurrent gate (ccm_scrub_verify_many, or ccm_scrub_verify_many_tagged with --check tagged)
 // and prints ONE JSON line with the same fields as k8s_cc_manager_b200.devices.ScrubReport (the
@@ -13,7 +13,10 @@
 // read-back found non-zero bytes: what kind of dirt, as ccm_scrub_last_triage and ccm_last_triage_pages report it;
 // "mismatch_triage" with --mismatch-triage, which needs --check tagged and arms every GPU for the mismatch triage
 // (ccm_scrub_mismatch_triage), for a GPU whose tagged check found bytes off their tags: what kind of mismatch, as
-// ccm_scrub_last_mismatch_triage and ccm_last_mismatch_triage_pages report it).
+// ccm_scrub_last_mismatch_triage and ccm_last_mismatch_triage_pages report it; "cover" with --prove, which arms every
+// GPU for the coverage proof (ccm_scrub_prove), for every GPU whose passes finished, as ccm_scrub_last_cover and
+// ccm_last_cover_pages report it).  With --prove, a GPU that cannot be armed is never scrubbed unproven: nothing is
+// scrubbed and the exit code is 3.
 // Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
@@ -159,6 +162,36 @@ static void print_residue(const ccm_residue_report& r, int ordinal) {
   printf("}");
 }
 
+// The "cover" object: the fields of k8s_cc_manager_b200.devices.CoverReport, with the first 64 inexact pages.
+static void print_cover(const ccm_cover_report& c, int ordinal) {
+  static const char* const names[3] = {"first", "check", "readback"};
+  printf(", \"cover\": {\"bytes_mapped\": %llu, \"pages_mapped\": %llu, \"va_base\": %llu, \"ms_prove\": %.3f, "
+         "\"proved\": %d, \"covered\": %d, \"passes\": [",
+         (unsigned long long)c.bytes_mapped, (unsigned long long)c.pages_mapped, (unsigned long long)c.va_base, c.ms_prove,
+         c.proved, c.covered);
+  for (int k = 0; k < 3; ++k) {
+    const ccm_cover_pass& p = c.pass[k];
+    printf("%s{\"name\": \"%s\", \"ran\": %d, \"bytes_counted\": %llu, \"bytes_missing\": %llu, \"bytes_extra\": %llu, "
+           "\"bytes_outside\": %llu, \"pages_short\": %llu, \"pages_over\": %llu, \"first_short_page\": %llu}",
+           k ? ", " : "", names[k], p.ran, (unsigned long long)p.bytes_counted, (unsigned long long)p.bytes_missing,
+           (unsigned long long)p.bytes_extra, (unsigned long long)p.bytes_outside, (unsigned long long)p.pages_short,
+           (unsigned long long)p.pages_over, (unsigned long long)p.first_short_page);
+  }
+  printf("], \"pages\": [");
+  uint64_t n = 0;
+  std::vector<ccm_cover_page> v;
+  if (!c.covered && ccm_last_cover_pages(ordinal, nullptr, 0, &n) == CCM_OK) {
+    v.resize(n);
+    if (n && ccm_last_cover_pages(ordinal, v.data(), n, &n) != CCM_OK) v.clear();
+  }
+  const size_t keep = 64;   // k8s_cc_manager_b200.devices.COVER_PAGES
+  for (size_t k = 0; k < v.size() && k < keep; ++k)
+    printf("%s{\"page\": %llu, \"chunk\": %u, \"expected\": %u, \"first\": %u, \"check\": %u, \"readback\": %u}",
+           k ? ", " : "", (unsigned long long)v[k].page, v[k].chunk, v[k].expected, v[k].count[0], v[k].count[1],
+           v[k].count[2]);
+  printf("], \"pages_truncated\": %d}", v.size() > keep);
+}
+
 // The "mismatch_triage" object: the fields of k8s_cc_manager_b200.devices.TriageReport for the mismatch page map, with
 // the first 64 pages that did not clear (devices.TRIAGE_PAGES).
 static void print_mismatch_triage(const ccm_triage_report& t, int ordinal) {
@@ -194,14 +227,14 @@ static void print_mismatch_triage(const ccm_triage_report& t, int ordinal) {
 
 static int usage(const char* argv0) {
   fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] "
-          "[--triage] [--mismatch-triage] [--triage-hold-ms MS] (--all | --bdf <bdf> ...)\n", argv0);
+          "[--triage] [--mismatch-triage] [--triage-hold-ms MS] [--prove] (--all | --bdf <bdf> ...)\n", argv0);
   return 2;
 }
 
 int main(int argc, char** argv) {
   std::vector<std::string> bdfs;
   unsigned long long bytes = 0;
-  bool all = false, tagged = false, residue = false, triage = false, mismatch_triage = false;
+  bool all = false, tagged = false, residue = false, triage = false, mismatch_triage = false, prove = false;
   unsigned long triage_hold_ms = 100;   // k8s_cc_manager_b200.devices.TRIAGE_HOLD_MS
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
@@ -209,6 +242,7 @@ int main(int argc, char** argv) {
     else if (a == "--residue") residue = true;
     else if (a == "--triage") triage = true;
     else if (a == "--mismatch-triage") mismatch_triage = true;
+    else if (a == "--prove") prove = true;
     else if (a == "--triage-hold-ms" && i + 1 < argc) {
       triage_hold_ms = strtoul(argv[++i], nullptr, 10);
       if (triage_hold_ms == 0 || triage_hold_ms > CCM_TRIAGE_MAX_HOLD_MS) return usage(argv[0]);
@@ -261,6 +295,16 @@ int main(int argc, char** argv) {
   std::vector<ccm_tag_result> tags(res.size());
   std::vector<ccm_residue_report> census(residue ? res.size() : 0);
   double wall_ms = 0;
+  std::vector<int> parmed;   // ordinals armed for the coverage proof: all of them, or the gate does not run
+  for (size_t i = 0; prove && i < ordinals.size(); ++i) {
+    const int rc = ordinals[i] >= 0 ? ccm_scrub_prove(ordinals[i], 1) : CCM_ERR_NO_CUDA;
+    if (rc != CCM_OK) {
+      fprintf(stderr, "cannot arm the coverage proof on %s: %s\n", names[i].c_str(), ccm_strerror(rc));
+      for (int o : parmed) ccm_scrub_prove(o, 0);
+      return 3;
+    }
+    parmed.push_back(ordinals[i]);
+  }
   std::vector<int> armed;   // ordinals armed for the triage, disarmed once the gate is done
   for (size_t i = 0; triage && i < ordinals.size(); ++i)
     if (ordinals[i] >= 0 && ccm_scrub_triage(ordinals[i], (uint32_t)triage_hold_ms) == CCM_OK) armed.push_back(ordinals[i]);
@@ -275,6 +319,7 @@ int main(int argc, char** argv) {
   else ccm_scrub_verify_many((int)devs.size(), devs.data(), bytes, res.data(), &wall_ms);
   for (int o : armed) ccm_scrub_triage(o, 0);
   for (int o : marmed) ccm_scrub_mismatch_triage(o, 0);
+  for (int o : parmed) ccm_scrub_prove(o, 0);
   bool clean = true;
   printf("{\"wall_ms\": %.3f, \"reports\": [", wall_ms);
   for (size_t i = 0; i < devs.size(); ++i) {
@@ -305,6 +350,10 @@ int main(int argc, char** argv) {
     if (mismatch_triage && tags[i].mismatch_bytes != 0 && ccm_scrub_last_mismatch_triage(ordinals[i], &t) == CCM_OK &&
         t.triaged)
       print_mismatch_triage(t, ordinals[i]);
+    ccm_cover_report c;
+    const bool proved = prove && ccm_scrub_last_cover(ordinals[i], &c) == CCM_OK && c.proved;
+    if (proved) print_cover(c, ordinals[i]);
+    clean = clean && (!prove || proved);   // a proof that was asked for and did not run fails the gate
     printf("}");
   }
   printf("]}\n");

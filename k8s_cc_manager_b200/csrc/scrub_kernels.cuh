@@ -30,6 +30,8 @@
 //   tag_fill_kernel / tag_check_zero_kernel              the tagged gate's known-answer pass
 //   locate_dirt_kernel                                   where the dirt is, after a failed read-back
 //   census_zero_kernel / census_tag_fill_kernel          what the first pass found before it erased it
+//   cover_*_pass                                         proving twins of the six above that run a product call's
+//                                                        passes: they count the bytes they walk per 2 MiB page
 //   fill_pattern_kernel                                  seeded test pattern (tests only)
 // The grab loop (grab_chunks) and the epilogue after the last whole chunk or tile (finish_region,
 // ragged_bytes) are written once.  The five compile-time-shape kernels are one frame (default_kernel)
@@ -1146,6 +1148,149 @@ census_tag_fill_kernel(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t se
   CensusOp<true> op{seed, {out}, records, base};
   default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, op);
   op.ragged_windows(s);
+  op.book.flush();
+}
+
+// ------------------------------------------------------------ coverage proof
+// A read-back that reads nothing returns what a read-back of clean memory returns, so a pass that skipped part of its
+// range cannot be told from one that walked it by its result.  The proving twins below run the same op on the same
+// frame (default_kernel: shape, grab words, PDL, loads and stores) and count, on the device, the bytes each of them
+// processed on every 2 MiB page of the mapping: the host compares the counts against the mapping itself.
+//
+// The cover map of one pass: u32 words, one per page of offset (address - base) >> kPageShift, and a last word, the
+// "outside" slot, for any byte whose page would lie past it (or before base).  Zero before and after every call.
+struct CoverOut {
+  uint32_t* map;
+  uint64_t base;     // address of the map's page 0
+  uint32_t outside;  // index of the outside slot (the map's last word)
+};
+
+__device__ __forceinline__ uint32_t cover_word(const CoverOut& c, uint64_t a) {
+  const uint64_t off = a - c.base;
+  if ((int64_t)off < 0) return c.outside;
+  const uint64_t page = off >> kPageShift;
+  return page < c.outside ? (uint32_t)page : c.outside;
+}
+
+// n bytes (n <= kPageBytes) from address a, by one thread: split at a page boundary, as the page maps split a chunk.
+__device__ __forceinline__ void cover_add(const CoverOut& c, uint64_t a, uint32_t n) {
+  const uint32_t room = kPageBytes - (uint32_t)((a - c.base) & (kPageBytes - 1));
+  const uint32_t lo = n < room ? n : room;
+  atomicAdd(c.map + cover_word(c, a), lo);
+  if (n > lo) atomicAdd(c.map + cover_word(c, a + lo), n - lo);
+}
+
+// n bytes (n <= 16) from address a, by every active lane: the lanes whose bytes start on one page add up and one of
+// them issues the atomic; the rare bytes past a page boundary go one atomic per lane.
+__device__ __forceinline__ void cover_lanes(const CoverOut& c, uint64_t a, uint32_t n) {
+  const uint32_t room = kPageBytes - (uint32_t)((a - c.base) & (kPageBytes - 1));
+  const uint32_t lo = n < room ? n : room;
+  const uint32_t w = cover_word(c, a);
+#if defined(__CUDA_ARCH__) && __CUDA_ARCH__ < 800
+  atomicAdd(c.map + w, lo);
+#else
+  const uint32_t peers = __match_any_sync(__activemask(), w);
+  const uint32_t sum = __reduce_add_sync(peers, lo);
+  if ((threadIdx.x & 31u) == (uint32_t)(__ffs(peers) - 1)) atomicAdd(c.map + w, sum);
+#endif
+  if (n > lo) atomicAdd(c.map + cover_word(c, a + lo), n - lo);
+}
+
+// The op of a proving kernel: `op` does the work, and what it did is counted into `cover` after it, in program order.
+// A chunk by thread 0 (its p is the chunk's first byte) once the CTA's chunk body is issued; leftover vectors and ragged
+// bytes by every lane that takes one.  BYTES = false for the window ops, whose byte() does nothing: their kernels take
+// the ragged head and tail window by window, and count them there (cover_ragged_windows).
+template <typename Op, bool BYTES = true>
+struct CoverOp {
+  Op& op;
+  CoverOut cover;
+  template <int THREADS, int PER_THREAD, typename P>
+  __device__ __forceinline__ void chunk(P p) {
+    op.template chunk<THREADS, PER_THREAD>(p);
+    if (threadIdx.x == 0) cover_add(cover, addr(p), (uint32_t)THREADS * PER_THREAD * 16u);
+  }
+  template <typename P>
+  __device__ __forceinline__ void vec(P p) {
+    op.vec(p);
+    cover_lanes(cover, addr(p), 16u);
+  }
+  template <typename P>
+  __device__ __forceinline__ void byte(P p) {
+    op.byte(p);
+    if constexpr (BYTES) cover_lanes(cover, addr(p), 1u);
+  }
+};
+
+// The ragged head and tail windows the window ops (tag check, census) take after the frame: the part inside the region.
+__device__ __forceinline__ void cover_ragged_windows(const RegionSplit& s, const CoverOut& c) {
+  uint64_t w0 = 0, lo = 0, hi = 0;
+  if (ragged_window(s, w0, lo, hi) && hi > lo) cover_lanes(c, lo, (uint32_t)(hi - lo));
+}
+
+// Proving twin of scrub_st128_fast_kernel.
+template <int THREADS, int PER_THREAD, int POL>
+__global__ void __launch_bounds__(THREADS)
+cover_zero_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, unsigned long long* zero_on_exit, CoverOut cover) {
+  ZeroOp<16, POL> op{0};
+  CoverOp<ZeroOp<16, POL>> cop{op, cover};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, zero_on_exit, cop);
+}
+
+// Proving twin of verify_ld128_fast_kernel (descending).
+template <int THREADS, int PER_THREAD, int POL>
+__global__ void __launch_bounds__(THREADS)
+cover_read_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, unsigned long long* counter, CoverOut cover) {
+  CountNonzeroOp<16, POL> op{0};
+  CoverOp<CountNonzeroOp<16, POL>> cop{op, cover};
+  default_kernel<THREADS, PER_THREAD, true>(s, nchunks, ctl, nullptr, cop);
+  block_accumulate(op.cnt, counter);
+}
+
+// Proving twin of tag_fill_kernel.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS)
+cover_tag_fill_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed, CoverOut cover) {
+  TagFillOp op{seed};
+  CoverOp<TagFillOp> cop{op, cover};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, cop);
+}
+
+// Proving twin of tag_check_zero_kernel.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS)
+cover_tag_check_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed, unsigned long long* mismatch,
+                       LocateOut out, uint64_t base, CoverOut cover) {
+  TagCheckZeroOp op{seed, {out}, base};
+  CoverOp<TagCheckZeroOp, false> cop{op, cover};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, cop);
+  op.ragged_windows(s);
+  cover_ragged_windows(s, cover);
+  op.book.flush();
+  block_accumulate(op.cnt, mismatch);
+}
+
+// Proving twins of census_zero_kernel and census_tag_fill_kernel.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS, 1)
+cover_census_zero_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, LocateOut out, MaskRecord* records,
+                         uint64_t base, CoverOut cover) {
+  CensusOp<false> op{0, {out}, records, base};
+  CoverOp<CensusOp<false>, false> cop{op, cover};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, cop);
+  op.ragged_windows(s);
+  cover_ragged_windows(s, cover);
+  op.book.flush();
+}
+
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS, 1)
+cover_census_tag_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t seed, LocateOut out,
+                        MaskRecord* records, uint64_t base, CoverOut cover) {
+  CensusOp<true> op{seed, {out}, records, base};
+  CoverOp<CensusOp<true>, false> cop{op, cover};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, cop);
+  op.ragged_windows(s);
+  cover_ragged_windows(s, cover);
   op.book.flush();
 }
 

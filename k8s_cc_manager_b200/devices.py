@@ -32,7 +32,8 @@ class GpuError(Exception):
     carries its DirtReport as `.dirt`; a tagged scrub whose check found bytes off their tags carries its
     MismatchReport as `.mismatch`; a census call carries its ResidueReport (what the first pass erased) as
     `.residue`; a triage call that read back dirt carries its TriageReport (what kind of dirt) as `.triage`; a mismatch
-    triage call whose tagged check failed carries its TriageReport (what kind of mismatch) as `.mismatch_triage`."""
+    triage call whose tagged check failed carries its TriageReport (what kind of mismatch) as `.mismatch_triage`; a
+    proving call carries its CoverReport (how many bytes each pass walked on every page) as `.cover`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
@@ -516,9 +517,117 @@ def _triage_hold(hold_ms: int) -> int:
     return int(hold_ms)
 
 
+COVER_PAGES = 64   # inexact pages a CoverReport keeps
+
+
+@dataclass
+class CoverPage:
+    """One page some pass of a proving call did not count exactly (include/ccm.h: ccm_cover_page)."""
+    page: int
+    chunk: int
+    expected: int      # bytes every pass that ran had to count on it
+    first: int         # bytes the first pass, the tagged check and the read-back counted
+    check: int
+    readback: int
+
+    def describe(self) -> str:
+        return (f"page {self.page} (chunk {self.chunk}): expected {self.expected}, first {self.first}, "
+                f"check {self.check}, read-back {self.readback}")
+
+
+@dataclass
+class CoverPass:
+    """What one pass counted against what the call mapped (include/ccm.h: ccm_cover_pass)."""
+    name: str          # "first", "check" or "readback"
+    ran: int
+    bytes_counted: int
+    bytes_missing: int
+    bytes_extra: int
+    bytes_outside: int
+    pages_short: int
+    pages_over: int
+    first_short_page: int
+
+
+@dataclass
+class CoverReport:
+    """The coverage proof of one product call (include/ccm.h: ccm_cover_report): every pass counted on the device the
+    bytes its kernels processed on each 2 MiB page, and `covered` says each pass that ran walked every mapped byte
+    exactly once.  `pages` are the first COVER_PAGES inexact pages."""
+    bytes_mapped: int
+    pages_mapped: int
+    va_base: int
+    ms_prove: float
+    proved: int
+    covered: int
+    passes: List[CoverPass] = field(default_factory=list)
+    pages: List[CoverPage] = field(default_factory=list)
+    pages_truncated: int = 0
+
+    @classmethod
+    def from_native(cls, r: N.CoverReport, pages: "Optional[List[CoverPage]]" = None) -> "CoverReport":
+        passes = [CoverPass(name, *(getattr(r.passes[k], f) for f, _ in N.CoverPass._fields_ if f != "reserved"))
+                  for k, name in enumerate(N.COVER_PASSES)]
+        pages = pages or []
+        return cls(r.bytes_mapped, r.pages_mapped, r.va_base, r.ms_prove, r.proved, r.covered, passes,
+                   pages[:COVER_PAGES], int(len(pages) > COVER_PAGES))
+
+    @classmethod
+    def from_json(cls, d: dict) -> "CoverReport":
+        return cls(**{**d, "passes": [CoverPass(**p) for p in d["passes"]],
+                      "pages": [CoverPage(**p) for p in d["pages"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    def short_pass(self) -> "Optional[CoverPass]":
+        """The first pass that ran and did not count every page exactly (None when covered)."""
+        return next((p for p in self.passes if p.ran and (p.bytes_missing or p.bytes_extra)), None)
+
+    def summary(self, first: int = 4) -> str:
+        """One line for an operator: what was mapped and, when a pass was short, which one and on which pages."""
+        line = f"{self.bytes_mapped} bytes on {self.pages_mapped} pages"
+        bad = self.short_pass()
+        if bad is None:
+            return line + ": every pass covered every byte once (" + ", ".join(p.name for p in self.passes if p.ran) + ")"
+        line += (f": the {bad.name} pass counted {bad.bytes_counted} bytes ({bad.bytes_missing} missing, "
+                 f"{bad.bytes_extra} extra) with {bad.pages_short} pages short")
+        if self.pages:
+            more = " (+more)" if self.pages_truncated or len(self.pages) > first else ""
+            line += "; " + "; ".join(p.describe() for p in self.pages[:first]) + more
+        return line
+
+
+def last_cover_pages(cuda_ordinal: int) -> "Optional[List[CoverPage]]":
+    """The inexact pages of the last proving call on a CUDA device (include/ccm.h: ccm_last_cover_pages), ascending;
+    None when they cannot be read."""
+    n = C.c_uint64(0)
+    if cuda_ordinal < 0 or N.lib().ccm_last_cover_pages(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
+        return None
+    buf = (N.CoverPage * max(1, n.value))()
+    if N.lib().ccm_last_cover_pages(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
+        return None
+    return [CoverPage(p.page, p.chunk, p.expected, *p.count) for p in buf[:n.value]]
+
+
+def last_cover(cuda_ordinal: int) -> "Optional[CoverReport]":
+    """The coverage report of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_cover), with its
+    first inexact pages; None when it cannot be read."""
+    out = N.CoverReport()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_cover(cuda_ordinal, C.byref(out)) != N.OK:
+        return None
+    return CoverReport.from_native(out, last_cover_pages(cuda_ordinal) if out.proved and not out.covered else None)
+
+
+def _arm_prove(cuda_ordinal: int, on: bool) -> int:
+    """Arms or disarms the coverage proof on a CUDA device; the library's status (a call that asked for the proof and
+    could not arm it fails with it: it is never run unproven)."""
+    return N.lib().ccm_scrub_prove(cuda_ordinal, int(on)) if cuda_ordinal >= 0 else N.ERR_NO_CUDA
+
+
 # The reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
 _REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport),
-            ("mismatch_triage", TriageReport))
+            ("mismatch_triage", TriageReport), ("cover", CoverReport))
 
 
 @dataclass
@@ -563,6 +672,9 @@ class ScrubReport:
     # call (mismatch_triage=True) that triaged: one whose tagged check found bytes off their tags.  Not a dataclass
     # field either.
     mismatch_triage = None
+    # How many bytes each pass walked on every page (a CoverReport), set for every report of a proving call
+    # (prove=True) whose passes finished.  Not a dataclass field either.
+    cover = None
 
     @property
     def clean(self) -> bool:
@@ -622,7 +734,7 @@ class ScrubReport:
 
 
 def _attach_reports(rep: ScrubReport, cuda_ordinal: int, census: "N.ResidueReport | None",
-                    triage: bool = False, mismatch_triage: bool = False) -> None:
+                    triage: bool = False, mismatch_triage: bool = False, prove: bool = False) -> None:
     """Attaches to the report of a call what that call found: the census's report, and the device's last dirt /
     mismatch report when the call counted non-zero / mismatched bytes; each report that booked a window with its page
     map's digest; for a triage call whose read-back found non-zero bytes, the triage report when it ran; and for a
@@ -639,6 +751,9 @@ def _attach_reports(rep: ScrubReport, cuda_ordinal: int, census: "N.ResidueRepor
     if mismatch_triage and rep.mismatch_bytes:
         report = last_mismatch_triage(cuda_ordinal)
         rep.mismatch_triage = report if report is not None and report.triaged else None
+    if prove:
+        report = last_cover(cuda_ordinal)
+        rep.cover = report if report is not None and report.proved else None
     for attr, _ in _REPORTS:
         report = getattr(rep, attr)
         if isinstance(report, _WindowReport) and getattr(report, report.WINDOWS):
@@ -711,7 +826,8 @@ class NvidiaDevice:
 
     # -- NEW: HBM scrub-and-verify ---------------------------------------------
     def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
-                         triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False) -> ScrubReport:
+                         triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False,
+                         prove: bool = False) -> ScrubReport:
         """Zero-fills and reads back this GPU's HBM (nbytes=0: all the context can map).
         check="tagged" first writes and checks an address-tagged known answer
         (include/ccm.h: ccm_scrub_verify_tagged).  residue=True runs the census in the first pass and attaches what
@@ -723,6 +839,9 @@ class NvidiaDevice:
         (include/ccm.h: ccm_scrub_mismatch_triage): when the tagged check finds bytes off their tags, those pages are
         re-tagged, checked and zeroed, held for `triage_hold_ms` and read for zeros, and what kind of mismatch it is
         comes attached as `.mismatch_triage`; it never changes the verdict either.
+        prove=True arms the coverage proof for this call (include/ccm.h: ccm_scrub_prove): every pass counts on the
+        device the bytes it walked on each page, the report comes attached as `.cover`, and a pass that missed or
+        repeated a byte fails the call with ERR_UNCOVERED.  A device that cannot be armed fails the call.
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
         if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
@@ -734,9 +853,12 @@ class NvidiaDevice:
             tag = N.TagResult()
         _mismatch_triage_check(mismatch_triage, check)
         hold = _triage_hold(triage_hold_ms) if triage or mismatch_triage else 0
-        armed = triage and _arm_triage(self.cuda_ordinal, hold)
-        marmed = mismatch_triage and _arm_mismatch_triage(self.cuda_ordinal, hold)
+        armed = marmed = False
         try:
+            if prove:
+                _check(_arm_prove(self.cuda_ordinal, True), "scrub_and_verify (coverage proof)", self.bdf)
+            armed = triage and _arm_triage(self.cuda_ordinal, hold)
+            marmed = mismatch_triage and _arm_mismatch_triage(self.cuda_ordinal, hold)
             if residue:
                 census = N.ResidueReport()
                 rc = N.lib().ccm_scrub_verify_residue(self.index, nbytes, C.byref(tag) if tag is not None else None,
@@ -751,8 +873,12 @@ class NvidiaDevice:
                 _arm_triage(self.cuda_ordinal, 0)
             if marmed:
                 _arm_mismatch_triage(self.cuda_ordinal, 0)
+            if prove:
+                _arm_prove(self.cuda_ordinal, False)
         rep = ScrubReport.from_native(self.bdf, res, tag)
-        _attach_reports(rep, self.cuda_ordinal, census, armed, marmed)
+        _attach_reports(rep, self.cuda_ordinal, census, armed, marmed, prove)
+        if err is None and prove and rep.cover is None:   # a proof that was asked for and did not run
+            err = GpuError(f"scrub_and_verify on {self.bdf}: the coverage proof did not run", N.ERR_UNCOVERED)
         if err is not None:
             for attr, _ in _REPORTS:
                 setattr(err, attr, getattr(rep, attr))
@@ -802,17 +928,40 @@ def find_gpus() -> Tuple[List[NvidiaDevice], int]:
 def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
                           check: str = "zero", residue: bool = False, triage: bool = False,
                           triage_hold_ms: int = TRIAGE_HOLD_MS,
-                          mismatch_triage: bool = False) -> Tuple[List[ScrubReport], float]:
+                          mismatch_triage: bool = False, prove: bool = False) -> Tuple[List[ScrubReport], float]:
     """Concurrent multi-context scrub of several GPUs through ONE native call
     (ccm_scrub_verify_many: one host thread + primary context + stream per GPU, no
     peer access, no collective; check="tagged": ccm_scrub_verify_many_tagged; residue=True:
     ccm_scrub_verify_many_residue, each report with its `.residue`; triage=True: every GPU armed for the dirt
     triage, as in NvidiaDevice.scrub_and_verify; mismatch_triage=True: every GPU armed for the mismatch triage, as
-    there).  Returns
+    there; prove=True: every GPU armed for the coverage proof, and a GPU that cannot be armed is not scrubbed: its
+    report carries the arming's status).  Returns
     (reports, wall_ms); never raises for a per-device failure — inspect report.status /
     report.clean."""
     tagged = _check_mode(check)
     _mismatch_triage_check(mismatch_triage, check)
+    if prove:
+        refused = {}
+        for d in devices:
+            rc = _arm_prove(d.cuda_ordinal, True)
+            if rc != N.OK:
+                refused[d.index] = ScrubReport.from_native(d.bdf, N.ScrubResult(status=rc))
+        try:
+            reports, wall = scrub_and_verify_many([d for d in devices if d.index not in refused], nbytes, check,
+                                                  residue, triage, triage_hold_ms, mismatch_triage)
+        finally:
+            for d in devices:
+                if d.index not in refused:
+                    _arm_prove(d.cuda_ordinal, False)
+        it = iter(reports)
+        reports = [refused[d.index] if d.index in refused else next(it) for d in devices]
+        for rep, d in zip(reports, devices):
+            if d.index not in refused:
+                report = last_cover(d.cuda_ordinal)
+                rep.cover = report if report is not None and report.proved else None
+                if rep.status == N.OK and rep.cover is None:   # a proof that was asked for and did not run
+                    rep.status = N.ERR_UNCOVERED
+        return reports, wall
     n = len(devices)
     if n == 0:
         return [], 0.0
@@ -892,11 +1041,15 @@ class ScrubbingProxy:
         return native.wait_scrub_released() if native is not None else (0.0, 0.0)
 
     def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
-                         triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False) -> ScrubReport:
+                         triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False,
+                         prove: bool = False) -> ScrubReport:
         native = object.__getattribute__(self, "_native")
         _mismatch_triage_check(mismatch_triage, check)
         if native is None:
             raise GpuError(f"no CUDA device with PCI address {self._foreign.bdf}: HBM scrub cannot run", N.ERR_NO_CUDA)
+        if prove:
+            return native.scrub_and_verify(nbytes, check=check, residue=residue, triage=triage,
+                                           triage_hold_ms=triage_hold_ms, mismatch_triage=mismatch_triage, prove=True)
         if mismatch_triage:
             return native.scrub_and_verify(nbytes, check=check, residue=residue, triage=triage,
                                            triage_hold_ms=triage_hold_ms, mismatch_triage=True)

@@ -63,6 +63,7 @@ VALID_MODES = ("on", "off", "devtools", "ppcie")
 SCRUB_SKIPPED_ANNOTATION = "nvidia.com/cc-manager.scrub-skipped"
 RESIDUE_MODES = ("off", "report")   # CC_SCRUB_RESIDUE
 TRIAGE_MODES = ("off", "report")    # CC_SCRUB_TRIAGE, CC_SCRUB_MISMATCH_TRIAGE
+PROOF_MODES = ("off", "require")    # CC_SCRUB_PROOF
 # How long the dirt and mismatch triages wait before their last re-read of the pages they re-wrote: long enough for an
 # agent that still writes this GPU's memory to show itself, short against a transition.
 SCRUB_TRIAGE_HOLD_MS = 100
@@ -109,7 +110,7 @@ class CCManager:
                  scrub_mode: Optional[str] = None, scrub_bytes: Optional[int] = None,
                  max_parallel: Optional[int] = None, scrub_check: Optional[str] = None,
                  scrub_residue: Optional[str] = None, scrub_triage: Optional[str] = None,
-                 scrub_mismatch_triage: Optional[str] = None):
+                 scrub_mismatch_triage: Optional[str] = None, scrub_proof: Optional[str] = None):
         env = os.environ
         self.operator_namespace = env.get("OPERATOR_NAMESPACE", "gpu-operator")
         self.evict_operator_components = env.get("EVICT_OPERATOR_COMPONENTS", "true").lower() == "true"
@@ -170,6 +171,14 @@ class CCManager:
         if self.scrub_mismatch_triage == "report" and self.scrub_check != "tagged":
             raise ValueError("CC_SCRUB_MISMATCH_TRIAGE=report triages what the tagged check finds: it needs "
                              f"CC_SCRUB_CHECK=tagged, not {self.scrub_check!r}")
+        # off:     the gate's verdict rests on what its kernels counted.
+        # require: every pass of the gate also counts, on the device, the bytes it walked on every 2 MiB page, and a GPU
+        #          on which a pass missed or repeated a byte fails the gate (ccm_scrub_prove, DESIGN.md §5h).  A check,
+        #          not a report: a device that cannot prove its coverage fails the gate.  Logged and kept in
+        #          last_transition["scrub_cover"].
+        self.scrub_proof = (scrub_proof or env.get("CC_SCRUB_PROOF", "off")).lower()
+        if self.scrub_proof not in PROOF_MODES:
+            raise ValueError(f"CC_SCRUB_PROOF must be 'off' or 'require', not {self.scrub_proof!r}")
         self.max_parallel = int(max_parallel if max_parallel is not None else env.get("CC_MAX_PARALLEL", "0"))
         # "full-HBM" is enforced, not assumed: when scrubbing everything (scrub_bytes == 0) a GPU on
         # which less than this fraction of DEVICE memory was zeroed and read back fails the gate
@@ -559,6 +568,8 @@ class CCManager:
             cmd += ["--triage", "--triage-hold-ms", str(SCRUB_TRIAGE_HOLD_MS)]
         if self.mismatch_triage:
             cmd += ["--mismatch-triage"] + ([] if self.triage else ["--triage-hold-ms", str(SCRUB_TRIAGE_HOLD_MS)])
+        if self.prove:
+            cmd += ["--prove"]
         for gpu in gpus:
             cmd += ["--bdf", gpu.bdf]
         env = dict(os.environ)
@@ -572,6 +583,29 @@ class CCManager:
         payload = _json.loads(lines[-1])
         return [_devices.ScrubReport.from_json(r) for r in payload["reports"]]
 
+    @property
+    def prove(self) -> bool:
+        return self.scrub_proof == "require"
+
+    def _scrub_call(self, gpu, **kwargs):
+        """The one call every per-device gate path makes: with CC_SCRUB_PROOF=require it also asks for the coverage
+        proof.  A device whose scrub_and_verify cannot take `prove` fails the gate: it is never scrubbed unproven in its
+        place."""
+        if self.prove:
+            kwargs["prove"] = True
+            try:
+                inspect.signature(gpu.scrub_and_verify).bind(self.scrub_bytes, **kwargs)
+            except (TypeError, ValueError):
+                raise ScrubFailure(f"device {gpu.bdf} cannot prove its HBM coverage (CC_SCRUB_PROOF=require); refusing "
+                                   "to release it") from None
+        return gpu.scrub_and_verify(self.scrub_bytes, **kwargs)
+
+    def _scrub_many(self, natives: list, **kwargs):
+        """The one native fan-out call of the gate, with the coverage proof under CC_SCRUB_PROOF=require."""
+        if self.prove:
+            kwargs["prove"] = True
+        return _devices.scrub_and_verify_many(natives, self.scrub_bytes, **kwargs)
+
     def _scrub_checked(self, gpu):
         """The tagged gate on one device.  A device that cannot run it fails the gate: it is never
         scrubbed zero-only in its place."""
@@ -580,7 +614,7 @@ class CCManager:
         except (TypeError, ValueError):
             raise ScrubFailure(f"device {gpu.bdf} cannot run the {self.scrub_check} HBM check "
                                f"(CC_SCRUB_CHECK={self.scrub_check}); refusing to release it") from None
-        rep = gpu.scrub_and_verify(self.scrub_bytes, check=self.scrub_check)
+        rep = self._scrub_call(gpu, check=self.scrub_check)
         if getattr(rep, "check", "zero") != self.scrub_check:
             raise ScrubFailure(f"device {gpu.bdf} returned a {getattr(rep, 'check', 'zero')} scrub report for "
                                f"CC_SCRUB_CHECK={self.scrub_check}; refusing to release it")
@@ -599,7 +633,7 @@ class CCManager:
             logger.warning("Device %s cannot report HBM residue (CC_SCRUB_RESIDUE=report): its gate runs without "
                            "the census", gpu.bdf)
             return self._scrub_one(gpu, census=False)
-        return gpu.scrub_and_verify(self.scrub_bytes, check=self.scrub_check, residue=True)
+        return self._scrub_call(gpu, check=self.scrub_check, residue=True)
 
     @property
     def triage(self) -> bool:
@@ -618,7 +652,7 @@ class CCManager:
             logger.warning("Device %s cannot triage HBM dirt (CC_SCRUB_TRIAGE=report): its gate runs without the "
                            "triage", gpu.bdf)
             return self._scrub_one(gpu, census)
-        rep = gpu.scrub_and_verify(self.scrub_bytes, **kwargs)
+        rep = self._scrub_call(gpu, **kwargs)
         if getattr(rep, "check", "zero") != self.scrub_check:   # as _scrub_checked: never zero-only in its place
             raise ScrubFailure(f"device {gpu.bdf} returned a {getattr(rep, 'check', 'zero')} scrub report for "
                                f"CC_SCRUB_CHECK={self.scrub_check}; refusing to release it")
@@ -642,7 +676,7 @@ class CCManager:
             logger.warning("Device %s cannot triage HBM tag mismatches (CC_SCRUB_MISMATCH_TRIAGE=report): its gate "
                            "runs without the mismatch triage", gpu.bdf)
             return self._scrub_with_triage(gpu, self.census) if self.triage else self._scrub_one(gpu, self.census)
-        rep = gpu.scrub_and_verify(self.scrub_bytes, **kwargs)
+        rep = self._scrub_call(gpu, **kwargs)
         if getattr(rep, "check", "zero") != self.scrub_check:   # as _scrub_checked: never zero-only in its place
             raise ScrubFailure(f"device {gpu.bdf} returned a {getattr(rep, 'check', 'zero')} scrub report for "
                                f"CC_SCRUB_CHECK={self.scrub_check}; refusing to release it")
@@ -652,7 +686,7 @@ class CCManager:
         if census:
             return self._scrub_with_residue(gpu)
         if self.scrub_check == "zero":
-            return gpu.scrub_and_verify(self.scrub_bytes)   # the call every scrubbing device takes
+            return self._scrub_call(gpu)   # the call every scrubbing device takes
         return self._scrub_checked(gpu)
 
     # The window reports a scrub report or GpuError may carry, in the order they are logged: (attribute, key of
@@ -679,7 +713,13 @@ class CCManager:
 
     def _note_reports(self, bdf: str, holder) -> None:
         """Logs every window report `holder` carries and keeps it in last_transition: the gate hands the memory back
-        right after the verdict, so this is the only look anyone gets at it."""
+        right after the verdict, so this is the only look anyone gets at it.  The coverage proof comes first: INFO when
+        every pass covered every byte, ERROR naming the short pass and its pages when not."""
+        cover = getattr(holder, "cover", None)
+        if cover is not None:
+            self.last_transition.setdefault("scrub_cover", {})[bdf] = cover
+            logger.log(logging.INFO if cover.covered else logging.ERROR, "HBM coverage proof on %s: %s", bdf,
+                       cover.summary())
         for attr, key, level, line in self._REPORT_NOTES + self._TRIAGE_NOTES:
             report = getattr(holder, attr, None)
             if report is not None:
@@ -701,20 +741,18 @@ class CCManager:
                 extra = {"residue": True} if self.census else {}
                 if self.triage:
                     extra["triage"] = True
-                reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes, check=self.scrub_check,
-                                                            triage_hold_ms=SCRUB_TRIAGE_HOLD_MS, mismatch_triage=True,
-                                                            **extra)
+                reports, _ = self._scrub_many(natives, check=self.scrub_check, triage_hold_ms=SCRUB_TRIAGE_HOLD_MS,
+                                              mismatch_triage=True, **extra)
             elif self.triage:
                 extra = {"residue": True} if self.census else {}
-                reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes, check=self.scrub_check,
-                                                            triage=True, triage_hold_ms=SCRUB_TRIAGE_HOLD_MS, **extra)
+                reports, _ = self._scrub_many(natives, check=self.scrub_check, triage=True,
+                                              triage_hold_ms=SCRUB_TRIAGE_HOLD_MS, **extra)
             elif self.census:
-                reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes, check=self.scrub_check,
-                                                            residue=True)
+                reports, _ = self._scrub_many(natives, check=self.scrub_check, residue=True)
             elif self.scrub_check == "zero":
-                reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes)
+                reports, _ = self._scrub_many(natives)
             else:
-                reports, _ = _devices.scrub_and_verify_many(natives, self.scrub_bytes, check=self.scrub_check)
+                reports, _ = self._scrub_many(natives, check=self.scrub_check)
             for rep, gpu in zip(reports, gpus):
                 rep.bdf = gpu.bdf
         else:
@@ -743,7 +781,12 @@ class CCManager:
                     f"HBM scrub failed on {rep.bdf}: status={rep.status} "
                     f"nonzero_bytes={rep.nonzero_bytes} of {rep.bytes_scrubbed}"
                     + (f" mismatch_bytes={mismatch} (bytes that did not hold their address tag)"
-                       if self.scrub_check == "tagged" else ""))
+                       if self.scrub_check == "tagged" else "")
+                    + (" (a pass did not walk every mapped byte exactly once: see the coverage proof)"
+                       if rep.status == _devices.N.ERR_UNCOVERED else ""))
+            if self.prove and getattr(rep, "cover", None) is None:
+                raise ScrubFailure(f"HBM scrub on {rep.bdf} carries no coverage proof (CC_SCRUB_PROOF=require); "
+                                   "refusing to release it")
             if self.scrub_bytes == 0 and rep.coverage < self.scrub_min_coverage:
                 raise ScrubFailure(
                     f"HBM scrub on {rep.bdf} covered only {100 * rep.coverage:.2f}% of device memory "
@@ -1009,6 +1052,9 @@ def build_arg_parser() -> argparse.ArgumentParser:
                         help="with --scrub-check tagged, after a failed check, re-tag, check and re-read the pages off "
                              "their tags and report whether the mismatch stays, returns or clears (never changes the "
                              "verdict; default: $CC_SCRUB_MISMATCH_TRIAGE or off)")
+    parser.add_argument("--scrub-proof", default=None, choices=PROOF_MODES,
+                        help="require: every pass of the scrub gate counts the bytes it walked on every 2 MiB page, and "
+                             "a GPU whose pass missed or repeated a byte fails the gate (default: $CC_SCRUB_PROOF or off)")
     return parser
 
 
@@ -1034,7 +1080,7 @@ def main(argv: Optional[List[str]] = None) -> None:
         CCManager(node_name=args.node_name, default_mode=default_mode, host_cc=host_cc,
                   kubeconfig=args.kubeconfig, scrub_mode=args.scrub_mode, scrub_check=args.scrub_check,
                   scrub_residue=args.scrub_residue, scrub_triage=args.scrub_triage,
-                  scrub_mismatch_triage=args.scrub_mismatch_triage,
+                  scrub_mismatch_triage=args.scrub_mismatch_triage, scrub_proof=args.scrub_proof,
                   device_source=_device_source_from_env()).run()
     except KeyboardInterrupt:
         logger.info("Shutting down...")
