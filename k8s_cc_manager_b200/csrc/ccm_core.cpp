@@ -700,6 +700,8 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
   else if (k == "triage_stay") d.drill.triage_stay = v < 0 ? 0 : (uint64_t)v;
   else if (k == "triage_return") d.drill.triage_return = v < 0 ? 0 : (uint64_t)v;
   else if (k == "cover_skip") d.drill.cover_skip = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "probe_mismatch") d.drill.probe_mismatch = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "probe_dirt") d.drill.probe_dirt = v < 0 ? 0 : (uint64_t)v;
   else if (k == "cover_pass") {
     if (v < 0 || v > CCM_PASS_READBACK) { set_error("sim key 'cover_pass' takes 0..3, not %lld", (long long)v); return CCM_ERR_INVALID; }
     d.drill.cover_pass = v == 0 ? (int)CCM_PASS_READBACK : (int)v;
@@ -754,6 +756,8 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "tag_flood") *value = d.drill.tag_flood;
     else if (k == "cover_skip") *value = (int64_t)d.drill.cover_skip;
     else if (k == "cover_pass") *value = d.drill.cover_pass;
+    else if (k == "probe_mismatch") *value = (int64_t)d.drill.probe_mismatch;
+    else if (k == "probe_dirt") *value = (int64_t)d.drill.probe_dirt;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

@@ -15,6 +15,7 @@
 #include <functional>
 #include <memory>
 #include <mutex>
+#include <random>
 #include <string>
 #include <thread>
 #include <vector>
@@ -196,6 +197,10 @@ struct ScrubEngine {
   GatePasses gate;                          // the product call's passes, while it enqueues them
   ccm_cover_report cover{};                 // report of the last product call (ccm_scrub_last_cover)
   std::vector<ccm_cover_page> cover_pages;  // and its inexact pages (ccm_last_cover_pages)
+  bool probe_armed = false;                 // the alias probe is armed (ccm_scrub_probe)
+  bool probe_ready = false;                 // its kernels are resident
+  int probe_ctas[3] = {};                   // and how many CTAs of each step (P1, P2, P3) one SM holds at once
+  ccm_probe_report probe{};                 // report of the last product call (ccm_scrub_last_probe)
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -251,6 +256,13 @@ static constexpr int kCensusThreads = 512, kCensusPer = 16;
 #define CCM_COVER_TAG_CHECK cover_tag_check_pass<kTagThreads, kTagPer>
 #define CCM_COVER_CENSUS_ZERO cover_census_zero_pass<kCensusThreads, kCensusPer>
 #define CCM_COVER_CENSUS_TAG cover_census_tag_pass<kCensusThreads, kCensusPer>
+// The alias probe: 256-thread CTAs, 4 windows in flight per thread (scattered 32-byte sectors: the rate is set by how
+// many are in flight, not by the bytes).  Each step launches as many CTAs per SM as its registers let one SM hold at
+// once (ptxas on sm_90a: P1 31, P2 48, P3 45 registers, so 8, 5 and 5 CTAs), so a launch runs in one wave.
+static constexpr int kProbeThreads = 256, kProbePer = 4;
+#define CCM_PROBE_FILL alias_probe_fill_pass<kProbeThreads, kProbePer>
+#define CCM_PROBE_CHECK alias_probe_check_pass<kProbeThreads, kProbePer>
+#define CCM_PROBE_REREAD alias_probe_reread_pass<kProbeThreads, kProbePer>
 
 const char* default_kernel_names() {
   static const std::string names = [] {
@@ -375,6 +387,7 @@ int engine_teardown(int ordinal) {
   if (e->h_cover) cudaFreeHost(e->h_cover);
   e->d_cover = nullptr;
   e->h_cover = nullptr;
+  e->probe_ready = false;
   e->d_counter = nullptr;
   e->h_counter = nullptr;
   e->d_records = nullptr;
@@ -1179,6 +1192,143 @@ static void end_gate(ScrubEngine* e) {
   e->gate = GatePasses();
 }
 
+// ------------------------------------------------------------------ alias probe
+// Makes the probe kernels resident (a whole-HBM call cannot load a module once everything is mapped).  The caller
+// holds e->mu.
+static int ensure_probe(ScrubEngine* e) {
+  if (e->probe_ready) return CCM_OK;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  cudaFuncAttributes fa;
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_PROBE_FILL));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_PROBE_CHECK));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_PROBE_REREAD));
+  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e->probe_ctas[0], CCM_PROBE_FILL, kProbeThreads, 0));
+  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e->probe_ctas[1], CCM_PROBE_CHECK, kProbeThreads, 0));
+  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e->probe_ctas[2], CCM_PROBE_REREAD, kProbeThreads, 0));
+  for (int& c : e->probe_ctas) c = std::max(c, 1);
+  e->probe_ready = true;
+  return CCM_OK;
+}
+
+// The probe windows of [addr, addr + n): the first 4096-aligned address w0 whose 32 bytes lie inside, and how many
+// windows follow it at the stride.
+static void probe_windows_of(uint64_t addr, uint64_t n, uint64_t* w0, uint64_t* nwin) {
+  *w0 = (addr + kProbeStride - 1) & ~(kProbeStride - 1);
+  *nwin = *w0 + kProbeWindow <= addr + n ? (addr + n - kProbeWindow - *w0) / kProbeStride + 1 : 0;
+}
+
+// The alias probe (ccm.h: ccm_scrub_probe) over `chunks` (each with its offset in what the reports describe; the caller
+// holds e->mu, and every kernel of the call has finished): P1 over every chunk, the "probe_mismatch" drill, P2, the
+// "probe_dirt" drill, P3, one launch per chunk per step in order.  Fills *rep (probed = 1) and *p3 (P3's count); after
+// P2 mismatches, *mrep (classified against `spans`, chunk_of(offset)) and the mismatch page map.  After an error it
+// drops the check book.
+template <typename ChunkOf>
+static int run_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& chunks,
+                     const std::vector<CheckSpan>& spans, uint32_t seed, const ScrubDrill& drill, uint64_t va_base,
+                     ccm_probe_report* rep, ccm_mismatch_report* mrep, uint64_t* p3, ChunkOf&& chunk_of) {
+  memset(rep, 0, sizeof *rep);
+  rep->seed = seed;
+  rep->va_base = va_base;
+  // one launch of step k (0 = P1, 1 = P2, 2 = P3) per chunk with windows
+  auto step = [&](int k, auto&& launch) -> int {
+    const uint64_t max_grid = (uint64_t)e->sm_count * e->probe_ctas[k];
+    for (const CheckSpan& c : chunks) {
+      uint64_t w0 = 0, nwin = 0;
+      probe_windows_of(c.addr, c.bytes, &w0, &nwin);
+      if (nwin == 0) continue;
+      const uint64_t batches = (nwin + kProbeThreads * kProbePer - 1) / (kProbeThreads * kProbePer);
+      launch(w0, nwin, (int)std::min<uint64_t>(batches, max_grid), c.addr - c.offset);
+      g_launches++;
+      rep->launches++;
+      CCM_CUDA(cudaGetLastError());
+    }
+    return CCM_OK;
+  };
+  // drills: the first byte of each of the first k windows, in launch order
+  auto xor_windows = [&](uint64_t k) -> int {
+    for (const CheckSpan& c : chunks) {
+      uint64_t w0 = 0, nwin = 0;
+      probe_windows_of(c.addr, c.bytes, &w0, &nwin);
+      for (uint64_t i = 0; i < nwin && k; ++i, --k) {
+        xor_byte_kernel<<<1, 1, 0, st>>>((uint8_t*)(uintptr_t)(w0 + i * kProbeStride));
+        g_launches++;
+        rep->launches++;
+        CCM_CUDA(cudaGetLastError());
+      }
+    }
+    return CCM_OK;
+  };
+  int rc = CCM_OK;
+  float ms = 0;
+  auto run = [&]() -> int {
+    CCM_CUDA(cudaMemsetAsync(e->d_counter + kMismatch, 0, sizeof(unsigned long long), st));
+    CCM_CUDA(cudaMemsetAsync(e->d_counter + kNonzero, 0, sizeof(unsigned long long), st));
+    CCM_CUDA(cudaEventRecord(e->ev[0], st));
+    if (int r2 = step(0, [&](uint64_t w0, uint64_t n, int grid, uint64_t) {
+          CCM_PROBE_FILL<<<grid, kProbeThreads, 0, st>>>(w0, n, seed);
+        }))
+      return r2;
+    if (int r2 = xor_windows(drill.probe_mismatch)) return r2;
+    if (int r2 = step(1, [&](uint64_t w0, uint64_t n, int grid, uint64_t base) {
+          CCM_PROBE_CHECK<<<grid, kProbeThreads, 0, st>>>(w0, n, seed, e->d_counter + kMismatch, e->book_out(kCheckBook),
+                                                         base);
+        }))
+      return r2;
+    if (int r2 = xor_windows(drill.probe_dirt)) return r2;
+    if (int r2 = step(2, [&](uint64_t w0, uint64_t n, int grid, uint64_t) {
+          CCM_PROBE_REREAD<<<grid, kProbeThreads, 0, st>>>(w0, n, e->d_counter + kNonzero);
+        }))
+      return r2;
+    CCM_CUDA(cudaEventRecord(e->ev[1], st));
+    CCM_CUDA(cudaMemcpyAsync(e->h_counter, e->d_counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CCM_CUDA(cudaMemcpyAsync(e->h_counter + 1, e->d_counter + kMismatch, sizeof(unsigned long long),
+                             cudaMemcpyDeviceToHost, st));
+    CCM_CUDA(cudaStreamSynchronize(st));
+    CCM_CUDA(cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]));
+    return CCM_OK;
+  };
+  if ((rc = run()) != CCM_OK) { drop_book(e, kCheckBook, st); return rc; }
+  for (const CheckSpan& c : chunks) {
+    uint64_t w0 = 0, nwin = 0;
+    probe_windows_of(c.addr, c.bytes, &w0, &nwin);
+    rep->windows += nwin;
+  }
+  rep->bytes_probed = rep->windows * kProbeWindow;
+  rep->reread_nonzero_bytes = *p3 = (uint64_t)e->h_counter[0];
+  rep->mismatch_bytes = (uint64_t)e->h_counter[1];
+  rep->ms_probe = ms;
+  rep->probed = 1;
+  e->pages[kCheckBook].clear();
+  memset(mrep, 0, sizeof *mrep);
+  mrep->located = 1;
+  mrep->seed = seed;
+  mrep->va_base = va_base;
+  if (rep->mismatch_bytes != 0) {
+    if ((rc = take_mismatch(e, st, rep->mismatch_bytes, seed, va_base, spans, mrep, chunk_of)) != CCM_OK) {
+      drop_book(e, kCheckBook, st);
+      e->pages[kCheckBook].clear();
+      return rc;
+    }
+    rep->mismatch_windows = mrep->mismatch_windows;
+  }
+  return CCM_OK;
+}
+
+// The product call's probe: armed, zero gate, clean read-back.  A seed per call; e->probe and (after mismatches)
+// e->mismatch get the reports.
+template <typename ChunkOf>
+static int gate_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& chunks,
+                      const std::vector<CheckSpan>& spans, const ScrubDrill& drill, uint64_t va_base,
+                      ccm_probe_report* out, uint64_t* p3, ChunkOf&& chunk_of) {
+  const uint32_t seed = std::random_device{}();
+  ccm_mismatch_report mrep;
+  const int rc = run_probe(e, st, chunks, spans, seed, drill, va_base, out, &mrep, p3, chunk_of);
+  if (rc != CCM_OK) { memset(out, 0, sizeof *out); return rc; }
+  e->probe = *out;
+  if (out->mismatch_bytes != 0) e->mismatch = mrep;
+  return CCM_OK;
+}
+
 // ------------------------------------------------------------------ what kind of dirt
 // One contiguous piece of the dirty memory the triage re-zeroes and re-reads: `bytes` at device address `addr`,
 // `offset` bytes from the dirt report's va_base, inside span `span` of what the call mapped.
@@ -1672,6 +1822,18 @@ static int arena_cover(ScrubEngine* e, bool tagged, ccm_cover_report* out) {
                     [&](uint64_t o) { return segment_of(e->segs, o); });
 }
 
+// The alias probe of the fallback path, after its read-back: segment by segment, offsets into the concatenated
+// segments, chunk = segment index.  *nz = P3's count.
+static int arena_probe(ScrubEngine* e, const ScrubDrill& drill, ccm_probe_report* out, uint64_t* nz) {
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  int rc = need_arena(e); if (rc) return rc;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  const std::vector<CheckSpan> spans = arena_spans(e->segs);
+  return gate_probe(e, e->stream, spans, spans, drill, (uint64_t)(uintptr_t)e->segs.front().ptr, out, nz,
+                    [&](uint64_t o) { return segment_of(e->segs, o); });
+}
+
 // ------------------------------------------------------- VMM (driver API, lazy)
 // The product call maps HBM in chunks through the virtual-memory-management API so
 // that (a) the chunks sit in ONE contiguous virtual range (one verify launch) and (b)
@@ -1741,7 +1903,7 @@ static bool async_release_enabled() { return env_u64("CCM_ASYNC_RELEASE", 1) != 
 // * the verdict is returned as soon as the 8-byte count is on the host; cuMemUnmap/cuMemRelease
 //   (serialised node-wide by the driver) run on the engine's reaper thread.
 static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDrill& drill, bool node_fanout,
-                                  ccm_scrub_result* r, ccm_cover_report* cover) {
+                                  ccm_scrub_result* r, ccm_cover_report* cover, ccm_probe_report* probe) {
   const VmmApi& api = vmm();
   if (!api.ok) return CCM_ERR_UNSUPPORTED;
   std::lock_guard<std::mutex> g(e->mu);
@@ -1805,6 +1967,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   int tag_timed = 0;
   std::vector<std::pair<uint64_t, uint64_t>> deferred;  // tagged: main-zone ranges, checked after the last mapping
   std::vector<std::pair<uint64_t, uint32_t>> pieces;    // (offset, handle index) of every mapped piece, ascending
+  std::vector<CheckSpan> iters;                         // every iteration of the mapping loop, for the alias probe
   bool checked = false;                                 // tagged: a check was enqueued (its book may be non-zero)
   // Census call: the first pass over each mapping (the scrub, or the tag fill) is the census of the same range.
   ccm_residue_report* res = current_residue_call();
@@ -1891,6 +2054,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     }
     aliased |= alias != 0;
     m.mapped = off + n;
+    iters.push_back({(uint64_t)m.base + off, n, off});
     // fault drill: the previous tenant's data, in place before anything scrubs this chunk
     if (drill.poison) {
       cudaError_t perr = cudaMemsetAsync((void*)(m.base + off), drill.poison, n, st);
@@ -1967,6 +2131,12 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
                                [](uint64_t v, const std::pair<uint64_t, uint32_t>& pc) { return v < pc.first; });
     return it == pieces.begin() ? 0u : std::prev(it)->second;
   };
+  // ---- alias probe: armed zero gate whose read-back was clean, after the last read-back -----------------------
+  if (rc == CCM_OK && probe && r->nonzero_bytes == 0 && mapped) {
+    uint64_t p3 = 0;
+    rc = gate_probe(e, st, iters, {{(uint64_t)m.base, mapped, 0}}, drill, (uint64_t)m.base, probe, &p3, chunk_of);
+    if (rc == CCM_OK) r->nonzero_bytes = p3;
+  }
   // ---- coverage proof: one copy of the cover maps, no launch ------------------------------------------------
   if (rc == CCM_OK && e->gate.prove) rc = take_cover(e, st, mapped, (uint64_t)m.base, tag != nullptr, cover, chunk_of);
   // ---- a failed tagged check: where were the tags wrong?  The checks booked it; one copy, no launch ---------
@@ -2034,7 +2204,8 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   drill.inject = inject;
   ccm_tag_result* tag = current_tag_call();
   ccm_residue_report* res = current_residue_call();
-  bool prove = false;
+  bool prove = false, probe_armed = false;
+  int probe_rc = CCM_OK;   // an armed device whose probe kernels cannot be made resident runs no call
   {
     std::lock_guard<std::mutex> g(e->mu);
     memset(&e->dirt, 0, sizeof e->dirt);  // every call replaces the reports of the last one
@@ -2048,7 +2219,11 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     if (res) e->pages[kCensusBook].clear();
     memset(&e->cover, 0, sizeof e->cover);
     e->cover_pages.clear();
+    memset(&e->probe, 0, sizeof e->probe);
     prove = e->prove;
+    // the alias probe is for the zero gate: a tagged call's check already covers every window
+    probe_armed = e->probe_armed && tag == nullptr;
+    if (probe_armed) probe_rc = ensure_probe(e);
   }
   ccm_scrub_result r;
   memset(&r, 0, sizeof r);
@@ -2058,10 +2233,18 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   // and so does a proving call, with the proving twins of the default kernels
   r.scrub_variant = res || prove ? CCM_SCRUB_ST128 : resolve_scrub_variant(CCM_SCRUB_AUTO);
   r.verify_variant = prove ? CCM_VERIFY_LD128 : resolve_verify_variant(CCM_VERIFY_AUTO);
+  if (probe_rc != CCM_OK) {
+    r.status = probe_rc;
+    if (out) *out = r;
+    return probe_rc;
+  }
   int rc = CCM_ERR_UNSUPPORTED;
   ccm_cover_report cover;   // this call's own copy of the coverage report
   memset(&cover, 0, sizeof cover);
-  if (env_u64("CCM_PIPELINE", 1) != 0) rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r, &cover);
+  ccm_probe_report probe;   // and of the probe report
+  memset(&probe, 0, sizeof probe);
+  ccm_probe_report* probe_out = probe_armed ? &probe : nullptr;
+  if (env_u64("CCM_PIPELINE", 1) != 0) rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r, &cover, probe_out);
   if (rc == CCM_ERR_UNSUPPORTED) {
     // plain path: one cudaMalloc'ed arena, whole-arena scrub, whole-arena verify (the drills act per
     // segment: poison before the scrub, flood + inject between the scrub and the verify)
@@ -2092,6 +2275,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       }
       if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
       if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
+      if (rc == CCM_OK && probe_out && nz == 0) rc = arena_probe(e, drill, probe_out, &nz);
       if (rc == CCM_OK) rc = arena_cover(e, tag != nullptr, &cover);
       if (rc == CCM_OK && nz != 0) arena_locate(e, drill);
       if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) arena_triage_mismatch(e, tag->seed, drill);
@@ -2118,6 +2302,13 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   } else if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) {
     set_error("tagged scrub found %llu bytes that did not hold their tag (and %llu non-zero bytes after the zeroing) "
               "on CUDA device %d", (unsigned long long)tag->mismatch_bytes, (unsigned long long)r.nonzero_bytes, e->ordinal);
+    rc = CCM_ERR_MISMATCH;
+  } else if (rc == CCM_OK && probe.probed && probe.mismatch_bytes != 0) {
+    set_error("HBM alias probe found %llu bytes that did not hold their tag in %llu 16-byte windows of its %llu probe "
+              "windows (and %llu non-zero bytes after the zeroing) on CUDA device %d: a page is mapped twice or does not "
+              "keep what is stored to it", (unsigned long long)probe.mismatch_bytes,
+              (unsigned long long)probe.mismatch_windows, (unsigned long long)probe.windows,
+              (unsigned long long)r.nonzero_bytes, e->ordinal);
     rc = CCM_ERR_MISMATCH;
   } else if (rc == CCM_OK && r.nonzero_bytes != 0) {
     set_error("scrub verify found %llu non-zero bytes on CUDA device %d", (unsigned long long)r.nonzero_bytes, e->ordinal);
@@ -2476,5 +2667,64 @@ extern "C" int ccm_last_cover_pages(int cuda_ordinal, ccm_cover_page* out, uint6
   std::lock_guard<std::mutex> g(e->mu);
   *n = e->cover_pages.size();
   if (cap) memcpy(out, e->cover_pages.data(), std::min<uint64_t>(cap, *n) * sizeof(ccm_cover_page));
+  return CCM_OK;
+}
+
+// ------------------------------------------------------------------------- alias probe
+static_assert(sizeof(ccm_probe_report) == 80 && offsetof(ccm_probe_report, seed) == 40 &&
+              offsetof(ccm_probe_report, va_base) == 48 && offsetof(ccm_probe_report, probed) == 64 &&
+              CCM_PROBE_STRIDE == kProbeStride && CCM_PROBE_WINDOW == kProbeWindow,
+              "ccm_probe_report keeps its layout, and the windows their place and size");
+
+extern "C" int ccm_scrub_probe(int cuda_ordinal, int on) {
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  // disarming an engine that was never created leaves nothing armed (and starts no context)
+  ScrubEngine* e = on ? engine_for(cuda_ordinal) : engine_lookup(cuda_ordinal);
+  if (!e) return on ? CCM_ERR_NO_CUDA : CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  if (on) {
+    CCM_ENSURE_READY(e);
+    if (int rc = ensure_probe(e)) return rc;
+  }
+  e->probe_armed = on != 0;
+  return CCM_OK;
+}
+
+extern "C" int ccm_scrub_last_probe(int cuda_ordinal, ccm_probe_report* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  *out = e->probe;
+  return CCM_OK;
+}
+
+extern "C" int ccm_region_probe(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream,
+                                ccm_probe_report* out, ccm_mismatch_report* mismatch) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  if (mismatch) memset(mismatch, 0, sizeof *mismatch);
+  ScrubEngine* e = engine_for(cuda_ordinal);
+  if (!e) return CCM_ERR_NO_CUDA;
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  if (int rc = ensure_probe(e)) return rc;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  const uint64_t base = (uint64_t)(uintptr_t)dptr;
+  const std::vector<CheckSpan> spans{{base, bytes, 0}};
+  ccm_mismatch_report rep;
+  uint64_t p3 = 0;
+  const int rc = run_probe(e, e->pick(stream), spans, spans, seed, ScrubDrill(), base, out, &rep, &p3,
+                           [](uint64_t) { return 0u; });
+  if (rc != CCM_OK) { memset(out, 0, sizeof *out); return rc; }
+  if (mismatch) *mismatch = rep;
   return CCM_OK;
 }

@@ -1,7 +1,7 @@
 // ccm-scrub — native command-line front end of the HBM scrub gate (links libccm.so).
 //
 //   ccm-scrub [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] [--triage]
-//             [--mismatch-triage] [--triage-hold-ms MS] [--prove] (--all | --bdf <pci address> ...)
+//             [--mismatch-triage] [--triage-hold-ms MS] [--prove] [--probe] (--all | --bdf <pci address> ...)
 //
 // Runs the concurrent gate (ccm_scrub_verify_many, or ccm_scrub_verify_many_tagged with --check tagged)
 // and prints ONE JSON line with the same fields as k8s_cc_manager_b200.devices.ScrubReport (the
@@ -15,8 +15,10 @@
 // (ccm_scrub_mismatch_triage), for a GPU whose tagged check found bytes off their tags: what kind of mismatch, as
 // ccm_scrub_last_mismatch_triage and ccm_last_mismatch_triage_pages report it; "cover" with --prove, which arms every
 // GPU for the coverage proof (ccm_scrub_prove), for every GPU whose passes finished, as ccm_scrub_last_cover and
-// ccm_last_cover_pages report it).  With --prove, a GPU that cannot be armed is never scrubbed unproven: nothing is
-// scrubbed and the exit code is 3.
+// ccm_last_cover_pages report it; "probe" with --probe, which refuses --check tagged and arms every GPU for the alias
+// probe (ccm_scrub_probe), for every GPU whose probe ran, as ccm_scrub_last_probe reports it, with "mismatch" when it
+// found bytes off their tags).  With --prove or --probe, a GPU that cannot be armed is never scrubbed without: nothing
+// is scrubbed and the exit code is 3.
 // Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
@@ -227,14 +229,25 @@ static void print_mismatch_triage(const ccm_triage_report& t, int ordinal) {
 
 static int usage(const char* argv0) {
   fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] "
-          "[--triage] [--mismatch-triage] [--triage-hold-ms MS] [--prove] (--all | --bdf <bdf> ...)\n", argv0);
+          "[--triage] [--mismatch-triage] [--triage-hold-ms MS] [--prove] [--probe] (--all | --bdf <bdf> ...)\n", argv0);
   return 2;
+}
+
+// The "probe" object: the fields of k8s_cc_manager_b200.devices.ProbeReport.
+static void print_probe(const ccm_probe_report& p) {
+  printf(", \"probe\": {\"windows\": %llu, \"bytes_probed\": %llu, \"mismatch_bytes\": %llu, \"mismatch_windows\": %llu, "
+         "\"reread_nonzero_bytes\": %llu, \"seed\": %u, \"launches\": %u, \"va_base\": %llu, \"ms_probe\": %.3f, "
+         "\"probed\": %d}",
+         (unsigned long long)p.windows, (unsigned long long)p.bytes_probed, (unsigned long long)p.mismatch_bytes,
+         (unsigned long long)p.mismatch_windows, (unsigned long long)p.reread_nonzero_bytes, p.seed, p.launches,
+         (unsigned long long)p.va_base, p.ms_probe, p.probed);
 }
 
 int main(int argc, char** argv) {
   std::vector<std::string> bdfs;
   unsigned long long bytes = 0;
-  bool all = false, tagged = false, residue = false, triage = false, mismatch_triage = false, prove = false;
+  bool all = false, tagged = false, residue = false, triage = false, mismatch_triage = false, prove = false,
+       probe = false;
   unsigned long triage_hold_ms = 100;   // k8s_cc_manager_b200.devices.TRIAGE_HOLD_MS
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
@@ -243,6 +256,7 @@ int main(int argc, char** argv) {
     else if (a == "--triage") triage = true;
     else if (a == "--mismatch-triage") mismatch_triage = true;
     else if (a == "--prove") prove = true;
+    else if (a == "--probe") probe = true;
     else if (a == "--triage-hold-ms" && i + 1 < argc) {
       triage_hold_ms = strtoul(argv[++i], nullptr, 10);
       if (triage_hold_ms == 0 || triage_hold_ms > CCM_TRIAGE_MAX_HOLD_MS) return usage(argv[0]);
@@ -263,6 +277,10 @@ int main(int argc, char** argv) {
   if (!all && bdfs.empty()) return usage(argv[0]);
   if (mismatch_triage && !tagged) {
     fprintf(stderr, "--mismatch-triage needs --check tagged\n");
+    return usage(argv[0]);
+  }
+  if (probe && tagged) {
+    fprintf(stderr, "--probe is for --check zero: the tagged check already covers every probe window\n");
     return usage(argv[0]);
   }
 
@@ -305,6 +323,17 @@ int main(int argc, char** argv) {
     }
     parmed.push_back(ordinals[i]);
   }
+  std::vector<int> probed;   // ordinals armed for the alias probe: all of them, or the gate does not run
+  for (size_t i = 0; probe && i < ordinals.size(); ++i) {
+    const int rc = ordinals[i] >= 0 ? ccm_scrub_probe(ordinals[i], 1) : CCM_ERR_NO_CUDA;
+    if (rc != CCM_OK) {
+      fprintf(stderr, "cannot arm the alias probe on %s: %s\n", names[i].c_str(), ccm_strerror(rc));
+      for (int o : probed) ccm_scrub_probe(o, 0);
+      for (int o : parmed) ccm_scrub_prove(o, 0);
+      return 3;
+    }
+    probed.push_back(ordinals[i]);
+  }
   std::vector<int> armed;   // ordinals armed for the triage, disarmed once the gate is done
   for (size_t i = 0; triage && i < ordinals.size(); ++i)
     if (ordinals[i] >= 0 && ccm_scrub_triage(ordinals[i], (uint32_t)triage_hold_ms) == CCM_OK) armed.push_back(ordinals[i]);
@@ -320,6 +349,7 @@ int main(int argc, char** argv) {
   for (int o : armed) ccm_scrub_triage(o, 0);
   for (int o : marmed) ccm_scrub_mismatch_triage(o, 0);
   for (int o : parmed) ccm_scrub_prove(o, 0);
+  for (int o : probed) ccm_scrub_probe(o, 0);
   bool clean = true;
   printf("{\"wall_ms\": %.3f, \"reports\": [", wall_ms);
   for (size_t i = 0; i < devs.size(); ++i) {
@@ -341,8 +371,12 @@ int main(int argc, char** argv) {
     }
     ccm_dirt_report d;
     if (r.nonzero_bytes != 0 && ccm_scrub_last_dirt(ordinals[i], &d) == CCM_OK) print_dirt(d, ordinals[i]);
+    ccm_probe_report pr;
+    const bool ran_probe = probe && ccm_scrub_last_probe(ordinals[i], &pr) == CCM_OK && pr.probed;
     ccm_mismatch_report m;
     if (tagged && tags[i].mismatch_bytes != 0 && ccm_scrub_last_mismatch(ordinals[i], &m) == CCM_OK) print_mismatch(m, ordinals[i]);
+    // --probe refuses --check tagged: at most one of the two prints the mismatch report
+    if (ran_probe && pr.mismatch_bytes != 0 && ccm_scrub_last_mismatch(ordinals[i], &m) == CCM_OK) print_mismatch(m, ordinals[i]);
     if (residue) print_residue(census[i], ordinals[i]);
     ccm_triage_report t;
     if (triage && r.nonzero_bytes != 0 && ccm_scrub_last_triage(ordinals[i], &t) == CCM_OK && t.triaged)
@@ -354,6 +388,7 @@ int main(int argc, char** argv) {
     const bool proved = prove && ccm_scrub_last_cover(ordinals[i], &c) == CCM_OK && c.proved;
     if (proved) print_cover(c, ordinals[i]);
     clean = clean && (!prove || proved);   // a proof that was asked for and did not run fails the gate
+    if (ran_probe) print_probe(pr);
     printf("}");
   }
   printf("]}\n");

@@ -1294,6 +1294,141 @@ cover_census_tag_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t see
   op.book.flush();
 }
 
+// ------------------------------------------------------------ alias probe
+// Two virtual views of one physical page both read back zero, so the zero gate cannot see them.  An alias is a
+// page-table event, so one known-answer window per 4 KiB page (the smallest page the MMU maps) is enough to catch it:
+// the later view's tags overwrite the earlier view's tags in the shared page.  A probe WINDOW is the 32-byte sector at
+// a 4096-aligned address; its position depends only on the address modulo 4096, so two views of one physical page
+// probe the same sector.  One launch covers the windows w0 + i * kProbeStride, i < nwin, of one mapped chunk (the host
+// computes w0, the chunk's first window, and nwin).  As the proving twins, the three kernels' names do not end in
+// `kernel`, so the existing kernel-name checks do not list them; tests/test_alias_probe_gpu.py launches all three.
+constexpr uint64_t kProbeStride = 4096;
+constexpr uint32_t kProbeWindow = 32;
+
+// Batches of THREADS * PER windows, window i of a batch on lane i % THREADS, PER windows in flight per thread; the
+// windows after the last whole batch one per thread.  op.batch<K>(a, step) takes the K windows a, a + step, ...
+template <int THREADS, int PER, typename Op>
+__device__ __forceinline__ void probe_windows(uint64_t w0, uint64_t nwin, Op& op) {
+  constexpr uint64_t kBatch = (uint64_t)THREADS * PER;
+  const uint64_t nbatch = nwin / kBatch;
+  for (uint64_t b = blockIdx.x; b < nbatch; b += gridDim.x)
+    op.template batch<PER>(w0 + (b * kBatch + threadIdx.x) * kProbeStride, (uint64_t)THREADS * kProbeStride);
+  for (uint64_t i = nbatch * kBatch + (uint64_t)blockIdx.x * THREADS + threadIdx.x; i < nwin;
+       i += (uint64_t)gridDim.x * THREADS)
+    op.template batch<1>(w0 + i * kProbeStride, 0);
+}
+
+// P1: the tags of `seed` into every window (two 16-byte stores).
+struct ProbeFillOp {
+  uint32_t seed;
+  template <int K>
+  __device__ __forceinline__ void batch(uint64_t a, uint64_t step) {
+#pragma unroll
+    for (int u = 0; u < K; ++u) {
+      const uint64_t q = a + u * step;
+      st16((void*)(uintptr_t)q, tag_vec(seed, q));
+      st16((void*)(uintptr_t)(q + 16), tag_vec(seed, q + 16));
+    }
+  }
+};
+
+// P2: every window checked against its tags, then zeroed.  All loads are issued first and the exact count of bytes
+// off their tags is branch-free; only a batch whose count is non-zero takes the branch, which books each 16-byte half
+// with the tag check's rules (TagCheckZeroOp::single: mask, record while slots last, page map by warp reduction).
+struct ProbeCheckOp {
+  TagCheckZeroOp op;   // seed, book, base, cnt
+  template <int K>
+  __device__ __forceinline__ void batch(uint64_t a, uint64_t step) {
+    uint4 v[K][2];
+#pragma unroll
+    for (int u = 0; u < K; ++u) {
+      v[u][0] = ld16_cs((const void*)(uintptr_t)(a + u * step));
+      v[u][1] = ld16_cs((const void*)(uintptr_t)(a + u * step + 16));
+    }
+    uint32_t n = 0;
+#pragma unroll
+    for (int u = 0; u < K; ++u)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint4 t = tag_vec(op.seed, a + u * step + 16 * h);
+        n += nonzero_bytes_in_word(v[u][h].x ^ t.x) + nonzero_bytes_in_word(v[u][h].y ^ t.y) +
+             nonzero_bytes_in_word(v[u][h].z ^ t.z) + nonzero_bytes_in_word(v[u][h].w ^ t.w);
+      }
+    if (n != 0) {
+      // The branch reads the batch's windows again, one at a time: they come from L2 (this thread loaded them a moment
+      // ago) and nothing has stored over them yet, so the loaded words die before it, as in TagCheckZeroOp::chunk.
+      // Keeping them live through the eight bookings would take the registers of two more CTAs per SM.
+#pragma unroll 1
+      for (int u = 0; u < K; ++u)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t q = a + u * step + 16 * h;
+          const uint4 x = ld16_cs((const void*)(uintptr_t)q);
+          op.single(q - op.base, TagCheckZeroOp::diff_mask(x, tag_vec(op.seed, q)), Vec16{{x.x, x.y, x.z, x.w}});
+        }
+    }
+#pragma unroll
+    for (int u = 0; u < K; ++u) {
+      st16((void*)(uintptr_t)(a + u * step), make_uint4(0, 0, 0, 0));
+      st16((void*)(uintptr_t)(a + u * step + 16), make_uint4(0, 0, 0, 0));
+    }
+    op.cnt += n;
+  }
+};
+
+// P3: the non-zero bytes of every window (OR first; the exact count only for a batch that is not all zero).
+struct ProbeRereadOp {
+  uint64_t cnt = 0;
+  template <int K>
+  __device__ __forceinline__ void batch(uint64_t a, uint64_t step) {
+    Vec16 v[K][2];
+#pragma unroll
+    for (int u = 0; u < K; ++u) {
+      v[u][0] = ld16<kPolStreaming>((const void*)(uintptr_t)(a + u * step), 0);
+      v[u][1] = ld16<kPolStreaming>((const void*)(uintptr_t)(a + u * step + 16), 0);
+    }
+    uint32_t any = 0;
+#pragma unroll
+    for (int u = 0; u < K; ++u)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) any |= v[u][0].w[k] | v[u][1].w[k];
+    if (any != 0) {
+      uint32_t n = 0;
+#pragma unroll
+      for (int u = 0; u < K; ++u)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) n += nonzero_bytes_in_word(v[u][0].w[k]) + nonzero_bytes_in_word(v[u][1].w[k]);
+      cnt += n;
+    }
+  }
+};
+
+template <int THREADS, int PER>
+__global__ void __launch_bounds__(THREADS)
+alias_probe_fill_pass(uint64_t w0, uint64_t nwin, uint32_t seed) {
+  ProbeFillOp op{seed};
+  probe_windows<THREADS, PER>(w0, nwin, op);
+}
+
+// Bytes off their tags into *mismatch (one atomic per CTA), the windows that differ into `out` with offsets from `base`.
+template <int THREADS, int PER>
+__global__ void __launch_bounds__(THREADS)
+alias_probe_check_pass(uint64_t w0, uint64_t nwin, uint32_t seed, unsigned long long* mismatch, LocateOut out,
+                         uint64_t base) {
+  ProbeCheckOp op{{seed, {out}, base}};
+  probe_windows<THREADS, PER>(w0, nwin, op);
+  op.op.book.flush();
+  block_accumulate(op.op.cnt, mismatch);
+}
+
+template <int THREADS, int PER>
+__global__ void __launch_bounds__(THREADS)
+alias_probe_reread_pass(uint64_t w0, uint64_t nwin, unsigned long long* nonzero) {
+  ProbeRereadOp op;
+  probe_windows<THREADS, PER>(w0, nwin, op);
+  block_accumulate(op.cnt, nonzero);
+}
+
 // ------------------------------------------------------------ test scaffolding
 __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
   x += 0x9E3779B97F4A7C15ull;

@@ -33,7 +33,8 @@ class GpuError(Exception):
     MismatchReport as `.mismatch`; a census call carries its ResidueReport (what the first pass erased) as
     `.residue`; a triage call that read back dirt carries its TriageReport (what kind of dirt) as `.triage`; a mismatch
     triage call whose tagged check failed carries its TriageReport (what kind of mismatch) as `.mismatch_triage`; a
-    proving call carries its CoverReport (how many bytes each pass walked on every page) as `.cover`."""
+    proving call carries its CoverReport (how many bytes each pass walked on every page) as `.cover`; a probing call
+    carries its ProbeReport (what the alias probe found) as `.probe`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
@@ -625,9 +626,81 @@ def _arm_prove(cuda_ordinal: int, on: bool) -> int:
     return N.lib().ccm_scrub_prove(cuda_ordinal, int(on)) if cuda_ordinal >= 0 else N.ERR_NO_CUDA
 
 
+@dataclass
+class ProbeReport:
+    """The alias probe of one product call (include/ccm.h: ccm_probe_report): one 32-byte window per 4 KiB page of
+    every mapped chunk was tagged (P1), checked and zeroed (P2), and read for zeros (P3).  A page mapped twice shows as
+    bytes off their tags (mismatch_bytes; where they are comes as the call's `.mismatch`)."""
+    windows: int
+    bytes_probed: int
+    mismatch_bytes: int
+    mismatch_windows: int      # 16-byte windows of the mismatch report
+    reread_nonzero_bytes: int
+    seed: int
+    launches: int
+    va_base: int
+    ms_probe: float
+    probed: int
+
+    @classmethod
+    def from_native(cls, r: N.ProbeReport) -> "ProbeReport":
+        return cls(*(getattr(r, f) for f, _ in N.ProbeReport._fields_ if f != "reserved"))
+
+    @classmethod
+    def from_json(cls, d: dict) -> "ProbeReport":
+        return cls(**d)
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    @property
+    def held(self) -> bool:
+        """Every window held its tags and read back zero."""
+        return self.mismatch_bytes == 0 and self.reread_nonzero_bytes == 0
+
+    def summary(self) -> str:
+        """One line for an operator."""
+        line = f"{self.windows} windows ({self.bytes_probed} bytes) in {self.ms_probe:.2f} ms"
+        if self.held:
+            return line + ": every window held its tags and read back zero"
+        return (line + f": {self.mismatch_bytes} bytes off their tags in {self.mismatch_windows} 16-byte windows, "
+                f"{self.reread_nonzero_bytes} non-zero bytes after the zeroing")
+
+
+def last_probe(cuda_ordinal: int) -> "Optional[ProbeReport]":
+    """The alias probe report of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_probe); None
+    when it cannot be read."""
+    out = N.ProbeReport()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_probe(cuda_ordinal, C.byref(out)) != N.OK:
+        return None
+    return ProbeReport.from_native(out)
+
+
+def _arm_probe(cuda_ordinal: int, on: bool) -> int:
+    """Arms or disarms the alias probe on a CUDA device; the library's status."""
+    return N.lib().ccm_scrub_probe(cuda_ordinal, int(on)) if cuda_ordinal >= 0 else N.ERR_NO_CUDA
+
+
+def _probe_check(probe: bool, check: str) -> None:
+    """The alias probe is a check of the zero gate: the tagged check already covers every window."""
+    if probe and check == "tagged":
+        raise ValueError("probe=True is for check='zero': the tagged check already covers every probe window")
+
+
+def _attach_probe(rep: "ScrubReport", cuda_ordinal: int) -> None:
+    """The probe report of a call that probed, and where its tags were wrong when they were."""
+    report = last_probe(cuda_ordinal)
+    rep.probe = report if report is not None and report.probed else None
+    if rep.probe is not None and rep.probe.mismatch_bytes:
+        rep.mismatch = last_mismatch(cuda_ordinal)
+        if rep.mismatch is not None and rep.mismatch.mismatch_windows:
+            pages = last_page_map(cuda_ordinal, rep.mismatch.BOOK)
+            rep.mismatch.pages = pages.digest() if pages is not None else None
+
+
 # The reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
 _REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport),
-            ("mismatch_triage", TriageReport), ("cover", CoverReport))
+            ("mismatch_triage", TriageReport), ("cover", CoverReport), ("probe", ProbeReport))
 
 
 @dataclass
@@ -675,6 +748,9 @@ class ScrubReport:
     # How many bytes each pass walked on every page (a CoverReport), set for every report of a proving call
     # (prove=True) whose passes finished.  Not a dataclass field either.
     cover = None
+    # What the alias probe found (a ProbeReport), set for every report of a probing call (probe=True) that probed: one
+    # whose read-back was clean.  Not a dataclass field either.
+    probe = None
 
     @property
     def clean(self) -> bool:
@@ -827,7 +903,7 @@ class NvidiaDevice:
     # -- NEW: HBM scrub-and-verify ---------------------------------------------
     def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
                          triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False,
-                         prove: bool = False) -> ScrubReport:
+                         prove: bool = False, probe: bool = False) -> ScrubReport:
         """Zero-fills and reads back this GPU's HBM (nbytes=0: all the context can map).
         check="tagged" first writes and checks an address-tagged known answer
         (include/ccm.h: ccm_scrub_verify_tagged).  residue=True runs the census in the first pass and attaches what
@@ -842,6 +918,10 @@ class NvidiaDevice:
         prove=True arms the coverage proof for this call (include/ccm.h: ccm_scrub_prove): every pass counts on the
         device the bytes it walked on each page, the report comes attached as `.cover`, and a pass that missed or
         repeated a byte fails the call with ERR_UNCOVERED.  A device that cannot be armed fails the call.
+        probe=True (check="zero" only, else ValueError) arms the alias probe for this call (include/ccm.h:
+        ccm_scrub_probe): after a clean read-back, one 32-byte window per 4 KiB page is tagged, checked and zeroed and
+        read for zeros; the report comes attached as `.probe`, and a window off its tags (a page mapped twice) fails
+        the call with ERR_MISMATCH and attaches where as `.mismatch`.  A device that cannot be armed fails the call.
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
         if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
@@ -852,11 +932,14 @@ class NvidiaDevice:
         if _check_mode(check):
             tag = N.TagResult()
         _mismatch_triage_check(mismatch_triage, check)
+        _probe_check(probe, check)
         hold = _triage_hold(triage_hold_ms) if triage or mismatch_triage else 0
         armed = marmed = False
         try:
             if prove:
                 _check(_arm_prove(self.cuda_ordinal, True), "scrub_and_verify (coverage proof)", self.bdf)
+            if probe:
+                _check(_arm_probe(self.cuda_ordinal, True), "scrub_and_verify (alias probe)", self.bdf)
             armed = triage and _arm_triage(self.cuda_ordinal, hold)
             marmed = mismatch_triage and _arm_mismatch_triage(self.cuda_ordinal, hold)
             if residue:
@@ -875,8 +958,12 @@ class NvidiaDevice:
                 _arm_mismatch_triage(self.cuda_ordinal, 0)
             if prove:
                 _arm_prove(self.cuda_ordinal, False)
+            if probe:
+                _arm_probe(self.cuda_ordinal, False)
         rep = ScrubReport.from_native(self.bdf, res, tag)
         _attach_reports(rep, self.cuda_ordinal, census, armed, marmed, prove)
+        if probe:
+            _attach_probe(rep, self.cuda_ordinal)
         if err is None and prove and rep.cover is None:   # a proof that was asked for and did not run
             err = GpuError(f"scrub_and_verify on {self.bdf}: the coverage proof did not run", N.ERR_UNCOVERED)
         if err is not None:
@@ -928,39 +1015,50 @@ def find_gpus() -> Tuple[List[NvidiaDevice], int]:
 def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
                           check: str = "zero", residue: bool = False, triage: bool = False,
                           triage_hold_ms: int = TRIAGE_HOLD_MS,
-                          mismatch_triage: bool = False, prove: bool = False) -> Tuple[List[ScrubReport], float]:
+                          mismatch_triage: bool = False, prove: bool = False,
+                          probe: bool = False) -> Tuple[List[ScrubReport], float]:
     """Concurrent multi-context scrub of several GPUs through ONE native call
     (ccm_scrub_verify_many: one host thread + primary context + stream per GPU, no
     peer access, no collective; check="tagged": ccm_scrub_verify_many_tagged; residue=True:
     ccm_scrub_verify_many_residue, each report with its `.residue`; triage=True: every GPU armed for the dirt
     triage, as in NvidiaDevice.scrub_and_verify; mismatch_triage=True: every GPU armed for the mismatch triage, as
     there; prove=True: every GPU armed for the coverage proof, and a GPU that cannot be armed is not scrubbed: its
-    report carries the arming's status).  Returns
+    report carries the arming's status; probe=True: every GPU armed for the alias probe, likewise).  Returns
     (reports, wall_ms); never raises for a per-device failure — inspect report.status /
     report.clean."""
     tagged = _check_mode(check)
     _mismatch_triage_check(mismatch_triage, check)
-    if prove:
-        refused = {}
-        for d in devices:
-            rc = _arm_prove(d.cuda_ordinal, True)
-            if rc != N.OK:
-                refused[d.index] = ScrubReport.from_native(d.bdf, N.ScrubResult(status=rc))
+    _probe_check(probe, check)
+    if prove or probe:
+        # every check asked for is armed on a device before it is scrubbed; a device that refuses one is not scrubbed
+        # (its report carries that arming's status, and no report of a call that did not run)
+        arms = [arm for on, arm in ((prove, _arm_prove), (probe, _arm_probe)) if on]
+        refused, armed = {}, []
         try:
-            reports, wall = scrub_and_verify_many([d for d in devices if d.index not in refused], nbytes, check,
-                                                  residue, triage, triage_hold_ms, mismatch_triage)
-        finally:
             for d in devices:
-                if d.index not in refused:
-                    _arm_prove(d.cuda_ordinal, False)
+                for arm in arms:
+                    rc = arm(d.cuda_ordinal, True)
+                    if rc != N.OK:
+                        refused[d.index] = ScrubReport.from_native(d.bdf, N.ScrubResult(status=rc))
+                        break
+                    armed.append((d, arm))
+            ran = [d for d in devices if d.index not in refused]
+            reports, wall = scrub_and_verify_many(ran, nbytes, check, residue, triage, triage_hold_ms, mismatch_triage)
+        finally:
+            for d, arm in armed:
+                arm(d.cuda_ordinal, False)
         it = iter(reports)
         reports = [refused[d.index] if d.index in refused else next(it) for d in devices]
         for rep, d in zip(reports, devices):
-            if d.index not in refused:
+            if d.index in refused:
+                continue
+            if prove:
                 report = last_cover(d.cuda_ordinal)
                 rep.cover = report if report is not None and report.proved else None
                 if rep.status == N.OK and rep.cover is None:   # a proof that was asked for and did not run
                     rep.status = N.ERR_UNCOVERED
+            if probe:
+                _attach_probe(rep, d.cuda_ordinal)
         return reports, wall
     n = len(devices)
     if n == 0:
@@ -1042,11 +1140,16 @@ class ScrubbingProxy:
 
     def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
                          triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False,
-                         prove: bool = False) -> ScrubReport:
+                         prove: bool = False, probe: bool = False) -> ScrubReport:
         native = object.__getattribute__(self, "_native")
         _mismatch_triage_check(mismatch_triage, check)
+        _probe_check(probe, check)
         if native is None:
             raise GpuError(f"no CUDA device with PCI address {self._foreign.bdf}: HBM scrub cannot run", N.ERR_NO_CUDA)
+        if probe:
+            return native.scrub_and_verify(nbytes, check=check, residue=residue, triage=triage,
+                                           triage_hold_ms=triage_hold_ms, mismatch_triage=mismatch_triage, prove=prove,
+                                           probe=True)
         if prove:
             return native.scrub_and_verify(nbytes, check=check, residue=residue, triage=triage,
                                            triage_hold_ms=triage_hold_ms, mismatch_triage=mismatch_triage, prove=True)

@@ -64,6 +64,7 @@ SCRUB_SKIPPED_ANNOTATION = "nvidia.com/cc-manager.scrub-skipped"
 RESIDUE_MODES = ("off", "report")   # CC_SCRUB_RESIDUE
 TRIAGE_MODES = ("off", "report")    # CC_SCRUB_TRIAGE, CC_SCRUB_MISMATCH_TRIAGE
 PROOF_MODES = ("off", "require")    # CC_SCRUB_PROOF
+ALIAS_PROBE_MODES = ("off", "require")   # CC_SCRUB_ALIAS_PROBE
 # How long the dirt and mismatch triages wait before their last re-read of the pages they re-wrote: long enough for an
 # agent that still writes this GPU's memory to show itself, short against a transition.
 SCRUB_TRIAGE_HOLD_MS = 100
@@ -110,7 +111,8 @@ class CCManager:
                  scrub_mode: Optional[str] = None, scrub_bytes: Optional[int] = None,
                  max_parallel: Optional[int] = None, scrub_check: Optional[str] = None,
                  scrub_residue: Optional[str] = None, scrub_triage: Optional[str] = None,
-                 scrub_mismatch_triage: Optional[str] = None, scrub_proof: Optional[str] = None):
+                 scrub_mismatch_triage: Optional[str] = None, scrub_proof: Optional[str] = None,
+                 scrub_alias_probe: Optional[str] = None):
         env = os.environ
         self.operator_namespace = env.get("OPERATOR_NAMESPACE", "gpu-operator")
         self.evict_operator_components = env.get("EVICT_OPERATOR_COMPONENTS", "true").lower() == "true"
@@ -179,6 +181,18 @@ class CCManager:
         self.scrub_proof = (scrub_proof or env.get("CC_SCRUB_PROOF", "off")).lower()
         if self.scrub_proof not in PROOF_MODES:
             raise ValueError(f"CC_SCRUB_PROOF must be 'off' or 'require', not {self.scrub_proof!r}")
+        # off:     the zero gate cannot see a page mapped twice: both views read back zero.
+        # require: after a clean read-back, the zero gate also tags, checks and re-reads one 32-byte window per 4 KiB
+        #          page (ccm_scrub_probe, DESIGN.md §5i), and a GPU on which a window lost its tags (a page mapped twice)
+        #          fails the gate.  A check, not a report: a device that cannot probe fails the gate.  The tagged check
+        #          already covers every window, so it is refused with CC_SCRUB_CHECK=tagged.  Logged and kept in
+        #          last_transition["scrub_probe"].
+        self.scrub_alias_probe = (scrub_alias_probe or env.get("CC_SCRUB_ALIAS_PROBE", "off")).lower()
+        if self.scrub_alias_probe not in ALIAS_PROBE_MODES:
+            raise ValueError(f"CC_SCRUB_ALIAS_PROBE must be 'off' or 'require', not {self.scrub_alias_probe!r}")
+        if self.scrub_alias_probe == "require" and self.scrub_check == "tagged":
+            raise ValueError("CC_SCRUB_ALIAS_PROBE=require probes the zero gate; CC_SCRUB_CHECK=tagged already checks "
+                             "every probe window: use one or the other")
         self.max_parallel = int(max_parallel if max_parallel is not None else env.get("CC_MAX_PARALLEL", "0"))
         # "full-HBM" is enforced, not assumed: when scrubbing everything (scrub_bytes == 0) a GPU on
         # which less than this fraction of DEVICE memory was zeroed and read back fails the gate
@@ -570,6 +584,8 @@ class CCManager:
             cmd += ["--mismatch-triage"] + ([] if self.triage else ["--triage-hold-ms", str(SCRUB_TRIAGE_HOLD_MS)])
         if self.prove:
             cmd += ["--prove"]
+        if self.alias_probe:
+            cmd += ["--probe"]
         for gpu in gpus:
             cmd += ["--bdf", gpu.bdf]
         env = dict(os.environ)
@@ -587,10 +603,14 @@ class CCManager:
     def prove(self) -> bool:
         return self.scrub_proof == "require"
 
+    @property
+    def alias_probe(self) -> bool:
+        return self.scrub_alias_probe == "require"
+
     def _scrub_call(self, gpu, **kwargs):
         """The one call every per-device gate path makes: with CC_SCRUB_PROOF=require it also asks for the coverage
-        proof.  A device whose scrub_and_verify cannot take `prove` fails the gate: it is never scrubbed unproven in its
-        place."""
+        proof, with CC_SCRUB_ALIAS_PROBE=require for the alias probe.  A device whose scrub_and_verify cannot take
+        `prove` (`probe`) fails the gate: it is never scrubbed without them in its place."""
         if self.prove:
             kwargs["prove"] = True
             try:
@@ -598,12 +618,22 @@ class CCManager:
             except (TypeError, ValueError):
                 raise ScrubFailure(f"device {gpu.bdf} cannot prove its HBM coverage (CC_SCRUB_PROOF=require); refusing "
                                    "to release it") from None
+        if self.alias_probe:
+            kwargs["probe"] = True
+            try:
+                inspect.signature(gpu.scrub_and_verify).bind(self.scrub_bytes, **kwargs)
+            except (TypeError, ValueError):
+                raise ScrubFailure(f"device {gpu.bdf} cannot probe its HBM for pages mapped twice "
+                                   "(CC_SCRUB_ALIAS_PROBE=require); refusing to release it") from None
         return gpu.scrub_and_verify(self.scrub_bytes, **kwargs)
 
     def _scrub_many(self, natives: list, **kwargs):
-        """The one native fan-out call of the gate, with the coverage proof under CC_SCRUB_PROOF=require."""
+        """The one native fan-out call of the gate, with the coverage proof under CC_SCRUB_PROOF=require and the alias
+        probe under CC_SCRUB_ALIAS_PROBE=require."""
         if self.prove:
             kwargs["prove"] = True
+        if self.alias_probe:
+            kwargs["probe"] = True
         return _devices.scrub_and_verify_many(natives, self.scrub_bytes, **kwargs)
 
     def _scrub_checked(self, gpu):
@@ -720,6 +750,10 @@ class CCManager:
             self.last_transition.setdefault("scrub_cover", {})[bdf] = cover
             logger.log(logging.INFO if cover.covered else logging.ERROR, "HBM coverage proof on %s: %s", bdf,
                        cover.summary())
+        probe = getattr(holder, "probe", None)
+        if probe is not None:
+            self.last_transition.setdefault("scrub_probe", {})[bdf] = probe
+            logger.log(logging.INFO if probe.held else logging.ERROR, "HBM alias probe on %s: %s", bdf, probe.summary())
         for attr, key, level, line in self._REPORT_NOTES + self._TRIAGE_NOTES:
             report = getattr(holder, attr, None)
             if report is not None:
@@ -783,9 +817,14 @@ class CCManager:
                     + (f" mismatch_bytes={mismatch} (bytes that did not hold their address tag)"
                        if self.scrub_check == "tagged" else "")
                     + (" (a pass did not walk every mapped byte exactly once: see the coverage proof)"
-                       if rep.status == _devices.N.ERR_UNCOVERED else ""))
+                       if rep.status == _devices.N.ERR_UNCOVERED else "")
+                    + (" (a probe window did not hold its tags: see the alias probe)"
+                       if getattr(getattr(rep, "probe", None), "mismatch_bytes", 0) else ""))
             if self.prove and getattr(rep, "cover", None) is None:
                 raise ScrubFailure(f"HBM scrub on {rep.bdf} carries no coverage proof (CC_SCRUB_PROOF=require); "
+                                   "refusing to release it")
+            if self.alias_probe and getattr(rep, "probe", None) is None:
+                raise ScrubFailure(f"HBM scrub on {rep.bdf} carries no alias probe (CC_SCRUB_ALIAS_PROBE=require); "
                                    "refusing to release it")
             if self.scrub_bytes == 0 and rep.coverage < self.scrub_min_coverage:
                 raise ScrubFailure(
@@ -1055,6 +1094,10 @@ def build_arg_parser() -> argparse.ArgumentParser:
     parser.add_argument("--scrub-proof", default=None, choices=PROOF_MODES,
                         help="require: every pass of the scrub gate counts the bytes it walked on every 2 MiB page, and "
                              "a GPU whose pass missed or repeated a byte fails the gate (default: $CC_SCRUB_PROOF or off)")
+    parser.add_argument("--scrub-alias-probe", default=None, choices=ALIAS_PROBE_MODES,
+                        help="require: after a clean read-back, the zero gate tags, checks and re-reads one 32-byte "
+                             "window per 4 KiB page, and a GPU with a page mapped twice fails the gate (not with "
+                             "--scrub-check tagged; default: $CC_SCRUB_ALIAS_PROBE or off)")
     return parser
 
 
@@ -1081,6 +1124,7 @@ def main(argv: Optional[List[str]] = None) -> None:
                   kubeconfig=args.kubeconfig, scrub_mode=args.scrub_mode, scrub_check=args.scrub_check,
                   scrub_residue=args.scrub_residue, scrub_triage=args.scrub_triage,
                   scrub_mismatch_triage=args.scrub_mismatch_triage, scrub_proof=args.scrub_proof,
+                  scrub_alias_probe=args.scrub_alias_probe,
                   device_source=_device_source_from_env()).run()
     except KeyboardInterrupt:
         logger.info("Shutting down...")

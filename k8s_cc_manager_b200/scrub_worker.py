@@ -10,7 +10,8 @@ short-lived process and reads ONE JSON line back; the process exit returns every
 Output (stdout, last line):  {"wall_ms": ..., "reports": [ {ScrubReport fields}, ... ]}
 (the tagged-gate fields only with --check tagged; "residue" only with --residue; "triage" only with --triage, for a
 GPU whose read-back found non-zero bytes; "mismatch_triage" only with --mismatch-triage, for a GPU whose tagged check
-found bytes off their tags; "cover" only with --prove, for every GPU whose passes finished).
+found bytes off their tags; "cover" only with --prove, for every GPU whose passes finished; "probe" only with --probe,
+for every GPU whose alias probe ran).
 Exit code: 0 if every GPU is clean, 3 if the gate failed, 2 on usage errors.
 """
 from __future__ import annotations
@@ -25,15 +26,22 @@ from . import devices as D
 
 
 def run(bdfs: List[str], nbytes: int, check: str = "zero", residue: bool = False, triage_hold_ms: int = 0,
-        mismatch_triage_hold_ms: int = 0, prove: bool = False) -> dict:
+        mismatch_triage_hold_ms: int = 0, prove: bool = False, probe: bool = False) -> dict:
     """triage_hold_ms > 0 arms the dirt triage with that hold, mismatch_triage_hold_ms > 0 the mismatch triage (with
-    the same hold when both are armed); prove arms the coverage proof."""
+    the same hold when both are armed); prove arms the coverage proof, probe the alias probe."""
     by_bdf = {d.bdf: d for d in D.find_gpus()[0] if d.is_gpu()}
     missing = [b for b in bdfs if b not in by_bdf]
     if missing:
         raise SystemExit(f"unknown GPU(s): {', '.join(missing)} (known: {', '.join(sorted(by_bdf))})")
     devs = [by_bdf[b] for b in bdfs]
-    if prove:
+    if probe:
+        reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check, residue=residue,
+                                                   triage=bool(triage_hold_ms),
+                                                   triage_hold_ms=mismatch_triage_hold_ms or triage_hold_ms or
+                                                   D.TRIAGE_HOLD_MS,
+                                                   mismatch_triage=bool(mismatch_triage_hold_ms), prove=prove,
+                                                   probe=True)
+    elif prove:
         reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check, residue=residue,
                                                    triage=bool(triage_hold_ms),
                                                    triage_hold_ms=mismatch_triage_hold_ms or triage_hold_ms or
@@ -71,6 +79,9 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap.add_argument("--prove", action="store_true",
                     help="prove that every pass walked every mapped byte exactly once; a GPU whose pass did not fails "
                          "the gate")
+    ap.add_argument("--probe", action="store_true",
+                    help="with --check zero, after a clean read-back, tag, check and re-read one 32-byte window per 4 KiB "
+                         "page; a GPU with a page mapped twice fails the gate")
     ap.add_argument("--triage-hold-ms", type=int, default=D.TRIAGE_HOLD_MS,
                     help="the triages' hold before their last re-read (default %(default)s)")
     args = ap.parse_args(argv)
@@ -78,11 +89,13 @@ def main(argv: Optional[List[str]] = None) -> int:
         ap.error("at least one --bdf is required")
     if args.mismatch_triage and args.check != "tagged":
         ap.error("--mismatch-triage needs --check tagged")
+    if args.probe and args.check == "tagged":
+        ap.error("--probe is for --check zero: the tagged check already covers every probe window")
     if args.backend:
         D.select_backend(args.backend)
     out = run([b.lower() for b in args.bdf], args.bytes, args.check, args.residue,
               args.triage_hold_ms if args.triage else 0, args.triage_hold_ms if args.mismatch_triage else 0,
-              args.prove)
+              args.prove, args.probe)
     print(json.dumps(out), flush=True)
     return 0 if all(r["status"] == 0 and r["nonzero_bytes"] == 0 and r.get("mismatch_bytes", 0) == 0
                     for r in out["reports"]) else 3
