@@ -702,6 +702,11 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
   else if (k == "cover_skip") d.drill.cover_skip = v < 0 ? 0 : (uint64_t)v;
   else if (k == "probe_mismatch") d.drill.probe_mismatch = v < 0 ? 0 : (uint64_t)v;
   else if (k == "probe_dirt") d.drill.probe_dirt = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "probe_skip") d.drill.probe_skip = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "probe_skip_step") {
+    if (v < 0 || v > 3) { set_error("sim key 'probe_skip_step' takes 0..3, not %lld", (long long)v); return CCM_ERR_INVALID; }
+    d.drill.probe_skip_step = v == 0 ? 2 : (int)v;
+  }
   else if (k == "cover_pass") {
     if (v < 0 || v > CCM_PASS_READBACK) { set_error("sim key 'cover_pass' takes 0..3, not %lld", (long long)v); return CCM_ERR_INVALID; }
     d.drill.cover_pass = v == 0 ? (int)CCM_PASS_READBACK : (int)v;
@@ -758,6 +763,8 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "cover_pass") *value = d.drill.cover_pass;
     else if (k == "probe_mismatch") *value = (int64_t)d.drill.probe_mismatch;
     else if (k == "probe_dirt") *value = (int64_t)d.drill.probe_dirt;
+    else if (k == "probe_skip") *value = (int64_t)d.drill.probe_skip;
+    else if (k == "probe_skip_step") *value = d.drill.probe_skip_step;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

@@ -61,6 +61,9 @@ int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, b
 // Drills of the alias probe (sim keys "probe_mismatch", "probe_dirt"; ccm.h), only in a call that probes:
 //   probe_mismatch: the first byte of each of the first that many probe windows is XORed between P1 and P2;
 //   probe_dirt:     the same bytes, between P2 and P3.
+// Drill of the probe proof (sim keys "probe_skip", "probe_skip_step"; ccm.h), in every call that probes:
+//   probe_skip:     the first launch of step probe_skip_step (1..3 = P1..P3; the sim key's 0 is stored as 2) starts
+//                   that many windows later and takes that many fewer (at most all of its windows).
 struct ScrubDrill {
   uint64_t inject = 0;
   int poison = 0;
@@ -75,6 +78,8 @@ struct ScrubDrill {
   int cover_pass = CCM_PASS_READBACK;
   uint64_t probe_mismatch = 0;
   uint64_t probe_dirt = 0;
+  uint64_t probe_skip = 0;
+  int probe_skip_step = 2;
 };
 // inject: the call's "scrub_inject" budget.  Its poison and flood drills are those current_scrub_drill()
 // returns on the calling thread.  (The engine entry points keep the signatures that host-only builds of

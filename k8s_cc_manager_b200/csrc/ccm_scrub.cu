@@ -160,8 +160,10 @@ struct GatePasses {
   std::vector<Span> spans;   // what the call holds, and the address of page 0 of the pages its bytes lie on
   int skip_pass = 0;     // drill "cover_skip": pending for the first launch of this pass (CCM_PASS_*; 0 = none)
   uint64_t skip = 0;
+  bool pcover_dirty = false;   // the probe's proving twins counted into the probe cover maps, not yet taken
 };
 static constexpr int kPasses = 3;   // CCM_PASS_FIRST, CHECK, READBACK
+static constexpr int kSteps = 3;    // the alias probe's P1, P2, P3
 
 struct ScrubEngine {
   int ordinal = -1;
@@ -201,6 +203,12 @@ struct ScrubEngine {
   bool probe_ready = false;                 // its kernels are resident
   int probe_ctas[3] = {};                   // and how many CTAs of each step (P1, P2, P3) one SM holds at once
   ccm_probe_report probe{};                 // report of the last product call (ccm_scrub_last_probe)
+  // probe proof (a call both proven and probed): kSteps maps of npages words, as d_cover, and their pinned copy
+  uint32_t* d_pcover = nullptr;
+  uint32_t* h_pcover = nullptr;
+  int pcover_ctas[3] = {};                  // CTAs per SM of each step's proving twin
+  ccm_probe_cover pcover{};                 // report of the last product call (ccm_scrub_last_probe_cover)
+  std::vector<ccm_probe_cover_page> pcover_pages;   // and its inexact pages (ccm_last_probe_cover_pages)
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -263,6 +271,10 @@ static constexpr int kProbeThreads = 256, kProbePer = 4;
 #define CCM_PROBE_FILL alias_probe_fill_pass<kProbeThreads, kProbePer>
 #define CCM_PROBE_CHECK alias_probe_check_pass<kProbeThreads, kProbePer>
 #define CCM_PROBE_REREAD alias_probe_reread_pass<kProbeThreads, kProbePer>
+// Their proving twins (probe proof): the same shapes.
+#define CCM_COVER_PROBE_FILL cover_probe_fill_pass<kProbeThreads, kProbePer>
+#define CCM_COVER_PROBE_CHECK cover_probe_check_pass<kProbeThreads, kProbePer>
+#define CCM_COVER_PROBE_REREAD cover_probe_reread_pass<kProbeThreads, kProbePer>
 
 const char* default_kernel_names() {
   static const std::string names = [] {
@@ -387,6 +399,10 @@ int engine_teardown(int ordinal) {
   if (e->h_cover) cudaFreeHost(e->h_cover);
   e->d_cover = nullptr;
   e->h_cover = nullptr;
+  if (e->d_pcover) cudaFree(e->d_pcover);
+  if (e->h_pcover) cudaFreeHost(e->h_pcover);
+  e->d_pcover = nullptr;
+  e->h_pcover = nullptr;
   e->probe_ready = false;
   e->d_counter = nullptr;
   e->h_counter = nullptr;
@@ -1185,8 +1201,9 @@ static int begin_gate(ScrubEngine* e, const ScrubDrill& drill) {
 // maps are zero again for the next one.
 static void end_gate(ScrubEngine* e) {
   std::lock_guard<std::mutex> g(e->mu);
-  if (e->gate.prove && e->d_cover && e->ready && cudaSetDevice(e->ordinal) == cudaSuccess) {
-    cudaMemsetAsync(e->d_cover, 0, kPasses * e->npages * sizeof(uint32_t), e->stream);
+  if ((e->gate.prove || e->gate.pcover_dirty) && e->ready && cudaSetDevice(e->ordinal) == cudaSuccess) {
+    if (e->gate.prove && e->d_cover) cudaMemsetAsync(e->d_cover, 0, kPasses * e->npages * sizeof(uint32_t), e->stream);
+    if (e->gate.pcover_dirty) cudaMemsetAsync(e->d_pcover, 0, kSteps * e->npages * sizeof(uint32_t), e->stream);
     cudaStreamSynchronize(e->stream);
   }
   e->gate = GatePasses();
@@ -1217,27 +1234,158 @@ static void probe_windows_of(uint64_t addr, uint64_t n, uint64_t* w0, uint64_t* 
   *nwin = *w0 + kProbeWindow <= addr + n ? (addr + n - kProbeWindow - *w0) / kProbeStride + 1 : 0;
 }
 
+// ------------------------------------------------------------------ probe proof
+// Sets aside the probe cover maps and their host copy, and makes the probe kernels' proving twins resident, the first
+// time a call is both proven and probed (before it maps anything).  The caller holds e->mu.
+static int ensure_probe_cover(ScrubEngine* e) {
+  if (e->d_pcover) return CCM_OK;
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  const size_t bytes = kSteps * e->npages * sizeof(uint32_t);
+  if (!e->h_pcover) CCM_CUDA(cudaHostAlloc(&e->h_pcover, bytes, cudaHostAllocDefault));
+  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e->pcover_ctas[0], CCM_COVER_PROBE_FILL, kProbeThreads, 0));
+  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e->pcover_ctas[1], CCM_COVER_PROBE_CHECK, kProbeThreads, 0));
+  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e->pcover_ctas[2], CCM_COVER_PROBE_REREAD, kProbeThreads, 0));
+  for (int& c : e->pcover_ctas) c = std::max(c, 1);
+  uint32_t* d = nullptr;
+  CCM_CUDA(cudaMalloc(&d, bytes));
+  const cudaError_t err = cudaMemset(d, 0, bytes);
+  if (err != cudaSuccess) {
+    cudaFree(d);
+    set_error("probe cover map memset failed: %s", cudaGetErrorString(err));
+    return CCM_ERR_CUDA;
+  }
+  e->d_pcover = d;
+  return CCM_OK;
+}
+
+// What every step of the probe must count on each of the np pages: CCM_PROBE_WINDOW bytes per window of `chunks`, on
+// the page its offset (c.offset + (window - c.addr)) starts on.  A window that crosses a page boundary splits its bytes
+// there, as the kernels' cover_lanes does (it cannot on 32-byte-aligned chunk offsets).  Chunks are walked page by page,
+// not window by window: a whole-HBM call has some 20 M windows.
+static std::vector<uint32_t> probe_cover_expected(const std::vector<CheckSpan>& chunks, uint64_t np) {
+  std::vector<uint32_t> exp(np, 0);
+  for (const CheckSpan& c : chunks) {
+    uint64_t w0 = 0, nwin = 0;
+    probe_windows_of(c.addr, c.bytes, &w0, &nwin);
+    if (nwin == 0) continue;
+    const uint64_t o0 = c.offset + (w0 - c.addr);   // offset of the chunk's first window
+    const uint64_t last = o0 + (nwin - 1) * kProbeStride;
+    for (uint64_t p = o0 / kPageBytes; p <= last / kPageBytes && p < np; ++p) {
+      const uint64_t lo = p * kPageBytes, hi = lo + kPageBytes;
+      const uint64_t i0 = lo <= o0 ? 0 : (lo - o0 + kProbeStride - 1) / kProbeStride;
+      const uint64_t i1 = std::min<uint64_t>(nwin, (hi - o0 + kProbeStride - 1) / kProbeStride);
+      if (i1 <= i0) continue;
+      exp[p] += (uint32_t)((i1 - i0) * kProbeWindow);
+      const uint64_t end = o0 + (i1 - 1) * kProbeStride + kProbeWindow;   // the page's last window, past its end?
+      if (end > hi) {
+        exp[p] -= (uint32_t)(end - hi);
+        if (p + 1 < np) exp[p + 1] += (uint32_t)(end - hi);
+      }
+    }
+  }
+  return exp;
+}
+
+// After the probe of a call both proven and probed (the caller holds e->mu): copies the probe cover maps once, zeroes
+// them for the next call, and compares every step against probe_cover_expected(chunks).  Fills *out (proved = 1),
+// e->pcover and e->pcover_pages; each inexact page gets chunk_of(page offset).
+template <typename ChunkOf>
+static int take_probe_cover(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& chunks, uint64_t va_base,
+                            ccm_probe_cover* out, ChunkOf&& chunk_of) {
+  const double t0 = now_ms();
+  const size_t bytes = kSteps * e->npages * sizeof(uint32_t);
+  CCM_CUDA(cudaMemcpyAsync(e->h_pcover, e->d_pcover, bytes, cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaMemsetAsync(e->d_pcover, 0, bytes, st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  e->gate.pcover_dirty = false;
+  const uint64_t np = e->npages - 1;   // pages of a map; word np is its outside slot
+  const std::vector<uint32_t> exp = probe_cover_expected(chunks, np);
+  ccm_probe_cover rep;
+  memset(&rep, 0, sizeof rep);
+  rep.va_base = va_base;
+  rep.proved = 1;
+  for (const CheckSpan& c : chunks) {
+    uint64_t w0 = 0, nwin = 0;
+    probe_windows_of(c.addr, c.bytes, &w0, &nwin);
+    rep.windows_expected += nwin;
+  }
+  uint64_t counted[kSteps] = {}, missing[kSteps] = {}, extra[kSteps] = {};   // bytes
+  std::vector<ccm_probe_cover_page> pages;
+  for (uint64_t p = 0; p < np; ++p) {
+    ccm_probe_cover_page cp;
+    memset(&cp, 0, sizeof cp);
+    cp.page = p;
+    cp.expected = exp[p];
+    bool exact = true;
+    for (int k = 0; k < kSteps; ++k) {
+      const uint32_t c = e->h_pcover[k * e->npages + p];
+      ccm_probe_cover_step& ps = rep.step[k];
+      cp.count[k] = c;
+      counted[k] += c;
+      if (c < exp[p]) {
+        if (ps.pages_short++ == 0) ps.first_short_page = p;
+        missing[k] += exp[p] - c;
+      } else if (c > exp[p]) {
+        ps.pages_over++;
+        extra[k] += c - exp[p];
+      }
+      exact &= c == exp[p];
+    }
+    if (!exact) {
+      cp.chunk = chunk_of(p * kPageBytes);
+      pages.push_back(cp);
+    }
+  }
+  rep.covered = 1;
+  for (int k = 0; k < kSteps; ++k) {
+    ccm_probe_cover_step& ps = rep.step[k];
+    const uint64_t outside = e->h_pcover[k * e->npages + np];
+    ps.ran = 1;
+    ps.windows_outside = (outside + kProbeWindow - 1) / kProbeWindow;
+    ps.windows_counted = (counted[k] + outside + kProbeWindow - 1) / kProbeWindow;
+    ps.windows_missing = (missing[k] + kProbeWindow - 1) / kProbeWindow;
+    ps.windows_extra = (extra[k] + outside + kProbeWindow - 1) / kProbeWindow;
+    if (missing[k] || extra[k] || outside) rep.covered = 0;
+  }
+  rep.ms_prove = now_ms() - t0;
+  e->pcover = *out = rep;
+  e->pcover_pages.swap(pages);
+  return CCM_OK;
+}
+
 // The alias probe (ccm.h: ccm_scrub_probe) over `chunks` (each with its offset in what the reports describe; the caller
 // holds e->mu, and every kernel of the call has finished): P1 over every chunk, the "probe_mismatch" drill, P2, the
 // "probe_dirt" drill, P3, one launch per chunk per step in order.  Fills *rep (probed = 1) and *p3 (P3's count); after
 // P2 mismatches, *mrep (classified against `spans`, chunk_of(offset)) and the mismatch page map.  After an error it
-// drops the check book.
+// drops the check book.  prove: the proving twins run instead, each step into its probe cover map (the caller takes
+// them), with page 0 at each chunk's c.addr - c.offset.
 template <typename ChunkOf>
 static int run_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& chunks,
                      const std::vector<CheckSpan>& spans, uint32_t seed, const ScrubDrill& drill, uint64_t va_base,
-                     ccm_probe_report* rep, ccm_mismatch_report* mrep, uint64_t* p3, ChunkOf&& chunk_of) {
+                     bool prove, ccm_probe_report* rep, ccm_mismatch_report* mrep, uint64_t* p3, ChunkOf&& chunk_of) {
   memset(rep, 0, sizeof *rep);
   rep->seed = seed;
   rep->va_base = va_base;
-  // one launch of step k (0 = P1, 1 = P2, 2 = P3) per chunk with windows
+  if (prove) e->gate.pcover_dirty = true;
+  uint64_t skip = drill.probe_skip;   // "probe_skip": pending for the first launch of step probe_skip_step
+  // one launch of step k (0 = P1, 1 = P2, 2 = P3) per chunk with windows; the grid from the launched kernel's occupancy
   auto step = [&](int k, auto&& launch) -> int {
-    const uint64_t max_grid = (uint64_t)e->sm_count * e->probe_ctas[k];
+    const uint64_t max_grid = (uint64_t)e->sm_count * (prove ? e->pcover_ctas[k] : e->probe_ctas[k]);
     for (const CheckSpan& c : chunks) {
       uint64_t w0 = 0, nwin = 0;
       probe_windows_of(c.addr, c.bytes, &w0, &nwin);
       if (nwin == 0) continue;
       const uint64_t batches = (nwin + kProbeThreads * kProbePer - 1) / (kProbeThreads * kProbePer);
-      launch(w0, nwin, (int)std::min<uint64_t>(batches, max_grid), c.addr - c.offset);
+      const int grid = (int)std::min<uint64_t>(batches, max_grid);
+      const uint64_t base = c.addr - c.offset;
+      const CoverOut cv{prove ? e->d_pcover + (uint64_t)k * e->npages : nullptr, base, (uint32_t)(e->npages - 1)};
+      if (skip && k + 1 == drill.probe_skip_step) {
+        const uint64_t s = std::min(skip, nwin);
+        w0 += s * kProbeStride;
+        nwin -= s;
+        skip = 0;
+      }
+      launch(w0, nwin, grid, base, cv);
       g_launches++;
       rep->launches++;
       CCM_CUDA(cudaGetLastError());
@@ -1264,19 +1412,25 @@ static int run_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpa
     CCM_CUDA(cudaMemsetAsync(e->d_counter + kMismatch, 0, sizeof(unsigned long long), st));
     CCM_CUDA(cudaMemsetAsync(e->d_counter + kNonzero, 0, sizeof(unsigned long long), st));
     CCM_CUDA(cudaEventRecord(e->ev[0], st));
-    if (int r2 = step(0, [&](uint64_t w0, uint64_t n, int grid, uint64_t) {
-          CCM_PROBE_FILL<<<grid, kProbeThreads, 0, st>>>(w0, n, seed);
+    if (int r2 = step(0, [&](uint64_t w0, uint64_t n, int grid, uint64_t, const CoverOut& cv) {
+          if (prove) CCM_COVER_PROBE_FILL<<<grid, kProbeThreads, 0, st>>>(w0, n, seed, cv);
+          else CCM_PROBE_FILL<<<grid, kProbeThreads, 0, st>>>(w0, n, seed);
         }))
       return r2;
     if (int r2 = xor_windows(drill.probe_mismatch)) return r2;
-    if (int r2 = step(1, [&](uint64_t w0, uint64_t n, int grid, uint64_t base) {
-          CCM_PROBE_CHECK<<<grid, kProbeThreads, 0, st>>>(w0, n, seed, e->d_counter + kMismatch, e->book_out(kCheckBook),
-                                                         base);
+    if (int r2 = step(1, [&](uint64_t w0, uint64_t n, int grid, uint64_t base, const CoverOut& cv) {
+          if (prove)
+            CCM_COVER_PROBE_CHECK<<<grid, kProbeThreads, 0, st>>>(w0, n, seed, e->d_counter + kMismatch,
+                                                                  e->book_out(kCheckBook), base, cv);
+          else
+            CCM_PROBE_CHECK<<<grid, kProbeThreads, 0, st>>>(w0, n, seed, e->d_counter + kMismatch,
+                                                           e->book_out(kCheckBook), base);
         }))
       return r2;
     if (int r2 = xor_windows(drill.probe_dirt)) return r2;
-    if (int r2 = step(2, [&](uint64_t w0, uint64_t n, int grid, uint64_t) {
-          CCM_PROBE_REREAD<<<grid, kProbeThreads, 0, st>>>(w0, n, e->d_counter + kNonzero);
+    if (int r2 = step(2, [&](uint64_t w0, uint64_t n, int grid, uint64_t, const CoverOut& cv) {
+          if (prove) CCM_COVER_PROBE_REREAD<<<grid, kProbeThreads, 0, st>>>(w0, n, e->d_counter + kNonzero, cv);
+          else CCM_PROBE_REREAD<<<grid, kProbeThreads, 0, st>>>(w0, n, e->d_counter + kNonzero);
         }))
       return r2;
     CCM_CUDA(cudaEventRecord(e->ev[1], st));
@@ -1315,18 +1469,21 @@ static int run_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpa
 }
 
 // The product call's probe: armed, zero gate, clean read-back.  A seed per call; e->probe and (after mismatches)
-// e->mismatch get the reports.
+// e->mismatch get the reports.  A proven call (its passes still counting, and the probe cover maps set aside) proves
+// the probe too, into *pcover and e->pcover, with page 0 at va_base.
 template <typename ChunkOf>
 static int gate_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& chunks,
                       const std::vector<CheckSpan>& spans, const ScrubDrill& drill, uint64_t va_base,
-                      ccm_probe_report* out, uint64_t* p3, ChunkOf&& chunk_of) {
+                      ccm_probe_report* out, ccm_probe_cover* pcover, uint64_t* p3, ChunkOf&& chunk_of) {
   const uint32_t seed = std::random_device{}();
+  const bool prove = e->gate.prove && e->d_pcover;
   ccm_mismatch_report mrep;
-  const int rc = run_probe(e, st, chunks, spans, seed, drill, va_base, out, &mrep, p3, chunk_of);
+  int rc = run_probe(e, st, chunks, spans, seed, drill, va_base, prove, out, &mrep, p3, chunk_of);
   if (rc != CCM_OK) { memset(out, 0, sizeof *out); return rc; }
   e->probe = *out;
   if (out->mismatch_bytes != 0) e->mismatch = mrep;
-  return CCM_OK;
+  if (prove) rc = take_probe_cover(e, st, chunks, va_base, pcover, chunk_of);
+  return rc;
 }
 
 // ------------------------------------------------------------------ what kind of dirt
@@ -1824,13 +1981,14 @@ static int arena_cover(ScrubEngine* e, bool tagged, ccm_cover_report* out) {
 
 // The alias probe of the fallback path, after its read-back: segment by segment, offsets into the concatenated
 // segments, chunk = segment index.  *nz = P3's count.
-static int arena_probe(ScrubEngine* e, const ScrubDrill& drill, ccm_probe_report* out, uint64_t* nz) {
+static int arena_probe(ScrubEngine* e, const ScrubDrill& drill, ccm_probe_report* out, ccm_probe_cover* pcover,
+                       uint64_t* nz) {
   std::lock_guard<std::mutex> g(e->mu);
   CCM_ENSURE_READY(e);
   int rc = need_arena(e); if (rc) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
   const std::vector<CheckSpan> spans = arena_spans(e->segs);
-  return gate_probe(e, e->stream, spans, spans, drill, (uint64_t)(uintptr_t)e->segs.front().ptr, out, nz,
+  return gate_probe(e, e->stream, spans, spans, drill, (uint64_t)(uintptr_t)e->segs.front().ptr, out, pcover, nz,
                     [&](uint64_t o) { return segment_of(e->segs, o); });
 }
 
@@ -1903,7 +2061,8 @@ static bool async_release_enabled() { return env_u64("CCM_ASYNC_RELEASE", 1) != 
 // * the verdict is returned as soon as the 8-byte count is on the host; cuMemUnmap/cuMemRelease
 //   (serialised node-wide by the driver) run on the engine's reaper thread.
 static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDrill& drill, bool node_fanout,
-                                  ccm_scrub_result* r, ccm_cover_report* cover, ccm_probe_report* probe) {
+                                  ccm_scrub_result* r, ccm_cover_report* cover, ccm_probe_report* probe,
+                                  ccm_probe_cover* pcover) {
   const VmmApi& api = vmm();
   if (!api.ok) return CCM_ERR_UNSUPPORTED;
   std::lock_guard<std::mutex> g(e->mu);
@@ -2134,7 +2293,8 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   // ---- alias probe: armed zero gate whose read-back was clean, after the last read-back -----------------------
   if (rc == CCM_OK && probe && r->nonzero_bytes == 0 && mapped) {
     uint64_t p3 = 0;
-    rc = gate_probe(e, st, iters, {{(uint64_t)m.base, mapped, 0}}, drill, (uint64_t)m.base, probe, &p3, chunk_of);
+    rc = gate_probe(e, st, iters, {{(uint64_t)m.base, mapped, 0}}, drill, (uint64_t)m.base, probe, pcover, &p3,
+                    chunk_of);
     if (rc == CCM_OK) r->nonzero_bytes = p3;
   }
   // ---- coverage proof: one copy of the cover maps, no launch ------------------------------------------------
@@ -2220,10 +2380,13 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     memset(&e->cover, 0, sizeof e->cover);
     e->cover_pages.clear();
     memset(&e->probe, 0, sizeof e->probe);
+    memset(&e->pcover, 0, sizeof e->pcover);
+    e->pcover_pages.clear();
     prove = e->prove;
     // the alias probe is for the zero gate: a tagged call's check already covers every window
     probe_armed = e->probe_armed && tag == nullptr;
     if (probe_armed) probe_rc = ensure_probe(e);
+    if (probe_armed && prove && probe_rc == CCM_OK) probe_rc = ensure_probe_cover(e);
   }
   ccm_scrub_result r;
   memset(&r, 0, sizeof r);
@@ -2244,7 +2407,10 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   ccm_probe_report probe;   // and of the probe report
   memset(&probe, 0, sizeof probe);
   ccm_probe_report* probe_out = probe_armed ? &probe : nullptr;
-  if (env_u64("CCM_PIPELINE", 1) != 0) rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r, &cover, probe_out);
+  ccm_probe_cover pcover;   // and of the probe proof
+  memset(&pcover, 0, sizeof pcover);
+  if (env_u64("CCM_PIPELINE", 1) != 0)
+    rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r, &cover, probe_out, &pcover);
   if (rc == CCM_ERR_UNSUPPORTED) {
     // plain path: one cudaMalloc'ed arena, whole-arena scrub, whole-arena verify (the drills act per
     // segment: poison before the scrub, flood + inject between the scrub and the verify)
@@ -2275,7 +2441,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       }
       if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
       if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
-      if (rc == CCM_OK && probe_out && nz == 0) rc = arena_probe(e, drill, probe_out, &nz);
+      if (rc == CCM_OK && probe_out && nz == 0) rc = arena_probe(e, drill, probe_out, &pcover, &nz);
       if (rc == CCM_OK) rc = arena_cover(e, tag != nullptr, &cover);
       if (rc == CCM_OK && nz != 0) arena_locate(e, drill);
       if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) arena_triage_mismatch(e, tag->seed, drill);
@@ -2297,6 +2463,17 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
               "%llu extra; %llu pages short, first short page %llu)", e->ordinal, kPassNames[short_pass],
               (unsigned long long)ps.bytes_counted, (unsigned long long)cover.bytes_mapped,
               (unsigned long long)ps.bytes_missing, (unsigned long long)ps.bytes_extra,
+              (unsigned long long)ps.pages_short, (unsigned long long)ps.first_short_page);
+    rc = CCM_ERR_UNCOVERED;
+  } else if (rc == CCM_OK && pcover.proved && !pcover.covered) {
+    static const char* const kStepNames[kSteps] = {"P1 (tag)", "P2 (check)", "P3 (re-read)"};
+    int k = 0;
+    while (k + 1 < kSteps && !(pcover.step[k].windows_missing || pcover.step[k].windows_extra)) ++k;
+    const ccm_probe_cover_step& ps = pcover.step[k];
+    set_error("HBM alias probe proof failed on CUDA device %d: step %s counted %llu of %llu probe windows (%llu missing, "
+              "%llu extra; %llu pages short, first short page %llu)", e->ordinal, kStepNames[k],
+              (unsigned long long)ps.windows_counted, (unsigned long long)pcover.windows_expected,
+              (unsigned long long)ps.windows_missing, (unsigned long long)ps.windows_extra,
               (unsigned long long)ps.pages_short, (unsigned long long)ps.first_short_page);
     rc = CCM_ERR_UNCOVERED;
   } else if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) {
@@ -2707,6 +2884,43 @@ extern "C" int ccm_scrub_last_probe(int cuda_ordinal, ccm_probe_report* out) {
   return CCM_OK;
 }
 
+// ------------------------------------------------------------------------- probe proof
+static_assert(sizeof(ccm_probe_cover_step) == 64 && sizeof(ccm_probe_cover) == 224 &&
+              offsetof(ccm_probe_cover, step) == 32 && sizeof(ccm_probe_cover_page) == 32,
+              "probe cover structs keep their layout");
+
+extern "C" int ccm_scrub_last_probe_cover(int cuda_ordinal, ccm_probe_cover* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  *out = e->pcover;
+  return CCM_OK;
+}
+
+extern "C" int ccm_last_probe_cover_pages(int cuda_ordinal, ccm_probe_cover_page* out, uint64_t cap, uint64_t* n) {
+  if (!n || (cap && !out)) {
+    set_error("ccm_last_probe_cover_pages: cap %llu (needs n, and out when cap > 0)", (unsigned long long)cap);
+    return CCM_ERR_INVALID;
+  }
+  *n = 0;
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_lookup(cuda_ordinal);
+  if (!e) return CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  *n = e->pcover_pages.size();
+  if (cap) memcpy(out, e->pcover_pages.data(), std::min<uint64_t>(cap, *n) * sizeof(ccm_probe_cover_page));
+  return CCM_OK;
+}
+
 extern "C" int ccm_region_probe(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream,
                                 ccm_probe_report* out, ccm_mismatch_report* mismatch) {
   if (!out) return CCM_ERR_INVALID;
@@ -2722,7 +2936,7 @@ extern "C" int ccm_region_probe(int cuda_ordinal, void* dptr, uint64_t bytes, ui
   const std::vector<CheckSpan> spans{{base, bytes, 0}};
   ccm_mismatch_report rep;
   uint64_t p3 = 0;
-  const int rc = run_probe(e, e->pick(stream), spans, spans, seed, ScrubDrill(), base, out, &rep, &p3,
+  const int rc = run_probe(e, e->pick(stream), spans, spans, seed, ScrubDrill(), base, false, out, &rep, &p3,
                            [](uint64_t) { return 0u; });
   if (rc != CCM_OK) { memset(out, 0, sizeof *out); return rc; }
   if (mismatch) *mismatch = rep;

@@ -17,8 +17,9 @@
 // GPU for the coverage proof (ccm_scrub_prove), for every GPU whose passes finished, as ccm_scrub_last_cover and
 // ccm_last_cover_pages report it; "probe" with --probe, which refuses --check tagged and arms every GPU for the alias
 // probe (ccm_scrub_probe), for every GPU whose probe ran, as ccm_scrub_last_probe reports it, with "mismatch" when it
-// found bytes off their tags).  With --prove or --probe, a GPU that cannot be armed is never scrubbed without: nothing
-// is scrubbed and the exit code is 3.
+// found bytes off their tags); "probe_cover" with --prove and --probe, for every GPU whose probe ran, as
+// ccm_scrub_last_probe_cover and ccm_last_probe_cover_pages report it.  With --prove or --probe, a GPU that cannot be
+// armed is never scrubbed without: nothing is scrubbed and the exit code is 3.
 // Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
@@ -243,6 +244,8 @@ static void print_probe(const ccm_probe_report& p) {
          (unsigned long long)p.va_base, p.ms_probe, p.probed);
 }
 
+static void print_pcover(const ccm_probe_cover& c, int ordinal);   // after main
+
 int main(int argc, char** argv) {
   std::vector<std::string> bdfs;
   unsigned long long bytes = 0;
@@ -354,14 +357,20 @@ int main(int argc, char** argv) {
   printf("{\"wall_ms\": %.3f, \"reports\": [", wall_ms);
   for (size_t i = 0; i < devs.size(); ++i) {
     const ccm_scrub_result& r = res[i];
-    clean = clean && r.status == CCM_OK && r.nonzero_bytes == 0;
+    ccm_probe_report pr;
+    const bool ran_probe = probe && ccm_scrub_last_probe(ordinals[i], &pr) == CCM_OK && pr.probed;
+    ccm_probe_cover pc;
+    const bool probe_proved = prove && ran_probe && ccm_scrub_last_probe_cover(ordinals[i], &pc) == CCM_OK && pc.proved;
+    // a proving call that probed and has no probe proof fails in its own report, whoever reads it
+    const int status = r.status == CCM_OK && prove && ran_probe && !probe_proved ? (int)CCM_ERR_UNCOVERED : r.status;
+    clean = clean && status == CCM_OK && r.nonzero_bytes == 0;
     printf("%s{\"bdf\": \"%s\", \"bytes_requested\": %llu, \"bytes_scrubbed\": %llu, \"device_total_bytes\": %llu, "
            "\"nonzero_bytes\": %llu, \"ms_acquire\": %.3f, \"ms_scrub\": %.3f, \"ms_verify\": %.3f, \"ms_release\": %.3f, "
            "\"ms_total\": %.3f, \"segments\": %d, \"status\": %d, \"release_deferred\": %d, "
            "\"device_free_before\": %llu, \"bytes_unreached\": %llu, \"ms_release_wait\": %.3f, \"ms_gpu_span\": %.3f",
            i ? ", " : "", names[i].c_str(), (unsigned long long)r.bytes_requested, (unsigned long long)r.bytes_scrubbed,
            (unsigned long long)r.device_total_bytes, (unsigned long long)r.nonzero_bytes, r.ms_acquire, r.ms_scrub,
-           r.ms_verify, r.ms_release, r.ms_total, r.segments, r.status, r.release_deferred,
+           r.ms_verify, r.ms_release, r.ms_total, r.segments, status, r.release_deferred,
            (unsigned long long)r.device_free_before, (unsigned long long)r.bytes_unreached, r.ms_release_wait, r.ms_gpu_span);
     if (tagged) {
       const ccm_tag_result& t = tags[i];
@@ -371,8 +380,6 @@ int main(int argc, char** argv) {
     }
     ccm_dirt_report d;
     if (r.nonzero_bytes != 0 && ccm_scrub_last_dirt(ordinals[i], &d) == CCM_OK) print_dirt(d, ordinals[i]);
-    ccm_probe_report pr;
-    const bool ran_probe = probe && ccm_scrub_last_probe(ordinals[i], &pr) == CCM_OK && pr.probed;
     ccm_mismatch_report m;
     if (tagged && tags[i].mismatch_bytes != 0 && ccm_scrub_last_mismatch(ordinals[i], &m) == CCM_OK) print_mismatch(m, ordinals[i]);
     // --probe refuses --check tagged: at most one of the two prints the mismatch report
@@ -389,10 +396,41 @@ int main(int argc, char** argv) {
     if (proved) print_cover(c, ordinals[i]);
     clean = clean && (!prove || proved);   // a proof that was asked for and did not run fails the gate
     if (ran_probe) print_probe(pr);
+    if (probe_proved) print_pcover(pc, ordinals[i]);
     printf("}");
   }
   printf("]}\n");
   fflush(stdout);  // the verdict is out BEFORE the contexts are torn down: a parent can act on it right away
   ccm_device_release_many((int)devs.size(), devs.data(), nullptr);  // joins the deferred HBM release, drops the contexts
   return clean ? 0 : 3;
+}
+
+// The "probe_cover" object: the fields of k8s_cc_manager_b200.devices.ProbeCoverReport, with the first 64 inexact pages.
+static void print_pcover(const ccm_probe_cover& c, int ordinal) {
+  static const char* const names[3] = {"P1", "P2", "P3"};
+  printf(", \"probe_cover\": {\"windows_expected\": %llu, \"va_base\": %llu, \"ms_prove\": %.3f, \"proved\": %d, "
+         "\"covered\": %d, \"steps\": [",
+         (unsigned long long)c.windows_expected, (unsigned long long)c.va_base, c.ms_prove, c.proved, c.covered);
+  for (int k = 0; k < 3; ++k) {
+    const ccm_probe_cover_step& p = c.step[k];
+    printf("%s{\"name\": \"%s\", \"ran\": %d, \"windows_counted\": %llu, \"windows_missing\": %llu, "
+           "\"windows_extra\": %llu, \"windows_outside\": %llu, \"pages_short\": %llu, \"pages_over\": %llu, "
+           "\"first_short_page\": %llu}",
+           k ? ", " : "", names[k], p.ran, (unsigned long long)p.windows_counted, (unsigned long long)p.windows_missing,
+           (unsigned long long)p.windows_extra, (unsigned long long)p.windows_outside, (unsigned long long)p.pages_short,
+           (unsigned long long)p.pages_over, (unsigned long long)p.first_short_page);
+  }
+  printf("], \"pages\": [");
+  uint64_t n = 0;
+  std::vector<ccm_probe_cover_page> v;
+  if (!c.covered && ccm_last_probe_cover_pages(ordinal, nullptr, 0, &n) == CCM_OK) {
+    v.resize(n);
+    if (n && ccm_last_probe_cover_pages(ordinal, v.data(), n, &n) != CCM_OK) v.clear();
+  }
+  const size_t keep = 64;   // k8s_cc_manager_b200.devices.COVER_PAGES
+  for (size_t k = 0; k < v.size() && k < keep; ++k)
+    printf("%s{\"page\": %llu, \"chunk\": %u, \"expected\": %u, \"p1\": %u, \"p2\": %u, \"p3\": %u}",
+           k ? ", " : "", (unsigned long long)v[k].page, v[k].chunk, v[k].expected, v[k].count[0], v[k].count[1],
+           v[k].count[2]);
+  printf("], \"pages_truncated\": %d}", v.size() > keep);
 }

@@ -32,6 +32,8 @@
 //   census_zero_kernel / census_tag_fill_kernel          what the first pass found before it erased it
 //   cover_*_pass                                         proving twins of the six above that run a product call's
 //                                                        passes: they count the bytes they walk per 2 MiB page
+//   alias_probe_*_pass                                   the alias probe's three steps (one 32-byte window per 4 KiB)
+//   cover_probe_*_pass                                   their proving twins: they count the windows they take per page
 //   fill_pattern_kernel                                  seeded test pattern (tests only)
 // The grab loop (grab_chunks) and the epilogue after the last whole chunk or tile (finish_region,
 // ragged_bytes) are written once.  The five compile-time-shape kernels are one frame (default_kernel)
@@ -1180,7 +1182,7 @@ __device__ __forceinline__ void cover_add(const CoverOut& c, uint64_t a, uint32_
   if (n > lo) atomicAdd(c.map + cover_word(c, a + lo), n - lo);
 }
 
-// n bytes (n <= 16) from address a, by every active lane: the lanes whose bytes start on one page add up and one of
+// n bytes (n <= 32) from address a, by every active lane: the lanes whose bytes start on one page add up and one of
 // them issues the atomic; the rare bytes past a page boundary go one atomic per lane.
 __device__ __forceinline__ void cover_lanes(const CoverOut& c, uint64_t a, uint32_t n) {
   const uint32_t room = kPageBytes - (uint32_t)((a - c.base) & (kPageBytes - 1));
@@ -1426,6 +1428,49 @@ __global__ void __launch_bounds__(THREADS)
 alias_probe_reread_pass(uint64_t w0, uint64_t nwin, unsigned long long* nonzero) {
   ProbeRereadOp op;
   probe_windows<THREADS, PER>(w0, nwin, op);
+  block_accumulate(op.cnt, nonzero);
+}
+
+// The proving twins of the probe kernels: the same op through the same loop, and after each batch kProbeWindow bytes of
+// every window it took counted into `cover`, one window slot u at a time across the lanes.  The 32 lanes of a warp take
+// 32 consecutive windows (128 KiB), so a slot is normally one atomic per warp.
+template <typename Op>
+struct CoverProbeOp {
+  Op& op;
+  CoverOut cover;
+  template <int K>
+  __device__ __forceinline__ void batch(uint64_t a, uint64_t step) {
+    op.template batch<K>(a, step);
+#pragma unroll
+    for (int u = 0; u < K; ++u) cover_lanes(cover, a + u * step, kProbeWindow);
+  }
+};
+
+template <int THREADS, int PER>
+__global__ void __launch_bounds__(THREADS)
+cover_probe_fill_pass(uint64_t w0, uint64_t nwin, uint32_t seed, CoverOut cover) {
+  ProbeFillOp op{seed};
+  CoverProbeOp<ProbeFillOp> cop{op, cover};
+  probe_windows<THREADS, PER>(w0, nwin, cop);
+}
+
+template <int THREADS, int PER>
+__global__ void __launch_bounds__(THREADS)
+cover_probe_check_pass(uint64_t w0, uint64_t nwin, uint32_t seed, unsigned long long* mismatch, LocateOut out,
+                       uint64_t base, CoverOut cover) {
+  ProbeCheckOp op{{seed, {out}, base}};
+  CoverProbeOp<ProbeCheckOp> cop{op, cover};
+  probe_windows<THREADS, PER>(w0, nwin, cop);
+  op.op.book.flush();
+  block_accumulate(op.op.cnt, mismatch);
+}
+
+template <int THREADS, int PER>
+__global__ void __launch_bounds__(THREADS)
+cover_probe_reread_pass(uint64_t w0, uint64_t nwin, unsigned long long* nonzero, CoverOut cover) {
+  ProbeRereadOp op;
+  CoverProbeOp<ProbeRereadOp> cop{op, cover};
+  probe_windows<THREADS, PER>(w0, nwin, cop);
   block_accumulate(op.cnt, nonzero);
 }
 

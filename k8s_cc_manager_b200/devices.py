@@ -34,7 +34,8 @@ class GpuError(Exception):
     `.residue`; a triage call that read back dirt carries its TriageReport (what kind of dirt) as `.triage`; a mismatch
     triage call whose tagged check failed carries its TriageReport (what kind of mismatch) as `.mismatch_triage`; a
     proving call carries its CoverReport (how many bytes each pass walked on every page) as `.cover`; a probing call
-    carries its ProbeReport (what the alias probe found) as `.probe`."""
+    carries its ProbeReport (what the alias probe found) as `.probe`; a call both proving and probing carries its
+    ProbeCoverReport (how many windows each probe step took on every page) as `.probe_cover`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
@@ -687,8 +688,112 @@ def _probe_check(probe: bool, check: str) -> None:
         raise ValueError("probe=True is for check='zero': the tagged check already covers every probe window")
 
 
-def _attach_probe(rep: "ScrubReport", cuda_ordinal: int) -> None:
-    """The probe report of a call that probed, and where its tags were wrong when they were."""
+@dataclass
+class ProbeCoverPage:
+    """One page some step of a proven probe did not count exactly (include/ccm.h: ccm_probe_cover_page)."""
+    page: int
+    chunk: int
+    expected: int      # bytes (PROBE_WINDOW per window) every step had to count on it
+    p1: int            # bytes P1, P2 and P3 counted
+    p2: int
+    p3: int
+
+    def describe(self) -> str:
+        return (f"page {self.page} (chunk {self.chunk}): expected {self.expected}, P1 {self.p1}, P2 {self.p2}, "
+                f"P3 {self.p3}")
+
+
+@dataclass
+class ProbeCoverStep:
+    """What one probe step counted against the call's windows (include/ccm.h: ccm_probe_cover_step)."""
+    name: str          # "P1", "P2" or "P3"
+    ran: int
+    windows_counted: int
+    windows_missing: int
+    windows_extra: int
+    windows_outside: int
+    pages_short: int
+    pages_over: int
+    first_short_page: int
+
+
+@dataclass
+class ProbeCoverReport:
+    """The probe proof of one product call both proven and probed (include/ccm.h: ccm_probe_cover): every probe step
+    counted on the device the windows it took on each 2 MiB page, and `covered` says each took every probe window of
+    the call exactly once.  `pages` are the first COVER_PAGES inexact pages."""
+    windows_expected: int
+    va_base: int
+    ms_prove: float
+    proved: int
+    covered: int
+    steps: List[ProbeCoverStep] = field(default_factory=list)
+    pages: List[ProbeCoverPage] = field(default_factory=list)
+    pages_truncated: int = 0
+
+    @classmethod
+    def from_native(cls, r: N.ProbeCover, pages: "Optional[List[ProbeCoverPage]]" = None) -> "ProbeCoverReport":
+        steps = [ProbeCoverStep(name=name, **{f: getattr(r.steps[k], f) for f, _ in N.ProbeCoverStep._fields_
+                                              if f != "reserved"})
+                 for k, name in enumerate(N.PROBE_STEPS)]
+        pages = pages or []
+        return cls(r.windows_expected, r.va_base, r.ms_prove, r.proved, r.covered, steps, pages[:COVER_PAGES],
+                   int(len(pages) > COVER_PAGES))
+
+    @classmethod
+    def from_json(cls, d: dict) -> "ProbeCoverReport":
+        return cls(**{**d, "steps": [ProbeCoverStep(**p) for p in d["steps"]],
+                      "pages": [ProbeCoverPage(**p) for p in d["pages"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    def short_step(self) -> "Optional[ProbeCoverStep]":
+        """The first step that did not count every page exactly (None when covered)."""
+        return next((p for p in self.steps if p.ran and (p.windows_missing or p.windows_extra)), None)
+
+    def summary(self, first: int = 4) -> str:
+        """One line for an operator: how many windows the probe had and, when a step was short, which one and where."""
+        line = f"{self.windows_expected} probe windows"
+        bad = self.short_step()
+        if bad is None:
+            return line + ": every step took every window once (" + ", ".join(p.name for p in self.steps if p.ran) + ")"
+        line += (f": step {bad.name} counted {bad.windows_counted} windows ({bad.windows_missing} missing, "
+                 f"{bad.windows_extra} extra) with {bad.pages_short} pages short, first short page "
+                 f"{bad.first_short_page}")
+        if self.pages:
+            more = " (+more)" if self.pages_truncated or len(self.pages) > first else ""
+            line += "; " + "; ".join(p.describe() for p in self.pages[:first]) + more
+        return line
+
+
+def last_probe_cover_pages(cuda_ordinal: int) -> "Optional[List[ProbeCoverPage]]":
+    """The inexact pages of the last proven probe on a CUDA device (include/ccm.h: ccm_last_probe_cover_pages),
+    ascending; None when they cannot be read."""
+    n = C.c_uint64(0)
+    if cuda_ordinal < 0 or N.lib().ccm_last_probe_cover_pages(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
+        return None
+    buf = (N.ProbeCoverPage * max(1, n.value))()
+    if N.lib().ccm_last_probe_cover_pages(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
+        return None
+    return [ProbeCoverPage(p.page, p.chunk, p.expected, *p.count) for p in buf[:n.value]]
+
+
+def last_probe_cover(cuda_ordinal: int) -> "Optional[ProbeCoverReport]":
+    """The probe proof of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_probe_cover), with
+    its first inexact pages; None when it cannot be read."""
+    out = N.ProbeCover()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_probe_cover(cuda_ordinal, C.byref(out)) != N.OK:
+        return None
+    return ProbeCoverReport.from_native(out, last_probe_cover_pages(cuda_ordinal)
+                                        if out.proved and not out.covered else None)
+
+
+def _attach_probe(rep: "ScrubReport", cuda_ordinal: int, prove: bool = False) -> bool:
+    """The probe report of a call that probed, and where its tags were wrong when they were; for a proving call that
+    probed, the probe proof.  False for a proving call that probed and has no proof that ran: none could be read, or
+    the one read did not run.  (A stand-in library without ccm_scrub_last_probe_cover has no proof to give, and
+    its verdict stands; _native.lib() loads no libccm without it.)"""
     report = last_probe(cuda_ordinal)
     rep.probe = report if report is not None and report.probed else None
     if rep.probe is not None and rep.probe.mismatch_bytes:
@@ -696,11 +801,19 @@ def _attach_probe(rep: "ScrubReport", cuda_ordinal: int) -> None:
         if rep.mismatch is not None and rep.mismatch.mismatch_windows:
             pages = last_page_map(cuda_ordinal, rep.mismatch.BOOK)
             rep.mismatch.pages = pages.digest() if pages is not None else None
+    if prove and rep.probe is not None:
+        if not hasattr(N.lib(), "ccm_scrub_last_probe_cover"):
+            return True
+        pc = last_probe_cover(cuda_ordinal)
+        rep.probe_cover = pc if pc is not None and pc.proved else None
+        return rep.probe_cover is not None
+    return True
 
 
 # The reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
 _REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport),
-            ("mismatch_triage", TriageReport), ("cover", CoverReport), ("probe", ProbeReport))
+            ("mismatch_triage", TriageReport), ("cover", CoverReport), ("probe", ProbeReport),
+            ("probe_cover", ProbeCoverReport))
 
 
 @dataclass
@@ -751,6 +864,9 @@ class ScrubReport:
     # What the alias probe found (a ProbeReport), set for every report of a probing call (probe=True) that probed: one
     # whose read-back was clean.  Not a dataclass field either.
     probe = None
+    # How many windows each probe step took on every page (a ProbeCoverReport), set for every report of a call both
+    # proving and probing (prove=True, probe=True) that probed.  Not a dataclass field either.
+    probe_cover = None
 
     @property
     def clean(self) -> bool:
@@ -922,6 +1038,9 @@ class NvidiaDevice:
         ccm_scrub_probe): after a clean read-back, one 32-byte window per 4 KiB page is tagged, checked and zeroed and
         read for zeros; the report comes attached as `.probe`, and a window off its tags (a page mapped twice) fails
         the call with ERR_MISMATCH and attaches where as `.mismatch`.  A device that cannot be armed fails the call.
+        prove=True with probe=True also proves the probe: each probe step counts on the device the windows it took on
+        each page, the report comes attached as `.probe_cover`, and a step that missed or repeated a window fails the
+        call with ERR_UNCOVERED.
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
         if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
@@ -962,10 +1081,11 @@ class NvidiaDevice:
                 _arm_probe(self.cuda_ordinal, False)
         rep = ScrubReport.from_native(self.bdf, res, tag)
         _attach_reports(rep, self.cuda_ordinal, census, armed, marmed, prove)
-        if probe:
-            _attach_probe(rep, self.cuda_ordinal)
+        probe_proved = _attach_probe(rep, self.cuda_ordinal, prove) if probe else True
         if err is None and prove and rep.cover is None:   # a proof that was asked for and did not run
             err = GpuError(f"scrub_and_verify on {self.bdf}: the coverage proof did not run", N.ERR_UNCOVERED)
+        if err is None and not probe_proved:
+            err = GpuError(f"scrub_and_verify on {self.bdf}: the probe proof did not run", N.ERR_UNCOVERED)
         if err is not None:
             for attr, _ in _REPORTS:
                 setattr(err, attr, getattr(rep, attr))
@@ -1057,8 +1177,8 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
                 rep.cover = report if report is not None and report.proved else None
                 if rep.status == N.OK and rep.cover is None:   # a proof that was asked for and did not run
                     rep.status = N.ERR_UNCOVERED
-            if probe:
-                _attach_probe(rep, d.cuda_ordinal)
+            if probe and not _attach_probe(rep, d.cuda_ordinal, prove) and rep.status == N.OK:
+                rep.status = N.ERR_UNCOVERED   # a probe proof that was asked for and did not run
         return reports, wall
     n = len(devices)
     if n == 0:

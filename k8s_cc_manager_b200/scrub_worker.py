@@ -11,7 +11,7 @@ Output (stdout, last line):  {"wall_ms": ..., "reports": [ {ScrubReport fields},
 (the tagged-gate fields only with --check tagged; "residue" only with --residue; "triage" only with --triage, for a
 GPU whose read-back found non-zero bytes; "mismatch_triage" only with --mismatch-triage, for a GPU whose tagged check
 found bytes off their tags; "cover" only with --prove, for every GPU whose passes finished; "probe" only with --probe,
-for every GPU whose alias probe ran).
+for every GPU whose alias probe ran; "probe_cover" only with --prove and --probe, for every GPU whose alias probe ran).
 Exit code: 0 if every GPU is clean, 3 if the gate failed, 2 on usage errors.
 """
 from __future__ import annotations
@@ -77,8 +77,8 @@ def main(argv: Optional[List[str]] = None) -> int:
                     help="with --check tagged, after a failed check, re-tag, check and re-read the pages off their tags: "
                          "does the mismatch stay, return or clear (never fails the gate)")
     ap.add_argument("--prove", action="store_true",
-                    help="prove that every pass walked every mapped byte exactly once; a GPU whose pass did not fails "
-                         "the gate")
+                    help="prove that every pass walked every mapped byte exactly once (with --probe, that every probe "
+                         "step took every window once); a GPU whose pass or step did not fails the gate")
     ap.add_argument("--probe", action="store_true",
                     help="with --check zero, after a clean read-back, tag, check and re-read one 32-byte window per 4 KiB "
                          "page; a GPU with a page mapped twice fails the gate")
