@@ -150,14 +150,42 @@ struct VmmMapping {
   std::vector<CUmemGenericAllocationHandle> handles;
 };
 
+// One contiguous piece of what a call holds: `bytes` at device address `addr`, which lie `offset` bytes into what its
+// reports describe (the mapping, the concatenated segments, or the region).
+struct CheckSpan { uint64_t addr, bytes, offset; };
+
+// What a product call holds while its reports are taken, or what a region call covers: page 0 of the reports at
+// va_base, `bytes` in all, as the spans its checks, locate pass and triages walk (ascending offsets), the chunks its
+// alias probe launches over (each mapping-loop iteration, or each segment), and the allocation behind every offset.
+struct Held {
+  uint64_t va_base = 0, bytes = 0;
+  std::vector<CheckSpan> spans, probe_chunks;
+  std::vector<std::pair<uint64_t, uint32_t>> chunks;   // (offset, chunk) of every allocation's first byte, ascending
+  // The chunk of `offset`: that of the last allocation that starts at or before it, else the first.  Compared as
+  // signed: the head window of a raw region that does not start 16-aligned has a negative offset.  (A mapping or a
+  // segment starts aligned, so the product call never books one.)
+  uint32_t chunk_of(uint64_t offset) const {
+    auto it = std::upper_bound(chunks.begin(), chunks.end(), offset, [](uint64_t o, const std::pair<uint64_t, uint32_t>& c) {
+      return (int64_t)o < (int64_t)c.first;
+    });
+    if (it != chunks.begin()) --it;
+    return it == chunks.end() ? 0u : it->second;
+  }
+};
+
+// A raw region's hold: one span, one probe chunk, chunk 0.
+static Held region_held(const void* p, uint64_t bytes) {
+  const uint64_t a = (uint64_t)(uintptr_t)p;
+  return Held{a, bytes, {{a, bytes, 0}}, {{a, bytes, 0}}, {{0, 0u}}};
+}
+
 // The product call's passes while it enqueues them (ccm.h: ccm_scrub_prove, and the "cover_skip" drill).  Every range
 // launch of the scrub, census, tag fill, tag check and read-back asks it for its cover map (gate_launch); the locate pass
 // and the triages run after it is cleared.
 struct GatePasses {
   bool active = false;   // the call's passes are being enqueued
   bool prove = false;    // ... with the proving kernels, into the cover maps
-  struct Span { uint64_t addr, bytes, base; };
-  std::vector<Span> spans;   // what the call holds, and the address of page 0 of the pages its bytes lie on
+  std::vector<CheckSpan> spans;   // what the call holds (page 0 of the pages its bytes lie on: addr - offset)
   int skip_pass = 0;     // drill "cover_skip": pending for the first launch of this pass (CCM_PASS_*; 0 = none)
   uint64_t skip = 0;
   bool pcover_dirty = false;   // the probe's proving twins counted into the probe cover maps, not yet taken
@@ -585,8 +613,8 @@ static int gate_launch(ScrubEngine* e, int pass, const void* p, int grab, cudaSt
     const uint64_t a = (uint64_t)(uintptr_t)p;
     // a launch outside what the call holds counts into the outside slot: its offsets all lie past the map
     uint64_t base = a - (uint64_t)e->npages * kPageBytes;
-    for (const GatePasses::Span& sp : g.spans)
-      if (a >= sp.addr && a < sp.addr + sp.bytes) base = sp.base;
+    for (const CheckSpan& sp : g.spans)
+      if (a >= sp.addr && a < sp.addr + sp.bytes) base = sp.addr - sp.offset;
     *cover = CoverOut{e->d_cover + (uint64_t)(pass - 1) * e->npages, base, (uint32_t)(e->npages - 1)};
   }
   return CCM_OK;
@@ -935,9 +963,8 @@ static int read_book(ScrubEngine* e, Book b, cudaStream_t st, BookHead* head, st
 }
 
 // Completes the page map read_book() gathered for book `b`: ascending, one entry per page (a page that two fallback
-// segments share was read twice), each with the chunk of its first byte, chunk_of(page offset).
-template <typename ChunkOf>
-static void finish_pages(ScrubEngine* e, Book b, ChunkOf&& chunk_of) {
+// segments share was read twice), each with the chunk of its first byte, h.chunk_of(page offset).
+static void finish_pages(ScrubEngine* e, Book b, const Held& h) {
   std::vector<ccm_page_entry>& v = e->pages[b];
   std::sort(v.begin(), v.end(), [](const ccm_page_entry& x, const ccm_page_entry& y) { return x.page < y.page; });
   size_t k = 0;
@@ -946,7 +973,7 @@ static void finish_pages(ScrubEngine* e, Book b, ChunkOf&& chunk_of) {
     else v[k++] = v[i];
   }
   v.resize(k);
-  for (ccm_page_entry& p : v) p.chunk = chunk_of(p.page * (uint64_t)kPageBytes);
+  for (ccm_page_entry& p : v) p.chunk = h.chunk_of(p.page * (uint64_t)kPageBytes);
 }
 
 // Sorts a report's records by offset (signed: a head window that starts before the region comes first) and sets
@@ -970,11 +997,10 @@ static int locate_launch(ScrubEngine* e, const void* p, uint64_t n, uint64_t bas
 
 // One locate pass over [p, p+n) on `st` (synchronises; the caller holds e->mu).  The kernel books offsets from
 // p - shift (`shift`: the range's offset in what `rep` describes), and what it found is added to `rep`: each new record
-// gets the chunk chunk_of(offset), and its pages are appended to the dirt book's page map (read_book).  Records are
+// gets the chunk h.chunk_of(offset), and its pages are appended to the dirt book's page map (read_book).  Records are
 // kept while `rep` has room; sort_records() sorts them.
-template <typename ChunkOf>
 static int locate_range(ScrubEngine* e, const void* p, uint64_t n, uint64_t shift, cudaStream_t st,
-                        ccm_dirt_report* rep, ChunkOf&& chunk_of) {
+                        ccm_dirt_report* rep, const Held& h) {
   rep->located = 1;
   if (n == 0) return CCM_OK;
   float ms = 0;
@@ -991,31 +1017,27 @@ static int locate_range(ScrubEngine* e, const void* p, uint64_t n, uint64_t shif
   for (uint64_t i = 0; i < bk.nrecords && rep->nrecords < CCM_DIRT_RECORDS; ++i) {
     ccm_dirt_record& r = rep->records[rep->nrecords++];
     memcpy(&r, &e->h_book->dirt[i], sizeof r);
-    r.chunk = chunk_of(r.offset);
+    r.chunk = h.chunk_of(r.offset);
   }
   return CCM_OK;
 }
 
 // ------------------------------------------------------------------ where the tags were wrong
-// One contiguous piece of what a tagged call checked: `bytes` at device address `addr`, which lie `offset` bytes into
-// what the report describes (the mapping, the concatenated segments, or the region).
-struct CheckSpan { uint64_t addr, bytes, offset; };
-
-// After checks that counted mismatch_bytes != 0 (and finished): reads the check book and fills `rep`.  Offsets are as
-// the kernels booked them; every record is classified (ccm_mismatch.h) against `spans` (the ALIAS search covers
-// exactly them) and gets chunk_of(offset).
-template <typename ChunkOf>
-static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_bytes, uint32_t seed, uint64_t va_base,
-                         const std::vector<CheckSpan>& spans, ccm_mismatch_report* rep, ChunkOf&& chunk_of) {
+// After checks over `h` that counted mismatch_bytes != 0 (and finished): reads the check book and fills `rep`.  Offsets
+// are as the kernels booked them; every record is classified (ccm_mismatch.h) against h.spans (the ALIAS search covers
+// exactly them) and gets h.chunk_of(offset).
+static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_bytes, uint32_t seed, const Held& h,
+                         ccm_mismatch_report* rep) {
+  const std::vector<CheckSpan>& spans = h.spans;
   memset(rep, 0, sizeof *rep);
   rep->located = 1;
   rep->seed = seed;
-  rep->va_base = va_base;
+  rep->va_base = h.va_base;
   rep->mismatch_bytes = mismatch_bytes;
   BookHead bk;
   e->pages[kCheckBook].clear();
   if (int rc = read_book(e, kCheckBook, st, &bk)) return rc;
-  finish_pages(e, kCheckBook, chunk_of);
+  finish_pages(e, kCheckBook, h);
   rep->zero_windows = bk.count;
   rep->mismatch_windows = bk.windows;
   if (bk.windows == 0) return CCM_OK;
@@ -1040,7 +1062,7 @@ static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_byte
     const DirtRecord& d = e->h_book->dirt[i];
     ccm_mismatch_record& r = rep->records[rep->nrecords++];
     r.offset = d.offset;
-    r.chunk = chunk_of(d.offset);
+    r.chunk = h.chunk_of(d.offset);
     r.mask = d.mask;
     memcpy(r.bytes, &d.bytes, sizeof r.bytes);
     const CheckSpan& sp = span_at(d.offset);
@@ -1054,7 +1076,7 @@ static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_byte
       // offsets follow the span of the source's first present byte (a head window's source may start before it)
       const CheckSpan* src = span_holding(v.source + (uint64_t)(__builtin_ctz(present)));
       r.source_offset = src ? src->offset + (v.source - src->addr) : 0;
-      r.source_chunk = chunk_of(r.source_offset);
+      r.source_chunk = h.chunk_of(r.source_offset);
     }
   }
   sort_records(rep, bk.windows);
@@ -1062,19 +1084,17 @@ static int take_mismatch(ScrubEngine* e, cudaStream_t st, uint64_t mismatch_byte
 }
 
 // ------------------------------------------------------------------ what the first pass erased
-// After the census launches of one call have finished: reads the census book and fills `rep` (located = 1).  Offsets
-// are as the kernels booked them; every record gets chunk_of(offset).
-template <typename ChunkOf>
-static int take_residue(ScrubEngine* e, cudaStream_t st, uint64_t va_base, uint64_t examined, ccm_residue_report* rep,
-                        ChunkOf&& chunk_of) {
+// After the census launches of one call over `h` have finished: reads the census book and fills `rep` (located = 1).
+// Offsets are as the kernels booked them; every record gets h.chunk_of(offset).
+static int take_residue(ScrubEngine* e, cudaStream_t st, const Held& h, ccm_residue_report* rep) {
   memset(rep, 0, sizeof *rep);
   BookHead bk;
   e->pages[kCensusBook].clear();
   if (int rc = read_book(e, kCensusBook, st, &bk)) return rc;
-  finish_pages(e, kCensusBook, chunk_of);
+  finish_pages(e, kCensusBook, h);
   rep->located = 1;
-  rep->va_base = va_base;
-  rep->bytes_examined = examined;
+  rep->va_base = h.va_base;
+  rep->bytes_examined = h.bytes;
   rep->residue_bytes = bk.count;
   rep->residue_windows = bk.windows;
   if (bk.windows == 0) return CCM_OK;
@@ -1084,7 +1104,7 @@ static int take_residue(ScrubEngine* e, cudaStream_t st, uint64_t va_base, uint6
     const MaskRecord& m = e->h_book->mask[i];
     ccm_residue_record& r = rep->records[rep->nrecords++];
     r.offset = m.offset;
-    r.chunk = chunk_of(r.offset);
+    r.chunk = h.chunk_of(r.offset);
     r.mask = m.mask;
     r.reserved = 0;
   }
@@ -1120,11 +1140,10 @@ static int ensure_cover(ScrubEngine* e) {
 }
 
 // After the passes of a proving call have finished (the caller holds e->mu): copies the cover maps once, zeroes them
-// for the next call, and compares every pass that ran against what the call mapped, [0, mapped) from va_base.  Fills
-// e->cover (proved = 1) and e->cover_pages; each inexact page gets chunk_of(page offset).
-template <typename ChunkOf>
-static int take_cover(ScrubEngine* e, cudaStream_t st, uint64_t mapped, uint64_t va_base, bool tagged,
-                      ccm_cover_report* out, ChunkOf&& chunk_of) {
+// for the next call, and compares every pass that ran against what the call holds, [0, h.bytes) from h.va_base.  Fills
+// e->cover (proved = 1) and e->cover_pages; each inexact page gets h.chunk_of(page offset).
+static int take_cover(ScrubEngine* e, cudaStream_t st, const Held& h, bool tagged, ccm_cover_report* out) {
+  const uint64_t mapped = h.bytes;
   e->gate.prove = false;
   const double t0 = now_ms();
   const size_t bytes = kPasses * e->npages * sizeof(uint32_t);
@@ -1135,7 +1154,7 @@ static int take_cover(ScrubEngine* e, cudaStream_t st, uint64_t mapped, uint64_t
   memset(&rep, 0, sizeof rep);
   rep.bytes_mapped = mapped;
   rep.pages_mapped = (mapped + kPageBytes - 1) / kPageBytes;
-  rep.va_base = va_base;
+  rep.va_base = h.va_base;
   rep.proved = 1;
   const bool ran[kPasses] = {true, tagged, true};
   for (int k = 0; k < kPasses; ++k) rep.pass[k].ran = ran[k];
@@ -1165,7 +1184,7 @@ static int take_cover(ScrubEngine* e, cudaStream_t st, uint64_t mapped, uint64_t
       exact &= c == expected;
     }
     if (!exact) {
-      cp.chunk = chunk_of(lo);
+      cp.chunk = h.chunk_of(lo);
       pages.push_back(cp);
     }
   }
@@ -1287,11 +1306,10 @@ static std::vector<uint32_t> probe_cover_expected(const std::vector<CheckSpan>& 
 }
 
 // After the probe of a call both proven and probed (the caller holds e->mu): copies the probe cover maps once, zeroes
-// them for the next call, and compares every step against probe_cover_expected(chunks).  Fills *out (proved = 1),
-// e->pcover and e->pcover_pages; each inexact page gets chunk_of(page offset).
-template <typename ChunkOf>
-static int take_probe_cover(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& chunks, uint64_t va_base,
-                            ccm_probe_cover* out, ChunkOf&& chunk_of) {
+// them for the next call, and compares every step against probe_cover_expected(h.probe_chunks).  Fills *out
+// (proved = 1), e->pcover and e->pcover_pages; each inexact page gets h.chunk_of(page offset).
+static int take_probe_cover(ScrubEngine* e, cudaStream_t st, const Held& h, ccm_probe_cover* out) {
+  const std::vector<CheckSpan>& chunks = h.probe_chunks;
   const double t0 = now_ms();
   const size_t bytes = kSteps * e->npages * sizeof(uint32_t);
   CCM_CUDA(cudaMemcpyAsync(e->h_pcover, e->d_pcover, bytes, cudaMemcpyDeviceToHost, st));
@@ -1302,7 +1320,7 @@ static int take_probe_cover(ScrubEngine* e, cudaStream_t st, const std::vector<C
   const std::vector<uint32_t> exp = probe_cover_expected(chunks, np);
   ccm_probe_cover rep;
   memset(&rep, 0, sizeof rep);
-  rep.va_base = va_base;
+  rep.va_base = h.va_base;
   rep.proved = 1;
   for (const CheckSpan& c : chunks) {
     uint64_t w0 = 0, nwin = 0;
@@ -1332,7 +1350,7 @@ static int take_probe_cover(ScrubEngine* e, cudaStream_t st, const std::vector<C
       exact &= c == exp[p];
     }
     if (!exact) {
-      cp.chunk = chunk_of(p * kPageBytes);
+      cp.chunk = h.chunk_of(p * kPageBytes);
       pages.push_back(cp);
     }
   }
@@ -1353,19 +1371,18 @@ static int take_probe_cover(ScrubEngine* e, cudaStream_t st, const std::vector<C
   return CCM_OK;
 }
 
-// The alias probe (ccm.h: ccm_scrub_probe) over `chunks` (each with its offset in what the reports describe; the caller
-// holds e->mu, and every kernel of the call has finished): P1 over every chunk, the "probe_mismatch" drill, P2, the
-// "probe_dirt" drill, P3, one launch per chunk per step in order.  Fills *rep (probed = 1) and *p3 (P3's count); after
-// P2 mismatches, *mrep (classified against `spans`, chunk_of(offset)) and the mismatch page map.  After an error it
-// drops the check book.  prove: the proving twins run instead, each step into its probe cover map (the caller takes
-// them), with page 0 at each chunk's c.addr - c.offset.
-template <typename ChunkOf>
-static int run_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& chunks,
-                     const std::vector<CheckSpan>& spans, uint32_t seed, const ScrubDrill& drill, uint64_t va_base,
-                     bool prove, ccm_probe_report* rep, ccm_mismatch_report* mrep, uint64_t* p3, ChunkOf&& chunk_of) {
+// The alias probe (ccm.h: ccm_scrub_probe) over h.probe_chunks (each with its offset in what the reports describe; the
+// caller holds e->mu, and every kernel of the call has finished): P1 over every chunk, the "probe_mismatch" drill, P2,
+// the "probe_dirt" drill, P3, one launch per chunk per step in order.  Fills *rep (probed = 1) and *p3 (P3's count);
+// after P2 mismatches, *mrep (take_mismatch over `h`) and the mismatch page map.  After an error it drops the check
+// book.  prove: the proving twins run instead, each step into its probe cover map (the caller takes them), with page 0
+// at each chunk's c.addr - c.offset.
+static int run_probe(ScrubEngine* e, cudaStream_t st, const Held& h, uint32_t seed, const ScrubDrill& drill, bool prove,
+                     ccm_probe_report* rep, ccm_mismatch_report* mrep, uint64_t* p3) {
+  const std::vector<CheckSpan>& chunks = h.probe_chunks;
   memset(rep, 0, sizeof *rep);
   rep->seed = seed;
-  rep->va_base = va_base;
+  rep->va_base = h.va_base;
   if (prove) e->gate.pcover_dirty = true;
   uint64_t skip = drill.probe_skip;   // "probe_skip": pending for the first launch of step probe_skip_step
   // one launch of step k (0 = P1, 1 = P2, 2 = P3) per chunk with windows; the grid from the launched kernel's occupancy
@@ -1456,9 +1473,9 @@ static int run_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpa
   memset(mrep, 0, sizeof *mrep);
   mrep->located = 1;
   mrep->seed = seed;
-  mrep->va_base = va_base;
+  mrep->va_base = h.va_base;
   if (rep->mismatch_bytes != 0) {
-    if ((rc = take_mismatch(e, st, rep->mismatch_bytes, seed, va_base, spans, mrep, chunk_of)) != CCM_OK) {
+    if ((rc = take_mismatch(e, st, rep->mismatch_bytes, seed, h, mrep)) != CCM_OK) {
       drop_book(e, kCheckBook, st);
       e->pages[kCheckBook].clear();
       return rc;
@@ -1470,19 +1487,17 @@ static int run_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpa
 
 // The product call's probe: armed, zero gate, clean read-back.  A seed per call; e->probe and (after mismatches)
 // e->mismatch get the reports.  A proven call (its passes still counting, and the probe cover maps set aside) proves
-// the probe too, into *pcover and e->pcover, with page 0 at va_base.
-template <typename ChunkOf>
-static int gate_probe(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& chunks,
-                      const std::vector<CheckSpan>& spans, const ScrubDrill& drill, uint64_t va_base,
-                      ccm_probe_report* out, ccm_probe_cover* pcover, uint64_t* p3, ChunkOf&& chunk_of) {
+// the probe too, into *pcover and e->pcover, with page 0 at h.va_base.
+static int gate_probe(ScrubEngine* e, cudaStream_t st, const Held& h, const ScrubDrill& drill, ccm_probe_report* out,
+                      ccm_probe_cover* pcover, uint64_t* p3) {
   const uint32_t seed = std::random_device{}();
   const bool prove = e->gate.prove && e->d_pcover;
   ccm_mismatch_report mrep;
-  int rc = run_probe(e, st, chunks, spans, seed, drill, va_base, prove, out, &mrep, p3, chunk_of);
+  int rc = run_probe(e, st, h, seed, drill, prove, out, &mrep, p3);
   if (rc != CCM_OK) { memset(out, 0, sizeof *out); return rc; }
   e->probe = *out;
   if (out->mismatch_bytes != 0) e->mismatch = mrep;
-  if (prove) rc = take_probe_cover(e, st, chunks, va_base, pcover, chunk_of);
+  if (prove) rc = take_probe_cover(e, st, h, pcover);
   return rc;
 }
 
@@ -1642,6 +1657,54 @@ static void triage_mismatch(ScrubEngine* e, cudaStream_t st, const std::vector<C
       kCheckBook, kDirtBook};
   run_triage(e, st, spans, drill, e->pages[kCheckBook], e->mismatch.va_base, e->mtriage_hold_ms, steps, &e->mtriage,
              &e->mtriage_pages);
+}
+
+// The reports of a product call, on the VMM path and the fallback alike.  The caller holds e->mu, every pass of the
+// call has finished (`rc`: how they ended), and the call still holds `h`.  In order: the alias probe (armed zero gate
+// whose read-back was clean; *nonzero becomes P3's count), the coverage proof, where the tags were wrong (tagged call,
+// mismatch_bytes != 0), what the first pass erased (census call), where the dirt is and its triage (*nonzero != 0), and
+// the mismatch triage.  Only the probe and the proof can fail the call; the other reports are left empty when they
+// cannot be taken.  After a failure it takes nothing and drops the books the passes filled.
+static int finish_gate(ScrubEngine* e, cudaStream_t st, int rc, const Held& h, const ScrubDrill& drill,
+                       ccm_tag_result* tag, ccm_residue_report* res, uint64_t* nonzero, ccm_probe_report* probe,
+                       ccm_probe_cover* pcover, ccm_cover_report* cover) {
+  e->gate.active = false;   // the probe, the locate pass and the triages are not the call's passes
+  if (rc == CCM_OK && probe && *nonzero == 0 && h.bytes) {
+    uint64_t p3 = 0;
+    rc = gate_probe(e, st, h, drill, probe, pcover, &p3);
+    if (rc == CCM_OK) *nonzero = p3;
+  }
+  if (rc == CCM_OK && e->gate.prove) rc = take_cover(e, st, h, tag != nullptr, cover);
+  if (rc != CCM_OK) {
+    if (tag) drop_book(e, kCheckBook, st);
+    if (res) drop_book(e, kCensusBook, st);
+    return rc;
+  }
+  const bool mismatched = tag && tag->mismatch_bytes != 0;
+  if (mismatched) {
+    ccm_mismatch_report rep;
+    if (take_mismatch(e, st, tag->mismatch_bytes, tag->seed, h, &rep) == CCM_OK) e->mismatch = rep;
+  }
+  if (res && take_residue(e, st, h, res) != CCM_OK) memset(res, 0, sizeof *res);
+  if (*nonzero != 0) {   // one locate launch per span, before the memory goes back
+    ccm_dirt_report rep;
+    memset(&rep, 0, sizeof rep);
+    rep.va_base = h.va_base;
+    e->pages[kDirtBook].clear();
+    int lrc = CCM_OK;
+    for (const CheckSpan& sp : h.spans)
+      if ((lrc = locate_range(e, (const void*)(uintptr_t)sp.addr, sp.bytes, sp.offset, st, &rep, h)) != CCM_OK) break;
+    if (lrc == CCM_OK) {
+      sort_records(&rep, rep.dirty_windows);
+      finish_pages(e, kDirtBook, h);
+      e->dirt = rep;
+      triage_dirt(e, st, h.spans, drill);
+    } else {
+      e->pages[kDirtBook].clear();
+    }
+  }
+  if (mismatched) triage_mismatch(e, st, h.spans, drill, tag->seed);
+  return CCM_OK;
 }
 
 int engine_arena_scrub(ScrubEngine* e, int variant, const ccm_launch_cfg* cfg, void* stream, float* ms) {
@@ -1843,67 +1906,37 @@ static int arena_drill(ScrubEngine* e, int fill, uint64_t inject, uint64_t resid
   return CCM_OK;
 }
 
-// The segment a fallback offset (into the concatenated segments) lies in: the last one that starts at or before it.
-static uint32_t segment_of(const std::vector<Segment>& segs, uint64_t o) {
-  uint32_t i = 0;
-  uint64_t start = 0;
-  for (size_t k = 0; k < segs.size(); start += segs[k].bytes, ++k)
-    if ((int64_t)start <= (int64_t)o) i = (uint32_t)k;
-  return i;
-}
-
-// The zero gate's first pass on the fallback path, with the census: one census launch per segment (timed as the
-// scrub, *ms), offsets into the concatenated segments, chunk = segment index.
-static int arena_census(ScrubEngine* e, ccm_residue_report* res, float* ms) {
+// The zero gate's first pass on the fallback path, with the census: one census launch per segment (`spans`, offsets
+// into the concatenated segments), timed as the scrub (*ms).
+static int arena_census(ScrubEngine* e, const std::vector<CheckSpan>& spans, float* ms) {
   std::lock_guard<std::mutex> g(e->mu);
   CCM_ENSURE_READY(e);
   int rc = need_arena(e); if (rc) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->stream;
-  rc = run_timed(e, st, ms, [&]() -> int {
-    uint64_t shift = 0;
-    for (auto& s : e->segs) {
-      if (int rc2 = census_range(e, s.ptr, s.bytes, false, 0, st, (uint64_t)(uintptr_t)s.ptr - shift)) return rc2;
-      shift += s.bytes;
-    }
+  return run_timed(e, st, ms, [&]() -> int {
+    for (const CheckSpan& sp : spans)
+      if (int rc2 = census_range(e, (void*)(uintptr_t)sp.addr, sp.bytes, false, 0, st, sp.addr - sp.offset)) return rc2;
     return CCM_OK;
   });
-  if (rc) { drop_book(e, kCensusBook, st); return rc; }
-  return take_residue(e, st, (uint64_t)(uintptr_t)e->segs.front().ptr, e->arena_bytes, res,
-                      [&](uint64_t o) { return segment_of(e->segs, o); });
 }
 
-// What the fallback path holds, as the spans of its checks and triages: every segment, with its offset into the
-// concatenated segments.
-static std::vector<CheckSpan> arena_spans(const std::vector<Segment>& segs) {
-  std::vector<CheckSpan> spans;
-  uint64_t shift = 0;
-  for (const Segment& s : segs) {
-    spans.push_back({(uint64_t)(uintptr_t)s.ptr, s.bytes, shift});
-    shift += s.bytes;
-  }
-  return spans;
-}
-
-// Tagged pass of the product call's fallback path: tag every segment, then (after the "tag_flood" and "tag_inject"
-// drills) check and zero every segment.  Fills tag->mismatch_bytes, ->ms_tag, ->ms_check, ->va_base, and after
-// mismatches the engine's mismatch report (offsets into the concatenated segments, chunk = segment index).
-// res (census call): the fills are census fills, and `res` gets what they found.
-static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inject, int tag_flood,
-                           ccm_residue_report* res) {
+// Tagged pass of the product call's fallback path: tag every segment (`spans`), then (after the "tag_flood" and
+// "tag_inject" drills) check and zero every segment.  Fills tag->mismatch_bytes, ->ms_tag, ->ms_check and ->va_base.
+// census (census call): the fills are census fills.
+static int arena_tag_check(ScrubEngine* e, const std::vector<CheckSpan>& spans, ccm_tag_result* tag,
+                           uint64_t tag_inject, int tag_flood, bool census) {
   std::lock_guard<std::mutex> g(e->mu);
   CCM_ENSURE_READY(e);
   int rc = need_arena(e); if (rc) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
   cudaStream_t st = e->stream;
-  auto chunk_of = [&](uint64_t o) { return segment_of(e->segs, o); };
-  const std::vector<CheckSpan> spans = arena_spans(e->segs);
   // fills between ev[0] and ev[2], the drill, checks between ev[3] and ev[1]
   rc = run_counted(e, st, kMismatch, &tag->mismatch_bytes, nullptr, [&]() -> int {
     for (const CheckSpan& sp : spans) {
       void* p = (void*)(uintptr_t)sp.addr;
-      if (int rc2 = res ? census_range(e, p, sp.bytes, true, tag->seed, st, sp.addr - sp.offset)
-                        : tag_fill_range(e, p, sp.bytes, tag->seed, st))
+      if (int rc2 = census ? census_range(e, p, sp.bytes, true, tag->seed, st, sp.addr - sp.offset)
+                           : tag_fill_range(e, p, sp.bytes, tag->seed, st))
         return rc2;
     }
     CCM_CUDA(cudaEventRecord(e->ev[2], st));
@@ -1917,79 +1950,14 @@ static int arena_tag_check(ScrubEngine* e, ccm_tag_result* tag, uint64_t tag_inj
       if (int rc2 = tag_check_range(e, (void*)(uintptr_t)sp.addr, sp.bytes, tag->seed, st, sp.addr - sp.offset)) return rc2;
     return CCM_OK;
   });
-  if (rc) {
-    drop_book(e, kCheckBook, st);
-    if (res) drop_book(e, kCensusBook, st);
-    return rc;
-  }
+  if (rc) return rc;
   float a = 0, b = 0;
   CCM_CUDA(cudaEventElapsedTime(&a, e->ev[0], e->ev[2]));
   CCM_CUDA(cudaEventElapsedTime(&b, e->ev[3], e->ev[1]));
   tag->ms_tag = a;
   tag->ms_check = b;
   tag->va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
-  if (tag->mismatch_bytes != 0) {   // a failure of the report leaves it empty; it never changes the verdict
-    ccm_mismatch_report rep;
-    if (take_mismatch(e, st, tag->mismatch_bytes, tag->seed, tag->va_base, spans, &rep, chunk_of) == CCM_OK) e->mismatch = rep;
-  }
-  if (res) return take_residue(e, st, tag->va_base, e->arena_bytes, res, chunk_of);
   return CCM_OK;
-}
-
-// The dirt report of the fallback path: one locate pass per segment, offsets into the concatenated segments,
-// chunk = segment index.  A failure of the pass leaves the report empty; it never changes the verdict.  Then, when the
-// device is armed, the triage of the dirt, segment by segment (`drill`: the call's drills).
-static void arena_locate(ScrubEngine* e, const ScrubDrill& drill) {
-  std::lock_guard<std::mutex> g(e->mu);
-  if (!e->ready || e->segs.empty() || cudaSetDevice(e->ordinal) != cudaSuccess) return;
-  ccm_dirt_report rep;
-  memset(&rep, 0, sizeof rep);
-  rep.va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
-  e->pages[kDirtBook].clear();
-  uint64_t shift = 0;
-  for (size_t i = 0; i < e->segs.size(); ++i) {
-    if (locate_range(e, e->segs[i].ptr, e->segs[i].bytes, shift, e->stream, &rep, [i](uint64_t) { return (uint32_t)i; })) {
-      e->pages[kDirtBook].clear();
-      return;
-    }
-    shift += e->segs[i].bytes;
-  }
-  sort_records(&rep, rep.dirty_windows);
-  finish_pages(e, kDirtBook, [&](uint64_t o) { return segment_of(e->segs, o); });
-  e->dirt = rep;
-  triage_dirt(e, e->stream, arena_spans(e->segs), drill);
-}
-
-// The mismatch triage of the fallback path, when the device is armed: segment by segment, with the offsets of the
-// mismatch report (into the concatenated segments).
-static void arena_triage_mismatch(ScrubEngine* e, uint32_t seed, const ScrubDrill& drill) {
-  std::lock_guard<std::mutex> g(e->mu);
-  if (!e->ready || e->segs.empty() || cudaSetDevice(e->ordinal) != cudaSuccess) return;
-  triage_mismatch(e, e->stream, arena_spans(e->segs), drill, seed);
-}
-
-// The coverage proof of the fallback path, after its read-back: page offsets into the concatenated segments from the
-// first segment's address, chunk = segment index.
-static int arena_cover(ScrubEngine* e, bool tagged, ccm_cover_report* out) {
-  std::lock_guard<std::mutex> g(e->mu);
-  e->gate.active = false;
-  if (!e->gate.prove) return CCM_OK;
-  CCM_CUDA(cudaSetDevice(e->ordinal));
-  return take_cover(e, e->stream, e->arena_bytes, (uint64_t)(uintptr_t)e->segs.front().ptr, tagged, out,
-                    [&](uint64_t o) { return segment_of(e->segs, o); });
-}
-
-// The alias probe of the fallback path, after its read-back: segment by segment, offsets into the concatenated
-// segments, chunk = segment index.  *nz = P3's count.
-static int arena_probe(ScrubEngine* e, const ScrubDrill& drill, ccm_probe_report* out, ccm_probe_cover* pcover,
-                       uint64_t* nz) {
-  std::lock_guard<std::mutex> g(e->mu);
-  CCM_ENSURE_READY(e);
-  int rc = need_arena(e); if (rc) return rc;
-  CCM_CUDA(cudaSetDevice(e->ordinal));
-  const std::vector<CheckSpan> spans = arena_spans(e->segs);
-  return gate_probe(e, e->stream, spans, spans, drill, (uint64_t)(uintptr_t)e->segs.front().ptr, out, pcover, nz,
-                    [&](uint64_t o) { return segment_of(e->segs, o); });
 }
 
 // ------------------------------------------------------- VMM (driver API, lazy)
@@ -2109,7 +2077,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   VmmMapping m;
   if (api.AddressReserve(&m.base, va_bytes, 0, 0, 0) != CUDA_SUCCESS) return CCM_ERR_UNSUPPORTED;
   m.va_bytes = va_bytes;
-  e->gate.spans = {{(uint64_t)m.base, va_bytes, (uint64_t)m.base}};
+  e->gate.spans = {{(uint64_t)m.base, va_bytes, 0}};
   cudaStream_t st = e->stream;
   CUmemAccessDesc acc;
   memset(&acc, 0, sizeof acc);
@@ -2127,7 +2095,6 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   std::vector<std::pair<uint64_t, uint64_t>> deferred;  // tagged: main-zone ranges, checked after the last mapping
   std::vector<std::pair<uint64_t, uint32_t>> pieces;    // (offset, handle index) of every mapped piece, ascending
   std::vector<CheckSpan> iters;                         // every iteration of the mapping loop, for the alias probe
-  bool checked = false;                                 // tagged: a check was enqueued (its book may be non-zero)
   // Census call: the first pass over each mapping (the scrub, or the tag fill) is the census of the same range.
   ccm_residue_report* res = current_residue_call();
   uint64_t residue = drill.residue;                     // "scrub_residue" budget, spent in mapping order
@@ -2150,7 +2117,6 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     }
     cudaEvent_t* evs = timed < kMaxPipeChunks ? e->pipe_ev[timed] : nullptr;
     if (evs) cudaEventRecord(evs[0], st);
-    checked |= tag != nullptr;
     int rc2 = tag ? tag_check_range(e, (void*)(m.base + off), n, tag->seed, st, (uint64_t)m.base)
             : res ? census_range(e, (void*)(m.base + off), n, false, 0, st, (uint64_t)m.base)
                   : scrub_range(e, (void*)(m.base + off), n, CCM_SCRUB_AUTO, nullptr, st);
@@ -2249,7 +2215,6 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     rc = CCM_ERR_CUDA;
   cudaError_t serr = cudaStreamSynchronize(st);  // nothing may still touch the mapping below
   if (rc == CCM_OK && serr != cudaSuccess) { set_error("stream sync failed: %s", cudaGetErrorString(serr)); rc = CCM_ERR_CUDA; }
-  e->gate.active = false;   // the locate pass and the triages below are not the call's passes
 
   const uint64_t mapped = m.mapped;
   const int nchunks = (int)m.handles.size();
@@ -2285,53 +2250,9 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
       tag->va_base = mapped ? (uint64_t)m.base : 0;
     }
   }
-  auto chunk_of = [&](uint64_t o) {
-    auto it = std::upper_bound(pieces.begin(), pieces.end(), o,
-                               [](uint64_t v, const std::pair<uint64_t, uint32_t>& pc) { return v < pc.first; });
-    return it == pieces.begin() ? 0u : std::prev(it)->second;
-  };
-  // ---- alias probe: armed zero gate whose read-back was clean, after the last read-back -----------------------
-  if (rc == CCM_OK && probe && r->nonzero_bytes == 0 && mapped) {
-    uint64_t p3 = 0;
-    rc = gate_probe(e, st, iters, {{(uint64_t)m.base, mapped, 0}}, drill, (uint64_t)m.base, probe, pcover, &p3,
-                    chunk_of);
-    if (rc == CCM_OK) r->nonzero_bytes = p3;
-  }
-  // ---- coverage proof: one copy of the cover maps, no launch ------------------------------------------------
-  if (rc == CCM_OK && e->gate.prove) rc = take_cover(e, st, mapped, (uint64_t)m.base, tag != nullptr, cover, chunk_of);
-  // ---- a failed tagged check: where were the tags wrong?  The checks booked it; one copy, no launch ---------
-  if (checked && rc == CCM_OK && tag->mismatch_bytes != 0) {
-    ccm_mismatch_report rep;
-    const std::vector<CheckSpan> spans{{(uint64_t)m.base, mapped, 0}};
-    if (take_mismatch(e, st, tag->mismatch_bytes, tag->seed, (uint64_t)m.base, spans, &rep, chunk_of) == CCM_OK)
-      e->mismatch = rep;   // never changes the verdict
-  } else if (checked && rc != CCM_OK) {
-    drop_book(e, kCheckBook, st);
-  }
-  // ---- census call: what the first pass found.  The censuses booked it; one copy, no launch ----------------
-  if (res && rc == CCM_OK) {
-    if (take_residue(e, st, (uint64_t)m.base, mapped, res, chunk_of) != CCM_OK) memset(res, 0, sizeof *res);
-  } else if (res) {
-    drop_book(e, kCensusBook, st);
-  }
-  // ---- a failed read-back: where is the dirt?  One more launch, before the mapping goes back -------------
-  if (rc == CCM_OK && r->nonzero_bytes != 0) {
-    ccm_dirt_report rep;
-    memset(&rep, 0, sizeof rep);
-    rep.va_base = (uint64_t)m.base;
-    e->pages[kDirtBook].clear();
-    if (locate_range(e, (const void*)m.base, mapped, 0, st, &rep, chunk_of) == CCM_OK) {  // never changes the verdict
-      sort_records(&rep, rep.dirty_windows);
-      finish_pages(e, kDirtBook, chunk_of);
-      e->dirt = rep;
-      triage_dirt(e, st, {{(uint64_t)m.base, mapped, 0}}, drill);   // armed: what kind of dirt, while it is mapped
-    } else {
-      e->pages[kDirtBook].clear();
-    }
-  }
-  // ---- a failed tagged check, armed: what kind of mismatch, while it is mapped ----------------------------
-  if (checked && rc == CCM_OK && tag->mismatch_bytes != 0)
-    triage_mismatch(e, st, {{(uint64_t)m.base, mapped, 0}}, drill, tag->seed);
+  // ---- the reports, before the mapping goes back: an alias piece maps to handle 0 ----------------------------
+  const Held h{(uint64_t)m.base, mapped, {{(uint64_t)m.base, mapped, 0}}, std::move(iters), std::move(pieces)};
+  rc = finish_gate(e, st, rc, h, drill, tag, res, &r->nonzero_bytes, probe, pcover, cover);
   // ---- give the HBM back: on the reaper (default) or right here -----------------------
   if (rc == CCM_OK && async_release_enabled()) {
     r->release_deferred = 1;
@@ -2417,10 +2338,18 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     ccm_arena_info ai;
     rc = engine_arena_acquire(e, bytes, &ai);
     if (rc == CCM_OK) {
+      Held h;   // every segment, at its offset into the concatenated segments; chunk = segment index
       {
         std::lock_guard<std::mutex> g(e->mu);
         rc = begin_gate(e, drill);
-        for (const CheckSpan& sp : arena_spans(e->segs)) e->gate.spans.push_back({sp.addr, sp.bytes, sp.addr - sp.offset});
+        h.va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
+        for (const Segment& s : e->segs) {
+          h.chunks.emplace_back(h.bytes, (uint32_t)h.spans.size());
+          h.spans.push_back({(uint64_t)(uintptr_t)s.ptr, s.bytes, h.bytes});
+          h.bytes += s.bytes;
+        }
+        h.probe_chunks = h.spans;
+        e->gate.spans = h.spans;
       }
       r.ms_acquire = ai.ms_acquire;
       r.bytes_scrubbed = ai.bytes;
@@ -2432,19 +2361,20 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
       uint64_t nz = 0;
       if (rc == CCM_OK) rc = arena_drill(e, drill.poison, 0, drill.residue);
       if (rc == CCM_OK && tag) {
-        rc = arena_tag_check(e, tag, drill.tag_inject, drill.tag_flood, res);
+        rc = arena_tag_check(e, h.spans, tag, drill.tag_inject, drill.tag_flood, res != nullptr);
         ms_s = (float)tag->ms_check;
       } else if (rc == CCM_OK && res) {
-        rc = arena_census(e, res, &ms_s);
+        rc = arena_census(e, h.spans, &ms_s);
       } else if (rc == CCM_OK) {
         rc = engine_arena_scrub(e, CCM_SCRUB_AUTO, nullptr, nullptr, &ms_s);
       }
       if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
       if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
-      if (rc == CCM_OK && probe_out && nz == 0) rc = arena_probe(e, drill, probe_out, &pcover, &nz);
-      if (rc == CCM_OK) rc = arena_cover(e, tag != nullptr, &cover);
-      if (rc == CCM_OK && nz != 0) arena_locate(e, drill);
-      if (rc == CCM_OK && tag && tag->mismatch_bytes != 0) arena_triage_mismatch(e, tag->seed, drill);
+      {
+        std::lock_guard<std::mutex> g(e->mu);
+        if (rc == CCM_OK) rc = need_arena(e);   // torn down since the read-back: nothing is held any more
+        rc = finish_gate(e, e->stream, rc, h, drill, tag, res, &nz, probe_out, &pcover, &cover);
+      }
       r.ms_scrub = ms_s;
       r.ms_verify = ms_v;
       r.nonzero_bytes = nz;
@@ -2617,10 +2547,7 @@ extern "C" int ccm_region_tag_check_locate(int cuda_ordinal, void* dptr, uint64_
   rep.located = 1;
   rep.seed = seed;
   rep.va_base = base;
-  if (count != 0) {
-    const std::vector<CheckSpan> spans{{base, bytes, 0}};
-    if ((rc = take_mismatch(e, st, count, seed, base, spans, &rep, [](uint64_t) { return 0u; }))) return rc;
-  }
+  if (count != 0 && (rc = take_mismatch(e, st, count, seed, region_held(dptr, bytes), &rep))) return rc;
   *out = rep;
   return CCM_OK;
 }
@@ -2638,11 +2565,13 @@ extern "C" int ccm_region_census(int cuda_ordinal, void* dptr, uint64_t bytes, i
   cudaStream_t st = e->pick(stream);
   const uint64_t base = (uint64_t)(uintptr_t)dptr;
   if (int rc = census_range(e, dptr, bytes, store_tags != 0, seed, st, base)) { drop_book(e, kCensusBook, st); return rc; }
-  return take_residue(e, st, base, bytes, out, [](uint64_t) { return 0u; });
+  return take_residue(e, st, region_held(dptr, bytes), out);
 }
 
-// ------------------------------------------------------------------------- mismatch report
-extern "C" int ccm_scrub_last_mismatch(int cuda_ordinal, ccm_mismatch_report* out) {
+// ------------------------------------------------------------------------- the last product call's reports
+// The last report `rep` of one kind on a CUDA device.
+template <typename Report>
+static int last_report(int cuda_ordinal, Report* out, Report ScrubEngine::*rep) {
   if (!out) return CCM_ERR_INVALID;
   memset(out, 0, sizeof *out);
   if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
@@ -2652,51 +2581,15 @@ extern "C" int ccm_scrub_last_mismatch(int cuda_ordinal, ccm_mismatch_report* ou
   ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
   if (!e) return CCM_OK;
   std::lock_guard<std::mutex> g(e->mu);
-  *out = e->mismatch;
+  *out = e->*rep;
   return CCM_OK;
 }
 
-// ------------------------------------------------------------------------- dirt report
-extern "C" int ccm_scrub_last_dirt(int cuda_ordinal, ccm_dirt_report* out) {
-  if (!out) return CCM_ERR_INVALID;
-  memset(out, 0, sizeof *out);
-  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
-    set_error("no CUDA device with ordinal %d", cuda_ordinal);
-    return CCM_ERR_NO_CUDA;
-  }
-  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
-  if (!e) return CCM_OK;
-  std::lock_guard<std::mutex> g(e->mu);
-  *out = e->dirt;
-  return CCM_OK;
-}
-
-extern "C" int ccm_region_locate(int cuda_ordinal, const void* dptr, uint64_t bytes, void* stream, ccm_dirt_report* out) {
-  if (!out) return CCM_ERR_INVALID;
-  memset(out, 0, sizeof *out);
-  ScrubEngine* e = engine_for(cuda_ordinal);
-  if (!e) return CCM_ERR_NO_CUDA;
-  std::lock_guard<std::mutex> g(e->mu);
-  CCM_ENSURE_READY(e);
-  CCM_CUDA(cudaSetDevice(e->ordinal));
-  ccm_dirt_report rep;
-  memset(&rep, 0, sizeof rep);
-  rep.va_base = (uint64_t)(uintptr_t)dptr;
-  e->pages[kDirtBook].clear();
-  if (int rc = locate_range(e, dptr, bytes, 0, e->pick(stream), &rep, [](uint64_t) { return 0u; })) {
-    e->pages[kDirtBook].clear();
-    return rc;
-  }
-  sort_records(&rep, rep.dirty_windows);
-  finish_pages(e, kDirtBook, [](uint64_t) { return 0u; });
-  *out = rep;
-  return CCM_OK;
-}
-
-// ------------------------------------------------------------------------- page maps
-extern "C" int ccm_last_page_map(int cuda_ordinal, int book, ccm_page_entry* out, uint64_t cap, uint64_t* n) {
-  if (!n || (cap && !out) || book < CCM_BOOK_DIRT || book > CCM_BOOK_RESIDUE) {
-    set_error("ccm_last_page_map: book %d, cap %llu (needs n, and out when cap > 0)", book, (unsigned long long)cap);
+// The pages behind one report (`pages`: the engine's list of them, a member or a callable on the engine).
+template <typename Page, typename Pages>
+static int last_pages(const char* fn, int cuda_ordinal, Page* out, uint64_t cap, uint64_t* n, Pages pages) {
+  if (!n || (cap && !out)) {
+    set_error("%s: cap %llu (needs n, and out when cap > 0)", fn, (unsigned long long)cap);
     return CCM_ERR_INVALID;
   }
   *n = 0;
@@ -2707,10 +2600,53 @@ extern "C" int ccm_last_page_map(int cuda_ordinal, int book, ccm_page_entry* out
   ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no call ever reported anything (and none is started here)
   if (!e) return CCM_OK;
   std::lock_guard<std::mutex> g(e->mu);
-  const std::vector<ccm_page_entry>& v = e->pages[book - CCM_BOOK_DIRT];
+  const std::vector<Page>& v = std::invoke(pages, *e);
   *n = v.size();
-  if (cap) memcpy(out, v.data(), std::min<uint64_t>(cap, v.size()) * sizeof(ccm_page_entry));
+  if (cap) memcpy(out, v.data(), std::min<uint64_t>(cap, *n) * sizeof(Page));
   return CCM_OK;
+}
+
+// ------------------------------------------------------------------------- mismatch report
+extern "C" int ccm_scrub_last_mismatch(int cuda_ordinal, ccm_mismatch_report* out) {
+  return last_report(cuda_ordinal, out, &ScrubEngine::mismatch);
+}
+
+// ------------------------------------------------------------------------- dirt report
+extern "C" int ccm_scrub_last_dirt(int cuda_ordinal, ccm_dirt_report* out) {
+  return last_report(cuda_ordinal, out, &ScrubEngine::dirt);
+}
+
+extern "C" int ccm_region_locate(int cuda_ordinal, const void* dptr, uint64_t bytes, void* stream, ccm_dirt_report* out) {
+  if (!out) return CCM_ERR_INVALID;
+  memset(out, 0, sizeof *out);
+  ScrubEngine* e = engine_for(cuda_ordinal);
+  if (!e) return CCM_ERR_NO_CUDA;
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  const Held h = region_held(dptr, bytes);
+  ccm_dirt_report rep;
+  memset(&rep, 0, sizeof rep);
+  rep.va_base = h.va_base;
+  e->pages[kDirtBook].clear();
+  if (int rc = locate_range(e, dptr, bytes, 0, e->pick(stream), &rep, h)) {
+    e->pages[kDirtBook].clear();
+    return rc;
+  }
+  sort_records(&rep, rep.dirty_windows);
+  finish_pages(e, kDirtBook, h);
+  *out = rep;
+  return CCM_OK;
+}
+
+// ------------------------------------------------------------------------- page maps
+extern "C" int ccm_last_page_map(int cuda_ordinal, int book, ccm_page_entry* out, uint64_t cap, uint64_t* n) {
+  if (!n || (cap && !out) || book < CCM_BOOK_DIRT || book > CCM_BOOK_RESIDUE) {
+    set_error("ccm_last_page_map: book %d, cap %llu (needs n, and out when cap > 0)", book, (unsigned long long)cap);
+    return CCM_ERR_INVALID;
+  }
+  return last_pages("ccm_last_page_map", cuda_ordinal, out, cap, n,
+                    [book](const ScrubEngine& e) -> const std::vector<ccm_page_entry>& { return e.pages[book - CCM_BOOK_DIRT]; });
 }
 
 // ------------------------------------------------------------------------- dirt and mismatch triages
@@ -2734,52 +2670,16 @@ static int arm_triage(const char* fn, int cuda_ordinal, uint32_t hold_ms, uint32
   return CCM_OK;
 }
 
-// The last report of one triage (`rep`) on a CUDA device.
-static int last_triage(int cuda_ordinal, ccm_triage_report* out, ccm_triage_report ScrubEngine::*rep) {
-  if (!out) return CCM_ERR_INVALID;
-  memset(out, 0, sizeof *out);
-  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
-    set_error("no CUDA device with ordinal %d", cuda_ordinal);
-    return CCM_ERR_NO_CUDA;
-  }
-  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
-  if (!e) return CCM_OK;
-  std::lock_guard<std::mutex> g(e->mu);
-  *out = e->*rep;
-  return CCM_OK;
-}
-
-// The pages of that report (`pages`).
-static int last_triage_pages(const char* fn, int cuda_ordinal, ccm_triage_page* out, uint64_t cap, uint64_t* n,
-                             std::vector<ccm_triage_page> ScrubEngine::*pages) {
-  if (!n || (cap && !out)) {
-    set_error("%s: cap %llu (needs n, and out when cap > 0)", fn, (unsigned long long)cap);
-    return CCM_ERR_INVALID;
-  }
-  *n = 0;
-  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
-    set_error("no CUDA device with ordinal %d", cuda_ordinal);
-    return CCM_ERR_NO_CUDA;
-  }
-  ScrubEngine* e = engine_lookup(cuda_ordinal);
-  if (!e) return CCM_OK;
-  std::lock_guard<std::mutex> g(e->mu);
-  const std::vector<ccm_triage_page>& v = e->*pages;
-  *n = v.size();
-  if (cap) memcpy(out, v.data(), std::min<uint64_t>(cap, *n) * sizeof(ccm_triage_page));
-  return CCM_OK;
-}
-
 extern "C" int ccm_scrub_triage(int cuda_ordinal, uint32_t hold_ms) {
   return arm_triage("ccm_scrub_triage", cuda_ordinal, hold_ms, &ScrubEngine::triage_hold_ms);
 }
 
 extern "C" int ccm_scrub_last_triage(int cuda_ordinal, ccm_triage_report* out) {
-  return last_triage(cuda_ordinal, out, &ScrubEngine::triage);
+  return last_report(cuda_ordinal, out, &ScrubEngine::triage);
 }
 
 extern "C" int ccm_last_triage_pages(int cuda_ordinal, ccm_triage_page* out, uint64_t cap, uint64_t* n) {
-  return last_triage_pages("ccm_last_triage_pages", cuda_ordinal, out, cap, n, &ScrubEngine::triage_pages);
+  return last_pages("ccm_last_triage_pages", cuda_ordinal, out, cap, n, &ScrubEngine::triage_pages);
 }
 
 extern "C" int ccm_scrub_mismatch_triage(int cuda_ordinal, uint32_t hold_ms) {
@@ -2787,11 +2687,11 @@ extern "C" int ccm_scrub_mismatch_triage(int cuda_ordinal, uint32_t hold_ms) {
 }
 
 extern "C" int ccm_scrub_last_mismatch_triage(int cuda_ordinal, ccm_triage_report* out) {
-  return last_triage(cuda_ordinal, out, &ScrubEngine::mtriage);
+  return last_report(cuda_ordinal, out, &ScrubEngine::mtriage);
 }
 
 extern "C" int ccm_last_mismatch_triage_pages(int cuda_ordinal, ccm_triage_page* out, uint64_t cap, uint64_t* n) {
-  return last_triage_pages("ccm_last_mismatch_triage_pages", cuda_ordinal, out, cap, n, &ScrubEngine::mtriage_pages);
+  return last_pages("ccm_last_mismatch_triage_pages", cuda_ordinal, out, cap, n, &ScrubEngine::mtriage_pages);
 }
 
 // ------------------------------------------------------------------------- coverage proof
@@ -2816,35 +2716,11 @@ extern "C" int ccm_scrub_prove(int cuda_ordinal, int on) {
 }
 
 extern "C" int ccm_scrub_last_cover(int cuda_ordinal, ccm_cover_report* out) {
-  if (!out) return CCM_ERR_INVALID;
-  memset(out, 0, sizeof *out);
-  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
-    set_error("no CUDA device with ordinal %d", cuda_ordinal);
-    return CCM_ERR_NO_CUDA;
-  }
-  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
-  if (!e) return CCM_OK;
-  std::lock_guard<std::mutex> g(e->mu);
-  *out = e->cover;
-  return CCM_OK;
+  return last_report(cuda_ordinal, out, &ScrubEngine::cover);
 }
 
 extern "C" int ccm_last_cover_pages(int cuda_ordinal, ccm_cover_page* out, uint64_t cap, uint64_t* n) {
-  if (!n || (cap && !out)) {
-    set_error("ccm_last_cover_pages: cap %llu (needs n, and out when cap > 0)", (unsigned long long)cap);
-    return CCM_ERR_INVALID;
-  }
-  *n = 0;
-  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
-    set_error("no CUDA device with ordinal %d", cuda_ordinal);
-    return CCM_ERR_NO_CUDA;
-  }
-  ScrubEngine* e = engine_lookup(cuda_ordinal);
-  if (!e) return CCM_OK;
-  std::lock_guard<std::mutex> g(e->mu);
-  *n = e->cover_pages.size();
-  if (cap) memcpy(out, e->cover_pages.data(), std::min<uint64_t>(cap, *n) * sizeof(ccm_cover_page));
-  return CCM_OK;
+  return last_pages("ccm_last_cover_pages", cuda_ordinal, out, cap, n, &ScrubEngine::cover_pages);
 }
 
 // ------------------------------------------------------------------------- alias probe
@@ -2871,17 +2747,7 @@ extern "C" int ccm_scrub_probe(int cuda_ordinal, int on) {
 }
 
 extern "C" int ccm_scrub_last_probe(int cuda_ordinal, ccm_probe_report* out) {
-  if (!out) return CCM_ERR_INVALID;
-  memset(out, 0, sizeof *out);
-  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
-    set_error("no CUDA device with ordinal %d", cuda_ordinal);
-    return CCM_ERR_NO_CUDA;
-  }
-  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
-  if (!e) return CCM_OK;
-  std::lock_guard<std::mutex> g(e->mu);
-  *out = e->probe;
-  return CCM_OK;
+  return last_report(cuda_ordinal, out, &ScrubEngine::probe);
 }
 
 // ------------------------------------------------------------------------- probe proof
@@ -2890,35 +2756,11 @@ static_assert(sizeof(ccm_probe_cover_step) == 64 && sizeof(ccm_probe_cover) == 2
               "probe cover structs keep their layout");
 
 extern "C" int ccm_scrub_last_probe_cover(int cuda_ordinal, ccm_probe_cover* out) {
-  if (!out) return CCM_ERR_INVALID;
-  memset(out, 0, sizeof *out);
-  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
-    set_error("no CUDA device with ordinal %d", cuda_ordinal);
-    return CCM_ERR_NO_CUDA;
-  }
-  ScrubEngine* e = engine_lookup(cuda_ordinal);  // no engine: no product call ever ran (and none is started here)
-  if (!e) return CCM_OK;
-  std::lock_guard<std::mutex> g(e->mu);
-  *out = e->pcover;
-  return CCM_OK;
+  return last_report(cuda_ordinal, out, &ScrubEngine::pcover);
 }
 
 extern "C" int ccm_last_probe_cover_pages(int cuda_ordinal, ccm_probe_cover_page* out, uint64_t cap, uint64_t* n) {
-  if (!n || (cap && !out)) {
-    set_error("ccm_last_probe_cover_pages: cap %llu (needs n, and out when cap > 0)", (unsigned long long)cap);
-    return CCM_ERR_INVALID;
-  }
-  *n = 0;
-  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
-    set_error("no CUDA device with ordinal %d", cuda_ordinal);
-    return CCM_ERR_NO_CUDA;
-  }
-  ScrubEngine* e = engine_lookup(cuda_ordinal);
-  if (!e) return CCM_OK;
-  std::lock_guard<std::mutex> g(e->mu);
-  *n = e->pcover_pages.size();
-  if (cap) memcpy(out, e->pcover_pages.data(), std::min<uint64_t>(cap, *n) * sizeof(ccm_probe_cover_page));
-  return CCM_OK;
+  return last_pages("ccm_last_probe_cover_pages", cuda_ordinal, out, cap, n, &ScrubEngine::pcover_pages);
 }
 
 extern "C" int ccm_region_probe(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream,
@@ -2932,12 +2774,9 @@ extern "C" int ccm_region_probe(int cuda_ordinal, void* dptr, uint64_t bytes, ui
   CCM_ENSURE_READY(e);
   if (int rc = ensure_probe(e)) return rc;
   CCM_CUDA(cudaSetDevice(e->ordinal));
-  const uint64_t base = (uint64_t)(uintptr_t)dptr;
-  const std::vector<CheckSpan> spans{{base, bytes, 0}};
   ccm_mismatch_report rep;
   uint64_t p3 = 0;
-  const int rc = run_probe(e, e->pick(stream), spans, spans, seed, ScrubDrill(), base, false, out, &rep, &p3,
-                           [](uint64_t) { return 0u; });
+  const int rc = run_probe(e, e->pick(stream), region_held(dptr, bytes), seed, ScrubDrill(), false, out, &rep, &p3);
   if (rc != CCM_OK) { memset(out, 0, sizeof *out); return rc; }
   if (mismatch) *mismatch = rep;
   return CCM_OK;
