@@ -707,6 +707,14 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
     if (v < 0 || v > 3) { set_error("sim key 'probe_skip_step' takes 0..3, not %lld", (long long)v); return CCM_ERR_INVALID; }
     d.drill.probe_skip_step = v == 0 ? 2 : (int)v;
   }
+  else if (k == "report_skip") d.drill.report_skip = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "report_skip_step") {
+    if (v < 0 || v > (int64_t)CCM_REPORT_STEPS) {
+      set_error("sim key 'report_skip_step' takes 0..%u, not %lld", CCM_REPORT_STEPS, (long long)v);
+      return CCM_ERR_INVALID;
+    }
+    d.drill.report_skip_step = v == 0 ? (int)CCM_REPORT_DIRT_T3 : (int)v;
+  }
   else if (k == "cover_pass") {
     if (v < 0 || v > CCM_PASS_READBACK) { set_error("sim key 'cover_pass' takes 0..3, not %lld", (long long)v); return CCM_ERR_INVALID; }
     d.drill.cover_pass = v == 0 ? (int)CCM_PASS_READBACK : (int)v;
@@ -765,6 +773,8 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "probe_dirt") *value = (int64_t)d.drill.probe_dirt;
     else if (k == "probe_skip") *value = (int64_t)d.drill.probe_skip;
     else if (k == "probe_skip_step") *value = d.drill.probe_skip_step;
+    else if (k == "report_skip") *value = (int64_t)d.drill.report_skip;
+    else if (k == "report_skip_step") *value = d.drill.report_skip_step;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

@@ -64,6 +64,9 @@ int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, b
 // Drill of the probe proof (sim keys "probe_skip", "probe_skip_step"; ccm.h), in every call that probes:
 //   probe_skip:     the first launch of step probe_skip_step (1..3 = P1..P3; the sim key's 0 is stored as 2) starts
 //                   that many windows later and takes that many fewer (at most all of its windows).
+// Drill of the report proof (sim keys "report_skip", "report_skip_step"; ccm.h), armed or not:
+//   report_skip:    that many is written into the grab word of the first launch of report step report_skip_step
+//                   (CCM_REPORT_*; the sim key's 0 is stored as CCM_REPORT_DIRT_T3), just before it on the stream.
 struct ScrubDrill {
   uint64_t inject = 0;
   int poison = 0;
@@ -80,6 +83,8 @@ struct ScrubDrill {
   uint64_t probe_dirt = 0;
   uint64_t probe_skip = 0;
   int probe_skip_step = 2;
+  uint64_t report_skip = 0;
+  int report_skip_step = CCM_REPORT_DIRT_T3;
 };
 // inject: the call's "scrub_inject" budget.  Its poison and flood drills are those current_scrub_drill()
 // returns on the calling thread.  (The engine entry points keep the signatures that host-only builds of

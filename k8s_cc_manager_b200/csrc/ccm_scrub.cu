@@ -180,8 +180,12 @@ static Held region_held(const void* p, uint64_t bytes) {
 }
 
 // The product call's passes while it enqueues them (ccm.h: ccm_scrub_prove, and the "cover_skip" drill).  Every range
-// launch of the scrub, census, tag fill, tag check and read-back asks it for its cover map (gate_launch); the locate pass
-// and the triages run after it is cleared.
+// launch of the scrub, census, tag fill, tag check and read-back asks it for its cover map (gate_launch).  The locate
+// pass and the triages run after it is cleared, each step with `report` set (ccm.h: ccm_report_cover, and the
+// "report_skip" drill): their launches ask it for the report step's map.
+static constexpr int kPasses = 3;   // CCM_PASS_FIRST, CHECK, READBACK
+static constexpr int kSteps = 3;    // the alias probe's P1, P2, P3
+static constexpr int kReportSteps = (int)CCM_REPORT_STEPS;   // CCM_REPORT_LOCATE .. CCM_REPORT_MISMATCH_T3
 struct GatePasses {
   bool active = false;   // the call's passes are being enqueued
   bool prove = false;    // ... with the proving kernels, into the cover maps
@@ -189,9 +193,13 @@ struct GatePasses {
   int skip_pass = 0;     // drill "cover_skip": pending for the first launch of this pass (CCM_PASS_*; 0 = none)
   uint64_t skip = 0;
   bool pcover_dirty = false;   // the probe's proving twins counted into the probe cover maps, not yet taken
+  int report = 0;        // the report step (CCM_REPORT_*) being enqueued once the passes are over; 0 = none
+  bool report_prove = false;   // ... with the proving kernels, into the report cover maps
+  int skip_report = 0;   // drill "report_skip": pending for the first launch of this report step (0 = none)
+  uint64_t report_skip = 0;
+  uint64_t report_launches[kReportSteps] = {};   // launches of each report step
+  bool rcover_dirty = false;   // a report step's proving twins counted into its map, not yet taken
 };
-static constexpr int kPasses = 3;   // CCM_PASS_FIRST, CHECK, READBACK
-static constexpr int kSteps = 3;    // the alias probe's P1, P2, P3
 
 struct ScrubEngine {
   int ordinal = -1;
@@ -237,6 +245,10 @@ struct ScrubEngine {
   int pcover_ctas[3] = {};                  // CTAs per SM of each step's proving twin
   ccm_probe_cover pcover{};                 // report of the last product call (ccm_scrub_last_probe_cover)
   std::vector<ccm_probe_cover_page> pcover_pages;   // and its inexact pages (ccm_last_probe_cover_pages)
+  // report proof (a proven call that locates or triages): kReportSteps maps of npages words after the kPasses cover maps
+  // in d_cover (report_map), and their pinned copy at the same place in h_cover
+  ccm_report_cover rcover{};                // report of the last product call (ccm_scrub_last_report_cover)
+  std::vector<ccm_report_cover_page> rcover_pages;   // and its inexact pages (ccm_last_report_cover_pages)
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -252,6 +264,8 @@ struct ScrubEngine {
   // the grab word of a default kernel and its done word, one line further on
   GrabCtl ctl(int grab) const { return GrabCtl{d_counter + grab, d_counter + grab + 8}; }
   DirtRecord* book_records(Book b) const { return d_records + b * kDirtRecords; }
+  // the cover map of report step `step` (CCM_REPORT_*), and its host copy
+  uint64_t report_word(int step) const { return (uint64_t)(kPasses + step - 1) * npages; }
   uint32_t* book_pages(Book b) const { return d_pages + b * npages; }
   // The census records into book_records(kCensusBook) as MaskRecord, passed to it apart from its LocateOut.
   LocateOut book_out(Book b) const {
@@ -292,6 +306,7 @@ static constexpr int kCensusThreads = 512, kCensusPer = 16;
 #define CCM_COVER_TAG_CHECK cover_tag_check_pass<kTagThreads, kTagPer>
 #define CCM_COVER_CENSUS_ZERO cover_census_zero_pass<kCensusThreads, kCensusPer>
 #define CCM_COVER_CENSUS_TAG cover_census_tag_pass<kCensusThreads, kCensusPer>
+#define CCM_COVER_LOCATE cover_locate_pass<kLocateThreads, kLocatePer>
 // The alias probe: 256-thread CTAs, 4 windows in flight per thread (scattered 32-byte sectors: the rate is set by how
 // many are in flight, not by the bytes).  Each step launches as many CTAs per SM as its registers let one SM hold at
 // once (ptxas on sm_90a: P1 31, P2 48, P3 45 registers, so 8, 5 and 5 CTAs), so a launch runs in one wave.
@@ -597,25 +612,33 @@ static bool is_fast_scrub(int variant, const ccm_launch_cfg* cfg) {
   return cfg == nullptr && resolve_scrub_variant(variant) == CCM_SCRUB_ST128;
 }
 
-// Before a default-frame launch over [p, ...) that may belong to pass `pass` (CCM_PASS_*) of the product call, whose
-// GrabCtl pair is at word `grab`: *cover = the pass's cover map when the call proves (map == nullptr otherwise), and the
-// "cover_skip" drill, when it is pending for this pass, writes its count into the grab word first.
+// Before a default-frame launch over [p, ...) that may belong to pass `pass` (CCM_PASS_*) of the product call, or (once
+// its passes are over; pass 0 for the locate kernel) to its report step g.report, whose GrabCtl pair is at word `grab`:
+// *cover = the pass's or the step's cover map when the call proves it (map == nullptr otherwise), and the "cover_skip"
+// or "report_skip" drill, when it is pending for this pass or step, writes its count into the grab word first.
 static int gate_launch(ScrubEngine* e, int pass, const void* p, int grab, cudaStream_t st, CoverOut* cover) {
   GatePasses& g = e->gate;
   *cover = CoverOut{nullptr, 0, 0};
-  if (!g.active) return CCM_OK;
-  if (g.skip_pass == pass) {
-    e->h_counter[7] = g.skip;   // pinned and unchanged until the call ends: the copy runs in stream order
-    CCM_CUDA(cudaMemcpyAsync(e->d_counter + grab, e->h_counter + 7, sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
-    g.skip_pass = 0;
+  if (g.active ? pass == 0 : g.report == 0) return CCM_OK;
+  const bool report = !g.active;
+  if (report) g.report_launches[g.report - 1]++;
+  if (report ? g.skip_report == g.report : g.skip_pass == pass) {
+    // pinned and unchanged until the call ends: the copy runs in stream order
+    const int slot = report ? 6 : 7;
+    e->h_counter[slot] = report ? g.report_skip : g.skip;
+    CCM_CUDA(cudaMemcpyAsync(e->d_counter + grab, e->h_counter + slot, sizeof(unsigned long long), cudaMemcpyHostToDevice,
+                             st));
+    (report ? g.skip_report : g.skip_pass) = 0;
   }
-  if (g.prove) {
+  if (report ? g.report_prove : g.prove) {
     const uint64_t a = (uint64_t)(uintptr_t)p;
     // a launch outside what the call holds counts into the outside slot: its offsets all lie past the map
     uint64_t base = a - (uint64_t)e->npages * kPageBytes;
     for (const CheckSpan& sp : g.spans)
       if (a >= sp.addr && a < sp.addr + sp.bytes) base = sp.addr - sp.offset;
-    *cover = CoverOut{e->d_cover + (uint64_t)(pass - 1) * e->npages, base, (uint32_t)(e->npages - 1)};
+    const uint64_t word = report ? e->report_word(g.report) : (uint64_t)(pass - 1) * e->npages;
+    *cover = CoverOut{e->d_cover + word, base, (uint32_t)(e->npages - 1)};
+    g.rcover_dirty |= report;
   }
   return CCM_OK;
 }
@@ -986,10 +1009,16 @@ static void sort_records(Report* rep, uint64_t windows) {
 }
 
 // ------------------------------------------------------------------ locate the dirt
-// One locate launch over [p, p+n) on `st` (no sync) into the dirt book, with offsets from `base`.
+// One locate launch over [p, p+n) on `st` (no sync) into the dirt book, with offsets from `base`.  A proven report step
+// launches the proving twin (gate_launch).
 static int locate_launch(ScrubEngine* e, const void* p, uint64_t n, uint64_t base, cudaStream_t st) {
-  const cudaError_t err = launch_fast(CCM_LOCATE, kLocateThreads, kLocatePer, e, kLocateGrab, st,
-                                      split_region(p, n, 16, 128), e->book_out(kDirtBook), base);
+  CoverOut cv;
+  if (int rc = gate_launch(e, 0, p, kLocateGrab, st, &cv)) return rc;
+  const RegionSplit s = split_region(p, n, 16, 128);
+  const cudaError_t err =
+      cv.map ? launch_fast(CCM_COVER_LOCATE, kLocateThreads, kLocatePer, e, kLocateGrab, st, s, e->book_out(kDirtBook),
+                           base, cv)
+             : launch_fast(CCM_LOCATE, kLocateThreads, kLocatePer, e, kLocateGrab, st, s, e->book_out(kDirtBook), base);
   g_launches++;
   if (err != cudaSuccess) { set_error("locate launch failed: %s", cudaGetErrorString(err)); return CCM_ERR_CUDA; }
   return CCM_OK;
@@ -1114,11 +1143,12 @@ static int take_residue(ScrubEngine* e, cudaStream_t st, const Held& h, ccm_resi
 
 // ------------------------------------------------------------------ coverage proof
 // Sets aside the cover maps and their host copy, and makes the proving kernels resident (a whole-HBM call cannot load a
-// module once everything is mapped).  The caller holds e->mu.
+// module once everything is mapped).  The report proof's maps follow the passes' in the same allocation: a whole-HBM
+// call that fails has mapped everything by the time it locates.  The caller holds e->mu.
 static int ensure_cover(ScrubEngine* e) {
   if (e->d_cover) return CCM_OK;
   CCM_CUDA(cudaSetDevice(e->ordinal));
-  const size_t bytes = kPasses * e->npages * sizeof(uint32_t);
+  const size_t bytes = (kPasses + kReportSteps) * e->npages * sizeof(uint32_t);
   if (!e->h_cover) CCM_CUDA(cudaHostAlloc(&e->h_cover, bytes, cudaHostAllocDefault));
   cudaFuncAttributes fa;
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_ZERO));
@@ -1127,6 +1157,7 @@ static int ensure_cover(ScrubEngine* e) {
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_TAG_CHECK));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_CENSUS_ZERO));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_CENSUS_TAG));
+  CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_LOCATE));
   uint32_t* d = nullptr;
   CCM_CUDA(cudaMalloc(&d, bytes));
   const cudaError_t err = cudaMemset(d, 0, bytes);
@@ -1203,6 +1234,76 @@ static int take_cover(ScrubEngine* e, cudaStream_t st, const Held& h, bool tagge
   return CCM_OK;
 }
 
+// ------------------------------------------------------------------ report proof
+// What one report step over `pieces` (each `bytes` at `offset` from va_base: the spans of what the call holds, or the
+// runs of a triage) must count on each of the np pages: the bytes of the pieces that lie on it.
+template <typename Piece>
+static std::vector<uint32_t> report_cover_expected(const std::vector<Piece>& pieces, uint64_t np) {
+  std::vector<uint32_t> exp(np, 0);
+  for (const Piece& r : pieces)
+    for (uint64_t o = r.offset, end = r.offset + r.bytes; o < end;) {
+      const uint64_t p = o / kPageBytes, next = std::min<uint64_t>(end, (p + 1) * kPageBytes);
+      if (p < np) exp[p] += (uint32_t)(next - o);
+      o = next;
+    }
+  return exp;
+}
+
+// After report steps first .. first + n - 1 (CCM_REPORT_*) of a proven call over `pieces` (the caller holds e->mu and
+// their kernels have finished; ok = false when an error cut them short): zeroes their maps for the next report, and
+// when they ran to the end copies them first, all in one copy, and compares each step against
+// report_cover_expected(pieces) into e->rcover (proved = 1) and e->rcover_pages, each inexact page with
+// h.chunk_of(page offset).  After an error the steps keep ran = 0.
+template <typename Piece>
+static int take_report_cover(ScrubEngine* e, cudaStream_t st, const Held& h, int first, int n,
+                             const std::vector<Piece>& pieces, bool ok) {
+  const double t0 = now_ms();
+  const size_t bytes = (size_t)n * e->npages * sizeof(uint32_t);
+  uint32_t* const d = e->d_cover + e->report_word(first);
+  const uint32_t* const c = e->h_cover + e->report_word(first);
+  if (ok) CCM_CUDA(cudaMemcpyAsync((void*)c, d, bytes, cudaMemcpyDeviceToHost, st));
+  CCM_CUDA(cudaMemsetAsync(d, 0, bytes, st));
+  CCM_CUDA(cudaStreamSynchronize(st));
+  ccm_report_cover& rep = e->rcover;
+  if (!rep.proved) {
+    rep.proved = 1;
+    rep.covered = 1;
+    rep.va_base = h.va_base;
+  }
+  if (ok) {
+    const uint64_t np = e->npages - 1;   // pages of a map; word np is its outside slot
+    const std::vector<uint32_t> exp = report_cover_expected(pieces, np);
+    uint64_t total = 0;
+    for (const Piece& r : pieces) total += r.bytes;
+    for (int k = 0; k < n; ++k) {
+      const int step = first + k;
+      const uint32_t* m = c + (uint64_t)k * e->npages;
+      ccm_report_cover_step& ps = rep.step[step - 1];
+      ps.ran = 1;
+      ps.launches = e->gate.report_launches[step - 1];
+      ps.bytes_expected = total;
+      for (uint64_t p = 0; p < np; ++p) {
+        ps.bytes_counted += m[p];
+        if (m[p] == exp[p]) continue;
+        if (m[p] < exp[p]) {
+          if (ps.pages_short++ == 0) ps.first_short_page = p;
+          ps.bytes_missing += exp[p] - m[p];
+        } else {
+          ps.pages_over++;
+          ps.bytes_extra += m[p] - exp[p];
+        }
+        e->rcover_pages.push_back(ccm_report_cover_page{p, h.chunk_of(p * kPageBytes), step, exp[p], m[p]});
+      }
+      ps.bytes_outside = m[np];
+      ps.bytes_counted += m[np];
+      ps.bytes_extra += m[np];
+      if (ps.bytes_missing || ps.bytes_extra) rep.covered = 0;
+    }
+  }
+  rep.ms_prove += now_ms() - t0;
+  return CCM_OK;
+}
+
 // Starts the passes of one product call (the caller holds e->mu, before the call maps or launches anything): the
 // "cover_skip" drill pending, and when the device is armed, the cover maps set aside.  An armed call that cannot count
 // fails here: it never runs unproven.  The caller adds the spans of what it holds.
@@ -1210,6 +1311,7 @@ static int begin_gate(ScrubEngine* e, const ScrubDrill& drill) {
   e->gate = GatePasses();
   e->gate.active = true;
   if (drill.cover_skip) { e->gate.skip_pass = drill.cover_pass; e->gate.skip = drill.cover_skip; }
+  if (drill.report_skip) { e->gate.skip_report = drill.report_skip_step; e->gate.report_skip = drill.report_skip; }
   if (!e->prove) return CCM_OK;
   if (int rc = ensure_cover(e)) { e->gate.active = false; return rc; }
   e->gate.prove = true;
@@ -1220,9 +1322,12 @@ static int begin_gate(ScrubEngine* e, const ScrubDrill& drill) {
 // maps are zero again for the next one.
 static void end_gate(ScrubEngine* e) {
   std::lock_guard<std::mutex> g(e->mu);
-  if ((e->gate.prove || e->gate.pcover_dirty) && e->ready && cudaSetDevice(e->ordinal) == cudaSuccess) {
+  if ((e->gate.prove || e->gate.pcover_dirty || e->gate.rcover_dirty) && e->ready &&
+      cudaSetDevice(e->ordinal) == cudaSuccess) {
     if (e->gate.prove && e->d_cover) cudaMemsetAsync(e->d_cover, 0, kPasses * e->npages * sizeof(uint32_t), e->stream);
     if (e->gate.pcover_dirty) cudaMemsetAsync(e->d_pcover, 0, kSteps * e->npages * sizeof(uint32_t), e->stream);
+    if (e->gate.rcover_dirty)
+      cudaMemsetAsync(e->d_cover + e->report_word(1), 0, kReportSteps * e->npages * sizeof(uint32_t), e->stream);
     cudaStreamSynchronize(e->stream);
   }
   e->gate = GatePasses();
@@ -1525,10 +1630,12 @@ static std::vector<TriageRun> triage_runs(const std::vector<ccm_page_entry>& pag
 }
 
 // The steps of one triage: each enqueues one launch over one run on the triage's stream (no sync).  T2 and T3 book
-// into b2 and b3, which the triage reads back into page maps of its own.
+// into b2 and b3, which the triage reads back into page maps of its own.  Report steps r1, r1 + 1 and r1 + 2
+// (CCM_REPORT_*) are T1, T2 and T3 (gate_launch).
 struct TriageSteps {
   std::function<int(const TriageRun&)> t1, t2, t3;
   Book b2, b3;
+  int r1;
 };
 
 // A triage (ccm.h: ccm_scrub_triage, ccm_scrub_mismatch_triage), while the call still holds what it mapped (`spans`,
@@ -1536,8 +1643,9 @@ struct TriageSteps {
 // of `hold_ms`, then T3 (booked).  The drills XOR the first byte of each of the first "triage_stay" pages of `map`
 // between T1 and T2, and of the first "triage_return" pages between T2 and T3.  A page is STAYS when T2 booked bytes
 // on it, RETURNS when only T3 did, CLEARS otherwise; fills *report and *pages.  b2 and b3 must be zero when it starts
-// (read_book() left them so) and are zero when it ends.  After an error it drops them and leaves *report empty.
-static void run_triage(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& spans, const ScrubDrill& drill,
+// (read_book() left them so) and are zero when it ends.  After an error it drops them, leaves *report empty and returns
+// the error.
+static int run_triage(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& spans, const ScrubDrill& drill,
                        const std::vector<ccm_page_entry>& map, uint64_t va_base, uint32_t hold_ms,
                        const TriageSteps& steps, ccm_triage_report* report, std::vector<ccm_triage_page>* pages) {
   const double t0 = now_ms();
@@ -1554,30 +1662,34 @@ static void run_triage(ScrubEngine* e, cudaStream_t st, const std::vector<CheckS
     }
     return CCM_OK;
   };
-  // one step over every run: each launch, then (booked) its book read back into its head and page map
-  auto step = [&](const std::function<int(const TriageRun&)>& launch, Book b, BookHead* head,
+  // one step (report step rs) over every run: each launch, then (booked) its book read back into its head and page map
+  auto step = [&](int rs, const std::function<int(const TriageRun&)>& launch, Book b, BookHead* head,
                   std::vector<ccm_page_entry>* into) -> int {
+    e->gate.report = rs;
+    int rc = CCM_OK;
     for (const TriageRun& r : runs)
-      if (int rc = launch(r)) return rc;
+      if ((rc = launch(r)) != CCM_OK) break;
+    e->gate.report = 0;
+    if (rc != CCM_OK) return rc;
     return head ? read_book(e, b, st, head, into) : CCM_OK;
   };
   BookHead t2{}, t3{};
   std::vector<ccm_page_entry> map2, map3;
   double ms_hold = 0;
-  int rc = step(steps.t1, kBooks, nullptr, nullptr);                                                           // T1
+  int rc = step(steps.r1, steps.t1, kBooks, nullptr, nullptr);                                                 // T1
   if (rc == CCM_OK) rc = xor_pages(drill.triage_stay);
-  if (rc == CCM_OK) rc = step(steps.t2, steps.b2, &t2, &map2);                                                 // T2
+  if (rc == CCM_OK) rc = step(steps.r1 + 1, steps.t2, steps.b2, &t2, &map2);                                   // T2
   if (rc == CCM_OK) rc = xor_pages(drill.triage_return);
   if (rc == CCM_OK) {
     const double h0 = now_ms();
     std::this_thread::sleep_for(std::chrono::milliseconds(hold_ms));
     ms_hold = now_ms() - h0;
-    rc = step(steps.t3, steps.b3, &t3, &map3);                                                                 // T3
+    rc = step(steps.r1 + 2, steps.t3, steps.b3, &t3, &map3);                                                   // T3
   }
   if (rc != CCM_OK) {
     drop_book(e, steps.b2, st);
     if (steps.b3 != steps.b2) drop_book(e, steps.b3, st);
-    return;
+    return rc;
   }
 
   ccm_triage_report t;
@@ -1617,23 +1729,27 @@ static void run_triage(ScrubEngine* e, cudaStream_t st, const std::vector<CheckS
   t.ms_triage = now_ms() - t0;
   *report = t;
   pages->swap(out);
+  return CCM_OK;
 }
 
 // The triage of a failed read-back (ccm.h: ccm_scrub_triage).  Runs when the device is armed, after the locate pass
 // filled e->dirt and e->pages[kDirtBook], while the call still holds what it mapped (`spans`, offsets from the dirt
 // report's va_base; the caller holds e->mu).  Re-zeroes every run with the default scrub (T1), re-reads it with the
 // locate kernel (T2), waits the hold and re-reads it again (T3); T2 and T3 book into the dirt book.  Fills e->triage
-// and e->triage_pages.  Never changes the verdict or another report.
-static void triage_dirt(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& spans, const ScrubDrill& drill) {
+// and e->triage_pages.  Never changes the verdict or another report.  A proven call proves its steps
+// (CCM_REPORT_DIRT_T1..T3) over the runs of the page map.
+static void triage_dirt(ScrubEngine* e, cudaStream_t st, const Held& h, const ScrubDrill& drill) {
   if (e->triage_hold_ms == 0 || !e->dirt.located || e->pages[kDirtBook].empty()) return;
   auto locate = [&](const TriageRun& r) {
     return locate_launch(e, (const void*)(uintptr_t)r.addr, r.bytes, r.addr - r.offset, st);
   };
   const TriageSteps steps{
       [&](const TriageRun& r) { return scrub_range(e, (void*)(uintptr_t)r.addr, r.bytes, CCM_SCRUB_ST128, nullptr, st); },
-      locate, locate, kDirtBook, kDirtBook};
-  run_triage(e, st, spans, drill, e->pages[kDirtBook], e->dirt.va_base, e->triage_hold_ms, steps, &e->triage,
-             &e->triage_pages);
+      locate, locate, kDirtBook, kDirtBook, CCM_REPORT_DIRT_T1};
+  const int rc = run_triage(e, st, h.spans, drill, e->pages[kDirtBook], e->dirt.va_base, e->triage_hold_ms, steps,
+                            &e->triage, &e->triage_pages);
+  if (e->gate.report_prove)
+    take_report_cover(e, st, h, CCM_REPORT_DIRT_T1, 3, triage_runs(e->pages[kDirtBook], h.spans), rc == CCM_OK);
 }
 
 // The triage of a failed tagged check (ccm.h: ccm_scrub_mismatch_triage).  Runs when the device is armed, after
@@ -1642,9 +1758,9 @@ static void triage_dirt(ScrubEngine* e, cudaStream_t st, const std::vector<Check
 // Writes the tags of `seed` over every run again (T1), checks and zeroes it (T2, into the check book, with the base the
 // gate's check used, so its offsets and pages are the mismatch report's own), waits the hold and reads it for zeros
 // (T3, into the dirt book).  T2 leaves the runs zero, so no tag outlives the call.  Fills e->mtriage and
-// e->mtriage_pages.  Never changes the verdict or another report.
-static void triage_mismatch(ScrubEngine* e, cudaStream_t st, const std::vector<CheckSpan>& spans,
-                            const ScrubDrill& drill, uint32_t seed) {
+// e->mtriage_pages.  Never changes the verdict or another report.  A proven call proves its steps
+// (CCM_REPORT_MISMATCH_T1..T3) over the runs of the page map.
+static void triage_mismatch(ScrubEngine* e, cudaStream_t st, const Held& h, const ScrubDrill& drill, uint32_t seed) {
   if (e->mtriage_hold_ms == 0 || !e->mismatch.located || e->pages[kCheckBook].empty()) return;
   const TriageSteps steps{
       [&](const TriageRun& r) { return tag_fill_range(e, (void*)(uintptr_t)r.addr, r.bytes, seed, st); },
@@ -1654,9 +1770,11 @@ static void triage_mismatch(ScrubEngine* e, cudaStream_t st, const std::vector<C
       [&](const TriageRun& r) {
         return locate_launch(e, (const void*)(uintptr_t)r.addr, r.bytes, r.addr - r.offset, st);
       },
-      kCheckBook, kDirtBook};
-  run_triage(e, st, spans, drill, e->pages[kCheckBook], e->mismatch.va_base, e->mtriage_hold_ms, steps, &e->mtriage,
-             &e->mtriage_pages);
+      kCheckBook, kDirtBook, CCM_REPORT_MISMATCH_T1};
+  const int rc = run_triage(e, st, h.spans, drill, e->pages[kCheckBook], e->mismatch.va_base, e->mtriage_hold_ms, steps,
+                            &e->mtriage, &e->mtriage_pages);
+  if (e->gate.report_prove)
+    take_report_cover(e, st, h, CCM_REPORT_MISMATCH_T1, 3, triage_runs(e->pages[kCheckBook], h.spans), rc == CCM_OK);
 }
 
 // The reports of a product call, on the VMM path and the fallback alike.  The caller holds e->mu, every pass of the
@@ -1664,11 +1782,13 @@ static void triage_mismatch(ScrubEngine* e, cudaStream_t st, const std::vector<C
 // whose read-back was clean; *nonzero becomes P3's count), the coverage proof, where the tags were wrong (tagged call,
 // mismatch_bytes != 0), what the first pass erased (census call), where the dirt is and its triage (*nonzero != 0), and
 // the mismatch triage.  Only the probe and the proof can fail the call; the other reports are left empty when they
-// cannot be taken.  After a failure it takes nothing and drops the books the passes filled.
+// cannot be taken.  After a failure it takes nothing and drops the books the passes filled.  A proven call proves the
+// locate pass and the triages apart (ccm.h: ccm_report_cover), which never changes the call's result.
 static int finish_gate(ScrubEngine* e, cudaStream_t st, int rc, const Held& h, const ScrubDrill& drill,
                        ccm_tag_result* tag, ccm_residue_report* res, uint64_t* nonzero, ccm_probe_report* probe,
                        ccm_probe_cover* pcover, ccm_cover_report* cover) {
   e->gate.active = false;   // the probe, the locate pass and the triages are not the call's passes
+  e->gate.report_prove = e->gate.prove;   // take_cover() ends the passes' proof, not the reports'
   if (rc == CCM_OK && probe && *nonzero == 0 && h.bytes) {
     uint64_t p3 = 0;
     rc = gate_probe(e, st, h, drill, probe, pcover, &p3);
@@ -1692,18 +1812,21 @@ static int finish_gate(ScrubEngine* e, cudaStream_t st, int rc, const Held& h, c
     rep.va_base = h.va_base;
     e->pages[kDirtBook].clear();
     int lrc = CCM_OK;
+    e->gate.report = CCM_REPORT_LOCATE;
     for (const CheckSpan& sp : h.spans)
       if ((lrc = locate_range(e, (const void*)(uintptr_t)sp.addr, sp.bytes, sp.offset, st, &rep, h)) != CCM_OK) break;
+    e->gate.report = 0;
+    if (e->gate.report_prove) take_report_cover(e, st, h, CCM_REPORT_LOCATE, 1, h.spans, lrc == CCM_OK);
     if (lrc == CCM_OK) {
       sort_records(&rep, rep.dirty_windows);
       finish_pages(e, kDirtBook, h);
       e->dirt = rep;
-      triage_dirt(e, st, h.spans, drill);
+      triage_dirt(e, st, h, drill);
     } else {
       e->pages[kDirtBook].clear();
     }
   }
-  if (mismatched) triage_mismatch(e, st, h.spans, drill, tag->seed);
+  if (mismatched) triage_mismatch(e, st, h, drill, tag->seed);
   return CCM_OK;
 }
 
@@ -2303,6 +2426,8 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     memset(&e->probe, 0, sizeof e->probe);
     memset(&e->pcover, 0, sizeof e->pcover);
     e->pcover_pages.clear();
+    memset(&e->rcover, 0, sizeof e->rcover);
+    e->rcover_pages.clear();
     prove = e->prove;
     // the alias probe is for the zero gate: a tagged call's check already covers every window
     probe_armed = e->probe_armed && tag == nullptr;
@@ -2761,6 +2886,20 @@ extern "C" int ccm_scrub_last_probe_cover(int cuda_ordinal, ccm_probe_cover* out
 
 extern "C" int ccm_last_probe_cover_pages(int cuda_ordinal, ccm_probe_cover_page* out, uint64_t cap, uint64_t* n) {
   return last_pages("ccm_last_probe_cover_pages", cuda_ordinal, out, cap, n, &ScrubEngine::pcover_pages);
+}
+
+// ------------------------------------------------------------------------- report proof
+static_assert(sizeof(ccm_report_cover_step) == 80 && sizeof(ccm_report_cover) == 584 &&
+              offsetof(ccm_report_cover, step) == 24 && sizeof(ccm_report_cover_page) == 24 &&
+              offsetof(ccm_report_cover_page, step) == 12 && offsetof(ccm_report_cover_page, counted) == 20,
+              "report cover structs keep their layout");
+
+extern "C" int ccm_scrub_last_report_cover(int cuda_ordinal, ccm_report_cover* out) {
+  return last_report(cuda_ordinal, out, &ScrubEngine::rcover);
+}
+
+extern "C" int ccm_last_report_cover_pages(int cuda_ordinal, ccm_report_cover_page* out, uint64_t cap, uint64_t* n) {
+  return last_pages("ccm_last_report_cover_pages", cuda_ordinal, out, cap, n, &ScrubEngine::rcover_pages);
 }
 
 extern "C" int ccm_region_probe(int cuda_ordinal, void* dptr, uint64_t bytes, uint32_t seed, void* stream,

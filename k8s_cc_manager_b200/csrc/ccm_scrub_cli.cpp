@@ -18,8 +18,9 @@
 // ccm_last_cover_pages report it; "probe" with --probe, which refuses --check tagged and arms every GPU for the alias
 // probe (ccm_scrub_probe), for every GPU whose probe ran, as ccm_scrub_last_probe reports it, with "mismatch" when it
 // found bytes off their tags); "probe_cover" with --prove and --probe, for every GPU whose probe ran, as
-// ccm_scrub_last_probe_cover and ccm_last_probe_cover_pages report it.  With --prove or --probe, a GPU that cannot be
-// armed is never scrubbed without: nothing is scrubbed and the exit code is 3.
+// ccm_scrub_last_probe_cover and ccm_last_probe_cover_pages report it; "report_cover" with --prove, for every GPU that
+// located dirt or triaged, as ccm_scrub_last_report_cover and ccm_last_report_cover_pages report it.  With --prove or
+// --probe, a GPU that cannot be armed is never scrubbed without: nothing is scrubbed and the exit code is 3.
 // Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
@@ -234,6 +235,39 @@ static int usage(const char* argv0) {
   return 2;
 }
 
+// The "report_cover" object: the fields of k8s_cc_manager_b200.devices.ReportCoverReport, with the first 64 inexact
+// (step, page) entries.
+static void print_rcover(const ccm_report_cover& c, int ordinal) {
+  static const char* const names[CCM_REPORT_STEPS] = {"LOCATE",      "DIRT_T1",     "DIRT_T2",    "DIRT_T3",
+                                                      "MISMATCH_T1", "MISMATCH_T2", "MISMATCH_T3"};
+  printf(", \"report_cover\": {\"va_base\": %llu, \"ms_prove\": %.3f, \"proved\": %d, \"covered\": %d, \"steps\": [",
+         (unsigned long long)c.va_base, c.ms_prove, c.proved, c.covered);
+  for (unsigned k = 0; k < CCM_REPORT_STEPS; ++k) {
+    const ccm_report_cover_step& p = c.step[k];
+    printf("%s{\"name\": \"%s\", \"ran\": %d, \"launches\": %llu, \"bytes_expected\": %llu, \"bytes_counted\": %llu, "
+           "\"bytes_missing\": %llu, \"bytes_extra\": %llu, \"bytes_outside\": %llu, \"pages_short\": %llu, "
+           "\"pages_over\": %llu, \"first_short_page\": %llu}",
+           k ? ", " : "", names[k], p.ran, (unsigned long long)p.launches, (unsigned long long)p.bytes_expected,
+           (unsigned long long)p.bytes_counted, (unsigned long long)p.bytes_missing, (unsigned long long)p.bytes_extra,
+           (unsigned long long)p.bytes_outside, (unsigned long long)p.pages_short, (unsigned long long)p.pages_over,
+           (unsigned long long)p.first_short_page);
+  }
+  printf("], \"pages\": [");
+  uint64_t n = 0;
+  std::vector<ccm_report_cover_page> v;
+  if (!c.covered && ccm_last_report_cover_pages(ordinal, nullptr, 0, &n) == CCM_OK) {
+    v.resize(n);
+    if (n && ccm_last_report_cover_pages(ordinal, v.data(), n, &n) != CCM_OK) v.clear();
+  }
+  const size_t keep = 64;   // k8s_cc_manager_b200.devices.COVER_PAGES
+  for (size_t k = 0; k < v.size() && k < keep; ++k) {
+    const int step = v[k].step >= 1 && v[k].step <= (int)CCM_REPORT_STEPS ? v[k].step : 1;
+    printf("%s{\"page\": %llu, \"chunk\": %u, \"step\": \"%s\", \"expected\": %u, \"counted\": %u}", k ? ", " : "",
+           (unsigned long long)v[k].page, v[k].chunk, names[step - 1], v[k].expected, v[k].counted);
+  }
+  printf("], \"pages_truncated\": %d}", v.size() > keep);
+}
+
 // The "probe" object: the fields of k8s_cc_manager_b200.devices.ProbeReport.
 static void print_probe(const ccm_probe_report& p) {
   printf(", \"probe\": {\"windows\": %llu, \"bytes_probed\": %llu, \"mismatch_bytes\": %llu, \"mismatch_windows\": %llu, "
@@ -397,6 +431,8 @@ int main(int argc, char** argv) {
     clean = clean && (!prove || proved);   // a proof that was asked for and did not run fails the gate
     if (ran_probe) print_probe(pr);
     if (probe_proved) print_pcover(pc, ordinals[i]);
+    ccm_report_cover rc;
+    if (prove && ccm_scrub_last_report_cover(ordinals[i], &rc) == CCM_OK && rc.proved) print_rcover(rc, ordinals[i]);
     printf("}");
   }
   printf("]}\n");

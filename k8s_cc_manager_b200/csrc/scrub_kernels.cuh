@@ -31,8 +31,9 @@
 //   locate_dirt_kernel                                   where the dirt is, after a failed read-back
 //   census_zero_kernel / census_tag_fill_kernel          what the first pass found before it erased it
 //   cover_*_pass                                         proving twins of the six above that run a product call's
-//                                                        passes: they count the bytes they walk per 2 MiB page
-//   alias_probe_*_pass                                   the alias probe's three steps (one 32-byte window per 4 KiB)
+//                                                        passes: they count the bytes they walk per 2 MiB page;
+//                                                        cover_locate_pass also runs a failed call's reports
+//   alias_probe_*_pass                                  the alias probe's three steps (one 32-byte window per 4 KiB)
 //   cover_probe_*_pass                                   their proving twins: they count the windows they take per page
 //   fill_pattern_kernel                                  seeded test pattern (tests only)
 // The grab loop (grab_chunks) and the epilogue after the last whole chunk or tile (finish_region,
@@ -1290,6 +1291,18 @@ cover_census_tag_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, uint32_t see
                         MaskRecord* records, uint64_t base, CoverOut cover) {
   CensusOp<true> op{seed, {out}, records, base};
   CoverOp<CensusOp<true>, false> cop{op, cover};
+  default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, cop);
+  op.ragged_windows(s);
+  cover_ragged_windows(s, cover);
+  op.book.flush();
+}
+
+// Proving twin of locate_dirt_kernel: the locate pass and the triages' re-reads of a proven call that failed.
+template <int THREADS, int PER_THREAD>
+__global__ void __launch_bounds__(THREADS, 1)
+cover_locate_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, LocateOut out, uint64_t base, CoverOut cover) {
+  LocateOp op{{out}, base};
+  CoverOp<LocateOp, false> cop{op, cover};
   default_kernel<THREADS, PER_THREAD, false>(s, nchunks, ctl, nullptr, cop);
   op.ragged_windows(s);
   cover_ragged_windows(s, cover);

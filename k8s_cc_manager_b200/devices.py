@@ -35,7 +35,9 @@ class GpuError(Exception):
     triage call whose tagged check failed carries its TriageReport (what kind of mismatch) as `.mismatch_triage`; a
     proving call carries its CoverReport (how many bytes each pass walked on every page) as `.cover`; a probing call
     carries its ProbeReport (what the alias probe found) as `.probe`; a call both proving and probing carries its
-    ProbeCoverReport (how many windows each probe step took on every page) as `.probe_cover`."""
+    ProbeCoverReport (how many windows each probe step took on every page) as `.probe_cover`; a proving call that
+    located dirt or triaged carries its ReportCoverReport (how many bytes the locate pass and each triage step walked on
+    every page) as `.report_cover`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
@@ -810,10 +812,131 @@ def _attach_probe(rep: "ScrubReport", cuda_ordinal: int, prove: bool = False) ->
     return True
 
 
+@dataclass
+class ReportCoverPage:
+    """One page one step of a proven locate pass or triage did not count exactly (include/ccm.h:
+    ccm_report_cover_page)."""
+    page: int
+    chunk: int
+    step: str          # N.REPORT_STEPS
+    expected: int      # bytes the step had to count on it
+    counted: int       # bytes it counted
+
+    def describe(self) -> str:
+        return f"page {self.page} (chunk {self.chunk}): {self.step} counted {self.counted} of {self.expected} bytes"
+
+
+@dataclass
+class ReportCoverStep:
+    """What one step of a proven locate pass or triage counted (include/ccm.h: ccm_report_cover_step)."""
+    name: str          # N.REPORT_STEPS
+    ran: int
+    launches: int
+    bytes_expected: int
+    bytes_counted: int
+    bytes_missing: int
+    bytes_extra: int
+    bytes_outside: int
+    pages_short: int
+    pages_over: int
+    first_short_page: int
+
+
+# The report each step of the report proof walks for: the locate pass the dirt report, the triage steps their triage.
+REPORT_STEP_OF = {"LOCATE": "dirt", "DIRT_T1": "triage", "DIRT_T2": "triage", "DIRT_T3": "triage",
+                  "MISMATCH_T1": "mismatch_triage", "MISMATCH_T2": "mismatch_triage", "MISMATCH_T3": "mismatch_triage"}
+
+
+@dataclass
+class ReportCoverReport:
+    """The report proof of one proven product call that failed (include/ccm.h: ccm_report_cover): its locate pass and
+    every triage step it ran counted on the device the bytes they walked on each 2 MiB page, and `covered` says each
+    walked every byte of its reports exactly once.  It never changes the call's verdict: a short step says only which
+    pages of the dirt and triage reports rest on a kernel that missed bytes.  `pages` are the first COVER_PAGES
+    inexact (step, page) entries."""
+    va_base: int
+    ms_prove: float
+    proved: int
+    covered: int
+    steps: List[ReportCoverStep] = field(default_factory=list)
+    pages: List[ReportCoverPage] = field(default_factory=list)
+    pages_truncated: int = 0
+
+    @classmethod
+    def from_native(cls, r: N.ReportCover, pages: "Optional[List[ReportCoverPage]]" = None) -> "ReportCoverReport":
+        steps = [ReportCoverStep(name=name, **{f: getattr(r.steps[k], f) for f, _ in N.ReportCoverStep._fields_
+                                               if f != "reserved"})
+                 for k, name in enumerate(N.REPORT_STEPS)]
+        pages = pages or []
+        return cls(r.va_base, r.ms_prove, r.proved, r.covered, steps, pages[:COVER_PAGES], int(len(pages) > COVER_PAGES))
+
+    @classmethod
+    def from_json(cls, d: dict) -> "ReportCoverReport":
+        return cls(**{**d, "steps": [ReportCoverStep(**p) for p in d["steps"]],
+                      "pages": [ReportCoverPage(**p) for p in d["pages"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    def short_steps(self) -> "List[ReportCoverStep]":
+        """The steps that ran and did not count every page exactly."""
+        return [p for p in self.steps if p.ran and (p.bytes_missing or p.bytes_extra)]
+
+    def unproven_pages(self, report: str) -> "List[int]":
+        """The pages (of those kept) on which a step behind `report` ("dirt", "triage" or "mismatch_triage") was
+        inexact, ascending."""
+        return sorted({p.page for p in self.pages if REPORT_STEP_OF[p.step] == report})
+
+    def summary(self, first: int = 4) -> str:
+        """One line for an operator: which steps ran and, when one was short, which and where."""
+        ran = [p.name for p in self.steps if p.ran]
+        bad = self.short_steps()
+        if not bad:
+            return "every step walked every byte of its reports once (" + ", ".join(ran) + ")"
+        line = "; ".join(f"step {p.name} counted {p.bytes_counted} of {p.bytes_expected} bytes ({p.bytes_missing} "
+                         f"missing, {p.bytes_extra} extra) with {p.pages_short} pages short, first short page "
+                         f"{p.first_short_page}" for p in bad)
+        if self.pages:
+            more = " (+more)" if self.pages_truncated or len(self.pages) > first else ""
+            line += "; " + "; ".join(p.describe() for p in self.pages[:first]) + more
+        return line
+
+
+def last_report_cover_pages(cuda_ordinal: int) -> "Optional[List[ReportCoverPage]]":
+    """The inexact (step, page) entries of the last proven locate pass and triages on a CUDA device (include/ccm.h:
+    ccm_last_report_cover_pages), by step then page; None when they cannot be read."""
+    n = C.c_uint64(0)
+    if cuda_ordinal < 0 or N.lib().ccm_last_report_cover_pages(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
+        return None
+    buf = (N.ReportCoverPage * max(1, n.value))()
+    if N.lib().ccm_last_report_cover_pages(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
+        return None
+    return [ReportCoverPage(p.page, p.chunk, N.REPORT_STEPS[p.step - 1], p.expected, p.counted) for p in buf[:n.value]]
+
+
+def last_report_cover(cuda_ordinal: int) -> "Optional[ReportCoverReport]":
+    """The report proof of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_report_cover), with
+    its first inexact pages; None when it cannot be read."""
+    out = N.ReportCover()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_report_cover(cuda_ordinal, C.byref(out)) != N.OK:
+        return None
+    return ReportCoverReport.from_native(out, last_report_cover_pages(cuda_ordinal)
+                                         if out.proved and not out.covered else None)
+
+
+def _attach_report_cover(rep: "ScrubReport", cuda_ordinal: int) -> None:
+    """For a proving call that ran a locate pass or a triage, their proof.  (A stand-in library without
+    ccm_scrub_last_report_cover has none to give.)  Never changes the call's status."""
+    if not hasattr(N.lib(), "ccm_scrub_last_report_cover"):
+        return
+    report = last_report_cover(cuda_ordinal)
+    rep.report_cover = report if report is not None and report.proved else None
+
+
 # The reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
 _REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport),
             ("mismatch_triage", TriageReport), ("cover", CoverReport), ("probe", ProbeReport),
-            ("probe_cover", ProbeCoverReport))
+            ("probe_cover", ProbeCoverReport), ("report_cover", ReportCoverReport))
 
 
 @dataclass
@@ -867,6 +990,9 @@ class ScrubReport:
     # How many windows each probe step took on every page (a ProbeCoverReport), set for every report of a call both
     # proving and probing (prove=True, probe=True) that probed.  Not a dataclass field either.
     probe_cover = None
+    # How many bytes the locate pass and each triage step walked on every page (a ReportCoverReport), set for every
+    # report of a proving call (prove=True) that located dirt or triaged.  Not a dataclass field either.
+    report_cover = None
 
     @property
     def clean(self) -> bool:
@@ -1040,7 +1166,8 @@ class NvidiaDevice:
         the call with ERR_MISMATCH and attaches where as `.mismatch`.  A device that cannot be armed fails the call.
         prove=True with probe=True also proves the probe: each probe step counts on the device the windows it took on
         each page, the report comes attached as `.probe_cover`, and a step that missed or repeated a window fails the
-        call with ERR_UNCOVERED.
+        call with ERR_UNCOVERED.  A proving call that fails and locates its dirt or triages also proves its locate pass
+        and triage steps: the report comes attached as `.report_cover`, and never changes the verdict.
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
         if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
@@ -1082,6 +1209,8 @@ class NvidiaDevice:
         rep = ScrubReport.from_native(self.bdf, res, tag)
         _attach_reports(rep, self.cuda_ordinal, census, armed, marmed, prove)
         probe_proved = _attach_probe(rep, self.cuda_ordinal, prove) if probe else True
+        if prove:
+            _attach_report_cover(rep, self.cuda_ordinal)
         if err is None and prove and rep.cover is None:   # a proof that was asked for and did not run
             err = GpuError(f"scrub_and_verify on {self.bdf}: the coverage proof did not run", N.ERR_UNCOVERED)
         if err is None and not probe_proved:
@@ -1179,6 +1308,8 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
                     rep.status = N.ERR_UNCOVERED
             if probe and not _attach_probe(rep, d.cuda_ordinal, prove) and rep.status == N.OK:
                 rep.status = N.ERR_UNCOVERED   # a probe proof that was asked for and did not run
+            if prove:
+                _attach_report_cover(rep, d.cuda_ordinal)
         return reports, wall
     n = len(devices)
     if n == 0:

@@ -177,7 +177,9 @@ class CCManager:
         # require: every pass of the gate also counts, on the device, the bytes it walked on every 2 MiB page, and a GPU
         #          on which a pass missed or repeated a byte fails the gate (ccm_scrub_prove, DESIGN.md §5h).  A check,
         #          not a report: a device that cannot prove its coverage fails the gate.  Logged and kept in
-        #          last_transition["scrub_cover"].
+        #          last_transition["scrub_cover"].  A GPU that failed also proves its locate pass and triages (DESIGN.md
+        #          §5k): which pages of its dirt and triage reports rest on a step that missed bytes.  A report, not a
+        #          check: it never changes the verdict.  Logged and kept in last_transition["scrub_report_cover"].
         self.scrub_proof = (scrub_proof or env.get("CC_SCRUB_PROOF", "off")).lower()
         if self.scrub_proof not in PROOF_MODES:
             raise ValueError(f"CC_SCRUB_PROOF must be 'off' or 'require', not {self.scrub_proof!r}")
@@ -746,7 +748,8 @@ class CCManager:
     def _note_reports(self, bdf: str, holder) -> None:
         """Logs every window report `holder` carries and keeps it in last_transition: the gate hands the memory back
         right after the verdict, so this is the only look anyone gets at it.  The coverage proof comes first: INFO when
-        every pass covered every byte, ERROR naming the short pass and its pages when not."""
+        every pass covered every byte, ERROR naming the short pass and its pages when not.  The report proof of a GPU
+        that failed comes before its dirt and triage lines, which name the pages it left unproven."""
         cover = getattr(holder, "cover", None)
         if cover is not None:
             self.last_transition.setdefault("scrub_cover", {})[bdf] = cover
@@ -761,11 +764,21 @@ class CCManager:
             self.last_transition.setdefault("scrub_probe_cover", {})[bdf] = probe_cover
             logger.log(logging.INFO if probe_cover.covered else logging.ERROR, "HBM alias probe proof on %s: %s", bdf,
                        probe_cover.summary())
+        report_cover = getattr(holder, "report_cover", None)
+        if report_cover is not None:
+            self.last_transition.setdefault("scrub_report_cover", {})[bdf] = report_cover
+            logger.log(logging.INFO if report_cover.covered else logging.ERROR, "HBM report proof on %s: %s", bdf,
+                       report_cover.summary())
         for attr, key, level, line in self._REPORT_NOTES + self._TRIAGE_NOTES:
             report = getattr(holder, attr, None)
             if report is not None:
                 self.last_transition.setdefault(key, {})[bdf] = report
-                logger.log(level, line, bdf, report.summary())
+                note = report.summary()
+                unproven = report_cover.unproven_pages(attr) if report_cover is not None and attr in _devices.REPORT_STEP_OF.values() else []
+                if unproven:
+                    note += (f" (unproven on pages {', '.join(map(str, unproven))}: a step of the report proof was short "
+                             "there)")
+                logger.log(level, line, bdf, note)
                 pages = getattr(report, "pages", None) if attr in self._PAGE_NOTES else None
                 if pages is not None:
                     logger.log(level, self._PAGE_NOTES[attr], bdf, pages.summary())

@@ -11,7 +11,8 @@ Output (stdout, last line):  {"wall_ms": ..., "reports": [ {ScrubReport fields},
 (the tagged-gate fields only with --check tagged; "residue" only with --residue; "triage" only with --triage, for a
 GPU whose read-back found non-zero bytes; "mismatch_triage" only with --mismatch-triage, for a GPU whose tagged check
 found bytes off their tags; "cover" only with --prove, for every GPU whose passes finished; "probe" only with --probe,
-for every GPU whose alias probe ran; "probe_cover" only with --prove and --probe, for every GPU whose alias probe ran).
+for every GPU whose alias probe ran; "probe_cover" only with --prove and --probe, for every GPU whose alias probe ran;
+"report_cover" only with --prove, for every GPU that located dirt or triaged).
 Exit code: 0 if every GPU is clean, 3 if the gate failed, 2 on usage errors.
 """
 from __future__ import annotations
