@@ -1315,8 +1315,7 @@ cover_locate_pass(RegionSplit s, uint64_t nchunks, GrabCtl ctl, LocateOut out, u
 // the later view's tags overwrite the earlier view's tags in the shared page.  A probe WINDOW is the 32-byte sector at
 // a 4096-aligned address; its position depends only on the address modulo 4096, so two views of one physical page
 // probe the same sector.  One launch covers the windows w0 + i * kProbeStride, i < nwin, of one mapped chunk (the host
-// computes w0, the chunk's first window, and nwin).  As the proving twins, the three kernels' names do not end in
-// `kernel`, so the existing kernel-name checks do not list them; tests/test_alias_probe_gpu.py launches all three.
+// computes w0, the chunk's first window, and nwin).
 constexpr uint64_t kProbeStride = 4096;
 constexpr uint32_t kProbeWindow = 32;
 

@@ -5,7 +5,10 @@ The default scrub and verify kernels hand their grab and done words back zeroed 
 non-zero would make the next launch start at chunk `grab` and skip chunk 0 (scrub) or the last chunks
 (verify, which walks the chunks in descending order).  `launch_state_sequence` runs a fixed sequence of
 default-kernel calls, alternating the engine stream and a torch stream, and after every call dirties
-chunk 0 and the last whole chunk of the next region only.
+chunk 0 and the last whole chunk of the next region only.  Each region step runs every default-frame kernel that
+has a grab word of its own: read-back, locate, census, scrub, tag fill and tag check.  An armed step runs their
+proving twins (include/ccm.h: ccm_region_prove), which share the plain kernels' grab words, between plain steps,
+and each twin's cover map must hold every byte of the region.
 
 Run as a script (tests/test_scrub_exactness_gpu.py does, once with CCM_PDL=1 and once without — the
 library latches CCM_PDL once per process) it also drives PDL-chained arena steps and a product call with
@@ -25,6 +28,7 @@ for p in (ROOT, ROOT / "tests"):
         sys.path.insert(0, str(p))
 
 from k8s_cc_manager_b200 import _native as N  # noqa: E402
+from region_cover_calls import ArmedMap  # noqa: E402
 
 CHUNK = 128 * 1024          # bytes per grab of the default kernels
 MiB = 1 << 20
@@ -80,8 +84,67 @@ def dirty_arena_segments(lib, value: int = 0x5A) -> int:
     return len(offs)
 
 
+def region_step(lib, n: int, handle, armed: bool) -> list:
+    """One region step over n bytes at OFFSET, dirt in chunk 0 and the last whole chunk (or the first and last byte):
+    the read-back, the locate pass and the zero census each count it, the census and the scrub zero it, then the tag
+    fill and the tag check (which zeroes the region again) count the same bytes XORed into the tags.  Returns
+    [n or "armed n", [counted by each], [expected], bytes left non-zero after the zeroing passes, final read-back]."""
+    import torch
+    buf = torch.zeros(n + 256, dtype=torch.uint8, device="cuda")
+    assert buf.data_ptr() % 128 == 0
+    region = buf[OFFSET:OFFSET + n]
+    offs = torch.tensor(dirt_offsets(n), device="cuda")
+    region[offs] = 0xC3
+    torch.cuda.synchronize()
+    addr = region.data_ptr()
+    ptr = C.c_void_p(addr)
+    arm = ArmedMap(lib, addr, n, n) if armed else None
+    torch.cuda.synchronize()   # the map is zero before any stream launches into it
+    counted, left, maps = [], 0, []
+
+    def run(call, what):
+        """call() with the twins armed (and its map taken) when the step is armed."""
+        if arm is None:
+            return ok(call(), what)
+        with arm:
+            ok(call(), what)
+        torch.cuda.synchronize()
+        maps.append((what, arm.take()[0] == arm.want([(addr, n)])))
+        torch.cuda.synchronize()
+
+    nz = C.c_uint64(12345)
+    run(lambda: lib.ccm_region_verify(0, ptr, n, N.VERIFY_AUTO, None, handle(), C.byref(nz), None), "region_verify")
+    counted.append(nz.value)
+    d = N.DirtReport()
+    run(lambda: lib.ccm_region_locate(0, ptr, n, handle(), C.byref(d)), "region_locate")
+    counted.append(d.nonzero_bytes)
+    r = N.ResidueReport()
+    run(lambda: lib.ccm_region_census(0, ptr, n, 0, 0, handle(), C.byref(r)), "region_census")
+    counted.append(r.residue_bytes)
+    torch.cuda.synchronize()
+    left += int(torch.count_nonzero(region))
+    region[offs] = 0xC3
+    torch.cuda.synchronize()
+    run(lambda: lib.ccm_region_scrub(0, ptr, n, N.SCRUB_AUTO, None, handle(), None), "region_scrub")
+    torch.cuda.synchronize()
+    left += int(torch.count_nonzero(region))
+    run(lambda: lib.ccm_region_tag_fill(0, ptr, n, 0x600D, handle(), None), "region_tag_fill")
+    torch.cuda.synchronize()
+    region[offs] ^= 0xFF
+    torch.cuda.synchronize()
+    mm = C.c_uint64(12345)
+    run(lambda: lib.ccm_region_tag_check_zero(0, ptr, n, 0x600D, handle(), C.byref(mm), None), "region_tag_check")
+    counted.append(mm.value)
+    torch.cuda.synchronize()
+    left += int(torch.count_nonzero(region))
+    run(lambda: lib.ccm_region_verify(0, ptr, n, N.VERIFY_AUTO, None, handle(), C.byref(nz), None), "region_verify")
+    assert int(torch.count_nonzero(buf[:OFFSET])) == 0 and int(torch.count_nonzero(buf[OFFSET + n:])) == 0
+    assert all(exact for _, exact in maps), (n, [what for what, exact in maps if not exact])
+    return [f"armed {n}" if armed else n, counted, [offs.numel()] * 4, left, nz.value]
+
+
 def launch_state_sequence(lib) -> list[list]:
-    """Returns one [label, counted, expected, left after scrub, verify after scrub] row per step;
+    """Returns one [label, counted, expected, left after zeroing, verify after zeroing] row per step;
     raises on the first inexact result."""
     import torch
     stream = torch.cuda.Stream()
@@ -94,7 +157,9 @@ def launch_state_sequence(lib) -> list[list]:
         return h
 
     rows = []
-    steps = [CHUNK - 1, 1, 9 * CHUNK + 12345, "arena", CHUNK - 1, 40 * MiB + 3, 1, "arena", 9 * CHUNK + 12345]
+    # ("armed", n): the twins, each between plain launches on its grab word: no whole chunk, 1 byte, many chunks
+    steps = [CHUNK - 1, ("armed", CHUNK - 1), 1, ("armed", 1), 9 * CHUNK + 12345, ("armed", 9 * CHUNK + 12345),
+             "arena", CHUNK - 1, ("armed", 40 * MiB + 3), 40 * MiB + 3, 1, "arena", 9 * CHUNK + 12345]
     for step in steps:
         torch.cuda.synchronize()
         if step == "arena":
@@ -119,23 +184,8 @@ def launch_state_sequence(lib) -> list[list]:
                 ok(lib.ccm_arena_release(0), "arena_release")
             rows.append(["arena", counted, want, left, after])
         else:
-            n = step
-            buf = torch.zeros(n + 256, dtype=torch.uint8, device="cuda")
-            assert buf.data_ptr() % 128 == 0
-            region = buf[OFFSET:OFFSET + n]
-            offs = dirt_offsets(n)
-            region[torch.tensor(offs, device="cuda")] = 0xC3
-            torch.cuda.synchronize()
-            ptr = C.c_void_p(region.data_ptr())
-            nz = C.c_uint64(12345)
-            ok(lib.ccm_region_verify(0, ptr, n, N.VERIFY_AUTO, None, handle(), C.byref(nz), None), "region_verify")
-            counted = nz.value
-            ok(lib.ccm_region_scrub(0, ptr, n, N.SCRUB_AUTO, None, handle(), None), "region_scrub")
-            torch.cuda.synchronize()
-            left = int(torch.count_nonzero(region))
-            ok(lib.ccm_region_verify(0, ptr, n, N.VERIFY_AUTO, None, handle(), C.byref(nz), None), "region_verify")
-            rows.append([n, counted, len(offs), left, nz.value])
-            assert int(torch.count_nonzero(buf[:OFFSET])) == 0 and int(torch.count_nonzero(buf[OFFSET + n:])) == 0
+            armed = isinstance(step, tuple)
+            rows.append(region_step(lib, step[1] if armed else step, handle, armed))
         label, counted, want, left, after = rows[-1]
         assert (counted, left, after) == (want, 0, 0), f"step {label}: counted {counted} of {want} dirty bytes, " \
                                                         f"{left} left after the scrub, re-verify {after}"

@@ -6,6 +6,7 @@ against a same-run tag check; and the manager end to end.  The product calls run
 (tests/probe_calls.py), once with CCM_PDL=1 and once with CCM_PDL=0."""
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import json
 import logging
@@ -23,6 +24,8 @@ sys.path.insert(0, str(ROOT / "oracle"))
 import probe_oracle as PO  # noqa: E402
 import product_gate_calls as PGC  # noqa: E402
 import product_plan as PP  # noqa: E402
+import region_cover_calls as RCC  # noqa: E402
+import report_cover_oracle as RO  # noqa: E402
 import scenarios as SC  # noqa: E402
 from k8s_cc_manager_b200 import _native as N  # noqa: E402
 from k8s_cc_manager_b200 import devices as D  # noqa: E402
@@ -236,25 +239,106 @@ def region_probe(lib, ptr: int, n: int, seed: int):
     return rep, mm
 
 
+def probe_map(lib, ptr: int, n: int) -> RCC.ArmedMap:
+    """Three cover maps for an armed region probe over [ptr, ptr + n): one page, its base 7 bytes into the middle
+    window, so that window splits between the outside slot and page 0, and the windows past the page (a 4 MiB region)
+    count outside too."""
+    w0, k = PO.chunk_windows(ptr, n)
+    return RCC.ArmedMap(lib, ptr, n, 0, steps=3, at=(w0 + PO.STRIDE * (k // 2) + 7, 1))
+
+
 @pytest.mark.parametrize("start,n", [(0, 4 * MiB), (100, 4 * MiB), (100, 3 * 4096 - 100 + 32), (100, 3 * 4096 - 100 + 31),
                                      (4095, 2), (7, 4096 * 5 + 1000), (0, 31)])
 def test_region_probe_against_the_oracle(lib, start, n):
+    """Plain, then armed (include/ccm.h: ccm_region_prove), where the proving twins run: the same report and bytes both
+    times, and armed, three cover maps of the windows."""
     guard = 8192
     buf = torch.full((guard + start + n + guard,), 0xEE, dtype=torch.uint8, device="cuda")
     base = buf.data_ptr()
     ptr = base + guard + start
-    rep, mm = region_probe(lib, ptr, n, 0xABCD)
-    w0, k = PO.chunk_windows(ptr, n)
-    assert rep.probed == 1 and rep.windows == k and rep.bytes_probed == 32 * k and rep.seed == 0xABCD
-    assert rep.mismatch_bytes == 0 and rep.reread_nonzero_bytes == 0 and rep.va_base == ptr
-    assert rep.launches == (3 if k else 0) and mm.located == 1 and mm.mismatch_bytes == 0
-    host = buf.cpu().numpy()
-    want = host.copy()
-    want[:] = 0xEE
-    for i in range(k):
-        o = w0 + 4096 * i - base
-        want[o:o + 32] = 0
-    assert (host == want).all()   # the windows zero, every other byte (guards included) untouched
+    for armed in (False, True):
+        buf.fill_(0xEE)
+        arm = probe_map(lib, ptr, n) if armed else None
+        with arm or contextlib.nullcontext():
+            rep, mm = region_probe(lib, ptr, n, 0xABCD)
+        if arm:
+            assert arm.take() == [arm.want(RO.probe_parts([(ptr, n)]))] * 3, (arm.base - ptr, arm.pages)
+        w0, k = PO.chunk_windows(ptr, n)
+        assert rep.probed == 1 and rep.windows == k and rep.bytes_probed == 32 * k and rep.seed == 0xABCD, armed
+        assert rep.mismatch_bytes == 0 and rep.reread_nonzero_bytes == 0 and rep.va_base == ptr, armed
+        assert rep.launches == (3 if k else 0) and mm.located == 1 and mm.mismatch_bytes == 0, armed
+        host = buf.cpu().numpy()
+        want = host.copy()
+        want[:] = 0xEE
+        for i in range(k):
+            o = w0 + 4096 * i - base
+            want[o:o + 32] = 0
+        assert (host == want).all(), armed   # the windows zero, every other byte (guards included) untouched
+
+
+class _Prop(C.Structure):      # CUmemAllocationProp
+    _fields_ = [("type", C.c_int), ("handle_types", C.c_int), ("loc_type", C.c_int), ("loc_id", C.c_int),
+                ("win32", C.c_void_p), ("compression", C.c_ubyte), ("rdma", C.c_ubyte), ("usage", C.c_ushort),
+                ("reserved", C.c_ubyte * 4)]
+
+
+class _Access(C.Structure):    # CUmemAccessDesc
+    _fields_ = [("loc_type", C.c_int), ("loc_id", C.c_int), ("flags", C.c_int)]
+
+
+class TwoViews:
+    """One granule of device 0's memory mapped twice, end to end, through the driver's VMM calls: the region
+    [va, va + 2 * gran) is two virtual views of the same physical memory, the alias the probe looks for."""
+
+    def __enter__(self):
+        torch.zeros(1, device="cuda")   # the primary context, current on this thread
+        self.cu = cu = C.CDLL("libcuda.so.1")
+        prop = _Prop(type=1, loc_type=1, loc_id=torch.cuda.current_device())   # pinned, on the device
+        gran = C.c_size_t()
+        self.ok(cu.cuMemGetAllocationGranularity(C.byref(gran), C.byref(prop), 0))
+        self.gran = gran.value
+        self.handle, self.va = C.c_ulonglong(), C.c_ulonglong()
+        self.ok(cu.cuMemCreate(C.byref(self.handle), C.c_size_t(self.gran), C.byref(prop), C.c_ulonglong(0)))
+        self.ok(cu.cuMemAddressReserve(C.byref(self.va), C.c_size_t(2 * self.gran), C.c_size_t(0), C.c_ulonglong(0),
+                                       C.c_ulonglong(0)))
+        self.mapped = []
+        for k in range(2):
+            a = C.c_ulonglong(self.va.value + k * self.gran)
+            self.ok(cu.cuMemMap(a, C.c_size_t(self.gran), C.c_size_t(0), self.handle, C.c_ulonglong(0)))
+            self.mapped.append(a)
+        acc = _Access(loc_type=1, loc_id=prop.loc_id, flags=3)   # read and write
+        self.ok(cu.cuMemSetAccess(self.va, C.c_size_t(2 * self.gran), C.byref(acc), C.c_size_t(1)))
+        return self
+
+    def ok(self, rc):
+        assert rc == 0, f"CUDA driver error {rc}"
+
+    def __exit__(self, *exc):
+        torch.cuda.synchronize()
+        for a in self.mapped:
+            self.cu.cuMemUnmap(a, C.c_size_t(self.gran))
+        self.cu.cuMemAddressFree(self.va, C.c_size_t(2 * self.gran))
+        self.cu.cuMemRelease(self.handle)
+
+
+def test_region_probe_books_the_windows_of_a_second_view(lib):
+    """Off-tag bytes in the windows P2 checks: the second view's P1 overwrites the first view's tags (or the other way
+    round: one launch takes both views).  Plain and armed, every window of the pair whose tags were lost books off-tag
+    bytes, P2 zeroes both views, P3 reads zeros, and armed, each step counts every window on its page."""
+    with TwoViews() as tv:
+        ptr, n = tv.va.value, 2 * tv.gran
+        k = n // PO.STRIDE
+        for armed in (False, True):
+            arm = probe_map(lib, ptr, n) if armed else None
+            with arm or contextlib.nullcontext():
+                rep, mm = region_probe(lib, ptr, n, 0x5EED)
+            assert rep.probed == 1 and rep.windows == k and rep.reread_nonzero_bytes == 0, armed
+            # each pair of windows shares one sector: at least the view whose tags were lost is off them
+            assert rep.mismatch_bytes > 0 and mm.mismatch_bytes == rep.mismatch_bytes, (armed, rep.mismatch_bytes)
+            assert k // 2 <= mm.mismatch_windows <= 2 * k and mm.truncated == 1, (armed, mm.mismatch_windows)
+            if arm:
+                assert arm.take() == [arm.want(RO.probe_parts([(ptr, n)]))] * 3, (arm.base - ptr, arm.pages)
+
 
 
 def test_rate_bar_against_a_same_run_tag_check(lib):

@@ -13,6 +13,7 @@ import shutil
 import subprocess
 from pathlib import Path
 
+import numpy as np
 import pytest
 
 import report_cover_oracle as RO
@@ -70,8 +71,76 @@ def test_locate_walks_the_spans_and_the_triages_the_runs_of_their_own_map():
     assert sum(RO.per_page(RO.pieces("LOCATE", spans)).values()) == 10 * MiB
 
 
+# ---------------------------------------------------------------------------------- caller-owned maps (ccm_region_prove)
+def byte_walk_map(parts: list[tuple[int, int]], base: int, pages: int) -> list[int]:
+    """The map, one byte at a time: each byte's page from base, or the outside slot."""
+    m = np.zeros(pages + 1, np.int64)
+    for a, n in parts:
+        page = (np.arange(a, a + n, dtype=np.int64) - base) // PAGE
+        np.add.at(m, np.where((page >= 0) & (page < pages), page, pages), 1)
+    return m.tolist()
+
+
+A = 1 << 40   # an address
+MAP_CASES = [([(A + 5, 5 * MiB + 77)], A + 3 * MiB + 11, 1),               # below base, page 0, past it
+             ([(A + 5, 5 * MiB + 77)], A - PAGE + 9, 2),                      # the whole region inside, unaligned base
+             ([(A, 6 * MiB)], A, 3),                                          # exactly the map
+             ([(A + 100, 40)], A + 120, 0),                                   # no page: everything outside
+             ([(A + 7, 300), (A + 3 * PAGE - 17, 64), (A + 9 * MiB, 2 * MiB)], A + 1, 4)]
+
+
+@pytest.mark.parametrize("parts,base,pages", MAP_CASES)
+def test_cover_map_matches_a_byte_walk(parts, base, pages):
+    assert RO.cover_map(parts, base, pages) == byte_walk_map(parts, base, pages)
+    assert sum(RO.cover_map(parts, base, pages)) == sum(n for _, n in parts)
+    assert {p: v for p, v in RO.per_page(parts, base=base).items() if v} == RO.brute_counts(parts, 1, base=base)
+
+
+@pytest.mark.parametrize("chunk", [(A + 100, 4 * MiB), (A + 4096 - 9, 3 * 4096), (A + 4095, 2), (A, 31)])
+def test_probe_map_is_32_bytes_per_window(chunk):
+    w0, k = RO.PO.chunk_windows(*chunk)
+    parts = RO.probe_parts([chunk])
+    assert parts == [(w0 + 4096 * i, 32) for i in range(k)]
+    for base in (w0 + 7, w0 + 4096 * (k // 2) + 7, chunk[0] - PAGE + 1):
+        m = RO.cover_map(parts, base, 1)
+        assert m == byte_walk_map(parts, base, 1) and sum(m) == 32 * k, base
+
+
+def test_map_bases_cut_where_the_kernels_split():
+    """A region longer than a page and two chunks: base and every page boundary but the last cut a chunk of the body,
+    the last cuts the tail, and bytes lie before base and past the last page.  A shorter one: each cut on each side."""
+    CH = RO.CO.CHUNK
+    for addr in (A, A + 1, A + 17, A + 127):
+        for n in (PAGE + 2 * CH + 200, 16 * MiB + 3, (1 << 34) - 8, 3 * PAGE + 1 - (addr - A)):
+            head = (128 - addr % 128) % 128
+            base, pages = RO.map_base(addr, n, 0)
+            assert pages >= 1 and base > addr + head and (base - addr - head) % CH != 0, (addr, n)
+            assert addr + n - 2 <= base + pages * PAGE < addr + n, (addr, n)
+            m = RO.cover_map([(addr, n)], base, pages)
+            assert m[-1] == (base - addr) + (addr + n - base - pages * PAGE) and 0 < min(m[:-1]), (addr, n)
+        n = 3 * CH + 77
+        seen = {RO.map_base(addr, n, run) for run in range(8)}
+        assert len(seen) == 8 and {p for _, p in seen} == {1}, addr
+        for base, _ in seen:
+            assert addr < base < addr + n or addr < base + PAGE < addr + n
+
+
 # ---------------------------------------------------------------------------------- the C ABI
 ENTRY_POINTS = ("ccm_scrub_last_report_cover", "ccm_last_report_cover_pages")
+
+
+def test_region_prove_is_exported_and_refuses_a_missing_device(native):
+    lib = N.lib()
+    nm = subprocess.run(["nm", "-D", "--defined-only", str(N.LIB_PATH)], capture_output=True, text=True,
+                        check=True).stdout
+    assert "ccm_region_prove" in N.EXPORTED_SYMBOLS and re.search(r" T ccm_region_prove$", nm, re.M)
+    header = (ROOT / "include" / "ccm.h").read_text()
+    assert re.search(r"^int ccm_region_prove\(int cuda_ordinal, uint32_t\* map, uint64_t base, uint32_t pages\);",
+                     header, re.M)
+    words = (C.c_uint32 * 4)()
+    for ordinal in (-1, 1 << 12):
+        assert lib.ccm_region_prove(ordinal, C.cast(words, C.c_void_p), 0, 3) == N.ERR_NO_CUDA
+        assert lib.ccm_region_prove(ordinal, None, 0, 0) == N.ERR_NO_CUDA
 
 
 def test_entry_points_are_exported_and_refuse_what_they_must(native):

@@ -7,6 +7,10 @@
   count a zero region, dirt at the edges of the decomposition, address bit-planes and byte-value edges
   exactly, with non-zero guards around the region;
 * every 32-bit word once (16 GiB): the count is 4 x 255 x 2^24, above 2^32;
+* the proving twins of the default kernels (include/ccm.h: ccm_region_prove) once more at every placement of the
+  default scrub and verifier and over the 16 GiB: the same bytes and counts, and a cover map equal to the oracle's
+  (tests/report_cover_oracle.py), with page boundaries inside the head, a chunk, a vector and the tail; every other
+  variant armed at its first placement counts nothing;
 * launch-to-launch state of the default kernels, with and without programmatic dependent launch;
 * the product gate under every variant pair and to the last byte of a whole-HBM call.
 Cases and patterns come from tests/scrub_cases.py (checked on the CPU by
@@ -23,6 +27,7 @@ from pathlib import Path
 import pytest
 
 import scrub_cases as SC
+from region_cover_calls import ArmedMap
 from k8s_cc_manager_b200 import _native as N
 
 pytestmark = pytest.mark.gpu
@@ -80,27 +85,39 @@ def test_scrub_matrix_writes_exactly_its_region(lib, dev):
     assert max_len <= SC.MAX_LENGTH
     buf = guarded_buffer(torch, max_len, guard)
     gen = torch.Generator(device="cuda").manual_seed(20261015)
-    failures, runs = [], 0
+    failures, runs, armed_runs = [], 0, 0
     with torch.cuda.stream(stream):
         src = torch.randint(1, 256, (max_len,), dtype=torch.uint8, device="cuda", generator=gen)
         for case, g, full in plan:
             cfg = cfg_ref(case)
-            for o, n in SC.placements(g, full):
+            fast = SC.is_fast(case)
+            for i, (o, n) in enumerate(SC.placements(g, full)):
                 start, end = guard + o, guard + o + n
-                buf.fill_(SENTINEL)
-                buf[start:end].copy_(src[:n])
-                ok(lib.ccm_region_scrub(0, C.c_void_p(buf.data_ptr() + start), n, case.variant, cfg, h, None),
-                   case.label())
-                below = start - torch.count_nonzero(buf[:start] == SENTINEL)
-                inside = torch.count_nonzero(buf[start:end])
-                above = (buf.numel() - end) - torch.count_nonzero(buf[end:] == SENTINEL)
-                bad = torch.stack([below, inside, above]).tolist()
-                runs += 1
-                if any(bad):
-                    failures.append((case.label(), o, n, "below/inside/above", bad))
+                ptr = buf.data_ptr() + start
+                for armed in (False, True) if fast or i == 0 else (False,):
+                    buf.fill_(SENTINEL)
+                    buf[start:end].copy_(src[:n])
+                    arm = ArmedMap(lib, ptr, n, armed_runs) if armed else None
+                    if arm:
+                        with arm:
+                            ok(lib.ccm_region_scrub(0, C.c_void_p(ptr), n, case.variant, cfg, h, None), case.label())
+                        got, want = arm.take()[0], arm.want([(ptr, n)] if fast else [])
+                        armed_runs += 1
+                        if got != want:
+                            failures.append((case.label(), o, n, "cover map", arm.base - ptr, got, want))
+                    else:
+                        ok(lib.ccm_region_scrub(0, C.c_void_p(ptr), n, case.variant, cfg, h, None), case.label())
+                    below = start - torch.count_nonzero(buf[:start] == SENTINEL)
+                    inside = torch.count_nonzero(buf[start:end])
+                    above = (buf.numel() - end) - torch.count_nonzero(buf[end:] == SENTINEL)
+                    bad = torch.stack([below, inside, above]).tolist()
+                    runs += 1
+                    if any(bad):
+                        failures.append((case.label(), o, n, armed, "below/inside/above", bad))
     stream.synchronize()
     assert not failures, f"{len(failures)} of {runs} scrubs inexact, first: {failures[:10]}"
-    print(f"\nscrub matrix: {runs} scrubs over {len(plan)} launch shapes exact (guards {guard >> 10} KiB)")
+    print(f"\nscrub matrix: {runs} scrubs over {len(plan)} launch shapes exact (guards {guard >> 10} KiB), "
+          f"{armed_runs} of them armed")
 
 
 def test_verify_matrix_counts_exactly(lib, dev):
@@ -111,16 +128,27 @@ def test_verify_matrix_counts_exactly(lib, dev):
     guard = max([256 * 1024] + [g.chunk for g in geoms])
     guard = -(-guard // 512) * 512
     buf = guarded_buffer(torch, max_len, guard)
-    failures, runs = [], [0]
+    failures, runs = [], [0, 0]
 
     def count_all(verifiers, o, n, expect, what):
+        """Every verifier of the group, then the default one armed: the same count and a cover map of the region, or
+        (the first count of each placement) a group verifier armed: its count and an empty map."""
         ptr = C.c_void_p(buf.data_ptr() + guard + o)
-        for case in verifiers:
+        armed = [SC.FAST_VERIFY] + ([verifiers[0]] if what == "zero" and verifiers[0] != SC.FAST_VERIFY else [])
+        for case, arm in [(c, None) for c in verifiers] + [(c, ArmedMap(lib, ptr.value, n, runs[1])) for c in armed]:
             nz = C.c_uint64(1 << 63)
-            ok(lib.ccm_region_verify(0, ptr, n, case.variant, cfg_ref(case), h, C.byref(nz), None), case.label())
+            if arm:
+                with arm:
+                    ok(lib.ccm_region_verify(0, ptr, n, case.variant, cfg_ref(case), h, C.byref(nz), None), case.label())
+                got, want = arm.take()[0], arm.want([(ptr.value, n)] if case == SC.FAST_VERIFY else [])
+                runs[1] += 1
+                if got != want:
+                    failures.append((case.label(), o, n, what, "cover map", arm.base - ptr.value, got, want))
+            else:
+                ok(lib.ccm_region_verify(0, ptr, n, case.variant, cfg_ref(case), h, C.byref(nz), None), case.label())
             runs[0] += 1
             if nz.value != expect:
-                failures.append((case.label(), o, n, what, nz.value, expect))
+                failures.append((case.label(), o, n, what, arm is not None, nz.value, expect))
 
     with torch.cuda.stream(stream):
         for group, g in zip(groups, geoms):
@@ -147,7 +175,7 @@ def test_verify_matrix_counts_exactly(lib, dev):
                 count_all(verifiers, o, n, n, f"all {value:#x}")
     stream.synchronize()
     assert not failures, f"{len(failures)} of {runs[0]} counts inexact, first: {failures[:10]}"
-    print(f"\nverify matrix: {runs[0]} counts over {len(groups)} geometries exact")
+    print(f"\nverify matrix: {runs[0]} counts over {len(groups)} geometries exact, {runs[1]} of them armed")
 
 
 def test_every_32bit_word_is_counted_exactly(lib, dev):
@@ -179,6 +207,14 @@ def test_every_32bit_word_is_counted_exactly(lib, dev):
                    case.label())
                 if nz.value != want:
                     failures.append((case.label(), label, nz.value, want))
+            # the read-back's proving twin: the same count, and every byte of the 16 GiB on its page of the map
+            nz = C.c_uint64(0)
+            with ArmedMap(lib, ptr, n, 0) as arm:
+                ok(lib.ccm_region_verify(0, C.c_void_p(ptr), n, SC.FAST_VERIFY.variant, None, h, C.byref(nz), None),
+                   "armed")
+            got = arm.take()[0]
+            if nz.value != want or sum(got) != n or got != arm.want([(ptr, n)]):
+                failures.append(("armed", label, nz.value, want, sum(got), n, arm.pages, got[-1]))
     stream.synchronize()
     del words, raw
     torch.cuda.empty_cache()
@@ -187,10 +223,11 @@ def test_every_32bit_word_is_counted_exactly(lib, dev):
 
 def test_default_kernels_hand_back_clean_grab_state(lib, dev):
     """Dirt only in chunk 0 and the last whole chunk after each call: a grab word left non-zero by any
-    earlier launch (nchunks == 0, 1 byte, multi-chunk, segmented-arena step, either stream) skips one."""
+    earlier launch (nchunks == 0, 1 byte, multi-chunk, segmented-arena step, a proving twin, either stream)
+    skips one."""
     from default_kernel_steps import launch_state_sequence
     rows = launch_state_sequence(lib)
-    assert len(rows) == 9
+    assert len(rows) == 13 and sum(str(r[0]).startswith("armed") for r in rows) == 4
 
 
 def run_steps_child(pdl: str) -> dict:
@@ -209,6 +246,7 @@ def test_pdl_chained_steps_match_the_plain_launches(lib):
     assert all(step == [8, 0, 0] for step in with_pdl["arena_steps"]), with_pdl["arena_steps"]
     assert len(with_pdl["arena_steps"]) == 4
     assert all(r[1] == r[2] and r[3] == 0 and r[4] == 0 for r in with_pdl["sequence"])
+    assert len(with_pdl["sequence"]) == 13 and sum(str(r[0]).startswith("armed") for r in with_pdl["sequence"]) == 4
     assert with_pdl["product_dirty"] == [N.ERR_DIRTY, 8, 2 << 30]
 
 

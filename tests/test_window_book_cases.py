@@ -118,8 +118,6 @@ def test_masks_and_content():
 
 
 # ------------------------------------------------------------------ every kernel libccm.so defines, and who runs it
-KERNEL_RE = re.compile(r"ccm::(\w+kernel)(?:<[^>]*>)?\(")
-
 # kernel -> the GPU test that launches it ("file::test")
 KERNEL_TESTS = {
     "scrub_st_kernel": "test_scrub_exactness_gpu.py::test_scrub_matrix_writes_exactly_its_region",
@@ -135,19 +133,50 @@ KERNEL_TESTS = {
     "xor_byte_kernel": "test_window_books_gpu.py::test_record_limit_in_product_calls",
     "fill_byte_kernel": "test_scrub_gpu.py::test_segmented_arena",
     "fill_pattern_kernel": "test_scrub_gpu.py::test_seeded_pattern_count_matches_oracle",
+    # the proving twins, armed on caller-owned memory (include/ccm.h: ccm_region_prove)
+    "cover_zero_pass": "test_scrub_exactness_gpu.py::test_scrub_matrix_writes_exactly_its_region",
+    "cover_read_pass": "test_scrub_exactness_gpu.py::test_verify_matrix_counts_exactly",
+    "cover_tag_fill_pass": "test_window_books_gpu.py::test_placement_matrix",
+    "cover_tag_check_pass": "test_window_books_gpu.py::test_placement_matrix",
+    "cover_census_zero_pass": "test_window_books_gpu.py::test_placement_matrix",
+    "cover_census_tag_pass": "test_window_books_gpu.py::test_placement_matrix",
+    "cover_locate_pass": "test_window_books_gpu.py::test_placement_matrix",
+    "alias_probe_fill_pass": "test_alias_probe_gpu.py::test_region_probe_against_the_oracle",
+    "alias_probe_check_pass": "test_alias_probe_gpu.py::test_region_probe_against_the_oracle",
+    "alias_probe_reread_pass": "test_alias_probe_gpu.py::test_region_probe_against_the_oracle",
+    "cover_probe_fill_pass": "test_alias_probe_gpu.py::test_region_probe_against_the_oracle",
+    "cover_probe_check_pass": "test_alias_probe_gpu.py::test_region_probe_against_the_oracle",
+    "cover_probe_reread_pass": "test_alias_probe_gpu.py::test_region_probe_against_the_oracle",
 }
+ENTRY_RE = re.compile(r"^STT_FUNC\s+STB_GLOBAL\s+\S+\s+(\S+)$", re.M)
+KERNEL_RE = re.compile(r"^(?:void )?ccm::(\w+)(?:<[^>]*>)?\(")
+
+
+def device_kernels() -> list[str]:
+    """Every kernel entry of libccm.so's device code (its global functions), demangled."""
+    from k8s_cc_manager_b200 import build
+    cuobjdump = Path(build.find_nvcc()).parent / "cuobjdump"
+    assert cuobjdump.exists(), f"{cuobjdump} lists the kernels libccm.so defines; it ships with nvcc"
+    out = subprocess.run([str(cuobjdump), "-symbols", str(N.LIB_PATH)], check=True, capture_output=True,
+                         text=True).stdout
+    cxxfilt = shutil.which("c++filt")
+    assert cxxfilt, "c++filt (binutils) is needed to demangle the kernel names"
+    mangled = ENTRY_RE.findall(out)
+    return subprocess.run([cxxfilt], input="\n".join(mangled), check=True, capture_output=True,
+                          text=True).stdout.split("\n")[:len(mangled)]
 
 
 def test_every_kernel_is_launched_by_a_named_gpu_test():
-    nm = shutil.which("nm")
-    assert nm, "nm (binutils) is needed to list the kernels libccm.so defines"
-    out = subprocess.run([nm, "-C", "--defined-only", str(N.LIB_PATH)], check=True, capture_output=True,
-                         text=True).stdout
-    defined = set(KERNEL_RE.findall(out))
-    assert {"locate_dirt_kernel", "census_zero_kernel", "scrub_st_kernel"} <= defined, sorted(defined)
+    entries = device_kernels()
+    names = [KERNEL_RE.match(e) for e in entries]
+    assert all(names), [e for e, m in zip(entries, names) if not m]
+    defined = {m.group(1) for m in names}
+    assert {"locate_dirt_kernel", "cover_locate_pass", "alias_probe_check_pass"} <= defined, sorted(defined)
     missing = sorted(defined - set(KERNEL_TESTS))
     assert not missing, "kernels no GPU test is named for (add them to KERNEL_TESTS):\n  " + "\n  ".join(missing)
+    assert not set(KERNEL_TESTS) - defined, sorted(set(KERNEL_TESTS) - defined)
     for kernel, test in KERNEL_TESTS.items():
         fname, tname = test.split("::")
         src = (ROOT / "tests" / fname).read_text()
         assert re.search(rf"^def {tname}\(", src, re.M), (kernel, test)
+    print(f"\n{len(entries)} kernel entries, {len(defined)} kernels, each launched by a named GPU test")

@@ -1,9 +1,13 @@
 """The window books on one H100: the locate pass, the tag check and both censuses against the numpy oracles at every
 placement of tests/window_book_cases.py, with every 16-bit mask on every place they book from, at the 64-record limit
 (in single launches and in product calls on the pipelined and the fallback path), and across a seeded sequence of
-region passes and product calls on one engine, with the census error path in it."""
+region passes and product calls on one engine, with the census error path in it.  The placement matrix, every mask
+and the head and tail windows run each pass once more armed (include/ccm.h: ccm_region_prove): the proving twin must
+book, map and write exactly what the plain kernel did, and count every byte of the region on its page of a cover map
+whose page boundaries cut the region (tests/report_cover_oracle.py: map_base)."""
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import sys
 from dataclasses import dataclass
@@ -18,6 +22,7 @@ import dirt_oracle as DO  # noqa: E402
 import mismatch_oracle as MO  # noqa: E402
 import product_gate_calls as PGC  # noqa: E402
 import product_plan as PP  # noqa: E402
+import region_cover_calls as RCC  # noqa: E402
 import scrub_cases as CASES  # noqa: E402
 import tag_oracle as TO  # noqa: E402
 import window_book_cases as WB  # noqa: E402
@@ -33,6 +38,8 @@ GUARD_BYTE = 0xEE
 SEED = 0x7A61B00C
 DRILL_KEYS = PP.DRILL_KEYS + ("tag_inject", "scrub_alias", "scrub_residue")
 PASSES = ("locate", "check", "census0", "census1")
+PAGE_BOOK = {"locate": N.BOOK_DIRT, "check": N.BOOK_MISMATCH, "census0": N.BOOK_RESIDUE, "census1": N.BOOK_RESIDUE}
+ARMED_RUNS = {}           # test -> armed passes it ran
 
 
 @pytest.fixture(scope="module")
@@ -158,36 +165,60 @@ def census(lib, ptr, n, tags, seed=SEED) -> D.ResidueReport:
     return D.ResidueReport.from_native(r)
 
 
-def run_pass(lib, rig: Rig, kind: str, offset: int, region: np.ndarray, what, seed=SEED, zero_too=True) -> Book:
+def armed_map(lib, ptr: int, n: int, test: str) -> RCC.ArmedMap:
+    """A cover map for the next armed pass of `test` over [ptr, ptr + n); counts the pass."""
+    ARMED_RUNS[test] = ARMED_RUNS.get(test, 0) + 1
+    return RCC.ArmedMap(lib, ptr, n, sum(ARMED_RUNS.values()))
+
+
+def run_pass(lib, rig: Rig, kind: str, offset: int, region: np.ndarray, what, seed=SEED, zero_too=True,
+             armed: str | None = None) -> Book:
     """Runs one pass over `region` placed at `offset`, compares its book with the oracle and the slice's end state
     (guards unchanged; the region unchanged by locate, zero after the check and the zero census, the tags after the
-    tagged census).  For the check, the plain check-and-zero runs on the same input as well."""
+    tagged census).  For the check, the plain check-and-zero runs on the same input as well.  armed (the test's name):
+    everything once more with the proving twins, which must give the same book and page map, and cover maps of the
+    region."""
     n = region.size
-    ptr, host, bounds = rig.place(offset, region)
-    want = oracle(kind, region, ptr, seed)
-    if kind == "locate":
-        got = book_of(kind, locate(lib, ptr, n))
-    elif kind == "check":
-        got = book_of(kind, check_locate(lib, ptr, n, seed))
-    else:
-        got = book_of(kind, census(lib, ptr, n, kind == "census1", seed))
-    assert_book(got, want, (kind,) + tuple(what))
-    after = rig.read(bounds)
-    assert np.all(after[:GUARD] == GUARD_BYTE) and np.all(after[GUARD + n:] == GUARD_BYTE), (kind, what, "guards")
-    end = after[GUARD:GUARD + n]
-    if kind == "locate":
-        assert np.array_equal(end, region), (kind, what, "locate wrote the region")
-    elif kind == "census1":
-        assert np.array_equal(end, TO.tag_bytes(seed, ptr, n)), (kind, what, "not the tags")
-    else:
-        assert not end.any(), (kind, what, "region not zeroed")
-    if kind == "check" and zero_too:
-        rig.place(offset, region)
-        assert check_zero(lib, ptr, n, seed) == want.count, (what, "check_zero")
+    books, page_maps = [], []
+    for arm_it in (False, True) if armed else (False,):
+        ptr, host, bounds = rig.place(offset, region)
+        want = oracle(kind, region, ptr, seed)
+        arm = armed_map(lib, ptr, n, armed) if arm_it else contextlib.nullcontext()
+        with arm:
+            if kind == "locate":
+                got = book_of(kind, locate(lib, ptr, n))
+            elif kind == "check":
+                got = book_of(kind, check_locate(lib, ptr, n, seed))
+            else:
+                got = book_of(kind, census(lib, ptr, n, kind == "census1", seed))
+        if arm_it:
+            assert arm.take() == [arm.want([(ptr, n)])], (kind, what, "cover map", arm.base - ptr, arm.pages)
+        books.append(got)
+        page_maps.append(D.last_page_map(0, PAGE_BOOK[kind]).entries)
+        assert_book(got, want, (kind, arm_it) + tuple(what))
         after = rig.read(bounds)
-        assert not after[GUARD:GUARD + n].any() and np.all(after[:GUARD] == GUARD_BYTE), (what, "check_zero end state")
-        assert np.all(after[GUARD + n:] == GUARD_BYTE), (what, "check_zero guards")
-    return got
+        assert np.all(after[:GUARD] == GUARD_BYTE) and np.all(after[GUARD + n:] == GUARD_BYTE), (kind, what, "guards")
+        end = after[GUARD:GUARD + n]
+        if kind == "locate":
+            assert np.array_equal(end, region), (kind, what, "locate wrote the region")
+        elif kind == "census1":
+            assert np.array_equal(end, TO.tag_bytes(seed, ptr, n)), (kind, what, "not the tags")
+        else:
+            assert not end.any(), (kind, what, "region not zeroed")
+        if kind == "check" and zero_too:
+            rig.place(offset, region)
+            with arm:
+                assert check_zero(lib, ptr, n, seed) == want.count, (what, "check_zero")
+            if arm_it:
+                assert arm.take() == [arm.want([(ptr, n)])], (what, "check_zero cover map", arm.base - ptr)
+            after = rig.read(bounds)
+            assert not after[GUARD:GUARD + n].any() and np.all(after[:GUARD] == GUARD_BYTE), (what, "check_zero end")
+            assert np.all(after[GUARD + n:] == GUARD_BYTE), (what, "check_zero guards")
+    # which 64 records a truncated book keeps is not fixed: the rest of it is
+    same = [(b.count, b.windows, b.first, b.last, b.truncated, b.zero_windows, None if b.truncated else b.records)
+            for b in books]
+    assert all(x == same[0] for x in same) and all(m == page_maps[0] for m in page_maps), (kind, what, "armed")
+    return books[0]
 
 
 def content_for(kind: str, offset: int, n: int, windows, masks, rng, rig: Rig, seed=SEED) -> np.ndarray:
@@ -257,17 +288,22 @@ def test_placement_matrix(lib):
             for kind in PASSES:
                 seed = (SEED ^ (n * 131 + off)) & 0xFFFFFFFF or 1
                 region = placement_content(kind, g, off, n, ptr, dense, rng, seed)
-                got = run_pass(lib, rig, kind, off, region, (off, n, dense), seed)
+                got = run_pass(lib, rig, kind, off, region, (off, n, dense), seed, armed="placements")
                 seen.add((kind, "truncated" if got.truncated else "exact"))
                 if kind == "check":
                     seen |= {("kind", r[3]) for r in got.records}
-        # the fill alone: exactly the tags, nothing outside
-        _, _, bounds = rig.place(off, np.zeros(n, dtype=np.uint8))
-        assert lib.ccm_region_tag_fill(0, C.c_void_p(ptr), n, SEED, stream(), None) == 0, N.last_error()
-        after = rig.read(bounds)
-        assert np.array_equal(after[GUARD:GUARD + n], TO.tag_bytes(SEED, ptr, n)), (off, n, "tag fill")
-        assert np.all(after[:GUARD] == GUARD_BYTE) and np.all(after[GUARD + n:] == GUARD_BYTE), (off, n, "fill guards")
+        # the fill alone, plain and armed: exactly the tags, nothing outside
+        for arm in (contextlib.nullcontext(), armed_map(lib, ptr, n, "placements")):
+            _, _, bounds = rig.place(off, np.zeros(n, dtype=np.uint8))
+            with arm:
+                assert lib.ccm_region_tag_fill(0, C.c_void_p(ptr), n, SEED, stream(), None) == 0, N.last_error()
+            after = rig.read(bounds)
+            assert np.array_equal(after[GUARD:GUARD + n], TO.tag_bytes(SEED, ptr, n)), (off, n, "tag fill")
+            assert np.all(after[:GUARD] == GUARD_BYTE) and np.all(after[GUARD + n:] == GUARD_BYTE), (off, n, "guards")
+            if isinstance(arm, RCC.ArmedMap):
+                assert arm.take() == [arm.want([(ptr, n)])], (off, n, "tag fill cover map", arm.base - ptr, arm.pages)
     assert {(k, s) for k in PASSES for s in ("exact", "truncated")} <= seen, sorted(seen)
+    print(f"\nplacement matrix: {ARMED_RUNS['placements']} armed passes")
     assert {("kind", k) for k in ("zero", "alias", "partial", "foreign")} <= seen, sorted(seen)
 
 
@@ -321,8 +357,9 @@ def test_every_mask(lib, kind, path):
         off, n, wins = mask_layout(path, i // 64)
         wins = wins[:len(ms)]
         region = content_for(kind, off, n, wins, ms, rng, rig=rig)
-        got = run_pass(lib, rig, kind, off, region, (path, i), zero_too=False)
+        got = run_pass(lib, rig, kind, off, region, (path, i), zero_too=False, armed=f"mask {kind} {path}")
         assert not got.truncated and [(r[0], r[1]) for r in got.records] == list(zip(wins, ms)), (kind, path, i)
+    print(f"\nevery mask, {kind} on the {path} path: {ARMED_RUNS[f'mask {kind} {path}']} armed passes")
 
 
 @pytest.mark.parametrize("kind", PASSES)
@@ -338,8 +375,9 @@ def test_every_edge_mask_in_head_and_tail_windows(lib, kind):
         tm = masks[(i // 7 * 5) % len(masks)] & 0x7FFF or 0x4000
         wins, all_ms = heads[:len(ms)] + [tail], ms + [tm]
         region = content_for(kind, 16, n, wins, all_ms, rng, rig=rig)
-        got = run_pass(lib, rig, kind, 16, region, ("head/tail", i), zero_too=False)
+        got = run_pass(lib, rig, kind, 16, region, ("head/tail", i), zero_too=False, armed=f"head/tail {kind}")
         assert [(r[0], r[1]) for r in got.records] == list(zip(wins, all_ms)), (kind, i)
+    print(f"\nhead and tail windows, {kind}: {ARMED_RUNS[f'head/tail {kind}']} armed passes")
 
 
 @pytest.mark.parametrize("kind", PASSES)
