@@ -25,6 +25,7 @@
 
 #include "ccm_internal.h"
 #include "ccm_mismatch.h"
+#include "ccm_proof.h"
 #include "scrub_kernels.cuh"
 
 namespace ccm {
@@ -160,17 +161,8 @@ struct CheckSpan { uint64_t addr, bytes, offset; };
 struct Held {
   uint64_t va_base = 0, bytes = 0;
   std::vector<CheckSpan> spans, probe_chunks;
-  std::vector<std::pair<uint64_t, uint32_t>> chunks;   // (offset, chunk) of every allocation's first byte, ascending
-  // The chunk of `offset`: that of the last allocation that starts at or before it, else the first.  Compared as
-  // signed: the head window of a raw region that does not start 16-aligned has a negative offset.  (A mapping or a
-  // segment starts aligned, so the product call never books one.)
-  uint32_t chunk_of(uint64_t offset) const {
-    auto it = std::upper_bound(chunks.begin(), chunks.end(), offset, [](uint64_t o, const std::pair<uint64_t, uint32_t>& c) {
-      return (int64_t)o < (int64_t)c.first;
-    });
-    if (it != chunks.begin()) --it;
-    return it == chunks.end() ? 0u : it->second;
-  }
+  ccm_proof::ChunkTable chunks;   // (offset, chunk) of every allocation's first byte, ascending
+  uint32_t chunk_of(uint64_t offset) const { return ccm_proof::chunk_of(chunks, offset); }
 };
 
 // A raw region's hold: one span, one probe chunk, chunk 0.
@@ -182,23 +174,21 @@ static Held region_held(const void* p, uint64_t bytes) {
 // The product call's passes while it enqueues them (ccm.h: ccm_scrub_prove, and the "cover_skip" drill).  Every range
 // launch of the scrub, census, tag fill, tag check and read-back asks it for its cover map (gate_launch).  The locate
 // pass and the triages run after it is cleared, each step with `report` set (ccm.h: ccm_report_cover, and the
-// "report_skip" drill): their launches ask it for the report step's map.
+// "report_skip" drill): their launches ask it for the report step's map.  The cover maps lie end to end in d_cover:
+// map m = pass - 1 for a pass (CCM_PASS_*), kPasses + step - 1 for a report step (CCM_REPORT_*).
 static constexpr int kPasses = 3;   // CCM_PASS_FIRST, CHECK, READBACK
 static constexpr int kSteps = 3;    // the alias probe's P1, P2, P3
 static constexpr int kReportSteps = (int)CCM_REPORT_STEPS;   // CCM_REPORT_LOCATE .. CCM_REPORT_MISMATCH_T3
+static constexpr int kMaps = kPasses + kReportSteps;
+static constexpr uint32_t kProbeMapsBit = 1u << kMaps;   // GatePasses::touched: the probe's maps (d_pcover)
 struct GatePasses {
   bool active = false;   // the call's passes are being enqueued
-  bool prove = false;    // ... with the proving kernels, into the cover maps
+  bool prove = false;    // ... with the proving kernels, into the cover maps (and so are its report steps)
   std::vector<CheckSpan> spans;   // what the call holds (page 0 of the pages its bytes lie on: addr - offset)
-  int skip_pass = 0;     // drill "cover_skip": pending for the first launch of this pass (CCM_PASS_*; 0 = none)
-  uint64_t skip = 0;
-  bool pcover_dirty = false;   // the probe's proving twins counted into the probe cover maps, not yet taken
   int report = 0;        // the report step (CCM_REPORT_*) being enqueued once the passes are over; 0 = none
-  bool report_prove = false;   // ... with the proving kernels, into the report cover maps
-  int skip_report = 0;   // drill "report_skip": pending for the first launch of this report step (0 = none)
-  uint64_t report_skip = 0;
-  uint64_t report_launches[kReportSteps] = {};   // launches of each report step
-  bool rcover_dirty = false;   // a report step's proving twins counted into its map, not yet taken
+  uint64_t skip[kMaps] = {};       // drill "cover_skip" / "report_skip": pending for the first launch into map m
+  uint64_t launches[kMaps] = {};   // launches into map m
+  uint32_t touched = 0;  // bit m: proving twins counted into map m (kProbeMapsBit: the probe's), not yet taken
 };
 
 struct ScrubEngine {
@@ -230,7 +220,7 @@ struct ScrubEngine {
   ccm_triage_report mtriage{};              // report of the last product call (ccm_scrub_last_mismatch_triage)
   std::vector<ccm_triage_page> mtriage_pages;  // and its pages (ccm_last_mismatch_triage_pages)
   bool prove = false;                       // the coverage proof is armed (ccm_scrub_prove)
-  uint32_t* d_cover = nullptr;              // kPasses cover maps of npages words (the last: outside slot); zero between calls
+  uint32_t* d_cover = nullptr;              // kMaps cover maps of npages words (the last: outside slot); zero between calls
   uint32_t* h_cover = nullptr;              // pinned copy of all of them
   GatePasses gate;                          // the product call's passes, while it enqueues them
   CoverOut region_cover{nullptr, 0, 0};     // the caller's cover map of every launch outside a product call
@@ -247,8 +237,7 @@ struct ScrubEngine {
   int pcover_ctas[3] = {};                  // CTAs per SM of each step's proving twin
   ccm_probe_cover pcover{};                 // report of the last product call (ccm_scrub_last_probe_cover)
   std::vector<ccm_probe_cover_page> pcover_pages;   // and its inexact pages (ccm_last_probe_cover_pages)
-  // report proof (a proven call that locates or triages): kReportSteps maps of npages words after the kPasses cover maps
-  // in d_cover (report_map), and their pinned copy at the same place in h_cover
+  // report proof (a proven call that locates or triages): its maps follow the passes' in d_cover
   ccm_report_cover rcover{};                // report of the last product call (ccm_scrub_last_report_cover)
   std::vector<ccm_report_cover_page> rcover_pages;   // and its inexact pages (ccm_last_report_cover_pages)
   std::vector<Segment> segs;
@@ -266,8 +255,6 @@ struct ScrubEngine {
   // the grab word of a default kernel and its done word, one line further on
   GrabCtl ctl(int grab) const { return GrabCtl{d_counter + grab, d_counter + grab + 8}; }
   DirtRecord* book_records(Book b) const { return d_records + b * kDirtRecords; }
-  // the cover map of report step `step` (CCM_REPORT_*), and its host copy
-  uint64_t report_word(int step) const { return (uint64_t)(kPasses + step - 1) * npages; }
   uint32_t* book_pages(Book b) const { return d_pages + b * npages; }
   // The census records into book_records(kCensusBook) as MaskRecord, passed to it apart from its LocateOut.
   LocateOut book_out(Book b) const {
@@ -629,25 +616,25 @@ static int gate_launch(ScrubEngine* e, int pass, const void* p, int grab, cudaSt
     return CCM_OK;
   }
   if (g.active && pass == 0) return CCM_OK;
-  const bool report = !g.active;
-  if (report) g.report_launches[g.report - 1]++;
-  if (report ? g.skip_report == g.report : g.skip_pass == pass) {
-    // pinned and unchanged until the call ends: the copy runs in stream order
-    const int slot = report ? 6 : 7;
-    e->h_counter[slot] = report ? g.report_skip : g.skip;
+  const int m = g.active ? pass - 1 : kPasses + g.report - 1;
+  g.launches[m]++;
+  if (g.skip[m]) {
+    // pinned and unchanged until the call ends: the copy runs in stream order.  A call can drill a pass and a report
+    // step, so each has its own slot.
+    const int slot = m < kPasses ? 7 : 6;
+    e->h_counter[slot] = g.skip[m];
     CCM_CUDA(cudaMemcpyAsync(e->d_counter + grab, e->h_counter + slot, sizeof(unsigned long long), cudaMemcpyHostToDevice,
                              st));
-    (report ? g.skip_report : g.skip_pass) = 0;
+    g.skip[m] = 0;
   }
-  if (report ? g.report_prove : g.prove) {
+  if (g.prove) {
     const uint64_t a = (uint64_t)(uintptr_t)p;
     // a launch outside what the call holds counts into the outside slot: its offsets all lie past the map
     uint64_t base = a - (uint64_t)e->npages * kPageBytes;
     for (const CheckSpan& sp : g.spans)
       if (a >= sp.addr && a < sp.addr + sp.bytes) base = sp.addr - sp.offset;
-    const uint64_t word = report ? e->report_word(g.report) : (uint64_t)(pass - 1) * e->npages;
-    *cover = CoverOut{e->d_cover + word, base, (uint32_t)(e->npages - 1)};
-    g.rcover_dirty |= report;
+    *cover = CoverOut{e->d_cover + (uint64_t)m * e->npages, base, (uint32_t)(e->npages - 1)};
+    g.touched |= 1u << m;
   }
   return CCM_OK;
 }
@@ -1151,14 +1138,28 @@ static int take_residue(ScrubEngine* e, cudaStream_t st, const Held& h, ccm_resi
 }
 
 // ------------------------------------------------------------------ coverage proof
+// Sets aside n cover maps of npages words, zeroed, and (once) their pinned host copy.  The caller holds e->mu.
+static int alloc_maps(ScrubEngine* e, int n, const char* what, uint32_t** d_maps, uint32_t** h_maps) {
+  const size_t bytes = (size_t)n * e->npages * sizeof(uint32_t);
+  if (!*h_maps) CCM_CUDA(cudaHostAlloc(h_maps, bytes, cudaHostAllocDefault));
+  uint32_t* d = nullptr;
+  CCM_CUDA(cudaMalloc(&d, bytes));
+  const cudaError_t err = cudaMemset(d, 0, bytes);
+  if (err != cudaSuccess) {
+    cudaFree(d);
+    set_error("%s memset failed: %s", what, cudaGetErrorString(err));
+    return CCM_ERR_CUDA;
+  }
+  *d_maps = d;
+  return CCM_OK;
+}
+
 // Sets aside the cover maps and their host copy, and makes the proving kernels resident (a whole-HBM call cannot load a
 // module once everything is mapped).  The report proof's maps follow the passes' in the same allocation: a whole-HBM
 // call that fails has mapped everything by the time it locates.  The caller holds e->mu.
 static int ensure_cover(ScrubEngine* e) {
   if (e->d_cover) return CCM_OK;
   CCM_CUDA(cudaSetDevice(e->ordinal));
-  const size_t bytes = (kPasses + kReportSteps) * e->npages * sizeof(uint32_t);
-  if (!e->h_cover) CCM_CUDA(cudaHostAlloc(&e->h_cover, bytes, cudaHostAllocDefault));
   cudaFuncAttributes fa;
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_ZERO));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_READ));
@@ -1167,176 +1168,76 @@ static int ensure_cover(ScrubEngine* e) {
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_CENSUS_ZERO));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_CENSUS_TAG));
   CCM_CUDA(cudaFuncGetAttributes(&fa, CCM_COVER_LOCATE));
-  uint32_t* d = nullptr;
-  CCM_CUDA(cudaMalloc(&d, bytes));
-  const cudaError_t err = cudaMemset(d, 0, bytes);
-  if (err != cudaSuccess) {
-    cudaFree(d);
-    set_error("cover map memset failed: %s", cudaGetErrorString(err));
-    return CCM_ERR_CUDA;
-  }
-  e->d_cover = d;
-  return CCM_OK;
+  return alloc_maps(e, kMaps, "cover map", &e->d_cover, &e->h_cover);
 }
 
-// After the passes of a proving call have finished (the caller holds e->mu): copies the cover maps once, zeroes them
-// for the next call, and compares every pass that ran against what the call holds, [0, h.bytes) from h.va_base.  Fills
-// e->cover (proved = 1) and e->cover_pages; each inexact page gets h.chunk_of(page offset).
+// After the passes of a proving call have finished (the caller holds e->mu): copies the passes' maps once, zeroes them
+// for the next call, and compares every pass that ran against what the call holds (ccm_proof.h: fill_cover).  Fills
+// e->cover (proved = 1) and e->cover_pages.
 static int take_cover(ScrubEngine* e, cudaStream_t st, const Held& h, bool tagged, ccm_cover_report* out) {
-  const uint64_t mapped = h.bytes;
-  e->gate.prove = false;
   const double t0 = now_ms();
   const size_t bytes = kPasses * e->npages * sizeof(uint32_t);
   CCM_CUDA(cudaMemcpyAsync(e->h_cover, e->d_cover, bytes, cudaMemcpyDeviceToHost, st));
   CCM_CUDA(cudaMemsetAsync(e->d_cover, 0, bytes, st));
   CCM_CUDA(cudaStreamSynchronize(st));
-  ccm_cover_report rep;
-  memset(&rep, 0, sizeof rep);
-  rep.bytes_mapped = mapped;
-  rep.pages_mapped = (mapped + kPageBytes - 1) / kPageBytes;
-  rep.va_base = h.va_base;
-  rep.proved = 1;
+  e->gate.touched &= ~((1u << kPasses) - 1);
   const bool ran[kPasses] = {true, tagged, true};
-  for (int k = 0; k < kPasses; ++k) rep.pass[k].ran = ran[k];
-  const uint64_t np = e->npages - 1;   // pages of a map; word np is its outside slot
-  std::vector<ccm_cover_page> pages;
-  for (uint64_t p = 0; p < np; ++p) {
-    const uint64_t lo = p * kPageBytes;
-    const uint32_t expected = lo < mapped ? (uint32_t)std::min<uint64_t>(kPageBytes, mapped - lo) : 0u;
-    ccm_cover_page cp;
-    memset(&cp, 0, sizeof cp);
-    cp.page = p;
-    cp.expected = expected;
-    bool exact = true;
-    for (int k = 0; k < kPasses; ++k) {
-      if (!ran[k]) continue;
-      const uint32_t c = e->h_cover[k * e->npages + p];
-      ccm_cover_pass& ps = rep.pass[k];
-      cp.count[k] = c;
-      ps.bytes_counted += c;
-      if (c < expected) {
-        if (ps.pages_short++ == 0) ps.first_short_page = p;
-        ps.bytes_missing += expected - c;
-      } else if (c > expected) {
-        ps.pages_over++;
-        ps.bytes_extra += c - expected;
-      }
-      exact &= c == expected;
-    }
-    if (!exact) {
-      cp.chunk = h.chunk_of(lo);
-      pages.push_back(cp);
-    }
-  }
-  rep.covered = 1;
-  for (int k = 0; k < kPasses; ++k) {
-    if (!ran[k]) continue;
-    ccm_cover_pass& ps = rep.pass[k];
-    ps.bytes_outside = e->h_cover[k * e->npages + np];
-    ps.bytes_counted += ps.bytes_outside;
-    ps.bytes_extra += ps.bytes_outside;
-    if (ps.bytes_missing || ps.bytes_extra) rep.covered = 0;
-  }
-  rep.ms_prove = now_ms() - t0;
-  e->cover = *out = rep;
-  e->cover_pages.swap(pages);
+  ccm_proof::fill_cover(e->h_cover, e->npages - 1, h.spans, h.bytes, h.va_base, ran, h.chunks, &e->cover,
+                        &e->cover_pages);
+  e->cover.ms_prove = now_ms() - t0;
+  *out = e->cover;
   return CCM_OK;
 }
 
 // ------------------------------------------------------------------ report proof
-// What one report step over `pieces` (each `bytes` at `offset` from va_base: the spans of what the call holds, or the
-// runs of a triage) must count on each of the np pages: the bytes of the pieces that lie on it.
-template <typename Piece>
-static std::vector<uint32_t> report_cover_expected(const std::vector<Piece>& pieces, uint64_t np) {
-  std::vector<uint32_t> exp(np, 0);
-  for (const Piece& r : pieces)
-    for (uint64_t o = r.offset, end = r.offset + r.bytes; o < end;) {
-      const uint64_t p = o / kPageBytes, next = std::min<uint64_t>(end, (p + 1) * kPageBytes);
-      if (p < np) exp[p] += (uint32_t)(next - o);
-      o = next;
-    }
-  return exp;
-}
-
 // After report steps first .. first + n - 1 (CCM_REPORT_*) of a proven call over `pieces` (the caller holds e->mu and
 // their kernels have finished; ok = false when an error cut them short): zeroes their maps for the next report, and
-// when they ran to the end copies them first, all in one copy, and compares each step against
-// report_cover_expected(pieces) into e->rcover (proved = 1) and e->rcover_pages, each inexact page with
-// h.chunk_of(page offset).  After an error the steps keep ran = 0.
+// when they ran to the end copies them first, all in one copy, and compares each step against the bytes of `pieces`
+// (ccm_proof.h: fill_report_steps) into e->rcover (proved = 1) and e->rcover_pages.  After an error the steps keep
+// ran = 0.
 template <typename Piece>
 static int take_report_cover(ScrubEngine* e, cudaStream_t st, const Held& h, int first, int n,
                              const std::vector<Piece>& pieces, bool ok) {
   const double t0 = now_ms();
+  const int m = kPasses + first - 1;
   const size_t bytes = (size_t)n * e->npages * sizeof(uint32_t);
-  uint32_t* const d = e->d_cover + e->report_word(first);
-  const uint32_t* const c = e->h_cover + e->report_word(first);
-  if (ok) CCM_CUDA(cudaMemcpyAsync((void*)c, d, bytes, cudaMemcpyDeviceToHost, st));
+  uint32_t* const d = e->d_cover + (uint64_t)m * e->npages;
+  uint32_t* const maps = e->h_cover + (uint64_t)m * e->npages;
+  if (ok) CCM_CUDA(cudaMemcpyAsync(maps, d, bytes, cudaMemcpyDeviceToHost, st));
   CCM_CUDA(cudaMemsetAsync(d, 0, bytes, st));
   CCM_CUDA(cudaStreamSynchronize(st));
+  e->gate.touched &= ~(((1u << n) - 1) << m);
   ccm_report_cover& rep = e->rcover;
-  if (!rep.proved) {
-    rep.proved = 1;
-    rep.covered = 1;
-    rep.va_base = h.va_base;
-  }
-  if (ok) {
-    const uint64_t np = e->npages - 1;   // pages of a map; word np is its outside slot
-    const std::vector<uint32_t> exp = report_cover_expected(pieces, np);
-    uint64_t total = 0;
-    for (const Piece& r : pieces) total += r.bytes;
-    for (int k = 0; k < n; ++k) {
-      const int step = first + k;
-      const uint32_t* m = c + (uint64_t)k * e->npages;
-      ccm_report_cover_step& ps = rep.step[step - 1];
-      ps.ran = 1;
-      ps.launches = e->gate.report_launches[step - 1];
-      ps.bytes_expected = total;
-      for (uint64_t p = 0; p < np; ++p) {
-        ps.bytes_counted += m[p];
-        if (m[p] == exp[p]) continue;
-        if (m[p] < exp[p]) {
-          if (ps.pages_short++ == 0) ps.first_short_page = p;
-          ps.bytes_missing += exp[p] - m[p];
-        } else {
-          ps.pages_over++;
-          ps.bytes_extra += m[p] - exp[p];
-        }
-        e->rcover_pages.push_back(ccm_report_cover_page{p, h.chunk_of(p * kPageBytes), step, exp[p], m[p]});
-      }
-      ps.bytes_outside = m[np];
-      ps.bytes_counted += m[np];
-      ps.bytes_extra += m[np];
-      if (ps.bytes_missing || ps.bytes_extra) rep.covered = 0;
-    }
-  }
+  if (!rep.proved) { rep.proved = rep.covered = 1; rep.va_base = h.va_base; }
+  if (ok)
+    ccm_proof::fill_report_steps(maps, e->npages - 1, first, n, pieces, e->gate.launches + kPasses, h.chunks, &rep,
+                                 &e->rcover_pages);
   rep.ms_prove += now_ms() - t0;
   return CCM_OK;
 }
 
 // Starts the passes of one product call (the caller holds e->mu, before the call maps or launches anything): the
-// "cover_skip" drill pending, and when the device is armed, the cover maps set aside.  An armed call that cannot count
-// fails here: it never runs unproven.  The caller adds the spans of what it holds.
+// "cover_skip" and "report_skip" drills pending, and when the device is armed, the cover maps set aside.  An armed call
+// that cannot count fails here: it never runs unproven.  The caller adds the spans of what it holds.
 static int begin_gate(ScrubEngine* e, const ScrubDrill& drill) {
   e->gate = GatePasses();
   e->gate.active = true;
-  if (drill.cover_skip) { e->gate.skip_pass = drill.cover_pass; e->gate.skip = drill.cover_skip; }
-  if (drill.report_skip) { e->gate.skip_report = drill.report_skip_step; e->gate.report_skip = drill.report_skip; }
+  e->gate.skip[drill.cover_pass - 1] = drill.cover_skip;
+  e->gate.skip[kPasses + drill.report_skip_step - 1] = drill.report_skip;
   if (!e->prove) return CCM_OK;
   if (int rc = ensure_cover(e)) { e->gate.active = false; return rc; }
   e->gate.prove = true;
   return CCM_OK;
 }
 
-// Ends them after every call, whatever it returned.  An armed call cut short by an error leaves partial counts: the
-// maps are zero again for the next one.
+// Ends them after every call, whatever it returned.  An armed call cut short by an error leaves partial counts in the
+// maps it touched and did not take: they are zero again for the next one.
 static void end_gate(ScrubEngine* e) {
   std::lock_guard<std::mutex> g(e->mu);
-  if ((e->gate.prove || e->gate.pcover_dirty || e->gate.rcover_dirty) && e->ready &&
-      cudaSetDevice(e->ordinal) == cudaSuccess) {
-    if (e->gate.prove && e->d_cover) cudaMemsetAsync(e->d_cover, 0, kPasses * e->npages * sizeof(uint32_t), e->stream);
-    if (e->gate.pcover_dirty) cudaMemsetAsync(e->d_pcover, 0, kSteps * e->npages * sizeof(uint32_t), e->stream);
-    if (e->gate.rcover_dirty)
-      cudaMemsetAsync(e->d_cover + e->report_word(1), 0, kReportSteps * e->npages * sizeof(uint32_t), e->stream);
+  const uint32_t touched = e->gate.touched;
+  if (touched && e->ready && cudaSetDevice(e->ordinal) == cudaSuccess) {
+    if (touched & (kProbeMapsBit - 1)) cudaMemsetAsync(e->d_cover, 0, kMaps * e->npages * sizeof(uint32_t), e->stream);
+    if (touched & kProbeMapsBit) cudaMemsetAsync(e->d_pcover, 0, kSteps * e->npages * sizeof(uint32_t), e->stream);
     cudaStreamSynchronize(e->stream);
   }
   e->gate = GatePasses();
@@ -1360,128 +1261,34 @@ static int ensure_probe(ScrubEngine* e) {
   return CCM_OK;
 }
 
-// The probe windows of [addr, addr + n): the first 4096-aligned address w0 whose 32 bytes lie inside, and how many
-// windows follow it at the stride.
-static void probe_windows_of(uint64_t addr, uint64_t n, uint64_t* w0, uint64_t* nwin) {
-  *w0 = (addr + kProbeStride - 1) & ~(kProbeStride - 1);
-  *nwin = *w0 + kProbeWindow <= addr + n ? (addr + n - kProbeWindow - *w0) / kProbeStride + 1 : 0;
-}
-
 // ------------------------------------------------------------------ probe proof
 // Sets aside the probe cover maps and their host copy, and makes the probe kernels' proving twins resident, the first
-// time a call is both proven and probed (before it maps anything).  The caller holds e->mu.
+// time a call is both proven and probed (before it maps anything).  Apart from the passes' maps: a call that is not
+// probed does not give up their HBM.  The caller holds e->mu.
 static int ensure_probe_cover(ScrubEngine* e) {
   if (e->d_pcover) return CCM_OK;
   CCM_CUDA(cudaSetDevice(e->ordinal));
-  const size_t bytes = kSteps * e->npages * sizeof(uint32_t);
-  if (!e->h_pcover) CCM_CUDA(cudaHostAlloc(&e->h_pcover, bytes, cudaHostAllocDefault));
   CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e->pcover_ctas[0], CCM_COVER_PROBE_FILL, kProbeThreads, 0));
   CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e->pcover_ctas[1], CCM_COVER_PROBE_CHECK, kProbeThreads, 0));
   CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e->pcover_ctas[2], CCM_COVER_PROBE_REREAD, kProbeThreads, 0));
   for (int& c : e->pcover_ctas) c = std::max(c, 1);
-  uint32_t* d = nullptr;
-  CCM_CUDA(cudaMalloc(&d, bytes));
-  const cudaError_t err = cudaMemset(d, 0, bytes);
-  if (err != cudaSuccess) {
-    cudaFree(d);
-    set_error("probe cover map memset failed: %s", cudaGetErrorString(err));
-    return CCM_ERR_CUDA;
-  }
-  e->d_pcover = d;
-  return CCM_OK;
-}
-
-// What every step of the probe must count on each of the np pages: CCM_PROBE_WINDOW bytes per window of `chunks`, on
-// the page its offset (c.offset + (window - c.addr)) starts on.  A window that crosses a page boundary splits its bytes
-// there, as the kernels' cover_lanes does (it cannot on 32-byte-aligned chunk offsets).  Chunks are walked page by page,
-// not window by window: a whole-HBM call has some 20 M windows.
-static std::vector<uint32_t> probe_cover_expected(const std::vector<CheckSpan>& chunks, uint64_t np) {
-  std::vector<uint32_t> exp(np, 0);
-  for (const CheckSpan& c : chunks) {
-    uint64_t w0 = 0, nwin = 0;
-    probe_windows_of(c.addr, c.bytes, &w0, &nwin);
-    if (nwin == 0) continue;
-    const uint64_t o0 = c.offset + (w0 - c.addr);   // offset of the chunk's first window
-    const uint64_t last = o0 + (nwin - 1) * kProbeStride;
-    for (uint64_t p = o0 / kPageBytes; p <= last / kPageBytes && p < np; ++p) {
-      const uint64_t lo = p * kPageBytes, hi = lo + kPageBytes;
-      const uint64_t i0 = lo <= o0 ? 0 : (lo - o0 + kProbeStride - 1) / kProbeStride;
-      const uint64_t i1 = std::min<uint64_t>(nwin, (hi - o0 + kProbeStride - 1) / kProbeStride);
-      if (i1 <= i0) continue;
-      exp[p] += (uint32_t)((i1 - i0) * kProbeWindow);
-      const uint64_t end = o0 + (i1 - 1) * kProbeStride + kProbeWindow;   // the page's last window, past its end?
-      if (end > hi) {
-        exp[p] -= (uint32_t)(end - hi);
-        if (p + 1 < np) exp[p + 1] += (uint32_t)(end - hi);
-      }
-    }
-  }
-  return exp;
+  return alloc_maps(e, kSteps, "probe cover map", &e->d_pcover, &e->h_pcover);
 }
 
 // After the probe of a call both proven and probed (the caller holds e->mu): copies the probe cover maps once, zeroes
-// them for the next call, and compares every step against probe_cover_expected(h.probe_chunks).  Fills *out
-// (proved = 1), e->pcover and e->pcover_pages; each inexact page gets h.chunk_of(page offset).
+// them for the next call, and compares every step against the windows of h.probe_chunks (ccm_proof.h:
+// fill_probe_cover).  Fills *out (proved = 1), e->pcover and e->pcover_pages.
 static int take_probe_cover(ScrubEngine* e, cudaStream_t st, const Held& h, ccm_probe_cover* out) {
-  const std::vector<CheckSpan>& chunks = h.probe_chunks;
   const double t0 = now_ms();
   const size_t bytes = kSteps * e->npages * sizeof(uint32_t);
   CCM_CUDA(cudaMemcpyAsync(e->h_pcover, e->d_pcover, bytes, cudaMemcpyDeviceToHost, st));
   CCM_CUDA(cudaMemsetAsync(e->d_pcover, 0, bytes, st));
   CCM_CUDA(cudaStreamSynchronize(st));
-  e->gate.pcover_dirty = false;
-  const uint64_t np = e->npages - 1;   // pages of a map; word np is its outside slot
-  const std::vector<uint32_t> exp = probe_cover_expected(chunks, np);
-  ccm_probe_cover rep;
-  memset(&rep, 0, sizeof rep);
-  rep.va_base = h.va_base;
-  rep.proved = 1;
-  for (const CheckSpan& c : chunks) {
-    uint64_t w0 = 0, nwin = 0;
-    probe_windows_of(c.addr, c.bytes, &w0, &nwin);
-    rep.windows_expected += nwin;
-  }
-  uint64_t counted[kSteps] = {}, missing[kSteps] = {}, extra[kSteps] = {};   // bytes
-  std::vector<ccm_probe_cover_page> pages;
-  for (uint64_t p = 0; p < np; ++p) {
-    ccm_probe_cover_page cp;
-    memset(&cp, 0, sizeof cp);
-    cp.page = p;
-    cp.expected = exp[p];
-    bool exact = true;
-    for (int k = 0; k < kSteps; ++k) {
-      const uint32_t c = e->h_pcover[k * e->npages + p];
-      ccm_probe_cover_step& ps = rep.step[k];
-      cp.count[k] = c;
-      counted[k] += c;
-      if (c < exp[p]) {
-        if (ps.pages_short++ == 0) ps.first_short_page = p;
-        missing[k] += exp[p] - c;
-      } else if (c > exp[p]) {
-        ps.pages_over++;
-        extra[k] += c - exp[p];
-      }
-      exact &= c == exp[p];
-    }
-    if (!exact) {
-      cp.chunk = h.chunk_of(p * kPageBytes);
-      pages.push_back(cp);
-    }
-  }
-  rep.covered = 1;
-  for (int k = 0; k < kSteps; ++k) {
-    ccm_probe_cover_step& ps = rep.step[k];
-    const uint64_t outside = e->h_pcover[k * e->npages + np];
-    ps.ran = 1;
-    ps.windows_outside = (outside + kProbeWindow - 1) / kProbeWindow;
-    ps.windows_counted = (counted[k] + outside + kProbeWindow - 1) / kProbeWindow;
-    ps.windows_missing = (missing[k] + kProbeWindow - 1) / kProbeWindow;
-    ps.windows_extra = (extra[k] + outside + kProbeWindow - 1) / kProbeWindow;
-    if (missing[k] || extra[k] || outside) rep.covered = 0;
-  }
-  rep.ms_prove = now_ms() - t0;
-  e->pcover = *out = rep;
-  e->pcover_pages.swap(pages);
+  e->gate.touched &= ~kProbeMapsBit;
+  ccm_proof::fill_probe_cover(e->h_pcover, e->npages - 1, h.probe_chunks, h.va_base, h.chunks, &e->pcover,
+                              &e->pcover_pages);
+  e->pcover.ms_prove = now_ms() - t0;
+  *out = e->pcover;
   return CCM_OK;
 }
 
@@ -1504,7 +1311,7 @@ static int run_probe(ScrubEngine* e, cudaStream_t st, const Held& h, uint32_t se
     const uint64_t max_grid = (uint64_t)e->sm_count * (prove ? e->pcover_ctas[k] : e->probe_ctas[k]);
     for (const CheckSpan& c : chunks) {
       uint64_t w0 = 0, nwin = 0;
-      probe_windows_of(c.addr, c.bytes, &w0, &nwin);
+      ccm_proof::probe_windows_of(c.addr, c.bytes, &w0, &nwin);
       if (nwin == 0) continue;
       const uint64_t batches = (nwin + kProbeThreads * kProbePer - 1) / (kProbeThreads * kProbePer);
       const int grid = (int)std::min<uint64_t>(batches, max_grid);
@@ -1529,7 +1336,7 @@ static int run_probe(ScrubEngine* e, cudaStream_t st, const Held& h, uint32_t se
   auto xor_windows = [&](uint64_t k) -> int {
     for (const CheckSpan& c : chunks) {
       uint64_t w0 = 0, nwin = 0;
-      probe_windows_of(c.addr, c.bytes, &w0, &nwin);
+      ccm_proof::probe_windows_of(c.addr, c.bytes, &w0, &nwin);
       for (uint64_t i = 0; i < nwin && k; ++i, --k) {
         xor_byte_kernel<<<1, 1, 0, st>>>((uint8_t*)(uintptr_t)(w0 + i * kProbeStride));
         g_launches++;
@@ -1577,7 +1384,7 @@ static int run_probe(ScrubEngine* e, cudaStream_t st, const Held& h, uint32_t se
   if ((rc = run()) != CCM_OK) { drop_book(e, kCheckBook, st); return rc; }
   for (const CheckSpan& c : chunks) {
     uint64_t w0 = 0, nwin = 0;
-    probe_windows_of(c.addr, c.bytes, &w0, &nwin);
+    ccm_proof::probe_windows_of(c.addr, c.bytes, &w0, &nwin);
     rep->windows += nwin;
   }
   rep->bytes_probed = rep->windows * kProbeWindow;
@@ -1609,7 +1416,7 @@ static int gate_probe(ScrubEngine* e, cudaStream_t st, const Held& h, const Scru
   const uint32_t seed = std::random_device{}();
   const bool prove = e->gate.prove && e->d_pcover;
   const CoverOut maps{e->d_pcover, 0, (uint32_t)(e->npages - 1)};
-  if (prove) e->gate.pcover_dirty = true;
+  if (prove) e->gate.touched |= kProbeMapsBit;
   ccm_mismatch_report mrep;
   int rc = run_probe(e, st, h, seed, drill, prove ? &maps : nullptr, out, &mrep, p3);
   if (rc != CCM_OK) { memset(out, 0, sizeof *out); return rc; }
@@ -1761,7 +1568,7 @@ static void triage_dirt(ScrubEngine* e, cudaStream_t st, const Held& h, const Sc
       locate, locate, kDirtBook, kDirtBook, CCM_REPORT_DIRT_T1};
   const int rc = run_triage(e, st, h.spans, drill, e->pages[kDirtBook], e->dirt.va_base, e->triage_hold_ms, steps,
                             &e->triage, &e->triage_pages);
-  if (e->gate.report_prove)
+  if (e->gate.prove)
     take_report_cover(e, st, h, CCM_REPORT_DIRT_T1, 3, triage_runs(e->pages[kDirtBook], h.spans), rc == CCM_OK);
 }
 
@@ -1786,7 +1593,7 @@ static void triage_mismatch(ScrubEngine* e, cudaStream_t st, const Held& h, cons
       kCheckBook, kDirtBook, CCM_REPORT_MISMATCH_T1};
   const int rc = run_triage(e, st, h.spans, drill, e->pages[kCheckBook], e->mismatch.va_base, e->mtriage_hold_ms, steps,
                             &e->mtriage, &e->mtriage_pages);
-  if (e->gate.report_prove)
+  if (e->gate.prove)
     take_report_cover(e, st, h, CCM_REPORT_MISMATCH_T1, 3, triage_runs(e->pages[kCheckBook], h.spans), rc == CCM_OK);
 }
 
@@ -1801,7 +1608,6 @@ static int finish_gate(ScrubEngine* e, cudaStream_t st, int rc, const Held& h, c
                        ccm_tag_result* tag, ccm_residue_report* res, uint64_t* nonzero, ccm_probe_report* probe,
                        ccm_probe_cover* pcover, ccm_cover_report* cover) {
   e->gate.active = false;   // the probe, the locate pass and the triages are not the call's passes
-  e->gate.report_prove = e->gate.prove;   // take_cover() ends the passes' proof, not the reports'
   if (rc == CCM_OK && probe && *nonzero == 0 && h.bytes) {
     uint64_t p3 = 0;
     rc = gate_probe(e, st, h, drill, probe, pcover, &p3);
@@ -1829,7 +1635,7 @@ static int finish_gate(ScrubEngine* e, cudaStream_t st, int rc, const Held& h, c
     for (const CheckSpan& sp : h.spans)
       if ((lrc = locate_range(e, (const void*)(uintptr_t)sp.addr, sp.bytes, sp.offset, st, &rep, h)) != CCM_OK) break;
     e->gate.report = 0;
-    if (e->gate.report_prove) take_report_cover(e, st, h, CCM_REPORT_LOCATE, 1, h.spans, lrc == CCM_OK);
+    if (e->gate.prove) take_report_cover(e, st, h, CCM_REPORT_LOCATE, 1, h.spans, lrc == CCM_OK);
     if (lrc == CCM_OK) {
       sort_records(&rep, rep.dirty_windows);
       finish_pages(e, kDirtBook, h);

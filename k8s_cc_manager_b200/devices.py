@@ -161,13 +161,19 @@ class PageMap:
 def last_page_map(cuda_ordinal: int, book: int) -> "Optional[PageMap]":
     """The page map behind the last report of `book` (N.BOOK_DIRT / BOOK_MISMATCH / BOOK_RESIDUE) on a CUDA device
     (include/ccm.h: ccm_last_page_map); None when it cannot be read."""
+    entries = _read_pages("ccm_last_page_map", N.PageEntry, cuda_ordinal, book)
+    return PageMap(entries) if entries is not None else None
+
+
+def _read_pages(fn: str, ctype: type, cuda_ordinal: int, *args) -> "Optional[list]":
+    """The entries (`ctype`) the library's page reader `fn`(cuda_ordinal, *args, out, cap, n) gives; None if unread."""
     n = C.c_uint64(0)
-    if cuda_ordinal < 0 or N.lib().ccm_last_page_map(cuda_ordinal, book, None, 0, C.byref(n)) != N.OK:
+    if cuda_ordinal < 0 or getattr(N.lib(), fn)(cuda_ordinal, *args, None, 0, C.byref(n)) != N.OK:
         return None
-    buf = (N.PageEntry * max(1, n.value))()
-    if N.lib().ccm_last_page_map(cuda_ordinal, book, buf, n.value, C.byref(n)) != N.OK:
+    buf = (ctype * max(1, n.value))()
+    if getattr(N.lib(), fn)(cuda_ordinal, *args, buf, n.value, C.byref(n)) != N.OK:
         return None
-    return PageMap(buf[:n.value])
+    return buf[:n.value]
 
 
 class _WindowReport:
@@ -417,14 +423,9 @@ def last_mismatch_triage_pages(cuda_ordinal: int) -> "Optional[List[TriagePage]]
 
 
 def _triage_pages(cuda_ordinal: int, fn: str) -> "Optional[List[TriagePage]]":
-    n = C.c_uint64(0)
-    if cuda_ordinal < 0 or getattr(N.lib(), fn)(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
-        return None
-    buf = (N.TriagePage * max(1, n.value))()
-    if getattr(N.lib(), fn)(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
-        return None
-    return [TriagePage(p.page, p.chunk, N.TRIAGE_CLASSES.get(p.cls, str(p.cls)), p.dirt_bytes, p.t2_bytes, p.t3_bytes)
-            for p in buf[:n.value]]
+    pages = _read_pages(fn, N.TriagePage, cuda_ordinal)
+    return None if pages is None else [TriagePage(p.page, p.chunk, N.TRIAGE_CLASSES.get(p.cls, str(p.cls)),
+                                                  p.dirt_bytes, p.t2_bytes, p.t3_bytes) for p in pages]
 
 
 @dataclass
@@ -521,7 +522,48 @@ def _triage_hold(hold_ms: int) -> int:
     return int(hold_ms)
 
 
-COVER_PAGES = 64   # inexact pages a CoverReport keeps
+COVER_PAGES = 64   # inexact pages a CoverReport, ProbeCoverReport or ReportCoverReport keeps
+
+
+class _ProofReport:
+    """What the three proof reports share: their C struct, their JSON and the inexact pages they keep.  Each report is a
+    dataclass whose fields are those of its C struct, then its rows (ROWS, the struct's array of the same name: a ROW
+    per name of NAMES), `pages` (a list of PAGE) and `pages_truncated`."""
+    ROWS: str
+    ROW: type
+    NAMES: Tuple[str, ...]
+    PAGE: type
+
+    @classmethod
+    def from_native(cls, r, pages=None):
+        """The report of the C struct `r`, with the first COVER_PAGES of its inexact pages `pages`."""
+        rows = [cls.ROW(name=name, **{f: getattr(row, f) for f, _ in row._fields_ if f != "reserved"})
+                for name, row in zip(cls.NAMES, getattr(r, cls.ROWS))]
+        pages = pages or []
+        return cls(**{f.name: getattr(r, f.name) for f in dataclasses.fields(cls)[:-3]}, **{cls.ROWS: rows},
+                   pages=pages[:COVER_PAGES], pages_truncated=int(len(pages) > COVER_PAGES))
+
+    @classmethod
+    def _last(cls, cuda_ordinal: int, getter: str, native: type, read_pages):
+        """As _last_report, with the inexact pages (read_pages) of a report that proved and was not covered."""
+        out = native()
+        if cuda_ordinal < 0 or getattr(N.lib(), getter)(cuda_ordinal, C.byref(out)) != N.OK:
+            return None
+        return cls.from_native(out, read_pages(cuda_ordinal) if out.proved and not out.covered else None)
+
+    @classmethod
+    def from_json(cls, d: dict):
+        return cls(**{**d, cls.ROWS: [cls.ROW(**r) for r in d[cls.ROWS]], "pages": [cls.PAGE(**p) for p in d["pages"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    def _with_pages(self, line: str, first: int) -> str:
+        """`line`, then the first `first` inexact pages kept, and "(+more)" when there are others."""
+        if not self.pages:
+            return line
+        more = " (+more)" if self.pages_truncated or len(self.pages) > first else ""
+        return line + "; " + "; ".join(p.describe() for p in self.pages[:first]) + more
 
 
 @dataclass
@@ -554,7 +596,7 @@ class CoverPass:
 
 
 @dataclass
-class CoverReport:
+class CoverReport(_ProofReport):
     """The coverage proof of one product call (include/ccm.h: ccm_cover_report): every pass counted on the device the
     bytes its kernels processed on each 2 MiB page, and `covered` says each pass that ran walked every mapped byte
     exactly once.  `pages` are the first COVER_PAGES inexact pages."""
@@ -567,22 +609,7 @@ class CoverReport:
     passes: List[CoverPass] = field(default_factory=list)
     pages: List[CoverPage] = field(default_factory=list)
     pages_truncated: int = 0
-
-    @classmethod
-    def from_native(cls, r: N.CoverReport, pages: "Optional[List[CoverPage]]" = None) -> "CoverReport":
-        passes = [CoverPass(name, *(getattr(r.passes[k], f) for f, _ in N.CoverPass._fields_ if f != "reserved"))
-                  for k, name in enumerate(N.COVER_PASSES)]
-        pages = pages or []
-        return cls(r.bytes_mapped, r.pages_mapped, r.va_base, r.ms_prove, r.proved, r.covered, passes,
-                   pages[:COVER_PAGES], int(len(pages) > COVER_PAGES))
-
-    @classmethod
-    def from_json(cls, d: dict) -> "CoverReport":
-        return cls(**{**d, "passes": [CoverPass(**p) for p in d["passes"]],
-                      "pages": [CoverPage(**p) for p in d["pages"]]})
-
-    def as_json(self) -> dict:
-        return dataclasses.asdict(self)
+    ROWS, ROW, NAMES, PAGE = "passes", CoverPass, N.COVER_PASSES, CoverPage
 
     def short_pass(self) -> "Optional[CoverPass]":
         """The first pass that ran and did not count every page exactly (None when covered)."""
@@ -596,31 +623,20 @@ class CoverReport:
             return line + ": every pass covered every byte once (" + ", ".join(p.name for p in self.passes if p.ran) + ")"
         line += (f": the {bad.name} pass counted {bad.bytes_counted} bytes ({bad.bytes_missing} missing, "
                  f"{bad.bytes_extra} extra) with {bad.pages_short} pages short")
-        if self.pages:
-            more = " (+more)" if self.pages_truncated or len(self.pages) > first else ""
-            line += "; " + "; ".join(p.describe() for p in self.pages[:first]) + more
-        return line
+        return self._with_pages(line, first)
 
 
 def last_cover_pages(cuda_ordinal: int) -> "Optional[List[CoverPage]]":
     """The inexact pages of the last proving call on a CUDA device (include/ccm.h: ccm_last_cover_pages), ascending;
     None when they cannot be read."""
-    n = C.c_uint64(0)
-    if cuda_ordinal < 0 or N.lib().ccm_last_cover_pages(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
-        return None
-    buf = (N.CoverPage * max(1, n.value))()
-    if N.lib().ccm_last_cover_pages(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
-        return None
-    return [CoverPage(p.page, p.chunk, p.expected, *p.count) for p in buf[:n.value]]
+    pages = _read_pages("ccm_last_cover_pages", N.CoverPage, cuda_ordinal)
+    return None if pages is None else [CoverPage(p.page, p.chunk, p.expected, *p.count) for p in pages]
 
 
 def last_cover(cuda_ordinal: int) -> "Optional[CoverReport]":
     """The coverage report of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_cover), with its
     first inexact pages; None when it cannot be read."""
-    out = N.CoverReport()
-    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_cover(cuda_ordinal, C.byref(out)) != N.OK:
-        return None
-    return CoverReport.from_native(out, last_cover_pages(cuda_ordinal) if out.proved and not out.covered else None)
+    return CoverReport._last(cuda_ordinal, "ccm_scrub_last_cover", N.CoverReport, last_cover_pages)
 
 
 def _arm_prove(cuda_ordinal: int, on: bool) -> int:
@@ -720,7 +736,7 @@ class ProbeCoverStep:
 
 
 @dataclass
-class ProbeCoverReport:
+class ProbeCoverReport(_ProofReport):
     """The probe proof of one product call both proven and probed (include/ccm.h: ccm_probe_cover): every probe step
     counted on the device the windows it took on each 2 MiB page, and `covered` says each took every probe window of
     the call exactly once.  `pages` are the first COVER_PAGES inexact pages."""
@@ -732,23 +748,7 @@ class ProbeCoverReport:
     steps: List[ProbeCoverStep] = field(default_factory=list)
     pages: List[ProbeCoverPage] = field(default_factory=list)
     pages_truncated: int = 0
-
-    @classmethod
-    def from_native(cls, r: N.ProbeCover, pages: "Optional[List[ProbeCoverPage]]" = None) -> "ProbeCoverReport":
-        steps = [ProbeCoverStep(name=name, **{f: getattr(r.steps[k], f) for f, _ in N.ProbeCoverStep._fields_
-                                              if f != "reserved"})
-                 for k, name in enumerate(N.PROBE_STEPS)]
-        pages = pages or []
-        return cls(r.windows_expected, r.va_base, r.ms_prove, r.proved, r.covered, steps, pages[:COVER_PAGES],
-                   int(len(pages) > COVER_PAGES))
-
-    @classmethod
-    def from_json(cls, d: dict) -> "ProbeCoverReport":
-        return cls(**{**d, "steps": [ProbeCoverStep(**p) for p in d["steps"]],
-                      "pages": [ProbeCoverPage(**p) for p in d["pages"]]})
-
-    def as_json(self) -> dict:
-        return dataclasses.asdict(self)
+    ROWS, ROW, NAMES, PAGE = "steps", ProbeCoverStep, N.PROBE_STEPS, ProbeCoverPage
 
     def short_step(self) -> "Optional[ProbeCoverStep]":
         """The first step that did not count every page exactly (None when covered)."""
@@ -763,32 +763,20 @@ class ProbeCoverReport:
         line += (f": step {bad.name} counted {bad.windows_counted} windows ({bad.windows_missing} missing, "
                  f"{bad.windows_extra} extra) with {bad.pages_short} pages short, first short page "
                  f"{bad.first_short_page}")
-        if self.pages:
-            more = " (+more)" if self.pages_truncated or len(self.pages) > first else ""
-            line += "; " + "; ".join(p.describe() for p in self.pages[:first]) + more
-        return line
+        return self._with_pages(line, first)
 
 
 def last_probe_cover_pages(cuda_ordinal: int) -> "Optional[List[ProbeCoverPage]]":
     """The inexact pages of the last proven probe on a CUDA device (include/ccm.h: ccm_last_probe_cover_pages),
     ascending; None when they cannot be read."""
-    n = C.c_uint64(0)
-    if cuda_ordinal < 0 or N.lib().ccm_last_probe_cover_pages(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
-        return None
-    buf = (N.ProbeCoverPage * max(1, n.value))()
-    if N.lib().ccm_last_probe_cover_pages(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
-        return None
-    return [ProbeCoverPage(p.page, p.chunk, p.expected, *p.count) for p in buf[:n.value]]
+    pages = _read_pages("ccm_last_probe_cover_pages", N.ProbeCoverPage, cuda_ordinal)
+    return None if pages is None else [ProbeCoverPage(p.page, p.chunk, p.expected, *p.count) for p in pages]
 
 
 def last_probe_cover(cuda_ordinal: int) -> "Optional[ProbeCoverReport]":
     """The probe proof of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_probe_cover), with
     its first inexact pages; None when it cannot be read."""
-    out = N.ProbeCover()
-    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_probe_cover(cuda_ordinal, C.byref(out)) != N.OK:
-        return None
-    return ProbeCoverReport.from_native(out, last_probe_cover_pages(cuda_ordinal)
-                                        if out.proved and not out.covered else None)
+    return ProbeCoverReport._last(cuda_ordinal, "ccm_scrub_last_probe_cover", N.ProbeCover, last_probe_cover_pages)
 
 
 def _attach_probe(rep: "ScrubReport", cuda_ordinal: int, prove: bool = False) -> bool:
@@ -848,7 +836,7 @@ REPORT_STEP_OF = {"LOCATE": "dirt", "DIRT_T1": "triage", "DIRT_T2": "triage", "D
 
 
 @dataclass
-class ReportCoverReport:
+class ReportCoverReport(_ProofReport):
     """The report proof of one proven product call that failed (include/ccm.h: ccm_report_cover): its locate pass and
     every triage step it ran counted on the device the bytes they walked on each 2 MiB page, and `covered` says each
     walked every byte of its reports exactly once.  It never changes the call's verdict: a short step says only which
@@ -861,22 +849,7 @@ class ReportCoverReport:
     steps: List[ReportCoverStep] = field(default_factory=list)
     pages: List[ReportCoverPage] = field(default_factory=list)
     pages_truncated: int = 0
-
-    @classmethod
-    def from_native(cls, r: N.ReportCover, pages: "Optional[List[ReportCoverPage]]" = None) -> "ReportCoverReport":
-        steps = [ReportCoverStep(name=name, **{f: getattr(r.steps[k], f) for f, _ in N.ReportCoverStep._fields_
-                                               if f != "reserved"})
-                 for k, name in enumerate(N.REPORT_STEPS)]
-        pages = pages or []
-        return cls(r.va_base, r.ms_prove, r.proved, r.covered, steps, pages[:COVER_PAGES], int(len(pages) > COVER_PAGES))
-
-    @classmethod
-    def from_json(cls, d: dict) -> "ReportCoverReport":
-        return cls(**{**d, "steps": [ReportCoverStep(**p) for p in d["steps"]],
-                      "pages": [ReportCoverPage(**p) for p in d["pages"]]})
-
-    def as_json(self) -> dict:
-        return dataclasses.asdict(self)
+    ROWS, ROW, NAMES, PAGE = "steps", ReportCoverStep, N.REPORT_STEPS, ReportCoverPage
 
     def short_steps(self) -> "List[ReportCoverStep]":
         """The steps that ran and did not count every page exactly."""
@@ -896,32 +869,21 @@ class ReportCoverReport:
         line = "; ".join(f"step {p.name} counted {p.bytes_counted} of {p.bytes_expected} bytes ({p.bytes_missing} "
                          f"missing, {p.bytes_extra} extra) with {p.pages_short} pages short, first short page "
                          f"{p.first_short_page}" for p in bad)
-        if self.pages:
-            more = " (+more)" if self.pages_truncated or len(self.pages) > first else ""
-            line += "; " + "; ".join(p.describe() for p in self.pages[:first]) + more
-        return line
+        return self._with_pages(line, first)
 
 
 def last_report_cover_pages(cuda_ordinal: int) -> "Optional[List[ReportCoverPage]]":
     """The inexact (step, page) entries of the last proven locate pass and triages on a CUDA device (include/ccm.h:
     ccm_last_report_cover_pages), by step then page; None when they cannot be read."""
-    n = C.c_uint64(0)
-    if cuda_ordinal < 0 or N.lib().ccm_last_report_cover_pages(cuda_ordinal, None, 0, C.byref(n)) != N.OK:
-        return None
-    buf = (N.ReportCoverPage * max(1, n.value))()
-    if N.lib().ccm_last_report_cover_pages(cuda_ordinal, buf, n.value, C.byref(n)) != N.OK:
-        return None
-    return [ReportCoverPage(p.page, p.chunk, N.REPORT_STEPS[p.step - 1], p.expected, p.counted) for p in buf[:n.value]]
+    pages = _read_pages("ccm_last_report_cover_pages", N.ReportCoverPage, cuda_ordinal)
+    return None if pages is None else [ReportCoverPage(p.page, p.chunk, N.REPORT_STEPS[p.step - 1], p.expected,
+                                                       p.counted) for p in pages]
 
 
 def last_report_cover(cuda_ordinal: int) -> "Optional[ReportCoverReport]":
     """The report proof of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_report_cover), with
     its first inexact pages; None when it cannot be read."""
-    out = N.ReportCover()
-    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_report_cover(cuda_ordinal, C.byref(out)) != N.OK:
-        return None
-    return ReportCoverReport.from_native(out, last_report_cover_pages(cuda_ordinal)
-                                         if out.proved and not out.covered else None)
+    return ReportCoverReport._last(cuda_ordinal, "ccm_scrub_last_report_cover", N.ReportCover, last_report_cover_pages)
 
 
 def _attach_report_cover(rep: "ScrubReport", cuda_ordinal: int) -> None:
