@@ -1830,77 +1830,145 @@ static cudaError_t residue_drill(uint8_t* p, uint64_t n, uint64_t* budget, cudaS
   return err == cudaSuccess ? inject_dirt(p, n, budget, st) : err;
 }
 
-// Fault drills on the segments of the arena the product call's fallback path holds: every segment is
-// filled with `fill` (0 = no fill), then (residue != 0) drilled with "scrub_residue", then up to `inject` bytes are
-// dirtied, 4 candidates per segment.
-static int arena_drill(ScrubEngine* e, int fill, uint64_t inject, uint64_t residue = 0) {
-  if (!fill && !inject && !residue) return CCM_OK;
-  std::lock_guard<std::mutex> g(e->mu);
-  CCM_ENSURE_READY(e);
-  int rc = need_arena(e); if (rc) return rc;
-  CCM_CUDA(cudaSetDevice(e->ordinal));
-  const bool drill_residue = residue != 0;
-  for (auto& s : e->segs) {
-    if (fill) CCM_CUDA(cudaMemsetAsync(s.ptr, fill, s.bytes, e->stream));
-    if (drill_residue) CCM_CUDA(residue_drill(s.ptr, s.bytes, &residue, e->stream));
-    if (inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &inject, e->stream));
-  }
-  return CCM_OK;
+static int drill_failed(cudaError_t err) {
+  if (err == cudaSuccess) return CCM_OK;
+  set_error("scrub drill failed: %s", cudaGetErrorString(err));
+  return CCM_ERR_CUDA;
 }
 
-// The zero gate's first pass on the fallback path, with the census: one census launch per segment (`spans`, offsets
-// into the concatenated segments), timed as the scrub (*ms).
-static int arena_census(ScrubEngine* e, const std::vector<CheckSpan>& spans, float* ms) {
-  std::lock_guard<std::mutex> g(e->mu);
-  CCM_ENSURE_READY(e);
-  int rc = need_arena(e); if (rc) return rc;
-  CCM_CUDA(cudaSetDevice(e->ordinal));
-  cudaStream_t st = e->stream;
-  return run_timed(e, st, ms, [&]() -> int {
-    for (const CheckSpan& sp : spans)
-      if (int rc2 = census_range(e, (void*)(uintptr_t)sp.addr, sp.bytes, false, 0, st, sp.addr - sp.offset)) return rc2;
+// The passes and fault drills of one product call, in the order both its paths enqueue them on `st` (DESIGN.md §5a).
+// The caller holds e->mu from begin() to end() and calls held() and enqueue() as often as it likes in between: the VMM
+// path with one span at a time (each mapping, each range), the fallback once with every segment.  Each step runs each
+// of its phases over all its spans before the next phase, and the kernels get the base sp.addr - sp.offset.
+struct GateRun {
+  ScrubEngine* e;
+  cudaStream_t st;
+  const ScrubDrill& drill;
+  ccm_tag_result* tag;        // the tagged call's tag block, or nullptr
+  ccm_residue_report* res;    // the census call's report, or nullptr
+  bool interleave;            // enqueue() reads its spans back; otherwise end() reads back everything
+  uint64_t inject = drill.inject, tag_inject = drill.tag_inject;   // budgets, spent in enqueue order
+  uint64_t residue = drill.residue;                                 // budget, spent in held() order
+  int timed = 0, tag_timed = 0;   // pipe_ev and tag_ev brackets recorded (the first kMaxPipeChunks of each)
+
+  // Zeroes the counts and starts the call's span (ev[0]).
+  int begin() {
+    CCM_CUDA(cudaMemsetAsync(e->d_counter + kNonzero, 0, sizeof(unsigned long long), st));
+    if (tag) CCM_CUDA(cudaMemsetAsync(e->d_counter + kMismatch, 0, sizeof(unsigned long long), st));
+    cudaEventRecord(e->ev[0], st);
     return CCM_OK;
-  });
-}
+  }
 
-// Tagged pass of the product call's fallback path: tag every segment (`spans`), then (after the "tag_flood" and
-// "tag_inject" drills) check and zero every segment.  Fills tag->mismatch_bytes, ->ms_tag, ->ms_check and ->va_base.
-// census (census call): the fills are census fills.
-static int arena_tag_check(ScrubEngine* e, const std::vector<CheckSpan>& spans, ccm_tag_result* tag,
-                           uint64_t tag_inject, int tag_flood, bool census) {
-  std::lock_guard<std::mutex> g(e->mu);
-  CCM_ENSURE_READY(e);
-  int rc = need_arena(e); if (rc) return rc;
-  CCM_CUDA(cudaSetDevice(e->ordinal));
-  cudaStream_t st = e->stream;
-  // fills between ev[0] and ev[2], the drill, checks between ev[3] and ev[1]
-  rc = run_counted(e, st, kMismatch, &tag->mismatch_bytes, nullptr, [&]() -> int {
+  // Memory the call has just come to hold: the previous tenant's data ("scrub_poison") and a known residue
+  // ("scrub_residue") in place before anything scrubs it; then, in a tagged call, its tags (or the census with tags).
+  int held(const std::vector<CheckSpan>& spans) {
+    for (const CheckSpan& sp : spans) {
+      uint8_t* p = (uint8_t*)(uintptr_t)sp.addr;
+      cudaError_t err = drill.poison ? cudaMemsetAsync(p, drill.poison, sp.bytes, st) : cudaSuccess;
+      if (err == cudaSuccess && drill.residue) err = residue_drill(p, sp.bytes, &residue, st);
+      if (int rc = drill_failed(err)) return rc;
+    }
+    if (!tag) return CCM_OK;
+    cudaEvent_t* evs = tag_timed < kMaxPipeChunks ? e->tag_ev[tag_timed] : nullptr;
+    if (evs) cudaEventRecord(evs[0], st);
+    int rc = CCM_OK;
     for (const CheckSpan& sp : spans) {
       void* p = (void*)(uintptr_t)sp.addr;
-      if (int rc2 = census ? census_range(e, p, sp.bytes, true, tag->seed, st, sp.addr - sp.offset)
-                           : tag_fill_range(e, p, sp.bytes, tag->seed, st))
-        return rc2;
+      rc = res ? census_range(e, p, sp.bytes, true, tag->seed, st, sp.addr - sp.offset)
+               : tag_fill_range(e, p, sp.bytes, tag->seed, st);
+      if (rc != CCM_OK) break;
     }
-    CCM_CUDA(cudaEventRecord(e->ev[2], st));
-    for (auto& s : e->segs) {
-      if (tag_flood) CCM_CUDA(cudaMemsetAsync(s.ptr, tag_flood, s.bytes, st));
-      if (tag_inject) CCM_CUDA(inject_dirt(s.ptr, s.bytes, &tag_inject, st, true));
+    if (evs) { cudaEventRecord(evs[1], st); ++tag_timed; }
+    return rc;
+  }
+
+  // The scrub of `spans` (in a tagged call the check-and-zero, in a census call the census) inside one pipe_ev
+  // bracket, then the dirt its read-back MUST find, then (interleave) the read-back.  A tagged call's own drills act
+  // between its tags and its check.
+  int enqueue(const std::vector<CheckSpan>& spans) {
+    if (tag && (drill.tag_flood || tag_inject))
+      for (const CheckSpan& sp : spans) {
+        uint8_t* p = (uint8_t*)(uintptr_t)sp.addr;
+        cudaError_t err = drill.tag_flood ? cudaMemsetAsync(p, drill.tag_flood, sp.bytes, st) : cudaSuccess;
+        if (err == cudaSuccess && tag_inject) err = inject_dirt(p, sp.bytes, &tag_inject, st, true);
+        if (int rc = drill_failed(err)) return rc;
+      }
+    cudaEvent_t* evs = timed < kMaxPipeChunks ? e->pipe_ev[timed] : nullptr;
+    if (evs) cudaEventRecord(evs[0], st);
+    int rc = CCM_OK;
+    for (const CheckSpan& sp : spans) {
+      void* p = (void*)(uintptr_t)sp.addr;
+      rc = tag ? tag_check_range(e, p, sp.bytes, tag->seed, st, sp.addr - sp.offset)
+         : res ? census_range(e, p, sp.bytes, false, 0, st, sp.addr - sp.offset)
+               : scrub_range(e, p, sp.bytes, CCM_SCRUB_AUTO, nullptr, st);
+      if (rc != CCM_OK) break;
     }
-    CCM_CUDA(cudaEventRecord(e->ev[3], st));
-    // base = segment address - its offset: the offsets continue from one segment into the next
-    for (const CheckSpan& sp : spans)
-      if (int rc2 = tag_check_range(e, (void*)(uintptr_t)sp.addr, sp.bytes, tag->seed, st, sp.addr - sp.offset)) return rc2;
+    if (evs) cudaEventRecord(evs[1], st);
+    for (const CheckSpan& sp : spans) {
+      if (rc != CCM_OK) break;
+      uint8_t* p = (uint8_t*)(uintptr_t)sp.addr;
+      cudaError_t err = drill.flood ? cudaMemsetAsync(p, drill.flood, sp.bytes, st) : cudaSuccess;
+      if (err == cudaSuccess && inject) err = inject_dirt(p, sp.bytes, &inject, st);
+      rc = drill_failed(err);
+    }
+    if (interleave)
+      for (const CheckSpan& sp : spans)
+        if (rc == CCM_OK) rc = verify_range(e, (const void*)(uintptr_t)sp.addr, sp.bytes, CCM_VERIFY_AUTO, nullptr, st);
+    if (evs) { cudaEventRecord(evs[2], st); ++timed; }
+    return rc;
+  }
+
+  // After the passes enqueued so far (`rc`: how they ended): the read-back of everything the call holds (`spans`)
+  // unless enqueue() interleaved it, the counts to the host and one wait for the stream, whatever `rc` is, so that
+  // nothing touches the memory once this returns.  A call whose passes all ran gets its counts and kernel times into
+  // *r and the tag block.
+  int end(const std::vector<CheckSpan>& spans, int rc, ccm_scrub_result* r) {
+    if (rc == CCM_OK && !interleave) {
+      cudaEventRecord(e->ev[1], st);
+      for (const CheckSpan& sp : spans)
+        if (rc == CCM_OK) rc = verify_range(e, (const void*)(uintptr_t)sp.addr, sp.bytes, CCM_VERIFY_AUTO, nullptr, st);
+    }
+    cudaEventRecord(e->ev[2], st);
+    if (rc == CCM_OK &&
+        cudaMemcpyAsync(e->h_counter, e->d_counter + kNonzero, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                        st) != cudaSuccess)
+      rc = CCM_ERR_CUDA;
+    if (rc == CCM_OK && tag &&
+        cudaMemcpyAsync(e->h_counter + 1, e->d_counter + kMismatch, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                        st) != cudaSuccess)
+      rc = CCM_ERR_CUDA;
+    const cudaError_t serr = cudaStreamSynchronize(st);
+    if (rc == CCM_OK && serr != cudaSuccess) { set_error("stream sync failed: %s", cudaGetErrorString(serr)); rc = CCM_ERR_CUDA; }
+    if (rc != CCM_OK) return rc;
+    float span = 0, ms_s = 0, ms_v = 0;
+    cudaEventElapsedTime(&span, e->ev[0], e->ev[2]);
+    for (int i = 0; i < timed; ++i) {
+      float a = 0, b = 0;
+      cudaEventElapsedTime(&a, e->pipe_ev[i][0], e->pipe_ev[i][1]);
+      cudaEventElapsedTime(&b, e->pipe_ev[i][1], e->pipe_ev[i][2]);
+      ms_s += a;
+      ms_v += b;
+    }
+    if (!interleave) cudaEventElapsedTime(&ms_v, e->ev[1], e->ev[2]);
+    r->ms_scrub = ms_s;
+    r->ms_verify = ms_v;
+    r->ms_gpu_span = span;
+    r->nonzero_bytes = (uint64_t)*e->h_counter;
+    if (tag) {
+      float ms_t = 0;
+      for (int i = 0; i < tag_timed; ++i) {
+        float a = 0;
+        cudaEventElapsedTime(&a, e->tag_ev[i][0], e->tag_ev[i][1]);
+        ms_t += a;
+      }
+      tag->mismatch_bytes = (uint64_t)e->h_counter[1];
+      tag->ms_tag = ms_t;
+      tag->ms_check = ms_s;
+      tag->va_base = spans.empty() || spans.front().bytes == 0 ? 0 : spans.front().addr - spans.front().offset;
+    }
     return CCM_OK;
-  });
-  if (rc) return rc;
-  float a = 0, b = 0;
-  CCM_CUDA(cudaEventElapsedTime(&a, e->ev[0], e->ev[2]));
-  CCM_CUDA(cudaEventElapsedTime(&b, e->ev[3], e->ev[1]));
-  tag->ms_tag = a;
-  tag->ms_check = b;
-  tag->va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
-  return CCM_OK;
-}
+  }
+};
 
 // ------------------------------------------------------- VMM (driver API, lazy)
 // The product call maps HBM in chunks through the virtual-memory-management API so
@@ -2025,58 +2093,17 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
   memset(&acc, 0, sizeof acc);
   acc.location = prop.location;
   acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-  int rc = CCM_OK;
   double host_acquire = 0;
-  int timed = 0;  // chunks with an event triple (the first kMaxPipeChunks; a badly fragmented HBM may produce more)
-  uint64_t inject = drill.inject;  // one budget for all enqueued ranges, spent in enqueue order
   // Tagged gate: every mapping is tagged as soon as it is mapped, and the ranges are checked only after
   // the LAST mapping — a view that aliases an earlier chunk has overwritten that chunk's tags by then.
   ccm_tag_result* tag = current_tag_call();
-  uint64_t tag_inject = drill.tag_inject;
-  int tag_timed = 0;
-  std::vector<std::pair<uint64_t, uint64_t>> deferred;  // tagged: main-zone ranges, checked after the last mapping
+  std::vector<CheckSpan> deferred;                      // tagged: main-zone ranges, checked after the last mapping
   std::vector<std::pair<uint64_t, uint32_t>> pieces;    // (offset, handle index) of every mapped piece, ascending
   std::vector<CheckSpan> iters;                         // every iteration of the mapping loop, for the alias probe
-  // Census call: the first pass over each mapping (the scrub, or the tag fill) is the census of the same range.
-  ccm_residue_report* res = current_residue_call();
-  uint64_t residue = drill.residue;                     // "scrub_residue" budget, spent in mapping order
-  auto tag_fill = [&](uint64_t off, uint64_t n) -> int {
-    cudaEvent_t* evs = tag_timed < kMaxPipeChunks ? e->tag_ev[tag_timed] : nullptr;
-    if (evs) cudaEventRecord(evs[0], st);
-    const int rc2 = res ? census_range(e, (void*)(m.base + off), n, true, tag->seed, st, (uint64_t)m.base)
-                        : tag_fill_range(e, (void*)(m.base + off), n, tag->seed, st);
-    if (evs) { cudaEventRecord(evs[1], st); ++tag_timed; }
-    return rc2;
-  };
-
-  // enqueue scrub (+ read-back) of [off, off+n) with CUDA events around each kernel; in the tagged gate the
-  // scrub is the check-and-zero pass
-  auto enqueue = [&](uint64_t off, uint64_t n) -> int {
-    if (tag && (drill.tag_flood || tag_inject)) {
-      cudaError_t ierr = drill.tag_flood ? cudaMemsetAsync((void*)(m.base + off), drill.tag_flood, n, st) : cudaSuccess;
-      if (ierr == cudaSuccess && tag_inject) ierr = inject_dirt((uint8_t*)(m.base + off), n, &tag_inject, st, true);
-      if (ierr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(ierr)); return CCM_ERR_CUDA; }
-    }
-    cudaEvent_t* evs = timed < kMaxPipeChunks ? e->pipe_ev[timed] : nullptr;
-    if (evs) cudaEventRecord(evs[0], st);
-    int rc2 = tag ? tag_check_range(e, (void*)(m.base + off), n, tag->seed, st, (uint64_t)m.base)
-            : res ? census_range(e, (void*)(m.base + off), n, false, 0, st, (uint64_t)m.base)
-                  : scrub_range(e, (void*)(m.base + off), n, CCM_SCRUB_AUTO, nullptr, st);
-    if (evs) cudaEventRecord(evs[1], st);
-    // fault drills: dirt the read-back of this range MUST find
-    cudaError_t derr = cudaSuccess;
-    if (rc2 == CCM_OK && drill.flood) derr = cudaMemsetAsync((void*)(m.base + off), drill.flood, n, st);
-    if (rc2 == CCM_OK && derr == cudaSuccess && inject) derr = inject_dirt((uint8_t*)(m.base + off), n, &inject, st);
-    if (derr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(derr)); rc2 = CCM_ERR_CUDA; }
-    if (rc2 == CCM_OK && interleave) rc2 = verify_range(e, (const void*)(m.base + off), n, CCM_VERIFY_AUTO, nullptr, st);
-    if (evs) { cudaEventRecord(evs[2], st); ++timed; }
-    return rc2;
-  };
-
-  if (cudaMemsetAsync(e->d_counter, 0, sizeof(unsigned long long), st) != cudaSuccess) rc = CCM_ERR_CUDA;
-  if (tag && cudaMemsetAsync(e->d_counter + kMismatch, 0, sizeof(unsigned long long), st) != cudaSuccess) rc = CCM_ERR_CUDA;
+  GateRun run{e, st, drill, tag, current_residue_call(), interleave};
+  auto range = [&](uint64_t off, uint64_t n) { return std::vector<CheckSpan>{{(uint64_t)m.base + off, n, off}}; };
+  int rc = run.begin();
   bool aliased = false;  // "scrub_alias" drill done
-  cudaEventRecord(e->ev[0], st);
   uint64_t off = 0, tail_start = 0;
   bool in_tail = false;
   while (off < va_bytes && rc == CCM_OK) {
@@ -2122,79 +2149,30 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     aliased |= alias != 0;
     m.mapped = off + n;
     iters.push_back({(uint64_t)m.base + off, n, off});
-    // fault drill: the previous tenant's data, in place before anything scrubs this chunk
-    if (drill.poison) {
-      cudaError_t perr = cudaMemsetAsync((void*)(m.base + off), drill.poison, n, st);
-      if (perr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(perr)); rc = CCM_ERR_CUDA; break; }
-    }
-    if (drill.residue) {   // fault drill: a known residue, whatever the driver handed back
-      cudaError_t rerr = residue_drill((uint8_t*)(m.base + off), n, &residue, st);
-      if (rerr != cudaSuccess) { set_error("scrub drill failed: %s", cudaGetErrorString(rerr)); rc = CCM_ERR_CUDA; break; }
-    }
-    if (tag) rc = tag_fill(off, n);
+    rc = run.held(range(off, n));
     // tail-zone granules are scrubbed with ONE launch pair once the zone is mapped
     if (rc == CCM_OK && !in_tail && !map_first) {
-      if (tag) deferred.emplace_back(off, n);
-      else rc = enqueue(off, n);
+      if (tag) deferred.push_back(iters.back());
+      else rc = run.enqueue(range(off, n));
     }
     off += n;
     if (!in_tail && chunk < max_chunk) { chunk *= 2; if (chunk > max_chunk) chunk = max_chunk; }
   }
-  for (const auto& d : deferred) if (rc == CCM_OK) rc = enqueue(d.first, d.second);
-  if (rc == CCM_OK && map_first) { if (m.mapped) rc = enqueue(0, m.mapped); }
-  else if (rc == CCM_OK && in_tail && m.mapped > tail_start) rc = enqueue(tail_start, m.mapped - tail_start);
-  if (rc == CCM_OK && !interleave) {
-    cudaEventRecord(e->ev[1], st);
-    rc = verify_range(e, (const void*)m.base, m.mapped, CCM_VERIFY_AUTO, nullptr, st);
-  }
-  cudaEventRecord(e->ev[2], st);
-  if (rc == CCM_OK &&
-      cudaMemcpyAsync(e->h_counter, e->d_counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st) != cudaSuccess)
-    rc = CCM_ERR_CUDA;
-  if (rc == CCM_OK && tag &&
-      cudaMemcpyAsync(e->h_counter + 1, e->d_counter + kMismatch, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
-                      st) != cudaSuccess)
-    rc = CCM_ERR_CUDA;
-  cudaError_t serr = cudaStreamSynchronize(st);  // nothing may still touch the mapping below
-  if (rc == CCM_OK && serr != cudaSuccess) { set_error("stream sync failed: %s", cudaGetErrorString(serr)); rc = CCM_ERR_CUDA; }
+  for (const CheckSpan& d : deferred) if (rc == CCM_OK) rc = run.enqueue({d});
+  if (rc == CCM_OK && map_first) { if (m.mapped) rc = run.enqueue(range(0, m.mapped)); }
+  else if (rc == CCM_OK && in_tail && m.mapped > tail_start) rc = run.enqueue(range(tail_start, m.mapped - tail_start));
 
+  // ---- the reports, before the mapping goes back: an alias piece maps to handle 0 ----------------------------
   const uint64_t mapped = m.mapped;
-  const int nchunks = (int)m.handles.size();
+  const Held h{(uint64_t)m.base, mapped, range(0, mapped), std::move(iters), std::move(pieces)};
+  rc = run.end(h.spans, rc, r);
   if (rc == CCM_OK) {
-    float span = 0, ms_s = 0, ms_v = 0;
-    cudaEventElapsedTime(&span, e->ev[0], e->ev[2]);
-    for (int i = 0; i < timed; ++i) {
-      float a = 0, b = 0;
-      cudaEventElapsedTime(&a, e->pipe_ev[i][0], e->pipe_ev[i][1]);
-      cudaEventElapsedTime(&b, e->pipe_ev[i][1], e->pipe_ev[i][2]);
-      ms_s += a;
-      ms_v += b;
-    }
-    if (!interleave) cudaEventElapsedTime(&ms_v, e->ev[1], e->ev[2]);
     r->bytes_scrubbed = mapped;
     r->bytes_unreached = want_max && (uint64_t)fr > mapped ? (uint64_t)fr - mapped : 0;
-    r->segments = nchunks;
+    r->segments = (int)m.handles.size();
     r->ms_acquire = host_acquire;
-    r->ms_scrub = ms_s;
-    r->ms_verify = ms_v;
-    r->ms_gpu_span = span;
-    r->nonzero_bytes = (uint64_t)*e->h_counter;
-    if (tag) {
-      float ms_t = 0;
-      for (int i = 0; i < tag_timed; ++i) {
-        float a = 0;
-        cudaEventElapsedTime(&a, e->tag_ev[i][0], e->tag_ev[i][1]);
-        ms_t += a;
-      }
-      tag->mismatch_bytes = (uint64_t)e->h_counter[1];
-      tag->ms_tag = ms_t;
-      tag->ms_check = ms_s;
-      tag->va_base = mapped ? (uint64_t)m.base : 0;
-    }
   }
-  // ---- the reports, before the mapping goes back: an alias piece maps to handle 0 ----------------------------
-  const Held h{(uint64_t)m.base, mapped, {{(uint64_t)m.base, mapped, 0}}, std::move(iters), std::move(pieces)};
-  rc = finish_gate(e, st, rc, h, drill, tag, res, &r->nonzero_bytes, probe, pcover, cover);
+  rc = finish_gate(e, st, rc, h, drill, tag, run.res, &r->nonzero_bytes, probe, pcover, cover);
   // ---- give the HBM back: on the reaper (default) or right here -----------------------
   if (rc == CCM_OK && async_release_enabled()) {
     r->release_deferred = 1;
@@ -2218,6 +2196,31 @@ int engine_release_wait(ScrubEngine* e, double* ms_release, double* ms_waited) {
   if (ms_release) *ms_release = e->reaper_ms;
   if (ms_waited) *ms_waited = w;
   return CCM_OK;
+}
+
+// The passes of the product call's fallback over the arena engine_arena_acquire took (the caller holds e->mu until
+// finish_gate is done): *h = every segment, at its offset into the concatenated segments (chunk = segment index), and
+// each GateRun step once over all of them, the read-back after the last drill.  Whatever this returns, the caller ends
+// the gate and gives the arena back.
+static int arena_passes(ScrubEngine* e, const ScrubDrill& drill, ccm_tag_result* tag, ccm_residue_report* res,
+                        ccm_scrub_result* r, Held* h) {
+  CCM_ENSURE_READY(e);
+  if (int rc = need_arena(e)) return rc;   // torn down since it was acquired
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  if (int rc = begin_gate(e, drill)) return rc;
+  h->va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
+  for (const Segment& s : e->segs) {
+    h->chunks.emplace_back(h->bytes, (uint32_t)h->spans.size());
+    h->spans.push_back({(uint64_t)(uintptr_t)s.ptr, s.bytes, h->bytes});
+    h->bytes += s.bytes;
+  }
+  h->probe_chunks = h->spans;
+  e->gate.spans = h->spans;
+  GateRun run{e, e->stream, drill, tag, res, false};
+  int rc = run.begin();
+  if (rc == CCM_OK) rc = run.held(h->spans);
+  if (rc == CCM_OK) rc = run.enqueue(h->spans);
+  return run.end(h->spans, rc, r);
 }
 
 // --------------------------------------------------------------- product call
@@ -2282,46 +2285,18 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     ccm_arena_info ai;
     rc = engine_arena_acquire(e, bytes, &ai);
     if (rc == CCM_OK) {
-      Held h;   // every segment, at its offset into the concatenated segments; chunk = segment index
-      {
-        std::lock_guard<std::mutex> g(e->mu);
-        rc = begin_gate(e, drill);
-        h.va_base = (uint64_t)(uintptr_t)e->segs.front().ptr;
-        for (const Segment& s : e->segs) {
-          h.chunks.emplace_back(h.bytes, (uint32_t)h.spans.size());
-          h.spans.push_back({(uint64_t)(uintptr_t)s.ptr, s.bytes, h.bytes});
-          h.bytes += s.bytes;
-        }
-        h.probe_chunks = h.spans;
-        e->gate.spans = h.spans;
-      }
       r.ms_acquire = ai.ms_acquire;
       r.bytes_scrubbed = ai.bytes;
       r.device_total_bytes = ai.device_total_bytes;
       r.device_free_before = ai.device_free_before;
       r.bytes_unreached = bytes == 0 && ai.device_free_before > ai.bytes ? ai.device_free_before - ai.bytes : 0;
       r.segments = ai.segments;
-      float ms_s = 0, ms_v = 0;
-      uint64_t nz = 0;
-      if (rc == CCM_OK) rc = arena_drill(e, drill.poison, 0, drill.residue);
-      if (rc == CCM_OK && tag) {
-        rc = arena_tag_check(e, h.spans, tag, drill.tag_inject, drill.tag_flood, res != nullptr);
-        ms_s = (float)tag->ms_check;
-      } else if (rc == CCM_OK && res) {
-        rc = arena_census(e, h.spans, &ms_s);
-      } else if (rc == CCM_OK) {
-        rc = engine_arena_scrub(e, CCM_SCRUB_AUTO, nullptr, nullptr, &ms_s);
-      }
-      if (rc == CCM_OK) rc = arena_drill(e, drill.flood, drill.inject);
-      if (rc == CCM_OK) rc = engine_arena_verify(e, CCM_VERIFY_AUTO, nullptr, nullptr, &nz, &ms_v);
       {
         std::lock_guard<std::mutex> g(e->mu);
-        if (rc == CCM_OK) rc = need_arena(e);   // torn down since the read-back: nothing is held any more
-        rc = finish_gate(e, e->stream, rc, h, drill, tag, res, &nz, probe_out, &pcover, &cover);
+        Held h;
+        rc = arena_passes(e, drill, tag, res, &r, &h);
+        rc = finish_gate(e, e->stream, rc, h, drill, tag, res, &r.nonzero_bytes, probe_out, &pcover, &cover);
       }
-      r.ms_scrub = ms_s;
-      r.ms_verify = ms_v;
-      r.nonzero_bytes = nz;
       int rc2 = engine_arena_release(e, &r.ms_release);
       if (rc == CCM_OK) rc = rc2;
     }
