@@ -1,9 +1,10 @@
 """Drives failed product scrub gate calls on CUDA device 0, proven or not, and reports what each call returned and left:
-the result, the dirt, mismatch and triage reports with their page maps and triage pages, the report proof and its
-inexact pages, and the kernels launched.
+the result, the tag and census counts, the dirt, mismatch and triage reports with their page maps and triage pages, the
+coverage proof, the alias probe and its proof, the report proof and the inexact pages of each proof, the address the
+reports' offsets are from, and the kernels launched.
 
-Imported by tests/test_report_cover_gpu.py and benchmarks/report_proof.py.  Run as a script it reads a JSON list of
-calls from argv[1] (`[{"bytes": ..., "env": {...}, "drill": {"scrub_inject": 4}, "kind": "zero", "prove": 1,
+Imported by tests/test_report_cover_gpu.py, tests/test_gate_scenarios_gpu.py and benchmarks/report_proof.py.  Run as a script it reads a JSON list of
+calls from argv[1], or from the file argv[1] names after an "@" (`[{"bytes": ..., "env": {...}, "drill": {"scrub_inject": 4}, "kind": "zero", "prove": 1,
 "triage": 5, "mismatch_triage": 5, "probe": 0, "many": 0}, ...]`; kind is zero, tagged, census or census_tagged), makes
 them in this fresh process and prints one `RESULT <json>` line, so that CCM_PDL, which the library latches once per
 process, takes this process's value.  Not collected by pytest.
@@ -25,7 +26,8 @@ import cover_proof_calls as CPC  # noqa: E402
 import product_gate_calls as PGC  # noqa: E402
 from k8s_cc_manager_b200 import _native as N  # noqa: E402
 
-DRILL_KEYS = CPC.DRILL_KEYS + ("tag_flood", "triage_stay", "triage_return", "probe_dirt", "report_skip", "report_skip_step")
+DRILL_KEYS = CPC.DRILL_KEYS + ("tag_flood", "triage_stay", "triage_return", "probe_mismatch", "probe_dirt", "probe_skip",
+                               "probe_skip_step", "report_skip", "report_skip_step")
 STEP_FIELDS = [f for f, _ in N.ReportCoverStep._fields_ if f != "reserved"]
 
 
@@ -104,18 +106,35 @@ def call(lib, c: dict) -> dict:
     assert lib.ccm_scrub_last_cover(0, C.byref(cover)) == 0, N.last_error()
     left = CPC.reports(lib)
     left.update(triage_pages(lib))
+    probe, pcover = N.ProbeReport(), N.ProbeCover()
+    assert lib.ccm_scrub_last_probe(0, C.byref(probe)) == 0, N.last_error()
+    assert lib.ccm_scrub_last_probe_cover(0, C.byref(pcover)) == 0, N.last_error()
+    dirt, mismatch = N.DirtReport(), N.MismatchReport()
+    assert lib.ccm_scrub_last_dirt(0, C.byref(dirt)) == 0 and lib.ccm_scrub_last_mismatch(0, C.byref(mismatch)) == 0
     out = {"call": c, "rc": rc, "error": err, "launches": launches, "ms_verdict": ms_verdict,
            "results": [{f: getattr(r, f) for f in PGC.FIELDS} for r in res],
-           "cover": CPC.cover_dict(cover), "report_cover": report_cover(lib), "reports": left, "times": timings(lib)}
+           "cover": CPC.cover_dict(cover), "cover_pages": CPC.cover_pages(lib), "report_cover": report_cover(lib),
+           "reports": left, "times": timings(lib),
+           "probe": {f: getattr(probe, f) for f, _ in N.ProbeReport._fields_ if f not in ("reserved", "ms_probe")},
+           "probe_cover": {"proved": pcover.proved, "covered": pcover.covered, "windows_expected": pcover.windows_expected,
+                           "steps": [{f: getattr(s, f) for f, _ in N.ProbeCoverStep._fields_ if f != "reserved"}
+                                     for s in pcover.steps]}}
     PGC.release_wait(lib)
     if tags is not None:
-        out["tags"] = [{"mismatch_bytes": t.mismatch_bytes} for t in tags]
+        out["tags"] = [{"mismatch_bytes": t.mismatch_bytes, "seed": t.seed, "va_base": t.va_base} for t in tags]
+    if census is not None:
+        out["residue"] = [{"residue_bytes": r.residue_bytes, "residue_windows": r.residue_windows} for r in census]
+    # the address every offset of the call is from: the tags', the probe's or a report's (0 when none was kept)
+    out["va_base"] = next((v for v in ([t.va_base for t in tags] if tags is not None else []) +
+                           [probe.va_base, dirt.va_base, mismatch.va_base] if v), 0)
     return out
 
 
 def main() -> None:
     lib = PGC.open_lib()
-    print("RESULT " + json.dumps([call(lib, c) for c in json.loads(sys.argv[1])]), flush=True)
+    arg = sys.argv[1]
+    calls = json.loads(Path(arg[1:]).read_text() if arg.startswith("@") else arg)
+    print("RESULT " + json.dumps([call(lib, c) for c in calls]), flush=True)
 
 
 if __name__ == "__main__":
