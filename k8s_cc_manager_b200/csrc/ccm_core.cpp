@@ -285,23 +285,107 @@ int sim_scrub_hook(int dev, ScrubDrill* drill) {
 }
 
 // ------------------------------------------------------------------ NVML (dl)
-// Query-only view of the platform's CC state for the sysfs backend.
+// One loader for every NVML query of the library: libnvidia-ml.so.1 is opened and nvmlInit_v2 called once, and each
+// entry point is resolved with dlsym (no link-time NVML).  Only read-only queries are resolved.
 struct NvmlCcState { unsigned int environment, ccFeature, devToolsMode; };
+struct NvmlRemapHistogram { unsigned int max, high, partial, low, none; };
+using NvmlDevice = void*;
+struct Nvml {
+  void* lib = nullptr;
+  int init_rc = -1;   // nvmlInit_v2's return code
+  int (*cc_state)(NvmlCcState*) = nullptr;
+  int (*handle_by_bus)(const char*, NvmlDevice*) = nullptr;
+  int (*ecc_mode)(NvmlDevice, int*, int*) = nullptr;
+  int (*error_counter)(NvmlDevice, int, int, int, unsigned long long*) = nullptr;
+  int (*remapped_rows)(NvmlDevice, unsigned int*, unsigned int*, unsigned int*, unsigned int*) = nullptr;
+  int (*remap_histogram)(NvmlDevice, NvmlRemapHistogram*) = nullptr;
+};
+constexpr int kNvmlNotSupported = 3;   // NVML_ERROR_NOT_SUPPORTED
+
+// The loaded library, or nullptr with the error text set.
+static const Nvml* nvml() {
+  static const Nvml n = [] {
+    Nvml v;
+    v.lib = dlopen("libnvidia-ml.so.1", RTLD_LAZY | RTLD_LOCAL);
+    if (!v.lib) return v;
+    auto init = (int (*)())dlsym(v.lib, "nvmlInit_v2");
+    v.init_rc = init ? init() : -1;
+    v.cc_state = (decltype(v.cc_state))dlsym(v.lib, "nvmlSystemGetConfComputeState");
+    v.handle_by_bus = (decltype(v.handle_by_bus))dlsym(v.lib, "nvmlDeviceGetHandleByPciBusId_v2");
+    v.ecc_mode = (decltype(v.ecc_mode))dlsym(v.lib, "nvmlDeviceGetEccMode");
+    v.error_counter = (decltype(v.error_counter))dlsym(v.lib, "nvmlDeviceGetMemoryErrorCounter");
+    v.remapped_rows = (decltype(v.remapped_rows))dlsym(v.lib, "nvmlDeviceGetRemappedRows");
+    v.remap_histogram = (decltype(v.remap_histogram))dlsym(v.lib, "nvmlDeviceGetRowRemapperHistogram");
+    return v;
+  }();
+  if (!n.lib) { set_error("libnvidia-ml.so.1 not loadable"); return nullptr; }
+  if (n.init_rc != 0) { set_error("nvmlInit_v2 failed (%d)", n.init_rc); return nullptr; }
+  return &n;
+}
+
+// Query-only view of the platform's CC state for the sysfs backend.
 static int nvml_cc_state(int* mode) {
-  static void* lib = dlopen("libnvidia-ml.so.1", RTLD_LAZY | RTLD_LOCAL);
-  if (!lib) { set_error("libnvidia-ml.so.1 not loadable"); return CCM_ERR_UNSUPPORTED; }
-  using InitFn = int (*)();
-  using StateFn = int (*)(NvmlCcState*);
-  static InitFn init = (InitFn)dlsym(lib, "nvmlInit_v2");
-  static StateFn state = (StateFn)dlsym(lib, "nvmlSystemGetConfComputeState");
-  if (!init || !state) { set_error("NVML lacks nvmlSystemGetConfComputeState"); return CCM_ERR_UNSUPPORTED; }
-  static int inited = init();
-  if (inited != 0) { set_error("nvmlInit_v2 failed (%d)", inited); return CCM_ERR_IO; }
+  const Nvml* n = nvml();
+  if (!n) return CCM_ERR_UNSUPPORTED;
+  if (!n->cc_state) { set_error("NVML lacks nvmlSystemGetConfComputeState"); return CCM_ERR_UNSUPPORTED; }
   NvmlCcState s{};
-  int rc = state(&s);
-  if (rc != 0) { set_error("nvmlSystemGetConfComputeState failed (%d)", rc); return rc == 3 ? CCM_ERR_UNSUPPORTED : CCM_ERR_IO; }
+  int rc = n->cc_state(&s);
+  if (rc != 0) { set_error("nvmlSystemGetConfComputeState failed (%d)", rc); return rc == kNvmlNotSupported ? CCM_ERR_UNSUPPORTED : CCM_ERR_IO; }
   *mode = s.ccFeature ? (s.devToolsMode ? CCM_CC_DEVTOOLS : CCM_CC_ON) : CCM_CC_OFF;
   return CCM_OK;
+}
+
+int hbm_snapshot_bus(const char* bus_id, ccm_hbm_state* out) {
+  memset(out, 0, sizeof *out);
+  const auto t0 = Clock::now();
+  const Nvml* n = nvml();
+  int rc = CCM_OK;
+  NvmlDevice h = nullptr;
+  if (!n) rc = CCM_ERR_UNSUPPORTED;
+  else if (!n->handle_by_bus) { set_error("NVML lacks nvmlDeviceGetHandleByPciBusId_v2"); rc = CCM_ERR_UNSUPPORTED; }
+  else if (int hr = n->handle_by_bus(bus_id, &h)) { set_error("NVML has no device at %s (%d)", bus_id, hr); rc = CCM_ERR_UNSUPPORTED; }
+  if (rc != CCM_OK) {
+    for (int32_t& r : out->nvml_rc) r = kNvmlNotSupported;
+    out->ms_query = std::chrono::duration<double, std::milli>(Clock::now() - t0).count();
+    return rc;
+  }
+  // Each query: its return code in nvml_rc[k], its bit in `available` when it answered.
+  auto note = [&](int k, int qrc, const char* what) {
+    out->nvml_rc[k] = qrc;
+    if (qrc == 0) out->available |= 1u << k;
+    else if (qrc != kNvmlNotSupported && rc == CCM_OK) { set_error("%s on %s failed (%d)", what, bus_id, qrc); rc = CCM_ERR_IO; }
+  };
+  int cur = 0, pend = 0;
+  note(0, n->ecc_mode ? n->ecc_mode(h, &cur, &pend) : kNvmlNotSupported, "nvmlDeviceGetEccMode");
+  if (out->available & CCM_HBM_Q_ECC_MODE) { out->ecc_current = cur != 0; out->ecc_pending = pend != 0; }
+  constexpr int kCorrected = 0, kUncorrected = 1, kVolatile = 0, kDram = 2, kSram = 7;   // nvml.h enums
+  uint64_t* counts[4] = {&out->dram_corrected, &out->dram_uncorrected, &out->sram_corrected, &out->sram_uncorrected};
+  for (int k = 0; k < 4; ++k) {
+    unsigned long long c = 0;
+    note(1 + k, n->error_counter ? n->error_counter(h, k % 2 ? kUncorrected : kCorrected, kVolatile, k < 2 ? kDram : kSram, &c)
+                                 : kNvmlNotSupported, "nvmlDeviceGetMemoryErrorCounter");
+    if (out->available & (1u << (1 + k))) *counts[k] = c;
+  }
+  unsigned int corr = 0, unc = 0, pending = 0, failure = 0;
+  note(5, n->remapped_rows ? n->remapped_rows(h, &corr, &unc, &pending, &failure) : kNvmlNotSupported,
+       "nvmlDeviceGetRemappedRows");
+  if (out->available & CCM_HBM_Q_REMAPPED_ROWS) {
+    out->rows_corrected = corr;
+    out->rows_uncorrected = unc;
+    out->remap_pending = pending != 0;
+    out->remap_failure = failure != 0;
+  }
+  NvmlRemapHistogram hist{};
+  note(6, n->remap_histogram ? n->remap_histogram(h, &hist) : kNvmlNotSupported, "nvmlDeviceGetRowRemapperHistogram");
+  if (out->available & CCM_HBM_Q_REMAP_HISTOGRAM) {
+    out->hist_max = hist.max;
+    out->hist_high = hist.high;
+    out->hist_partial = hist.partial;
+    out->hist_low = hist.low;
+    out->hist_none = hist.none;
+  }
+  out->ms_query = std::chrono::duration<double, std::milli>(Clock::now() - t0).count();
+  return rc;
 }
 
 // ------------------------------------------------------------- register ops
@@ -434,6 +518,7 @@ const char* ccm_strerror(int status) {
     case CCM_ERR_NOT_BOOTED: return "device not booted since its last reset";
     case CCM_ERR_MISMATCH: return "HBM bytes did not hold their address tag (tagged scrub gate)";
     case CCM_ERR_UNCOVERED: return "a scrub gate pass did not walk every mapped byte exactly once (coverage proof)";
+    case CCM_ERR_HBM_HEALTH: return "the GPU's HBM ECC or row-remapping state is unfit or unknown (HBM health)";
   }
   return "unknown ccm status";
 }
@@ -475,6 +560,13 @@ int ccm_query_ppcie_mode(int dev, int* mode) {
 }
 int ccm_set_ppcie_mode(int dev, int mode) { return with_dev(dev, [&](Device& d) { return op_set_ppcie(d, mode); }); }
 int ccm_reset(int dev) { return with_dev(dev, [&](Device& d) { return op_reset(d); }); }
+int ccm_hbm_snapshot(int dev, ccm_hbm_state* out) {
+  if (!out) return CCM_ERR_INVALID;
+  char bdf[sizeof(ccm_dev_info::bdf)];
+  int rc = with_dev(dev, [&](Device& d) { memcpy(bdf, d.info.bdf, sizeof bdf); return (int)CCM_OK; });
+  if (rc) { memset(out, 0, sizeof *out); return rc; }
+  return hbm_snapshot_bus(bdf, out);
+}
 int ccm_wait_for_boot(int dev, int timeout_ms) { return with_dev(dev, [&](Device& d) { return op_wait_boot(d, timeout_ms); }); }
 
 // ------------------------------------------------------------------ scrub ABI
@@ -708,6 +800,17 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
     d.drill.probe_skip_step = v == 0 ? 2 : (int)v;
   }
   else if (k == "report_skip") d.drill.report_skip = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "hbm_uncorrected") d.drill.hbm.uncorrected = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "hbm_corrected") d.drill.hbm.corrected = v < 0 ? 0 : (uint64_t)v;
+  else if (k == "hbm_remap_pending") d.drill.hbm.remap_pending = v != 0;
+  else if (k == "hbm_remap_failure") d.drill.hbm.remap_failure = v != 0;
+  else if (k == "hbm_unavailable") {
+    if (v < 0 || v > (int64_t)ccm_health::kAllQueries) {
+      set_error("sim key 'hbm_unavailable' takes ccm_hbm_query bits (0..%u), not %lld", ccm_health::kAllQueries, (long long)v);
+      return CCM_ERR_INVALID;
+    }
+    d.drill.hbm.unavailable = (uint32_t)v;
+  }
   else if (k == "report_skip_step") {
     if (v < 0 || v > (int64_t)CCM_REPORT_STEPS) {
       set_error("sim key 'report_skip_step' takes 0..%u, not %lld", CCM_REPORT_STEPS, (long long)v);
@@ -775,6 +878,11 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "probe_skip_step") *value = d.drill.probe_skip_step;
     else if (k == "report_skip") *value = (int64_t)d.drill.report_skip;
     else if (k == "report_skip_step") *value = d.drill.report_skip_step;
+    else if (k == "hbm_uncorrected") *value = (int64_t)d.drill.hbm.uncorrected;
+    else if (k == "hbm_corrected") *value = (int64_t)d.drill.hbm.corrected;
+    else if (k == "hbm_remap_pending") *value = d.drill.hbm.remap_pending;
+    else if (k == "hbm_remap_failure") *value = d.drill.hbm.remap_failure;
+    else if (k == "hbm_unavailable") *value = d.drill.hbm.unavailable;
     else { set_error("unknown sim key '%s'", k.c_str()); return (int)CCM_ERR_INVALID; }
     return (int)CCM_OK;
   });

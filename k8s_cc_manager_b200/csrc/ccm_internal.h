@@ -7,6 +7,7 @@
 #include <string>
 
 #include "ccm.h"
+#include "ccm_health.h"
 
 namespace ccm {
 
@@ -67,6 +68,9 @@ int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, b
 // Drill of the report proof (sim keys "report_skip", "report_skip_step"; ccm.h), armed or not:
 //   report_skip:    that many is written into the grab word of the first launch of report step report_skip_step
 //                   (CCM_REPORT_*; the sim key's 0 is stored as CCM_REPORT_DIRT_T3), just before it on the stream.
+// Drills of the HBM health report (sim keys "hbm_uncorrected", "hbm_corrected", "hbm_remap_pending",
+// "hbm_remap_failure", "hbm_unavailable"; ccm.h), only in an armed call: layered on its second snapshot
+// (ccm_health::layer).
 struct ScrubDrill {
   uint64_t inject = 0;
   int poison = 0;
@@ -85,6 +89,7 @@ struct ScrubDrill {
   int probe_skip_step = 2;
   uint64_t report_skip = 0;
   int report_skip_step = CCM_REPORT_DIRT_T3;
+  ccm_health::Drills hbm;
 };
 // inject: the call's "scrub_inject" budget.  Its poison and flood drills are those current_scrub_drill()
 // returns on the calling thread.  (The engine entry points keep the signatures that host-only builds of
@@ -105,6 +110,8 @@ const char* default_kernel_names();
 int engine_teardown(int ordinal);
 
 // ---- implemented in ccm_core.cpp -------------------------------------------
+// One HBM health snapshot of the GPU at PCI address `bus_id` through NVML (include/ccm.h: ccm_hbm_state).
+int hbm_snapshot_bus(const char* bus_id, ccm_hbm_state* out);
 // Maps a device-table index to its CUDA ordinal (or a negative ccm_status).
 int cuda_ordinal_of(int dev);
 // sim fault hook for the scrub op (returns CCM_OK or CCM_ERR_FAULT) + trace line; *drill = the

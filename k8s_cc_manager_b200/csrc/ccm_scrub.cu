@@ -171,6 +171,37 @@ static Held region_held(const void* p, uint64_t bytes) {
   return Held{a, bytes, {{a, bytes, 0}}, {{a, bytes, 0}}, {{0, 0u}}};
 }
 
+// The HBM health report of one product call (ccm.h: ccm_scrub_health): the snapshot before the call maps anything
+// (begin), and the one after its reports (after: the first of its calls takes it, so every path can make one), with
+// the drills on top.  NVML needs no CUDA context, so a call whose kernels died still gets both.  Neither snapshot
+// changes the call's error text.
+struct HbmWatch {
+  int mode = 0;   // 0: the call is not armed, and reads nothing
+  const char* bus = nullptr;
+  ccm_health::Drills drills;
+  ccm_hbm_state before{}, post{};
+  bool taken = false;
+
+  void snap(ccm_hbm_state* s) {
+    const std::string err = last_error();
+    hbm_snapshot_bus(bus, s);
+    set_error("%s", err.c_str());
+  }
+  void begin() { if (mode) snap(&before); }
+  void after() {
+    if (!mode || taken) return;
+    taken = true;
+    snap(&post);
+    ccm_health::layer(&post, drills);
+  }
+  void judge(ccm_hbm_health* h) const {
+    memset(h, 0, sizeof *h);
+    ccm_health::judge(before, post, h);
+    h->mode = mode;
+    h->ms_health = before.ms_query + post.ms_query;
+  }
+};
+
 // The product call's passes while it enqueues them (ccm.h: ccm_scrub_prove, and the "cover_skip" drill).  Every range
 // launch of the scrub, census, tag fill, tag check and read-back asks it for its cover map (gate_launch).  The locate
 // pass and the triages run after it is cleared, each step with `report` set (ccm.h: ccm_report_cover, and the
@@ -240,6 +271,9 @@ struct ScrubEngine {
   // report proof (a proven call that locates or triages): its maps follow the passes' in d_cover
   ccm_report_cover rcover{};                // report of the last product call (ccm_scrub_last_report_cover)
   std::vector<ccm_report_cover_page> rcover_pages;   // and its inexact pages (ccm_last_report_cover_pages)
+  int health_mode = 0;                      // the HBM health report's arming (ccm_scrub_health): 0 off, 1, 2
+  char bus_id[32] = {};                     // the PCI bus id NVML knows the device by (set when armed)
+  ccm_hbm_health health{};                  // report of the last product call (ccm_scrub_last_health)
   std::vector<Segment> segs;
   uint64_t arena_bytes = 0;
   size_t total_bytes = 0;
@@ -2040,7 +2074,7 @@ static bool async_release_enabled() { return env_u64("CCM_ASYNC_RELEASE", 1) != 
 //   (serialised node-wide by the driver) run on the engine's reaper thread.
 static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDrill& drill, bool node_fanout,
                                   ccm_scrub_result* r, ccm_cover_report* cover, ccm_probe_report* probe,
-                                  ccm_probe_cover* pcover) {
+                                  ccm_probe_cover* pcover, HbmWatch* health) {
   const VmmApi& api = vmm();
   if (!api.ok) return CCM_ERR_UNSUPPORTED;
   std::lock_guard<std::mutex> g(e->mu);
@@ -2173,6 +2207,7 @@ static int scrub_verify_pipelined(ScrubEngine* e, uint64_t bytes, const ScrubDri
     r->ms_acquire = host_acquire;
   }
   rc = finish_gate(e, st, rc, h, drill, tag, run.res, &r->nonzero_bytes, probe, pcover, cover);
+  health->after();
   // ---- give the HBM back: on the reaper (default) or right here -----------------------
   if (rc == CCM_OK && async_release_enabled()) {
     r->release_deferred = 1;
@@ -2232,6 +2267,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   ccm_residue_report* res = current_residue_call();
   bool prove = false, probe_armed = false;
   int probe_rc = CCM_OK;   // an armed device whose probe kernels cannot be made resident runs no call
+  HbmWatch health;
   {
     std::lock_guard<std::mutex> g(e->mu);
     memset(&e->dirt, 0, sizeof e->dirt);  // every call replaces the reports of the last one
@@ -2250,6 +2286,9 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
     e->pcover_pages.clear();
     memset(&e->rcover, 0, sizeof e->rcover);
     e->rcover_pages.clear();
+    memset(&e->health, 0, sizeof e->health);
+    health.mode = e->health_mode;
+    health.bus = e->bus_id;
     prove = e->prove;
     // the alias probe is for the zero gate: a tagged call's check already covers every window
     probe_armed = e->probe_armed && tag == nullptr;
@@ -2277,8 +2316,10 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   ccm_probe_report* probe_out = probe_armed ? &probe : nullptr;
   ccm_probe_cover pcover;   // and of the probe proof
   memset(&pcover, 0, sizeof pcover);
+  health.drills = drill.hbm;
+  health.begin();
   if (env_u64("CCM_PIPELINE", 1) != 0)
-    rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r, &cover, probe_out, &pcover);
+    rc = scrub_verify_pipelined(e, bytes, drill, node_fanout, &r, &cover, probe_out, &pcover, &health);
   if (rc == CCM_ERR_UNSUPPORTED) {
     // plain path: one cudaMalloc'ed arena, whole-arena scrub, whole-arena verify (the drills act per
     // segment: poison before the scrub, flood + inject between the scrub and the verify)
@@ -2296,6 +2337,7 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
         Held h;
         rc = arena_passes(e, drill, tag, res, &r, &h);
         rc = finish_gate(e, e->stream, rc, h, drill, tag, res, &r.nonzero_bytes, probe_out, &pcover, &cover);
+        health.after();
       }
       int rc2 = engine_arena_release(e, &r.ms_release);
       if (rc == CCM_OK) rc = rc2;
@@ -2339,6 +2381,20 @@ int engine_scrub_verify(ScrubEngine* e, uint64_t bytes, uint64_t inject, bool no
   } else if (rc == CCM_OK && r.nonzero_bytes != 0) {
     set_error("scrub verify found %llu non-zero bytes on CUDA device %d", (unsigned long long)r.nonzero_bytes, e->ordinal);
     rc = CCM_ERR_DIRTY;
+  }
+  if (health.mode) {
+    health.after();   // a call that failed before its reports takes it here
+    ccm_hbm_health hh;
+    health.judge(&hh);
+    // the hardware's record explains the counts the passes found; an error that stopped the call keeps its status
+    const bool judged = rc == CCM_OK || rc == CCM_ERR_UNCOVERED || rc == CCM_ERR_MISMATCH || rc == CCM_ERR_DIRTY;
+    if (health.mode == 2 && judged && hh.verdict != CCM_HBM_FIT) {
+      set_error("HBM health of CUDA device %d (%s) is %s: %s", e->ordinal, e->bus_id,
+                hh.verdict == CCM_HBM_UNFIT ? "unfit" : "unknown", ccm_health::reasons(hh).c_str());
+      rc = CCM_ERR_HBM_HEALTH;
+    }
+    std::lock_guard<std::mutex> g(e->mu);
+    e->health = hh;
   }
   r.ms_total = now_ms() - t0;
   r.sm_count = e->sm_count;
@@ -2680,6 +2736,34 @@ extern "C" int ccm_scrub_probe(int cuda_ordinal, int on) {
 
 extern "C" int ccm_scrub_last_probe(int cuda_ordinal, ccm_probe_report* out) {
   return last_report(cuda_ordinal, out, &ScrubEngine::probe);
+}
+
+// ------------------------------------------------------------------------- HBM health
+static_assert(sizeof(ccm_hbm_state) == 120 && offsetof(ccm_hbm_state, available) == 76 &&
+              offsetof(ccm_hbm_state, ms_query) == 112 && sizeof(ccm_hbm_health) == 296 &&
+              offsetof(ccm_hbm_health, d_dram_corrected) == 240 && offsetof(ccm_hbm_health, mode) == 280,
+              "HBM health structs keep their layout");
+
+extern "C" int ccm_scrub_health(int cuda_ordinal, int mode) {
+  if (mode < 0 || mode > 2) {
+    set_error("ccm_scrub_health: mode %d (0 off, 1 report, 2 require)", mode);
+    return CCM_ERR_INVALID;
+  }
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  // disarming an engine that was never created leaves nothing armed (and starts no context)
+  ScrubEngine* e = mode ? engine_for(cuda_ordinal) : engine_lookup(cuda_ordinal);
+  if (!e) return mode ? CCM_ERR_NO_CUDA : CCM_OK;
+  std::lock_guard<std::mutex> g(e->mu);
+  if (mode) CCM_CUDA(cudaDeviceGetPCIBusId(e->bus_id, sizeof e->bus_id, e->ordinal));
+  e->health_mode = mode;
+  return CCM_OK;
+}
+
+extern "C" int ccm_scrub_last_health(int cuda_ordinal, ccm_hbm_health* out) {
+  return last_report(cuda_ordinal, out, &ScrubEngine::health);
 }
 
 // ------------------------------------------------------------------------- probe proof

@@ -1,7 +1,8 @@
 // ccm-scrub — native command-line front end of the HBM scrub gate (links libccm.so).
 //
 //   ccm-scrub [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] [--triage]
-//             [--mismatch-triage] [--triage-hold-ms MS] [--prove] [--probe] (--all | --bdf <pci address> ...)
+//             [--mismatch-triage] [--triage-hold-ms MS] [--prove] [--probe] [--health report|require]
+//             (--all | --bdf <pci address> ...)
 //
 // Runs the concurrent gate (ccm_scrub_verify_many, or ccm_scrub_verify_many_tagged with --check tagged)
 // and prints ONE JSON line with the same fields as k8s_cc_manager_b200.devices.ScrubReport (the
@@ -19,8 +20,10 @@
 // probe (ccm_scrub_probe), for every GPU whose probe ran, as ccm_scrub_last_probe reports it, with "mismatch" when it
 // found bytes off their tags); "probe_cover" with --prove and --probe, for every GPU whose probe ran, as
 // ccm_scrub_last_probe_cover and ccm_last_probe_cover_pages report it; "report_cover" with --prove, for every GPU that
-// located dirt or triaged, as ccm_scrub_last_report_cover and ccm_last_report_cover_pages report it.  With --prove or
-// --probe, a GPU that cannot be armed is never scrubbed without: nothing is scrubbed and the exit code is 3.
+// located dirt or triaged, as ccm_scrub_last_report_cover and ccm_last_report_cover_pages report it; "hbm_health" with
+// --health report or --health require, which arms every GPU for the HBM health report (ccm_scrub_health), as
+// ccm_scrub_last_health reports it (under require, a GPU armed and without one gets CCM_ERR_HBM_HEALTH).  With --prove,
+// --probe or --health, a GPU that cannot be armed is never scrubbed without: nothing is scrubbed and the exit code is 3.
 // Exit 0: every GPU clean; 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
@@ -33,6 +36,46 @@
 #include <vector>
 
 #include "ccm.h"
+
+// The "hbm_health" object: the fields of k8s_cc_manager_b200.devices.HbmHealth.
+static void print_snapshot(const char* key, const ccm_hbm_state& s) {
+  printf("\"%s\": {\"dram_corrected\": %llu, \"dram_uncorrected\": %llu, \"sram_corrected\": %llu, "
+         "\"sram_uncorrected\": %llu, \"ecc_current\": %u, \"ecc_pending\": %u, \"rows_corrected\": %u, "
+         "\"rows_uncorrected\": %u, \"remap_pending\": %u, \"remap_failure\": %u, \"hist_max\": %u, \"hist_high\": %u, "
+         "\"hist_partial\": %u, \"hist_low\": %u, \"hist_none\": %u, \"available\": %u, \"nvml_rc\": [",
+         key, (unsigned long long)s.dram_corrected, (unsigned long long)s.dram_uncorrected,
+         (unsigned long long)s.sram_corrected, (unsigned long long)s.sram_uncorrected, s.ecc_current, s.ecc_pending,
+         s.rows_corrected, s.rows_uncorrected, s.remap_pending, s.remap_failure, s.hist_max, s.hist_high, s.hist_partial,
+         s.hist_low, s.hist_none, s.available);
+  for (unsigned k = 0; k < CCM_HBM_QUERIES; ++k) printf("%s%d", k ? ", " : "", s.nvml_rc[k]);
+  printf("], \"ms_query\": %.3f}", s.ms_query);
+}
+
+static void print_names(uint32_t bits, const char* const* names, unsigned n) {
+  printf("[");
+  for (unsigned k = 0, first = 1; k < n; ++k)
+    if (bits >> k & 1) { printf("%s\"%s\"", first ? "" : ", ", names[k]); first = 0; }
+  printf("]");
+}
+
+static void print_health(const ccm_hbm_health& h) {
+  static const char* const kQueries[CCM_HBM_QUERIES] = {"ecc_mode", "dram_corrected", "dram_uncorrected", "sram_corrected",
+                                                        "sram_uncorrected", "remapped_rows", "remap_histogram"};
+  static const char* const kReasons[7] = {"dram_uncorrected", "sram_uncorrected", "remap_pending", "remap_failure",
+                                          "ecc_off", "no_answer", "went_down"};
+  printf(", \"hbm_health\": {");
+  print_snapshot("before", h.before);
+  printf(", ");
+  print_snapshot("after", h.after);
+  printf(", \"d_dram_corrected\": %lld, \"d_dram_uncorrected\": %lld, \"d_sram_corrected\": %lld, "
+         "\"d_sram_uncorrected\": %lld, \"ms_health\": %.3f, \"mode\": %d, \"verdict\": %d, \"reasons\": ",
+         (long long)h.d_dram_corrected, (long long)h.d_dram_uncorrected, (long long)h.d_sram_corrected,
+         (long long)h.d_sram_uncorrected, h.ms_health, h.mode, h.verdict);
+  print_names(h.reasons, kReasons, 7);
+  printf(", \"missing_queries\": ");
+  print_names(h.missing_queries, kQueries, CCM_HBM_QUERIES);
+  printf("}");
+}
 
 // The "triage" object: the fields of k8s_cc_manager_b200.devices.TriageReport, with the first 64 pages that did not clear
 // (devices.TRIAGE_PAGES).
@@ -231,7 +274,8 @@ static void print_mismatch_triage(const ccm_triage_report& t, int ordinal) {
 
 static int usage(const char* argv0) {
   fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] "
-          "[--triage] [--mismatch-triage] [--triage-hold-ms MS] [--prove] [--probe] (--all | --bdf <bdf> ...)\n", argv0);
+          "[--triage] [--mismatch-triage] [--triage-hold-ms MS] [--prove] [--probe] [--health report|require] "
+          "(--all | --bdf <bdf> ...)\n", argv0);
   return 2;
 }
 
@@ -286,6 +330,7 @@ int main(int argc, char** argv) {
   bool all = false, tagged = false, residue = false, triage = false, mismatch_triage = false, prove = false,
        probe = false;
   unsigned long triage_hold_ms = 100;   // k8s_cc_manager_b200.devices.TRIAGE_HOLD_MS
+  int health = 0;                       // ccm_scrub_health's mode: 0 off, 1 report, 2 require
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     if (a == "--all") all = true;
@@ -297,6 +342,11 @@ int main(int argc, char** argv) {
     else if (a == "--triage-hold-ms" && i + 1 < argc) {
       triage_hold_ms = strtoul(argv[++i], nullptr, 10);
       if (triage_hold_ms == 0 || triage_hold_ms > CCM_TRIAGE_MAX_HOLD_MS) return usage(argv[0]);
+    }
+    else if (a == "--health" && i + 1 < argc) {
+      std::string h = argv[++i];
+      if (h != "off" && h != "report" && h != "require") return usage(argv[0]);
+      health = h == "require" ? 2 : h == "report" ? 1 : 0;
     }
     else if (a == "--bdf" && i + 1 < argc) bdfs.emplace_back(argv[++i]);
     else if (a == "--bytes" && i + 1 < argc) bytes = strtoull(argv[++i], nullptr, 10);
@@ -371,6 +421,18 @@ int main(int argc, char** argv) {
     }
     probed.push_back(ordinals[i]);
   }
+  std::vector<int> harmed;   // ordinals armed for the HBM health report: all of them, or the gate does not run
+  for (size_t i = 0; health && i < ordinals.size(); ++i) {
+    const int rc = ordinals[i] >= 0 ? ccm_scrub_health(ordinals[i], health) : CCM_ERR_NO_CUDA;
+    if (rc != CCM_OK) {
+      fprintf(stderr, "cannot arm the HBM health report on %s: %s\n", names[i].c_str(), ccm_strerror(rc));
+      for (int o : harmed) ccm_scrub_health(o, 0);
+      for (int o : probed) ccm_scrub_probe(o, 0);
+      for (int o : parmed) ccm_scrub_prove(o, 0);
+      return 3;
+    }
+    harmed.push_back(ordinals[i]);
+  }
   std::vector<int> armed;   // ordinals armed for the triage, disarmed once the gate is done
   for (size_t i = 0; triage && i < ordinals.size(); ++i)
     if (ordinals[i] >= 0 && ccm_scrub_triage(ordinals[i], (uint32_t)triage_hold_ms) == CCM_OK) armed.push_back(ordinals[i]);
@@ -387,6 +449,7 @@ int main(int argc, char** argv) {
   for (int o : marmed) ccm_scrub_mismatch_triage(o, 0);
   for (int o : parmed) ccm_scrub_prove(o, 0);
   for (int o : probed) ccm_scrub_probe(o, 0);
+  for (int o : harmed) ccm_scrub_health(o, 0);
   bool clean = true;
   printf("{\"wall_ms\": %.3f, \"reports\": [", wall_ms);
   for (size_t i = 0; i < devs.size(); ++i) {
@@ -396,7 +459,10 @@ int main(int argc, char** argv) {
     ccm_probe_cover pc;
     const bool probe_proved = prove && ran_probe && ccm_scrub_last_probe_cover(ordinals[i], &pc) == CCM_OK && pc.proved;
     // a proving call that probed and has no probe proof fails in its own report, whoever reads it
-    const int status = r.status == CCM_OK && prove && ran_probe && !probe_proved ? (int)CCM_ERR_UNCOVERED : r.status;
+    int status = r.status == CCM_OK && prove && ran_probe && !probe_proved ? (int)CCM_ERR_UNCOVERED : r.status;
+    ccm_hbm_health hh;
+    const bool has_health = health && ccm_scrub_last_health(ordinals[i], &hh) == CCM_OK && hh.mode;
+    if (health == 2 && !has_health && status == CCM_OK) status = CCM_ERR_HBM_HEALTH;   // asked for and missing
     clean = clean && status == CCM_OK && r.nonzero_bytes == 0;
     printf("%s{\"bdf\": \"%s\", \"bytes_requested\": %llu, \"bytes_scrubbed\": %llu, \"device_total_bytes\": %llu, "
            "\"nonzero_bytes\": %llu, \"ms_acquire\": %.3f, \"ms_scrub\": %.3f, \"ms_verify\": %.3f, \"ms_release\": %.3f, "
@@ -433,6 +499,7 @@ int main(int argc, char** argv) {
     if (probe_proved) print_pcover(pc, ordinals[i]);
     ccm_report_cover rc;
     if (prove && ccm_scrub_last_report_cover(ordinals[i], &rc) == CCM_OK && rc.proved) print_rcover(rc, ordinals[i]);
+    if (has_health) print_health(hh);
     printf("}");
   }
   printf("]}\n");

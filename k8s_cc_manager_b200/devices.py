@@ -37,7 +37,8 @@ class GpuError(Exception):
     carries its ProbeReport (what the alias probe found) as `.probe`; a call both proving and probing carries its
     ProbeCoverReport (how many windows each probe step took on every page) as `.probe_cover`; a proving call that
     located dirt or triaged carries its ReportCoverReport (how many bytes the locate pass and each triage step walked on
-    every page) as `.report_cover`."""
+    every page) as `.report_cover`; a call armed for the HBM health report carries its HbmHealth (the GPU's ECC and
+    row-remapping state before and after the call) as `.health`."""
 
     def __init__(self, message: str, status: int = N.ERR_IO):
         super().__init__(message)
@@ -895,10 +896,169 @@ def _attach_report_cover(rep: "ScrubReport", cuda_ordinal: int) -> None:
     rep.report_cover = report if report is not None and report.proved else None
 
 
+@dataclass
+class HbmSnapshot:
+    """One NVML snapshot of a GPU's ECC and row-remapping state (include/ccm.h: ccm_hbm_state).  A query that did not
+    answer has its bit clear in `available`, its fields 0 and its NVML return code in `nvml_rc`."""
+    dram_corrected: int
+    dram_uncorrected: int
+    sram_corrected: int
+    sram_uncorrected: int
+    ecc_current: int
+    ecc_pending: int
+    rows_corrected: int
+    rows_uncorrected: int
+    remap_pending: int
+    remap_failure: int
+    hist_max: int
+    hist_high: int
+    hist_partial: int
+    hist_low: int
+    hist_none: int
+    available: int
+    nvml_rc: List[int]
+    ms_query: float
+
+    @classmethod
+    def from_native(cls, s: N.HbmState) -> "HbmSnapshot":
+        return cls(**{f: (list(getattr(s, f)) if f == "nvml_rc" else getattr(s, f))
+                      for f, _ in N.HbmState._fields_ if f != "reserved"})
+
+    def answered(self, query: str) -> bool:
+        """Whether the query (a name of N.HBM_QUERIES) answered."""
+        return bool(self.available >> N.HBM_QUERIES.index(query) & 1)
+
+    def unanswered(self) -> List[str]:
+        return [q for q in N.HBM_QUERIES if not self.answered(q)]
+
+
+def _delta(d: int, answered: bool) -> str:
+    return f"{d:+d}" if answered else "?"
+
+
+@dataclass
+class HbmHealth:
+    """The HBM health report of one armed product call (include/ccm.h: ccm_hbm_health): the GPU's ECC and row-remapping
+    state through NVML before the call mapped anything and after its reports, and the rule's verdict on the pair
+    (N.HBM_FIT, N.HBM_UNFIT, N.HBM_UNKNOWN) with its reasons (names of N.HBM_REASONS)."""
+    before: HbmSnapshot
+    after: HbmSnapshot
+    d_dram_corrected: int
+    d_dram_uncorrected: int
+    d_sram_corrected: int
+    d_sram_uncorrected: int
+    ms_health: float
+    mode: int
+    verdict: int
+    reasons: List[str]
+    missing_queries: List[str]
+
+    @classmethod
+    def from_native(cls, h: N.HbmHealth) -> "HbmHealth":
+        names = lambda bits, table: [n for k, n in enumerate(table) if bits >> k & 1]   # noqa: E731
+        return cls(HbmSnapshot.from_native(h.before), HbmSnapshot.from_native(h.after), h.d_dram_corrected,
+                   h.d_dram_uncorrected, h.d_sram_corrected, h.d_sram_uncorrected, h.ms_health, h.mode, h.verdict,
+                   names(h.reasons, N.HBM_REASONS), names(h.missing_queries, N.HBM_QUERIES))
+
+    @classmethod
+    def from_json(cls, d: dict) -> "HbmHealth":
+        return cls(**{**d, "before": HbmSnapshot(**d["before"]), "after": HbmSnapshot(**d["after"])})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    @property
+    def fit(self) -> bool:
+        return self.verdict == N.HBM_FIT
+
+    @property
+    def verdict_name(self) -> str:
+        return {N.HBM_FIT: "fit", N.HBM_UNFIT: "unfit", N.HBM_UNKNOWN: "unknown"}.get(self.verdict, "not judged")
+
+    def why(self) -> List[str]:
+        """The reasons of a report that is not fit, one phrase each, for an operator."""
+        a = self.after
+        phrases = {
+            "dram_uncorrected": f"uncorrected DRAM errors {self.d_dram_uncorrected:+d} during the gate",
+            "sram_uncorrected": f"uncorrected SRAM errors {self.d_sram_uncorrected:+d} during the gate",
+            "remap_pending": "a row remap is pending: the GPU must be reset before release",
+            "remap_failure": f"a row remap failed ({a.rows_uncorrected} rows remapped for uncorrected errors, "
+                             f"{a.hist_none} banks without spare rows): the GPU should go to RMA",
+            "ecc_off": "ECC is off",
+            "no_answer": "NVML did not answer " + ", ".join(
+                f"{q} ({self.before.nvml_rc[N.HBM_QUERIES.index(q)] or self.after.nvml_rc[N.HBM_QUERIES.index(q)]})"
+                for q in self.missing_queries),
+            "went_down": "an error counter went down between the snapshots (a reset in between)",
+        }
+        return [phrases[r] for r in self.reasons]
+
+    def summary(self) -> str:
+        """One line for an operator: ECC, the counter deltas over the gate and the remap state after it; then the
+        verdict's reasons when it is not fit."""
+        a, both = self.after, lambda q: self.before.answered(q) and self.after.answered(q)
+        ecc = ("on" if a.ecc_current else "off") if a.answered("ecc_mode") else "unknown"
+        line = (f"ECC {ecc}; DRAM corrected {_delta(self.d_dram_corrected, both('dram_corrected'))}, uncorrected "
+                f"{_delta(self.d_dram_uncorrected, both('dram_uncorrected'))} during the gate")
+        if self.d_sram_corrected or self.d_sram_uncorrected:
+            line += f"; SRAM corrected {self.d_sram_corrected:+d}, uncorrected {self.d_sram_uncorrected:+d}"
+        if a.answered("remapped_rows"):
+            line += (f"; rows remapped {a.rows_corrected}/{a.rows_uncorrected}, "
+                     f"{'remap pending' if a.remap_pending else 'none pending'}, "
+                     f"{'remap FAILED' if a.remap_failure else 'no failure'}")
+        else:
+            line += "; row remapping unknown"
+        if not self.fit:
+            line += f"; {self.verdict_name.upper()}: " + "; ".join(self.why())
+        return line
+
+
+def hbm_snapshot(dev) -> HbmSnapshot:
+    """One NVML snapshot of a GPU's ECC and row-remapping state (include/ccm.h: ccm_hbm_snapshot); `dev` is a device of
+    find_gpus() or its index.  Needs no CUDA context and changes nothing on the device.  A snapshot whose queries did
+    not all answer is returned as it is (see `available`); GpuError for an unknown device."""
+    index = dev if isinstance(dev, int) else dev.index
+    out = N.HbmState()
+    rc = N.lib().ccm_hbm_snapshot(index, C.byref(out))
+    if rc in (N.ERR_NO_DEVICE, N.ERR_INVALID):
+        _check(rc, "hbm_snapshot")
+    return HbmSnapshot.from_native(out)
+
+
+def last_health(cuda_ordinal: int) -> "Optional[HbmHealth]":
+    """The HBM health report of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_health); None
+    when it cannot be read or the call was not armed."""
+    out = N.HbmHealth()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_health(cuda_ordinal, C.byref(out)) != N.OK or not out.mode:
+        return None
+    return HbmHealth.from_native(out)
+
+
+def _health_mode(health: str) -> int:
+    """ccm_scrub_health's mode for 'off' / 'report' / 'require'; ValueError for anything else."""
+    if health not in N.HBM_HEALTH_MODES:
+        raise ValueError(f"HBM health must be 'off', 'report' or 'require', not {health!r}")
+    return N.HBM_HEALTH_MODES[health]
+
+
+def _arm_health(cuda_ordinal: int, mode: int) -> int:
+    """Arms (mode 1 or 2) or disarms (0) the HBM health report on a CUDA device; the library's status."""
+    return N.lib().ccm_scrub_health(cuda_ordinal, mode) if cuda_ordinal >= 0 else N.ERR_NO_CUDA
+
+
+def _attach_health(rep: "ScrubReport", cuda_ordinal: int, mode: int) -> None:
+    """The health report of an armed call; under 'require', a call that returned OK without one fails with
+    ERR_HBM_HEALTH (a report that was asked for and is missing is no evidence of health)."""
+    rep.health = last_health(cuda_ordinal)
+    if mode == N.HBM_HEALTH_MODES["require"] and rep.health is None and rep.status == N.OK:
+        rep.status = N.ERR_HBM_HEALTH
+
+
 # The reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
 _REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport),
             ("mismatch_triage", TriageReport), ("cover", CoverReport), ("probe", ProbeReport),
-            ("probe_cover", ProbeCoverReport), ("report_cover", ReportCoverReport))
+            ("probe_cover", ProbeCoverReport), ("report_cover", ReportCoverReport), ("health", HbmHealth))
+# The JSON key of a report whose attribute is not its key.
+_JSON_KEYS = {"health": "hbm_health"}
 
 
 @dataclass
@@ -955,6 +1115,9 @@ class ScrubReport:
     # How many bytes the locate pass and each triage step walked on every page (a ReportCoverReport), set for every
     # report of a proving call (prove=True) that located dirt or triaged.  Not a dataclass field either.
     report_cover = None
+    # The GPU's ECC and row-remapping state before and after the call (an HbmHealth), set for every report of a call
+    # armed for it (health="report" or "require").  Not a dataclass field either; its JSON key is "hbm_health".
+    health = None
 
     @property
     def clean(self) -> bool:
@@ -998,14 +1161,14 @@ class ScrubReport:
                 del d[name]
         for attr, _ in _REPORTS:
             if getattr(self, attr) is not None:
-                d[attr] = getattr(self, attr).as_json()
+                d[_JSON_KEYS.get(attr, attr)] = getattr(self, attr).as_json()
         return d
 
     @classmethod
     def from_json(cls, d: dict) -> "ScrubReport":
         """Inverse of as_json."""
         d = dict(d)
-        found = [(attr, kind, d.pop(attr, None)) for attr, kind in _REPORTS]
+        found = [(attr, kind, d.pop(_JSON_KEYS.get(attr, attr), None)) for attr, kind in _REPORTS]
         rep = cls(**d)
         for attr, kind, js in found:
             if js is not None:
@@ -1107,7 +1270,7 @@ class NvidiaDevice:
     # -- NEW: HBM scrub-and-verify ---------------------------------------------
     def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
                          triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False,
-                         prove: bool = False, probe: bool = False) -> ScrubReport:
+                         prove: bool = False, probe: bool = False, health: str = "off") -> ScrubReport:
         """Zero-fills and reads back this GPU's HBM (nbytes=0: all the context can map).
         check="tagged" first writes and checks an address-tagged known answer
         (include/ccm.h: ccm_scrub_verify_tagged).  residue=True runs the census in the first pass and attaches what
@@ -1130,6 +1293,11 @@ class NvidiaDevice:
         each page, the report comes attached as `.probe_cover`, and a step that missed or repeated a window fails the
         call with ERR_UNCOVERED.  A proving call that fails and locates its dirt or triages also proves its locate pass
         and triage steps: the report comes attached as `.report_cover`, and never changes the verdict.
+        health="report" or "require" arms the HBM health report for this call (include/ccm.h: ccm_scrub_health): the
+        GPU's ECC counters and row-remapping state are read through NVML before the call maps anything and after its
+        reports, and the report comes attached as `.health`.  Under "require" a GPU whose uncorrected count rose, whose
+        remap is pending or failed, whose ECC is off, or whose state could not be read fails the call with
+        ERR_HBM_HEALTH; "report" never changes the verdict.  A device that cannot be armed fails the call.
 
         Raises GpuError if the scrub cannot run (no CUDA device, no HBM, CUDA error),
         if any byte reads back non-zero, or (tagged) if any byte did not hold its tag.  When the read-back
@@ -1142,8 +1310,11 @@ class NvidiaDevice:
         _mismatch_triage_check(mismatch_triage, check)
         _probe_check(probe, check)
         hold = _triage_hold(triage_hold_ms) if triage or mismatch_triage else 0
+        hmode = _health_mode(health)
         armed = marmed = False
         try:
+            if hmode:
+                _check(_arm_health(self.cuda_ordinal, hmode), "scrub_and_verify (HBM health)", self.bdf)
             if prove:
                 _check(_arm_prove(self.cuda_ordinal, True), "scrub_and_verify (coverage proof)", self.bdf)
             if probe:
@@ -1168,6 +1339,8 @@ class NvidiaDevice:
                 _arm_prove(self.cuda_ordinal, False)
             if probe:
                 _arm_probe(self.cuda_ordinal, False)
+            if hmode:
+                _arm_health(self.cuda_ordinal, 0)
         rep = ScrubReport.from_native(self.bdf, res, tag)
         _attach_reports(rep, self.cuda_ordinal, census, armed, marmed, prove)
         probe_proved = _attach_probe(rep, self.cuda_ordinal, prove) if probe else True
@@ -1177,6 +1350,10 @@ class NvidiaDevice:
             err = GpuError(f"scrub_and_verify on {self.bdf}: the coverage proof did not run", N.ERR_UNCOVERED)
         if err is None and not probe_proved:
             err = GpuError(f"scrub_and_verify on {self.bdf}: the probe proof did not run", N.ERR_UNCOVERED)
+        if hmode:
+            _attach_health(rep, self.cuda_ordinal, hmode)
+            if err is None and rep.status == N.ERR_HBM_HEALTH:   # a report that was asked for and is missing
+                err = GpuError(f"scrub_and_verify on {self.bdf}: the HBM health report is missing", N.ERR_HBM_HEALTH)
         if err is not None:
             for attr, _ in _REPORTS:
                 setattr(err, attr, getattr(rep, attr))
@@ -1227,23 +1404,26 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
                           check: str = "zero", residue: bool = False, triage: bool = False,
                           triage_hold_ms: int = TRIAGE_HOLD_MS,
                           mismatch_triage: bool = False, prove: bool = False,
-                          probe: bool = False) -> Tuple[List[ScrubReport], float]:
+                          probe: bool = False, health: str = "off") -> Tuple[List[ScrubReport], float]:
     """Concurrent multi-context scrub of several GPUs through ONE native call
     (ccm_scrub_verify_many: one host thread + primary context + stream per GPU, no
     peer access, no collective; check="tagged": ccm_scrub_verify_many_tagged; residue=True:
     ccm_scrub_verify_many_residue, each report with its `.residue`; triage=True: every GPU armed for the dirt
     triage, as in NvidiaDevice.scrub_and_verify; mismatch_triage=True: every GPU armed for the mismatch triage, as
     there; prove=True: every GPU armed for the coverage proof, and a GPU that cannot be armed is not scrubbed: its
-    report carries the arming's status; probe=True: every GPU armed for the alias probe, likewise).  Returns
+    report carries the arming's status; probe=True: every GPU armed for the alias probe, likewise; health="report" or
+    "require": every GPU armed for the HBM health report, likewise, each report with its `.health`).  Returns
     (reports, wall_ms); never raises for a per-device failure — inspect report.status /
     report.clean."""
     tagged = _check_mode(check)
     _mismatch_triage_check(mismatch_triage, check)
     _probe_check(probe, check)
-    if prove or probe:
+    hmode = _health_mode(health)
+    if prove or probe or hmode:
         # every check asked for is armed on a device before it is scrubbed; a device that refuses one is not scrubbed
         # (its report carries that arming's status, and no report of a call that did not run)
-        arms = [arm for on, arm in ((prove, _arm_prove), (probe, _arm_probe)) if on]
+        arm_health = lambda ordinal, on: _arm_health(ordinal, hmode if on else 0)   # noqa: E731
+        arms = [arm for on, arm in ((prove, _arm_prove), (probe, _arm_probe), (hmode, arm_health)) if on]
         refused, armed = {}, []
         try:
             for d in devices:
@@ -1272,6 +1452,8 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
                 rep.status = N.ERR_UNCOVERED   # a probe proof that was asked for and did not run
             if prove:
                 _attach_report_cover(rep, d.cuda_ordinal)
+            if hmode:
+                _attach_health(rep, d.cuda_ordinal, hmode)
         return reports, wall
     n = len(devices)
     if n == 0:
@@ -1353,12 +1535,17 @@ class ScrubbingProxy:
 
     def scrub_and_verify(self, nbytes: int = 0, check: str = "zero", residue: bool = False, triage: bool = False,
                          triage_hold_ms: int = TRIAGE_HOLD_MS, mismatch_triage: bool = False,
-                         prove: bool = False, probe: bool = False) -> ScrubReport:
+                         prove: bool = False, probe: bool = False, health: str = "off") -> ScrubReport:
         native = object.__getattribute__(self, "_native")
         _mismatch_triage_check(mismatch_triage, check)
         _probe_check(probe, check)
+        _health_mode(health)
         if native is None:
             raise GpuError(f"no CUDA device with PCI address {self._foreign.bdf}: HBM scrub cannot run", N.ERR_NO_CUDA)
+        if health != "off":
+            return native.scrub_and_verify(nbytes, check=check, residue=residue, triage=triage,
+                                           triage_hold_ms=triage_hold_ms, mismatch_triage=mismatch_triage, prove=prove,
+                                           probe=probe, health=health)
         if probe:
             return native.scrub_and_verify(nbytes, check=check, residue=residue, triage=triage,
                                            triage_hold_ms=triage_hold_ms, mismatch_triage=mismatch_triage, prove=prove,

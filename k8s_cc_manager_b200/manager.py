@@ -65,6 +65,7 @@ RESIDUE_MODES = ("off", "report")   # CC_SCRUB_RESIDUE
 TRIAGE_MODES = ("off", "report")    # CC_SCRUB_TRIAGE, CC_SCRUB_MISMATCH_TRIAGE
 PROOF_MODES = ("off", "require")    # CC_SCRUB_PROOF
 ALIAS_PROBE_MODES = ("off", "require")   # CC_SCRUB_ALIAS_PROBE
+HBM_HEALTH_MODES = ("off", "report", "require")   # CC_SCRUB_HBM_HEALTH
 # How long the dirt and mismatch triages wait before their last re-read of the pages they re-wrote: long enough for an
 # agent that still writes this GPU's memory to show itself, short against a transition.
 SCRUB_TRIAGE_HOLD_MS = 100
@@ -112,7 +113,7 @@ class CCManager:
                  max_parallel: Optional[int] = None, scrub_check: Optional[str] = None,
                  scrub_residue: Optional[str] = None, scrub_triage: Optional[str] = None,
                  scrub_mismatch_triage: Optional[str] = None, scrub_proof: Optional[str] = None,
-                 scrub_alias_probe: Optional[str] = None):
+                 scrub_alias_probe: Optional[str] = None, scrub_hbm_health: Optional[str] = None):
         env = os.environ
         self.operator_namespace = env.get("OPERATOR_NAMESPACE", "gpu-operator")
         self.evict_operator_components = env.get("EVICT_OPERATOR_COMPONENTS", "true").lower() == "true"
@@ -197,6 +198,16 @@ class CCManager:
         if self.scrub_alias_probe == "require" and self.scrub_check == "tagged":
             raise ValueError("CC_SCRUB_ALIAS_PROBE=require probes the zero gate; CC_SCRUB_CHECK=tagged already checks "
                              "every probe window: use one or the other")
+        # off:     the gate judges HBM only by what its kernels read back, and ECC corrects a flipped cell on its way to
+        #          them: a memory fault during the gate goes unseen.
+        # report:  the gate also reads the GPU's ECC counters and row-remapping state through NVML before and after its
+        #          passes (ccm_scrub_health, DESIGN.md §5m).  Logged and kept in last_transition["scrub_hbm_health"].
+        # require: a GPU whose uncorrected error count rose during the gate, whose row remap is pending (it needs another
+        #          reset before it holds a tenant's data) or failed (RMA), whose ECC is off, or whose state could not be
+        #          read, fails the gate.  A check, not a report: a device without the report fails the gate.
+        self.scrub_hbm_health = (scrub_hbm_health or env.get("CC_SCRUB_HBM_HEALTH", "off")).lower()
+        if self.scrub_hbm_health not in HBM_HEALTH_MODES:
+            raise ValueError(f"CC_SCRUB_HBM_HEALTH must be 'off', 'report' or 'require', not {self.scrub_hbm_health!r}")
         self.max_parallel = int(max_parallel if max_parallel is not None else env.get("CC_MAX_PARALLEL", "0"))
         # "full-HBM" is enforced, not assumed: when scrubbing everything (scrub_bytes == 0) a GPU on
         # which less than this fraction of DEVICE memory was zeroed and read back fails the gate
@@ -590,6 +601,8 @@ class CCManager:
             cmd += ["--prove"]
         if self.alias_probe:
             cmd += ["--probe"]
+        if self.scrub_hbm_health != "off":
+            cmd += ["--health", self.scrub_hbm_health]
         for gpu in gpus:
             cmd += ["--bdf", gpu.bdf]
         env = dict(os.environ)
@@ -611,6 +624,10 @@ class CCManager:
     def alias_probe(self) -> bool:
         return self.scrub_alias_probe == "require"
 
+    @property
+    def hbm_health_required(self) -> bool:
+        return self.scrub_hbm_health == "require"
+
     def _scrub_call(self, gpu, **kwargs):
         """The one call every per-device gate path makes: with CC_SCRUB_PROOF=require it also asks for the coverage
         proof, with CC_SCRUB_ALIAS_PROBE=require for the alias probe.  A device whose scrub_and_verify cannot take
@@ -629,6 +646,16 @@ class CCManager:
             except (TypeError, ValueError):
                 raise ScrubFailure(f"device {gpu.bdf} cannot probe its HBM for pages mapped twice "
                                    "(CC_SCRUB_ALIAS_PROBE=require); refusing to release it") from None
+        if self.scrub_hbm_health != "off":
+            try:
+                inspect.signature(gpu.scrub_and_verify).bind(self.scrub_bytes, **kwargs, health=self.scrub_hbm_health)
+                kwargs["health"] = self.scrub_hbm_health
+            except (TypeError, ValueError):
+                if self.hbm_health_required:
+                    raise ScrubFailure(f"device {gpu.bdf} cannot report its HBM health (CC_SCRUB_HBM_HEALTH=require); "
+                                       "refusing to release it") from None
+                logger.warning("Device %s cannot report its HBM health (CC_SCRUB_HBM_HEALTH=report): its gate runs "
+                               "without it", gpu.bdf)
         return gpu.scrub_and_verify(self.scrub_bytes, **kwargs)
 
     def _scrub_many(self, natives: list, **kwargs):
@@ -638,6 +665,8 @@ class CCManager:
             kwargs["prove"] = True
         if self.alias_probe:
             kwargs["probe"] = True
+        if self.scrub_hbm_health != "off":
+            kwargs["health"] = self.scrub_hbm_health
         return _devices.scrub_and_verify_many(natives, self.scrub_bytes, **kwargs)
 
     def _scrub_checked(self, gpu):
@@ -764,6 +793,11 @@ class CCManager:
             self.last_transition.setdefault("scrub_probe_cover", {})[bdf] = probe_cover
             logger.log(logging.INFO if probe_cover.covered else logging.ERROR, "HBM alias probe proof on %s: %s", bdf,
                        probe_cover.summary())
+        health = getattr(holder, "health", None)
+        if health is not None:
+            self.last_transition.setdefault("scrub_hbm_health", {})[bdf] = health
+            level = logging.INFO if health.fit else logging.ERROR if self.hbm_health_required else logging.WARNING
+            logger.log(level, "HBM health on %s: %s", bdf, health.summary())
         report_cover = getattr(holder, "report_cover", None)
         if report_cover is not None:
             self.last_transition.setdefault("scrub_report_cover", {})[bdf] = report_cover
@@ -829,6 +863,13 @@ class CCManager:
         for rep in reports:
             self._note_reports(rep.bdf, rep)
         for rep in reports:
+            if self.hbm_health_required:   # the hardware's record comes first: it explains any count below
+                health = getattr(rep, "health", None)
+                if health is None:
+                    raise ScrubFailure(f"HBM scrub on {rep.bdf} carries no HBM health report "
+                                       "(CC_SCRUB_HBM_HEALTH=require); refusing to release it")
+                if not health.fit:
+                    raise ScrubFailure(f"HBM health on {rep.bdf} is {health.verdict_name}: " + "; ".join(health.why()))
             mismatch = getattr(rep, "mismatch_bytes", 0)
             probe_cover = getattr(rep, "probe_cover", None)
             probe_short = probe_cover is not None and not (probe_cover.proved and probe_cover.covered)
@@ -1124,6 +1165,11 @@ def build_arg_parser() -> argparse.ArgumentParser:
                         help="require: after a clean read-back, the zero gate tags, checks and re-reads one 32-byte "
                              "window per 4 KiB page, and a GPU with a page mapped twice fails the gate (not with "
                              "--scrub-check tagged; default: $CC_SCRUB_ALIAS_PROBE or off)")
+    parser.add_argument("--scrub-hbm-health", default=None, choices=HBM_HEALTH_MODES,
+                        help="report: read the GPUs' ECC counters and row-remapping state before and after the gate; "
+                             "require: a GPU whose memory failed during the gate, with a pending or failed row remap, "
+                             "ECC off, or a state that cannot be read fails the gate (default: $CC_SCRUB_HBM_HEALTH or "
+                             "off)")
     return parser
 
 
@@ -1150,7 +1196,7 @@ def main(argv: Optional[List[str]] = None) -> None:
                   kubeconfig=args.kubeconfig, scrub_mode=args.scrub_mode, scrub_check=args.scrub_check,
                   scrub_residue=args.scrub_residue, scrub_triage=args.scrub_triage,
                   scrub_mismatch_triage=args.scrub_mismatch_triage, scrub_proof=args.scrub_proof,
-                  scrub_alias_probe=args.scrub_alias_probe,
+                  scrub_alias_probe=args.scrub_alias_probe, scrub_hbm_health=args.scrub_hbm_health,
                   device_source=_device_source_from_env()).run()
     except KeyboardInterrupt:
         logger.info("Shutting down...")

@@ -12,7 +12,8 @@ Output (stdout, last line):  {"wall_ms": ..., "reports": [ {ScrubReport fields},
 GPU whose read-back found non-zero bytes; "mismatch_triage" only with --mismatch-triage, for a GPU whose tagged check
 found bytes off their tags; "cover" only with --prove, for every GPU whose passes finished; "probe" only with --probe,
 for every GPU whose alias probe ran; "probe_cover" only with --prove and --probe, for every GPU whose alias probe ran;
-"report_cover" only with --prove, for every GPU that located dirt or triaged).
+"report_cover" only with --prove, for every GPU that located dirt or triaged; "hbm_health" only with --health report
+or --health require, for every GPU that was armed).
 Exit code: 0 if every GPU is clean, 3 if the gate failed, 2 on usage errors.
 """
 from __future__ import annotations
@@ -27,15 +28,23 @@ from . import devices as D
 
 
 def run(bdfs: List[str], nbytes: int, check: str = "zero", residue: bool = False, triage_hold_ms: int = 0,
-        mismatch_triage_hold_ms: int = 0, prove: bool = False, probe: bool = False) -> dict:
+        mismatch_triage_hold_ms: int = 0, prove: bool = False, probe: bool = False, health: str = "off") -> dict:
     """triage_hold_ms > 0 arms the dirt triage with that hold, mismatch_triage_hold_ms > 0 the mismatch triage (with
-    the same hold when both are armed); prove arms the coverage proof, probe the alias probe."""
+    the same hold when both are armed); prove arms the coverage proof, probe the alias probe, health ('report' or
+    'require') the HBM health report."""
     by_bdf = {d.bdf: d for d in D.find_gpus()[0] if d.is_gpu()}
     missing = [b for b in bdfs if b not in by_bdf]
     if missing:
         raise SystemExit(f"unknown GPU(s): {', '.join(missing)} (known: {', '.join(sorted(by_bdf))})")
     devs = [by_bdf[b] for b in bdfs]
-    if probe:
+    if health != "off":
+        reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check, residue=residue,
+                                                   triage=bool(triage_hold_ms),
+                                                   triage_hold_ms=mismatch_triage_hold_ms or triage_hold_ms or
+                                                   D.TRIAGE_HOLD_MS,
+                                                   mismatch_triage=bool(mismatch_triage_hold_ms), prove=prove,
+                                                   probe=probe, health=health)
+    elif probe:
         reports, wall_ms = D.scrub_and_verify_many(devs, nbytes, check=check, residue=residue,
                                                    triage=bool(triage_hold_ms),
                                                    triage_hold_ms=mismatch_triage_hold_ms or triage_hold_ms or
@@ -83,6 +92,9 @@ def main(argv: Optional[List[str]] = None) -> int:
     ap.add_argument("--probe", action="store_true",
                     help="with --check zero, after a clean read-back, tag, check and re-read one 32-byte window per 4 KiB "
                          "page; a GPU with a page mapped twice fails the gate")
+    ap.add_argument("--health", choices=tuple(N.HBM_HEALTH_MODES), default="off",
+                    help="read the GPU's ECC counters and row-remapping state before and after the gate; require: a GPU "
+                         "whose memory failed during the gate, or whose state cannot be read, fails the gate")
     ap.add_argument("--triage-hold-ms", type=int, default=D.TRIAGE_HOLD_MS,
                     help="the triages' hold before their last re-read (default %(default)s)")
     args = ap.parse_args(argv)
@@ -96,7 +108,7 @@ def main(argv: Optional[List[str]] = None) -> int:
         D.select_backend(args.backend)
     out = run([b.lower() for b in args.bdf], args.bytes, args.check, args.residue,
               args.triage_hold_ms if args.triage else 0, args.triage_hold_ms if args.mismatch_triage else 0,
-              args.prove, args.probe)
+              args.prove, args.probe, args.health)
     print(json.dumps(out), flush=True)
     return 0 if all(r["status"] == 0 and r["nonzero_bytes"] == 0 and r.get("mismatch_bytes", 0) == 0
                     for r in out["reports"]) else 3
