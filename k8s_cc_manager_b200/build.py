@@ -45,20 +45,26 @@ def needs_build() -> bool:
     return any(p.stat().st_mtime > built for p in SOURCES + HEADERS + [CLI_SOURCE, Path(__file__)])
 
 
-def build(force: bool = False, verbose: bool = False) -> Path:
-    if not force and not needs_build():
-        return LIB_PATH
-    cmd = [find_nvcc(), *NVCC_FLAGS, "-I", str(REPO_ROOT / "include"), "-I", str(CSRC)]
+def compile_lib(src_dir: Path, include_dir: Path, out: Path, verbose: bool = False) -> Path:
+    """libccm.so from the sources under src_dir (laid out as csrc/) and include_dir, with the product's flags."""
+    cmd = [find_nvcc(), *NVCC_FLAGS, "-I", str(include_dir), "-I", str(src_dir)]
     if verbose:
         cmd += ["-Xptxas", "-v"]
-    cmd += [str(s) for s in SOURCES]
-    cmd += ["-o", str(LIB_PATH), "-ldl", "-lpthread"]
+    cmd += [str(src_dir / s.name) for s in SOURCES]
+    cmd += ["-o", str(out), "-ldl", "-lpthread"]
     proc = subprocess.run(cmd, capture_output=True, text=True)
     if proc.returncode != 0:
         sys.stderr.write(proc.stdout + proc.stderr)
-        raise RuntimeError(f"nvcc failed ({proc.returncode}) building {LIB_PATH}")
+        raise RuntimeError(f"nvcc failed ({proc.returncode}) building {out}")
     if verbose:
         sys.stderr.write(proc.stderr)
+    return out
+
+
+def build(force: bool = False, verbose: bool = False) -> Path:
+    if not force and not needs_build():
+        return LIB_PATH
+    compile_lib(CSRC, REPO_ROOT / "include", LIB_PATH, verbose)
     # native CLI front end (ccm-scrub): plain host C++, finds libccm.so next to itself
     gxx = shutil.which("g++") or "g++"
     cli = subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-I", str(REPO_ROOT / "include"), str(CLI_SOURCE),

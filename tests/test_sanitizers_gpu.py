@@ -22,9 +22,13 @@ and say so, and any other failure of that probe fails them.
 
 Open: no tool run has been measured yet, on any device.  The plain profiled run, which checks every result exactly,
 took 30 s on that H100.  The wall time of each tool's run is printed with its result and belongs here, beside the GPU
-and power limit it was measured at, once a device the tool instruments has run them; so do the two mutation checks each
-run exists for (racecheck must fail with the barrier between the writes and reads of `part` in WindowBook::flush
-dropped; memcheck must fail with ragged_bytes walking one byte past the tail).  TIMEOUT is a bound, not a measurement:
+and power limit it was measured at, once a device the tool instruments has run them.  That the driver's exact checks
+fail when a kernel is subtly wrong is shown without a sanitizer: tests/test_kernel_mutants.py runs the driver against
+copies of libccm.so with one value or loop-narrowing bug each, and requires it to fail on every one.  The two mutation
+checks each tool run exists for stay open (racecheck must fail with the barrier between the writes and reads of `part`
+in WindowBook::flush dropped; memcheck must fail with ragged_bytes walking one byte past the tail): both mutants race or
+access out of bounds on purpose, which a shared GPU must not be asked to run, and the tools do not instrument the H100
+that runs this suite (see above).  TIMEOUT is a bound, not a measurement:
 a run that reaches it fails, names itself and asks for smaller regions.  The regions stay at the sizes their tiling
 edges need (at most 34 MiB: every grabber of the default-frame kernels takes two grabs) and the product calls at a few
 2 MiB chunks, to keep the instrumented runs to minutes.
