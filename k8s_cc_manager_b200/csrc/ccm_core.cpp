@@ -822,6 +822,14 @@ static int sim_apply(Device& d, const std::string& k, int64_t v) {
     if (v < 0 || v > CCM_PASS_READBACK) { set_error("sim key 'cover_pass' takes 0..3, not %lld", (long long)v); return CCM_ERR_INVALID; }
     d.drill.cover_pass = v == 0 ? (int)CCM_PASS_READBACK : (int)v;
   }
+  else if (k == "cover_repeat") {
+    if (v < 0 || v > 15) { set_error("sim key 'cover_repeat' takes 0..15, not %lld", (long long)v); return CCM_ERR_INVALID; }
+    d.drill.cover_repeat = (uint32_t)v;
+  }
+  else if (k == "cover_lane_drop") {
+    if (v < 0 || v > 512) { set_error("sim key 'cover_lane_drop' takes 0..512, not %lld", (long long)v); return CCM_ERR_INVALID; }
+    d.drill.cover_lane_drop = (uint32_t)v;
+  }
   else if (k == "scrub_poison" || k == "scrub_flood" || k == "tag_flood") {
     if (v < 0 || v > 255) { set_error("sim key '%s' takes a byte value (0 = off), not %lld", k.c_str(), (long long)v); return CCM_ERR_INVALID; }
     (k == "scrub_poison" ? d.drill.poison : k == "scrub_flood" ? d.drill.flood : d.drill.tag_flood) = (int)v;
@@ -872,6 +880,8 @@ int ccm_sim_get(int dev, const char* key, int64_t* value) {
     else if (k == "tag_flood") *value = d.drill.tag_flood;
     else if (k == "cover_skip") *value = (int64_t)d.drill.cover_skip;
     else if (k == "cover_pass") *value = d.drill.cover_pass;
+    else if (k == "cover_repeat") *value = d.drill.cover_repeat;
+    else if (k == "cover_lane_drop") *value = d.drill.cover_lane_drop;
     else if (k == "probe_mismatch") *value = (int64_t)d.drill.probe_mismatch;
     else if (k == "probe_dirt") *value = (int64_t)d.drill.probe_dirt;
     else if (k == "probe_skip") *value = (int64_t)d.drill.probe_skip;

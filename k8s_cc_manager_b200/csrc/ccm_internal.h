@@ -59,6 +59,9 @@ int engine_arena_rw(ScrubEngine*, uint64_t offset, void* host, uint64_t bytes, b
 // Drill of the coverage proof (sim keys "cover_skip", "cover_pass"; ccm.h), armed or not:
 //   cover_skip:    that many is written into the grab word of the first default-frame launch of pass cover_pass
 //                  (CCM_PASS_*; the sim key's 0 is stored as CCM_PASS_READBACK), just before it on the stream.
+// Drills of the coverage ledger (sim keys "cover_repeat", "cover_lane_drop"; ccm.h), on pass cover_pass:
+//   cover_repeat:    k: the first page-aligned launch of at least a page is enqueued as three, repeating k chunks;
+//   cover_lane_drop: t + 1: in a proven call, thread t skips its share of chunk 0 of the first launch.
 // Drills of the alias probe (sim keys "probe_mismatch", "probe_dirt"; ccm.h), only in a call that probes:
 //   probe_mismatch: the first byte of each of the first that many probe windows is XORed between P1 and P2;
 //   probe_dirt:     the same bytes, between P2 and P3.
@@ -83,6 +86,8 @@ struct ScrubDrill {
   int tag_flood = 0;
   uint64_t cover_skip = 0;
   int cover_pass = CCM_PASS_READBACK;
+  uint32_t cover_repeat = 0;
+  uint32_t cover_lane_drop = 0;
   uint64_t probe_mismatch = 0;
   uint64_t probe_dirt = 0;
   uint64_t probe_skip = 0;

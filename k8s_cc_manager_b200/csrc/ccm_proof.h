@@ -2,7 +2,7 @@
 // ccm_cover_report, ccm_probe_cover, ccm_report_cover).  Plain C++17, no CUDA: a CPU test compiles it on its own.
 // A cover map is np words, word p the bytes counted on the 2 MiB page p from the call's va_base, then the outside slot
 // (bytes counted before va_base or past the last page).  A proof requires every page to count exactly what the call
-// expects on it, and the outside slot 0.
+// expects on it, and the outside slot 0.  The coverage ledger (ccm_cover_ledger) is the same per 128 KiB slot.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -167,6 +167,59 @@ void fill_cover(const uint32_t* maps, uint64_t np, const std::vector<Span>& span
     put_bytes(&rep->pass[k], t[k]);
   }
   rep->covered = t[0].exact() && t[1].exact() && t[2].exact();
+}
+
+constexpr uint64_t kSlotBytes = CCM_LEDGER_SLOT_BYTES;
+
+// The coverage ledger of a call that mapped bytes_mapped from va_base: `ledgers` are the three passes' ledgers, ns + 1
+// words each (ns slots, then the outside slot), end to end; ran[k] says pass k ran.  Every pass that ran must count
+// min(kSlotBytes, bytes_mapped - s * kSlotBytes) on every slot s of [0, bytes_mapped), 0 on every other slot and 0 in
+// the outside slot.  Fills *rep (proved = 1; ms_ledger is the caller's) and *slots, one entry per slot inexact in any
+// pass that ran, ascending.
+inline void fill_ledger(const uint32_t* ledgers, uint64_t ns, uint64_t bytes_mapped, uint64_t va_base, const bool ran[3],
+                        const ChunkTable& chunks, ccm_cover_ledger* rep, std::vector<ccm_ledger_slot>* slots) {
+  memset(rep, 0, sizeof *rep);
+  rep->bytes_mapped = bytes_mapped;
+  rep->slots_mapped = (bytes_mapped + kSlotBytes - 1) / kSlotBytes;
+  rep->va_base = va_base;
+  rep->proved = 1;
+  rep->exact = 1;
+  slots->clear();
+  for (uint64_t s = 0; s < ns; ++s) {
+    const uint32_t want = s * kSlotBytes < bytes_mapped ? (uint32_t)std::min(kSlotBytes, bytes_mapped - s * kSlotBytes) : 0u;
+    bool bad = false;
+    for (int k = 0; k < 3; ++k) {
+      if (!ran[k]) continue;
+      const uint32_t got = ledgers[k * (ns + 1) + s];
+      if (got == want) continue;
+      bad = true;
+      ccm_ledger_pass& p = rep->pass[k];
+      if (got < want) {
+        if (p.slots_short++ == 0) p.first_short_slot = s;
+        p.bytes_missing += want - got;
+      } else {
+        if (p.slots_over++ == 0) p.first_over_slot = s;
+        p.bytes_extra += got - want;
+      }
+    }
+    if (!bad) continue;
+    ccm_ledger_slot e;
+    memset(&e, 0, sizeof e);
+    e.slot = s;
+    e.chunk = chunk_of(chunks, s * kSlotBytes);
+    e.expected = want;
+    for (int k = 0; k < 3; ++k)
+      if (ran[k]) e.count[k] = ledgers[k * (ns + 1) + s];
+    slots->push_back(e);
+  }
+  for (int k = 0; k < 3; ++k) {
+    ccm_ledger_pass& p = rep->pass[k];
+    p.ran = ran[k];
+    if (!ran[k]) continue;
+    p.bytes_outside = ledgers[k * (ns + 1) + ns];
+    p.bytes_extra += p.bytes_outside;
+    if (p.bytes_missing || p.bytes_extra) rep->exact = 0;
+  }
 }
 
 inline uint64_t windows(uint64_t bytes) { return (bytes + kProbeWindow - 1) / kProbeWindow; }

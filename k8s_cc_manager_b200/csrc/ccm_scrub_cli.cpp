@@ -19,7 +19,8 @@
 // ccm_last_cover_pages report it; "probe" with --probe, which refuses --check tagged and arms every GPU for the alias
 // probe (ccm_scrub_probe), for every GPU whose probe ran, as ccm_scrub_last_probe reports it, with "mismatch" when it
 // found bytes off their tags); "probe_cover" with --prove and --probe, for every GPU whose probe ran, as
-// ccm_scrub_last_probe_cover and ccm_last_probe_cover_pages report it; "report_cover" with --prove, for every GPU that
+// ccm_scrub_last_probe_cover and ccm_last_probe_cover_pages report it; "cover_ledger" with --prove, for every GPU whose
+// passes finished, as ccm_scrub_last_ledger and ccm_last_ledger_slots report it; "report_cover" with --prove, for every GPU that
 // located dirt or triaged, as ccm_scrub_last_report_cover and ccm_last_report_cover_pages report it; "hbm_health" with
 // --health report or --health require, which arms every GPU for the HBM health report (ccm_scrub_health), as
 // ccm_scrub_last_health reports it (under require, a GPU armed and without one gets CCM_ERR_HBM_HEALTH).  With --prove,
@@ -279,6 +280,36 @@ static int usage(const char* argv0) {
   return 2;
 }
 
+// The "cover_ledger" object: the fields of k8s_cc_manager_b200.devices.CoverLedger, with the first 64 inexact slots.
+static void print_ledger(const ccm_cover_ledger& l, int ordinal) {
+  static const char* const names[3] = {"first", "check", "readback"};
+  printf(", \"cover_ledger\": {\"bytes_mapped\": %llu, \"slots_mapped\": %llu, \"va_base\": %llu, \"ms_ledger\": %.3f, "
+         "\"proved\": %d, \"exact\": %d, \"passes\": [",
+         (unsigned long long)l.bytes_mapped, (unsigned long long)l.slots_mapped, (unsigned long long)l.va_base,
+         l.ms_ledger, l.proved, l.exact);
+  for (int k = 0; k < 3; ++k) {
+    const ccm_ledger_pass& p = l.pass[k];
+    printf("%s{\"name\": \"%s\", \"ran\": %d, \"slots_short\": %llu, \"slots_over\": %llu, \"bytes_missing\": %llu, "
+           "\"bytes_extra\": %llu, \"bytes_outside\": %llu, \"first_short_slot\": %llu, \"first_over_slot\": %llu}",
+           k ? ", " : "", names[k], p.ran, (unsigned long long)p.slots_short, (unsigned long long)p.slots_over,
+           (unsigned long long)p.bytes_missing, (unsigned long long)p.bytes_extra, (unsigned long long)p.bytes_outside,
+           (unsigned long long)p.first_short_slot, (unsigned long long)p.first_over_slot);
+  }
+  printf("], \"slots\": [");
+  uint64_t n = 0;
+  std::vector<ccm_ledger_slot> v;
+  if (!l.exact && ccm_last_ledger_slots(ordinal, nullptr, 0, &n) == CCM_OK) {
+    v.resize(n);
+    if (n && ccm_last_ledger_slots(ordinal, v.data(), n, &n) != CCM_OK) v.clear();
+  }
+  const size_t keep = 64;   // k8s_cc_manager_b200.devices.LEDGER_SLOTS
+  for (size_t k = 0; k < v.size() && k < keep; ++k)
+    printf("%s{\"slot\": %llu, \"chunk\": %u, \"expected\": %u, \"first\": %u, \"check\": %u, \"readback\": %u}",
+           k ? ", " : "", (unsigned long long)v[k].slot, v[k].chunk, v[k].expected, v[k].count[0], v[k].count[1],
+           v[k].count[2]);
+  printf("], \"slots_truncated\": %d}", v.size() > keep);
+}
+
 // The "report_cover" object: the fields of k8s_cc_manager_b200.devices.ReportCoverReport, with the first 64 inexact
 // (step, page) entries.
 static void print_rcover(const ccm_report_cover& c, int ordinal) {
@@ -494,7 +525,10 @@ int main(int argc, char** argv) {
     ccm_cover_report c;
     const bool proved = prove && ccm_scrub_last_cover(ordinals[i], &c) == CCM_OK && c.proved;
     if (proved) print_cover(c, ordinals[i]);
-    clean = clean && (!prove || proved);   // a proof that was asked for and did not run fails the gate
+    ccm_cover_ledger lg;
+    const bool ledgered = proved && ccm_scrub_last_ledger(ordinals[i], &lg) == CCM_OK && lg.proved;
+    if (ledgered) print_ledger(lg, ordinals[i]);
+    clean = clean && (!prove || (proved && ledgered));   // a proof that was asked for and did not run fails the gate
     if (ran_probe) print_probe(pr);
     if (probe_proved) print_pcover(pc, ordinals[i]);
     ccm_report_cover rc;

@@ -33,7 +33,8 @@ class GpuError(Exception):
     MismatchReport as `.mismatch`; a census call carries its ResidueReport (what the first pass erased) as
     `.residue`; a triage call that read back dirt carries its TriageReport (what kind of dirt) as `.triage`; a mismatch
     triage call whose tagged check failed carries its TriageReport (what kind of mismatch) as `.mismatch_triage`; a
-    proving call carries its CoverReport (how many bytes each pass walked on every page) as `.cover`; a probing call
+    proving call carries its CoverReport (how many bytes each pass walked on every page) as `.cover` and its
+    CoverLedger (how many bytes every thread of each pass addressed on every 128 KiB slot) as `.ledger`; a probing call
     carries its ProbeReport (what the alias probe found) as `.probe`; a call both proving and probing carries its
     ProbeCoverReport (how many windows each probe step took on every page) as `.probe_cover`; a proving call that
     located dirt or triaged carries its ReportCoverReport (how many bytes the locate pass and each triage step walked on
@@ -640,6 +641,115 @@ def last_cover(cuda_ordinal: int) -> "Optional[CoverReport]":
     return CoverReport._last(cuda_ordinal, "ccm_scrub_last_cover", N.CoverReport, last_cover_pages)
 
 
+LEDGER_SLOTS = 64   # inexact slots a CoverLedger keeps
+
+
+@dataclass
+class LedgerSlot:
+    """One 128 KiB slot some pass of a proving call did not count exactly (include/ccm.h: ccm_ledger_slot)."""
+    slot: int
+    chunk: int
+    expected: int      # bytes every pass that ran had to count on it
+    first: int         # bytes the first pass, the tagged check and the read-back counted
+    check: int
+    readback: int
+
+    def describe(self) -> str:
+        return (f"slot {self.slot} (chunk {self.chunk}): expected {self.expected}, first {self.first}, "
+                f"check {self.check}, read-back {self.readback}")
+
+
+@dataclass
+class LedgerPass:
+    """What one pass counted per slot against what the call mapped (include/ccm.h: ccm_ledger_pass)."""
+    name: str          # "first", "check" or "readback"
+    ran: int
+    slots_short: int
+    slots_over: int
+    bytes_missing: int
+    bytes_extra: int
+    bytes_outside: int
+    first_short_slot: int
+    first_over_slot: int
+
+
+@dataclass
+class CoverLedger:
+    """The coverage ledger of one proving call (include/ccm.h: ccm_cover_ledger): every thread of every pass counted on
+    the device the bytes it addressed on each 128 KiB slot, and `exact` says each pass that ran walked every slot
+    exactly once.  A call can fail on its ledger while its CoverReport is covered (a chunk walked twice and another on
+    the same page skipped).  `slots` are the first LEDGER_SLOTS inexact slots."""
+    bytes_mapped: int
+    slots_mapped: int
+    va_base: int
+    ms_ledger: float
+    proved: int
+    exact: int
+    passes: List[LedgerPass] = field(default_factory=list)
+    slots: List[LedgerSlot] = field(default_factory=list)
+    slots_truncated: int = 0
+
+    @classmethod
+    def from_native(cls, r, slots=None) -> "CoverLedger":
+        passes = [LedgerPass(name, **{f: getattr(p, f) for f, _ in p._fields_ if f != "reserved"})
+                  for name, p in zip(N.COVER_PASSES, r.passes)]
+        slots = slots or []
+        return cls(r.bytes_mapped, r.slots_mapped, r.va_base, r.ms_ledger, r.proved, r.exact, passes,
+                   slots[:LEDGER_SLOTS], int(len(slots) > LEDGER_SLOTS))
+
+    @classmethod
+    def from_json(cls, d: dict) -> "CoverLedger":
+        return cls(**{**d, "passes": [LedgerPass(**p) for p in d["passes"]],
+                      "slots": [LedgerSlot(**x) for x in d["slots"]]})
+
+    def as_json(self) -> dict:
+        return dataclasses.asdict(self)
+
+    def inexact_pass(self) -> "Optional[LedgerPass]":
+        """The first pass that ran and did not count every slot exactly (None when exact)."""
+        return next((p for p in self.passes if p.ran and (p.bytes_missing or p.bytes_extra)), None)
+
+    def summary(self, first: int = 4) -> str:
+        """One line for an operator: what was mapped and, when a pass was inexact, which one and on which slots."""
+        line = f"{self.bytes_mapped} bytes on {self.slots_mapped} slots of 128 KiB"
+        bad = self.inexact_pass()
+        if bad is None:
+            return line + ": every pass walked every slot once (" + ", ".join(p.name for p in self.passes if p.ran) + ")"
+        line += (f": the {bad.name} pass has {bad.slots_short} slots short and {bad.slots_over} over "
+                 f"({bad.bytes_missing} bytes missing, {bad.bytes_extra} extra, {bad.bytes_outside} outside)")
+        if not self.slots:
+            return line
+        more = " (+more)" if self.slots_truncated or len(self.slots) > first else ""
+        return line + "; " + "; ".join(x.describe() for x in self.slots[:first]) + more
+
+
+def last_ledger_slots(cuda_ordinal: int) -> "Optional[List[LedgerSlot]]":
+    """The inexact slots of the last proving call on a CUDA device (include/ccm.h: ccm_last_ledger_slots), ascending;
+    None when they cannot be read."""
+    slots = _read_pages("ccm_last_ledger_slots", N.LedgerSlot, cuda_ordinal)
+    return None if slots is None else [LedgerSlot(x.slot, x.chunk, x.expected, *x.count) for x in slots]
+
+
+def last_ledger(cuda_ordinal: int) -> "Optional[CoverLedger]":
+    """The coverage ledger of the last product call on a CUDA device (include/ccm.h: ccm_scrub_last_ledger), with its
+    first inexact slots; None when it cannot be read."""
+    out = N.CoverLedger()
+    if cuda_ordinal < 0 or N.lib().ccm_scrub_last_ledger(cuda_ordinal, C.byref(out)) != N.OK:
+        return None
+    return CoverLedger.from_native(out, last_ledger_slots(cuda_ordinal) if out.proved and not out.exact else None)
+
+
+def _attach_ledger(rep: "ScrubReport", cuda_ordinal: int) -> bool:
+    """Attaches the coverage ledger of a proving call as `.ledger`; False when it cannot be read or did not run (the
+    call then fails with ERR_UNCOVERED, as a probe proof that did not run does).  A stand-in library without
+    ccm_scrub_last_ledger has no ledger to give."""
+    if not hasattr(N.lib(), "ccm_scrub_last_ledger"):
+        return True
+    ledger = last_ledger(cuda_ordinal)
+    rep.ledger = ledger if ledger is not None and ledger.proved else None
+    return rep.ledger is not None
+
+
 def _arm_prove(cuda_ordinal: int, on: bool) -> int:
     """Arms or disarms the coverage proof on a CUDA device; the library's status (a call that asked for the proof and
     could not arm it fails with it: it is never run unproven)."""
@@ -1056,9 +1166,10 @@ def _attach_health(rep: "ScrubReport", cuda_ordinal: int, mode: int) -> None:
 # The reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
 _REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport),
             ("mismatch_triage", TriageReport), ("cover", CoverReport), ("probe", ProbeReport),
-            ("probe_cover", ProbeCoverReport), ("report_cover", ReportCoverReport), ("health", HbmHealth))
+            ("probe_cover", ProbeCoverReport), ("report_cover", ReportCoverReport), ("health", HbmHealth),
+            ("ledger", CoverLedger))
 # The JSON key of a report whose attribute is not its key.
-_JSON_KEYS = {"health": "hbm_health"}
+_JSON_KEYS = {"health": "hbm_health", "ledger": "cover_ledger"}
 
 
 @dataclass
@@ -1118,6 +1229,9 @@ class ScrubReport:
     # The GPU's ECC and row-remapping state before and after the call (an HbmHealth), set for every report of a call
     # armed for it (health="report" or "require").  Not a dataclass field either; its JSON key is "hbm_health".
     health = None
+    # How many bytes every thread of each pass addressed on every 128 KiB slot (a CoverLedger), set for every report of
+    # a proving call (prove=True) whose passes finished.  Not a dataclass field either; its JSON key is "cover_ledger".
+    ledger = None
 
     @property
     def clean(self) -> bool:
@@ -1348,8 +1462,11 @@ class NvidiaDevice:
             _attach_report_cover(rep, self.cuda_ordinal)
         if err is None and prove and rep.cover is None:   # a proof that was asked for and did not run
             err = GpuError(f"scrub_and_verify on {self.bdf}: the coverage proof did not run", N.ERR_UNCOVERED)
+        ledger_ok = _attach_ledger(rep, self.cuda_ordinal) if prove else True
         if err is None and not probe_proved:
             err = GpuError(f"scrub_and_verify on {self.bdf}: the probe proof did not run", N.ERR_UNCOVERED)
+        if err is None and not ledger_ok:
+            err = GpuError(f"scrub_and_verify on {self.bdf}: the coverage ledger did not run", N.ERR_UNCOVERED)
         if hmode:
             _attach_health(rep, self.cuda_ordinal, hmode)
             if err is None and rep.status == N.ERR_HBM_HEALTH:   # a report that was asked for and is missing
@@ -1448,6 +1565,8 @@ def scrub_and_verify_many(devices: Sequence[NvidiaDevice], nbytes: int = 0,
                 rep.cover = report if report is not None and report.proved else None
                 if rep.status == N.OK and rep.cover is None:   # a proof that was asked for and did not run
                     rep.status = N.ERR_UNCOVERED
+                if not _attach_ledger(rep, d.cuda_ordinal) and rep.status == N.OK:
+                    rep.status = N.ERR_UNCOVERED   # a ledger that was asked for and did not run
             if probe and not _attach_probe(rep, d.cuda_ordinal, prove) and rep.status == N.OK:
                 rep.status = N.ERR_UNCOVERED   # a probe proof that was asked for and did not run
             if prove:

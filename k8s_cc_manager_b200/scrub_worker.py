@@ -10,7 +10,8 @@ short-lived process and reads ONE JSON line back; the process exit returns every
 Output (stdout, last line):  {"wall_ms": ..., "reports": [ {ScrubReport fields}, ... ]}
 (the tagged-gate fields only with --check tagged; "residue" only with --residue; "triage" only with --triage, for a
 GPU whose read-back found non-zero bytes; "mismatch_triage" only with --mismatch-triage, for a GPU whose tagged check
-found bytes off their tags; "cover" only with --prove, for every GPU whose passes finished; "probe" only with --probe,
+found bytes off their tags; "cover" and "cover_ledger" only with --prove, for every GPU whose passes finished; "probe"
+only with --probe,
 for every GPU whose alias probe ran; "probe_cover" only with --prove and --probe, for every GPU whose alias probe ran;
 "report_cover" only with --prove, for every GPU that located dirt or triaged; "hbm_health" only with --health report
 or --health require, for every GPU that was armed).
