@@ -20,7 +20,7 @@ CLI_SOURCE = CSRC / "ccm_scrub_cli.cpp"
 
 SOURCES = [CSRC / "ccm_scrub.cu", CSRC / "ccm_core.cpp"]
 HEADERS = [CSRC / "scrub_kernels.cuh", CSRC / "ccm_internal.h", CSRC / "ccm_mismatch.h", CSRC / "ccm_proof.h", CSRC / "ccm_health.h",
-           REPO_ROOT / "include" / "ccm.h"]
+           CSRC / "ccm_relay.h", REPO_ROOT / "include" / "ccm.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

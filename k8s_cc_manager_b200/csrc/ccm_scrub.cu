@@ -2885,6 +2885,31 @@ extern "C" int ccm_scrub_last_health(int cuda_ordinal, ccm_hbm_health* out) {
   return last_report(cuda_ordinal, out, &ScrubEngine::health);
 }
 
+// ------------------------------------------------------------------------- device memory (the relayed gate)
+extern "C" int ccm_device_memory(int cuda_ordinal, uint64_t* free_bytes, uint64_t* total_bytes) {
+  if (!free_bytes || !total_bytes) return CCM_ERR_INVALID;
+  *free_bytes = *total_bytes = 0;
+  if (cuda_ordinal < 0 || cuda_ordinal >= cuda_device_count()) {
+    set_error("no CUDA device with ordinal %d", cuda_ordinal);
+    return CCM_ERR_NO_CUDA;
+  }
+  ScrubEngine* e = engine_for(cuda_ordinal);
+  if (!e) return CCM_ERR_NO_CUDA;
+  std::lock_guard<std::mutex> g(e->mu);
+  CCM_ENSURE_READY(e);
+  // an armed zero-gate call that probes and proves sets these maps aside before it reads its free memory
+  if (e->probe_armed && e->prove) {
+    if (int rc = ensure_probe(e)) return rc;
+    if (int rc = ensure_probe_cover(e)) return rc;
+  }
+  CCM_CUDA(cudaSetDevice(e->ordinal));
+  size_t fr = 0, tot = 0;
+  CCM_CUDA(cudaMemGetInfo(&fr, &tot));
+  *free_bytes = fr;
+  *total_bytes = tot;
+  return CCM_OK;
+}
+
 // ------------------------------------------------------------------------- probe proof
 static_assert(sizeof(ccm_probe_cover_step) == 64 && sizeof(ccm_probe_cover) == 224 &&
               offsetof(ccm_probe_cover, step) == 32 && sizeof(ccm_probe_cover_page) == 32,

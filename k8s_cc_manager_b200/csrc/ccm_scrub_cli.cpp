@@ -25,18 +25,41 @@
 // --health report or --health require, which arms every GPU for the HBM health report (ccm_scrub_health), as
 // ccm_scrub_last_health reports it (under require, a GPU armed and without one gets CCM_ERR_HBM_HEALTH).  With --prove,
 // --probe or --health, a GPU that cannot be armed is never scrubbed without: nothing is scrubbed and the exit code is 3.
-// Exit 0: every GPU clean; 3: gate failed;
+//
+// --relay (whole-HBM only: it refuses --bytes other than 0) runs the gate twice, so that it also reaches the memory the
+// first gate's own CUDA context held (DESIGN.md §5n).  Before this process creates any context it starts leg A, its own
+// binary with --relay-first and the same options, fork + exec, stdin and stdout pipes to this process, killed when this
+// process dies and ending when its stdin closes.  A runs the gate exactly as a plain call does, prints the same line,
+// gives its HBM back (ccm_scrub_release_wait; its contexts stay), prints one "released" line and waits.  This process
+// then creates its engine on every GPU and arms it as A was armed, reads each GPU's free memory (ccm_device_memory),
+// closes A's stdin, reaps A, waits for the free memory to settle (ccm_relay.h), and runs leg B, the same gate: one JSON
+// line whose reports are leg B's, each with a "relay" object (ccm_relay::account), then "first", A's line verbatim, and
+// "first_pid".  When A fails or dies there is no leg B: A's line is printed as this call's, each report with
+// "relay": null, and the exit code is 3.  --relay-mark-mib N (a drill) has A hold N MiB of 0xA5 from its release until it
+// exits, a stand-in for a context footprint with a known content.
+// Exit 0: every GPU clean (with --relay: both legs, and every GPU's relay computed); 3: gate failed;
 // 2: usage.  Used by the manager for CC_SCRUB_ISOLATION=process (no Python start-up in the
 // child) and usable from the legacy shell engine (reference scripts/cc-manager.sh) as a
 // post-reset step.
+#include <fcntl.h>
+#include <sys/prctl.h>
+#include <sys/wait.h>
+#include <unistd.h>
+
+#include <cerrno>
+#include <chrono>
+#include <csignal>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "ccm.h"
+#include "ccm_relay.h"
 
 // The "hbm_health" object: the fields of k8s_cc_manager_b200.devices.HbmHealth.
 static void print_snapshot(const char* key, const ccm_hbm_state& s) {
@@ -276,7 +299,7 @@ static void print_mismatch_triage(const ccm_triage_report& t, int ordinal) {
 static int usage(const char* argv0) {
   fprintf(stderr, "usage: %s [--bytes N] [--backend sim|cudasim|sysfs] [--check zero|tagged] [--residue] "
           "[--triage] [--mismatch-triage] [--triage-hold-ms MS] [--prove] [--probe] [--health report|require] "
-          "(--all | --bdf <bdf> ...)\n", argv0);
+          "[--relay [--relay-mark-mib N]] (--all | --bdf <bdf> ...)\n", argv0);
   return 2;
 }
 
@@ -355,13 +378,36 @@ static void print_probe(const ccm_probe_report& p) {
 
 static void print_pcover(const ccm_probe_cover& c, int ordinal);   // after main
 
+// The gate one call runs, in a plain call and in each leg of a relay: its options and its GPUs.
+struct GateArgs {
+  unsigned long long bytes = 0;
+  bool tagged = false, residue = false, triage = false, mismatch_triage = false, prove = false, probe = false;
+  unsigned long triage_hold_ms = 100;   // k8s_cc_manager_b200.devices.TRIAGE_HOLD_MS
+  int health = 0;                       // ccm_scrub_health's mode: 0 off, 1 report, 2 require
+  std::vector<int> devs, ordinals;
+  std::vector<std::string> names;
+};
+
+// What the relay's second leg adds to that sequence: `armed` runs once every GPU is armed, before the gate (false: the
+// gate does not run), `report` prints more members of report i, `tail` more members after "reports".
+struct GateHooks {
+  std::function<bool()> armed;
+  std::function<void(size_t, const ccm_scrub_result&)> report;
+  std::function<void()> tail;
+};
+
+static int run_gate(const GateArgs& g, const GateHooks& hooks, std::vector<ccm_scrub_result>& res);   // after main
+static int relay_first(const GateArgs& g, unsigned long mark_mib);                                       // after main
+static int relay(const GateArgs& g, int argc, char** argv);                                              // after main
+
 int main(int argc, char** argv) {
   std::vector<std::string> bdfs;
   unsigned long long bytes = 0;
   bool all = false, tagged = false, residue = false, triage = false, mismatch_triage = false, prove = false,
-       probe = false;
+       probe = false, relay_on = false, relay_first_on = false;
   unsigned long triage_hold_ms = 100;   // k8s_cc_manager_b200.devices.TRIAGE_HOLD_MS
   int health = 0;                       // ccm_scrub_health's mode: 0 off, 1 report, 2 require
+  unsigned long mark_mib = 0;           // --relay-mark-mib
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     if (a == "--all") all = true;
@@ -370,6 +416,12 @@ int main(int argc, char** argv) {
     else if (a == "--mismatch-triage") mismatch_triage = true;
     else if (a == "--prove") prove = true;
     else if (a == "--probe") probe = true;
+    else if (a == "--relay") relay_on = true;
+    else if (a == "--relay-first") relay_first_on = true;
+    else if (a == "--relay-mark-mib" && i + 1 < argc) {
+      mark_mib = strtoul(argv[++i], nullptr, 10);
+      if (mark_mib == 0) return usage(argv[0]);
+    }
     else if (a == "--triage-hold-ms" && i + 1 < argc) {
       triage_hold_ms = strtoul(argv[++i], nullptr, 10);
       if (triage_hold_ms == 0 || triage_hold_ms > CCM_TRIAGE_MAX_HOLD_MS) return usage(argv[0]);
@@ -401,19 +453,36 @@ int main(int argc, char** argv) {
     fprintf(stderr, "--probe is for --check zero: the tagged check already covers every probe window\n");
     return usage(argv[0]);
   }
+  if (relay_on && relay_first_on) return usage(argv[0]);
+  if ((relay_on || relay_first_on) && bytes != 0) {
+    fprintf(stderr, "--relay is for the whole-HBM gate: it refuses --bytes other than 0\n");
+    return usage(argv[0]);
+  }
+  if (mark_mib && !relay_on && !relay_first_on) {
+    fprintf(stderr, "--relay-mark-mib needs --relay\n");
+    return usage(argv[0]);
+  }
 
+  GateArgs g;
+  g.bytes = bytes;
+  g.tagged = tagged;
+  g.residue = residue;
+  g.triage = triage;
+  g.mismatch_triage = mismatch_triage;
+  g.prove = prove;
+  g.probe = probe;
+  g.triage_hold_ms = triage_hold_ms;
+  g.health = health;
   int n = 0;
   ccm_enumerate(nullptr, 0, &n);
   std::vector<ccm_dev_info> infos(n > 0 ? n : 1);
   ccm_enumerate(infos.data(), n, &n);
-  std::vector<int> devs, ordinals;
-  std::vector<std::string> names;
   if (all) {
     for (int i = 0; i < n; ++i)
       if (infos[i].kind == CCM_KIND_GPU) {
-        devs.push_back(infos[i].index);
-        ordinals.push_back(infos[i].cuda_ordinal);
-        names.emplace_back(infos[i].bdf);
+        g.devs.push_back(infos[i].index);
+        g.ordinals.push_back(infos[i].cuda_ordinal);
+        g.names.emplace_back(infos[i].bdf);
       }
   } else {
     for (auto& want : bdfs) {
@@ -422,65 +491,87 @@ int main(int argc, char** argv) {
       for (int i = 0; i < n; ++i)
         if (infos[i].kind == CCM_KIND_GPU && want == infos[i].bdf) { found = infos[i].index; ordinal = infos[i].cuda_ordinal; }
       if (found < 0) { fprintf(stderr, "unknown GPU %s\n", want.c_str()); return 1; }
-      devs.push_back(found);
-      ordinals.push_back(ordinal);
-      names.push_back(want);
+      g.devs.push_back(found);
+      g.ordinals.push_back(ordinal);
+      g.names.push_back(want);
     }
   }
-  std::vector<ccm_scrub_result> res(devs.size() ? devs.size() : 1);
+  if (relay_first_on) return relay_first(g, mark_mib);
+  if (relay_on) return relay(g, argc, argv);
+  std::vector<ccm_scrub_result> res;
+  const int rc = run_gate(g, GateHooks(), res);
+  ccm_device_release_many((int)g.devs.size(), g.devs.data(), nullptr);  // joins the deferred HBM release, drops the contexts
+  return rc;
+}
+
+// Arms every GPU as `g` asks, runs the gate, disarms, prints the ONE JSON line and returns the exit code: 0 every GPU
+// clean, 3 the gate failed.  With --prove, --probe or --health a GPU that cannot be armed fails the gate before anything
+// is scrubbed, and nothing is printed.  `res` receives the results, one per GPU.
+static int run_gate(const GateArgs& g, const GateHooks& hooks, std::vector<ccm_scrub_result>& res) {
+  const std::vector<int>& devs = g.devs;
+  const std::vector<int>& ordinals = g.ordinals;
+  const std::vector<std::string>& names = g.names;
+  const bool tagged = g.tagged, residue = g.residue, triage = g.triage, mismatch_triage = g.mismatch_triage,
+             prove = g.prove, probe = g.probe;
+  const int health = g.health;
+  res.assign(devs.size() ? devs.size() : 1, ccm_scrub_result());
   std::vector<ccm_tag_result> tags(res.size());
   std::vector<ccm_residue_report> census(residue ? res.size() : 0);
   double wall_ms = 0;
   std::vector<int> parmed;   // ordinals armed for the coverage proof: all of them, or the gate does not run
+  std::vector<int> probed;   // ordinals armed for the alias probe: all of them, or the gate does not run
+  std::vector<int> harmed;   // ordinals armed for the HBM health report: all of them, or the gate does not run
+  std::vector<int> armed;    // ordinals armed for the triage, disarmed once the gate is done
+  std::vector<int> marmed;   // and for the mismatch triage
+  auto disarm = [&] {
+    for (int o : armed) ccm_scrub_triage(o, 0);
+    for (int o : marmed) ccm_scrub_mismatch_triage(o, 0);
+    for (int o : parmed) ccm_scrub_prove(o, 0);
+    for (int o : probed) ccm_scrub_probe(o, 0);
+    for (int o : harmed) ccm_scrub_health(o, 0);
+  };
   for (size_t i = 0; prove && i < ordinals.size(); ++i) {
     const int rc = ordinals[i] >= 0 ? ccm_scrub_prove(ordinals[i], 1) : CCM_ERR_NO_CUDA;
     if (rc != CCM_OK) {
       fprintf(stderr, "cannot arm the coverage proof on %s: %s\n", names[i].c_str(), ccm_strerror(rc));
-      for (int o : parmed) ccm_scrub_prove(o, 0);
+      disarm();
       return 3;
     }
     parmed.push_back(ordinals[i]);
   }
-  std::vector<int> probed;   // ordinals armed for the alias probe: all of them, or the gate does not run
   for (size_t i = 0; probe && i < ordinals.size(); ++i) {
     const int rc = ordinals[i] >= 0 ? ccm_scrub_probe(ordinals[i], 1) : CCM_ERR_NO_CUDA;
     if (rc != CCM_OK) {
       fprintf(stderr, "cannot arm the alias probe on %s: %s\n", names[i].c_str(), ccm_strerror(rc));
-      for (int o : probed) ccm_scrub_probe(o, 0);
-      for (int o : parmed) ccm_scrub_prove(o, 0);
+      disarm();
       return 3;
     }
     probed.push_back(ordinals[i]);
   }
-  std::vector<int> harmed;   // ordinals armed for the HBM health report: all of them, or the gate does not run
   for (size_t i = 0; health && i < ordinals.size(); ++i) {
     const int rc = ordinals[i] >= 0 ? ccm_scrub_health(ordinals[i], health) : CCM_ERR_NO_CUDA;
     if (rc != CCM_OK) {
       fprintf(stderr, "cannot arm the HBM health report on %s: %s\n", names[i].c_str(), ccm_strerror(rc));
-      for (int o : harmed) ccm_scrub_health(o, 0);
-      for (int o : probed) ccm_scrub_probe(o, 0);
-      for (int o : parmed) ccm_scrub_prove(o, 0);
+      disarm();
       return 3;
     }
     harmed.push_back(ordinals[i]);
   }
-  std::vector<int> armed;   // ordinals armed for the triage, disarmed once the gate is done
   for (size_t i = 0; triage && i < ordinals.size(); ++i)
-    if (ordinals[i] >= 0 && ccm_scrub_triage(ordinals[i], (uint32_t)triage_hold_ms) == CCM_OK) armed.push_back(ordinals[i]);
-  std::vector<int> marmed;   // and for the mismatch triage
+    if (ordinals[i] >= 0 && ccm_scrub_triage(ordinals[i], (uint32_t)g.triage_hold_ms) == CCM_OK) armed.push_back(ordinals[i]);
   for (size_t i = 0; mismatch_triage && i < ordinals.size(); ++i)
-    if (ordinals[i] >= 0 && ccm_scrub_mismatch_triage(ordinals[i], (uint32_t)triage_hold_ms) == CCM_OK)
+    if (ordinals[i] >= 0 && ccm_scrub_mismatch_triage(ordinals[i], (uint32_t)g.triage_hold_ms) == CCM_OK)
       marmed.push_back(ordinals[i]);
+  if (hooks.armed && !hooks.armed()) {
+    disarm();
+    return 3;
+  }
   if (residue)
-    ccm_scrub_verify_many_residue((int)devs.size(), devs.data(), bytes, tagged ? tags.data() : nullptr, census.data(),
+    ccm_scrub_verify_many_residue((int)devs.size(), devs.data(), g.bytes, tagged ? tags.data() : nullptr, census.data(),
                                   res.data(), &wall_ms);
-  else if (tagged) ccm_scrub_verify_many_tagged((int)devs.size(), devs.data(), bytes, tags.data(), res.data(), &wall_ms);
-  else ccm_scrub_verify_many((int)devs.size(), devs.data(), bytes, res.data(), &wall_ms);
-  for (int o : armed) ccm_scrub_triage(o, 0);
-  for (int o : marmed) ccm_scrub_mismatch_triage(o, 0);
-  for (int o : parmed) ccm_scrub_prove(o, 0);
-  for (int o : probed) ccm_scrub_probe(o, 0);
-  for (int o : harmed) ccm_scrub_health(o, 0);
+  else if (tagged) ccm_scrub_verify_many_tagged((int)devs.size(), devs.data(), g.bytes, tags.data(), res.data(), &wall_ms);
+  else ccm_scrub_verify_many((int)devs.size(), devs.data(), g.bytes, res.data(), &wall_ms);
+  disarm();
   bool clean = true;
   printf("{\"wall_ms\": %.3f, \"reports\": [", wall_ms);
   for (size_t i = 0; i < devs.size(); ++i) {
@@ -534,12 +625,229 @@ int main(int argc, char** argv) {
     ccm_report_cover rc;
     if (prove && ccm_scrub_last_report_cover(ordinals[i], &rc) == CCM_OK && rc.proved) print_rcover(rc, ordinals[i]);
     if (has_health) print_health(hh);
+    if (hooks.report) hooks.report(i, r);
     printf("}");
   }
-  printf("]}\n");
+  printf("]");
+  if (hooks.tail) hooks.tail();
+  printf("}\n");
   fflush(stdout);  // the verdict is out BEFORE the contexts are torn down: a parent can act on it right away
-  ccm_device_release_many((int)devs.size(), devs.data(), nullptr);  // joins the deferred HBM release, drops the contexts
   return clean ? 0 : 3;
+}
+
+// ------------------------------------------------------------------------------------------------ the relay
+using Clock = std::chrono::steady_clock;
+static double ms_since(Clock::time_point t0) {
+  return std::chrono::duration<double, std::milli>(Clock::now() - t0).count();
+}
+
+// The number after `"key": ` in the object of `line` whose "bdf" is `bdf`; false when there is none.
+static bool member(const std::string& line, const std::string& bdf, const char* key, uint64_t* v) {
+  const size_t at = line.find("{\"bdf\": \"" + bdf + "\"");
+  if (at == std::string::npos) return false;
+  const size_t end = line.find('}', at);
+  const size_t k = line.find(std::string("\"") + key + "\": ", at);
+  if (k == std::string::npos || k > end) return false;
+  *v = strtoull(line.c_str() + k + strlen(key) + 4, nullptr, 10);
+  return true;
+}
+
+// A payload of run_gate with `, "relay": null` closing every report.
+static std::string with_null_relay(const std::string& p) {
+  const std::string open = "\"reports\": [";
+  const size_t at = p.find(open);
+  if (at == std::string::npos) return p;
+  std::string out = p.substr(0, at + open.size());
+  int depth = 0;
+  bool str = false, esc = false;
+  for (size_t k = at + open.size(); k < p.size(); ++k) {
+    const char c = p[k];
+    if (str) {
+      if (esc) esc = false;
+      else if (c == '\\') esc = true;
+      else if (c == '"') str = false;
+    } else if (c == '"') {
+      str = true;
+    } else if (c == '{' || c == '[') {
+      ++depth;
+    } else if (c == '}' || c == ']') {
+      if (depth == 0) return out + p.substr(k);   // the end of "reports"
+      if (--depth == 0 && c == '}') out += ", \"relay\": null";
+    }
+    out += c;
+  }
+  return out;
+}
+
+// Leg A (--relay-first): the gate as a plain call runs it, its JSON line on stdout (a pipe to the process that started
+// it), then its HBM back with the driver and one "released" line, then the drill's marker when asked for, and then it
+// waits for stdin to close.  Its contexts stay until it exits: the second leg's context is created while they exist.
+static int relay_first(const GateArgs& g, unsigned long mark_mib) {
+  prctl(PR_SET_PDEATHSIG, SIGKILL);   // never outlive the process that started it
+  if (getppid() == 1) _exit(3);       // which may be gone already
+  std::vector<ccm_scrub_result> res;
+  const int rc = run_gate(g, GateHooks(), res);
+  printf("{\"released\": [");
+  for (size_t i = 0; i < g.devs.size(); ++i) {
+    double rel = 0, waited = 0;
+    ccm_scrub_release_wait(g.devs[i], &rel, &waited);   // not ccm_device_release_many: the contexts must stay
+    uint64_t marked = 0;
+    if (mark_mib) {
+      ccm_arena_info ai;
+      uint64_t nz = 0;
+      if (ccm_arena_acquire(g.devs[i], (uint64_t)mark_mib << 20, &ai) == CCM_OK &&
+          ccm_arena_fill(g.devs[i], 0xA5, nullptr) == CCM_OK &&
+          ccm_arena_verify(g.devs[i], CCM_VERIFY_AUTO, nullptr, nullptr, &nz, nullptr) == CCM_OK)
+        marked = nz;
+      else
+        fprintf(stderr, "cannot hold the %lu MiB marker on %s\n", mark_mib, g.names[i].c_str());
+    }
+    const ccm_scrub_result& r = res[i];
+    printf("%s{\"bdf\": \"%s\", \"device_total_bytes\": %llu, \"device_free_before\": %llu, \"bytes_unreached\": %llu, "
+           "\"ms_release\": %.3f, \"ms_waited\": %.3f, \"marked\": %llu}",
+           i ? ", " : "", g.names[i].c_str(), (unsigned long long)r.device_total_bytes,
+           (unsigned long long)r.device_free_before, (unsigned long long)r.bytes_unreached, rel, waited,
+           (unsigned long long)marked);
+  }
+  printf("], \"clean\": %d}\n", rc == 0);
+  fflush(stdout);
+  char b[256];
+  for (;;) {
+    const ssize_t n = read(0, b, sizeof b);
+    if (n == 0 || (n < 0 && errno != EINTR)) break;
+  }
+  _exit(rc);   // the exit frees the contexts (and the marker)
+}
+
+// The relay (--relay): leg A in a child started before this process creates any context, leg B here.
+static int relay(const GateArgs& g, int argc, char** argv) {
+  std::vector<std::string> args{"ccm-scrub"};
+  for (int i = 1; i < argc; ++i) args.emplace_back(strcmp(argv[i], "--relay") ? argv[i] : "--relay-first");
+  std::vector<char*> av;
+  for (auto& a : args) av.push_back(&a[0]);
+  av.push_back(nullptr);
+  int to_a[2], from_a[2];
+  if (pipe2(to_a, O_CLOEXEC) != 0 || pipe2(from_a, O_CLOEXEC) != 0) { perror("pipe2"); return 3; }
+  const pid_t parent = getpid();
+  const Clock::time_point t0 = Clock::now();
+  const pid_t pid = fork();   // fork + exec at once: this process has initialised the driver, and CUDA is not fork-safe
+  if (pid < 0) { perror("fork"); return 3; }
+  if (pid == 0) {
+    prctl(PR_SET_PDEATHSIG, SIGKILL);
+    if (getppid() != parent) _exit(127);
+    dup2(to_a[0], 0);
+    dup2(from_a[1], 1);
+    execv("/proc/self/exe", av.data());
+    _exit(127);
+  }
+  close(to_a[0]);
+  close(from_a[1]);
+  bool reaped = false;
+  int a_status = 0;
+  auto reap = [&] {
+    if (reaped) return;
+    close(to_a[1]);
+    while (waitpid(pid, &a_status, 0) < 0 && errno == EINTR) {}
+    reaped = true;
+  };
+  // A's JSON line, then its "released" line (none when it could not arm: then its gate did not run)
+  FILE* in = fdopen(from_a[0], "r");
+  std::string payload, released;
+  char* line = nullptr;
+  size_t cap = 0;
+  ssize_t len;
+  while (released.empty() && in && (len = getline(&line, &cap, in)) > 0) {
+    std::string l(line, (size_t)len);
+    while (!l.empty() && (l.back() == '\n' || l.back() == '\r')) l.pop_back();
+    if (l.rfind("{\"released\": ", 0) == 0) released = l;
+    else if (l.rfind("{\"wall_ms\": ", 0) == 0) payload = l;
+  }
+  free(line);
+  const double ms_first = ms_since(t0);
+  const bool a_clean = released.find("], \"clean\": 1}") != std::string::npos;
+  auto first = [&] { printf(", \"first\": %s, \"first_pid\": %d", payload.c_str(), (int)pid); };
+  if (payload.empty() || !a_clean) {   // A failed or died: no second leg, the gate has failed anyway
+    reap();
+    if (in) fclose(in);
+    if (payload.empty()) {
+      fprintf(stderr, "the first leg (pid %d) printed no report: %s\n", (int)pid,
+              WIFEXITED(a_status) ? "its gate did not run" : "it died");
+      return 3;
+    }
+    const std::string own = with_null_relay(payload);
+    printf("%s", own.substr(0, own.size() - 1).c_str());   // without its closing brace
+    first();
+    printf("}\n");
+    fflush(stdout);
+    return 3;
+  }
+  const size_t n = g.devs.size();
+  std::vector<uint64_t> held(n), tot(n);
+  std::vector<bool> have(n, false);
+  std::vector<ccm_relay::Settle> settle(n);
+  double ms_handover = 0, ms_settle = 0;
+  const Clock::time_point t_released = Clock::now();
+  GateHooks hooks;
+  hooks.armed = [&] {
+    // this leg's context exists and is armed: every allocation it needs is made by now
+    for (size_t i = 0; i < n; ++i) have[i] = ccm_device_memory(g.ordinals[i], &held[i], &tot[i]) == CCM_OK;
+    reap();
+    const Clock::time_point t_reaped = Clock::now();
+    ms_handover = std::chrono::duration<double, std::milli>(t_reaped - t_released).count();
+    if (!WIFEXITED(a_status) || WEXITSTATUS(a_status) != 0) {
+      fprintf(stderr, "the first leg (pid %d) did not exit cleanly (status %d): no second leg\n", (int)pid, a_status);
+      return false;
+    }
+    for (;;) {
+      const double ms = ms_since(t_reaped);
+      bool done = true;
+      for (size_t i = 0; i < n; ++i) {
+        uint64_t fr = 0, t = 0;
+        if (!have[i] || settle[i].done) continue;
+        if (ccm_device_memory(g.ordinals[i], &fr, &t) != CCM_OK) { have[i] = false; continue; }
+        done = settle[i].read(fr, ms) && done;
+      }
+      if (done) break;
+      std::this_thread::sleep_for(std::chrono::duration<double, std::milli>(ccm_relay::kSettlePollMs));
+    }
+    ms_settle = ms_since(t_reaped);
+    return true;
+  };
+  bool computed = true;
+  hooks.report = [&](size_t i, const ccm_scrub_result& r) {
+    ccm_relay::Inputs x;
+    x.total = r.device_total_bytes;
+    x.b_free_held = held[i];
+    x.b_free_settled = settle[i].free_bytes;
+    x.b_free_before = r.device_free_before;
+    x.b_unreached = r.bytes_unreached;
+    const std::string& bdf = g.names[i];
+    if (!have[i] || r.device_total_bytes == 0 || !member(released, bdf, "device_free_before", &x.a_free_before) ||
+        !member(released, bdf, "bytes_unreached", &x.a_unreached) || !member(released, bdf, "marked", &x.marked)) {
+      computed = false;
+      printf(", \"relay\": null");
+      return;
+    }
+    const ccm_relay::Relay v = ccm_relay::account(x);
+    printf(", \"relay\": {\"total\": %llu, \"a_free_before\": %llu, \"a_unreached\": %llu, \"b_free_held\": %llu, "
+           "\"b_free_settled\": %llu, \"b_free_before\": %llu, \"b_unreached\": %llu, \"marked\": %llu, "
+           "\"footprint_a\": %llu, \"freed\": %llu, \"held\": %llu, \"growth\": %llu, \"unreached\": %llu, "
+           "\"coverage\": %.9f, \"settled\": %d, \"settle_polls\": %d, \"ms_first\": %.3f, \"ms_handover\": %.3f, "
+           "\"ms_settle\": %.3f, \"ms_second\": %.3f}",
+           (unsigned long long)x.total, (unsigned long long)x.a_free_before, (unsigned long long)x.a_unreached,
+           (unsigned long long)x.b_free_held, (unsigned long long)x.b_free_settled, (unsigned long long)x.b_free_before,
+           (unsigned long long)x.b_unreached, (unsigned long long)x.marked, (unsigned long long)v.footprint_a,
+           (unsigned long long)v.freed, (unsigned long long)v.held, (unsigned long long)v.growth,
+           (unsigned long long)v.unreached, v.coverage, settle[i].settled, settle[i].polls, ms_first, ms_handover,
+           ms_settle, r.ms_total);
+  };
+  hooks.tail = first;
+  std::vector<ccm_scrub_result> res;
+  const int rc = run_gate(g, hooks, res);
+  reap();   // when arming failed, the hook never ran
+  if (in) fclose(in);
+  ccm_device_release_many((int)g.devs.size(), g.devs.data(), nullptr);
+  return rc == 0 && computed ? 0 : 3;
 }
 
 // The "probe_cover" object: the fields of k8s_cc_manager_b200.devices.ProbeCoverReport, with the first 64 inexact pages.

@@ -1163,11 +1163,76 @@ def _attach_health(rep: "ScrubReport", cuda_ordinal: int, mode: int) -> None:
         rep.status = N.ERR_HBM_HEALTH
 
 
+def _mib(n: int) -> str:
+    return f"{n / 2**20:.1f} MiB"
+
+
+@dataclass
+class RelayReport:
+    """What the relayed whole-HBM gate (ccm-scrub --relay, DESIGN.md §5n) reached on one GPU, in bytes: the inputs each
+    leg measured, the accounting rule's outputs (csrc/ccm_relay.h) and the phase times.  Leg A's gate ran in a first
+    process; this process's context was created while A's still existed, then A exited and leg B scrubbed what was free,
+    A's footprint included.  `first` is leg A's report for the GPU (a ScrubReport)."""
+    total: int
+    a_free_before: int
+    a_unreached: int
+    b_free_held: int
+    b_free_settled: int
+    b_free_before: int
+    b_unreached: int
+    marked: int
+    footprint_a: int      # total - a_free_before: what the device held beside leg A's mapping
+    freed: int            # b_free_settled - b_free_held: what A's exit gave back
+    held: int             # footprint_a - freed: memory neither leg could map
+    growth: int           # b_free_settled - b_free_before: what leg B's process allocated after the hand-over
+    unreached: int        # held + growth + a_unreached + b_unreached
+    coverage: float       # 1 - unreached / total
+    settled: int
+    settle_polls: int
+    ms_first: float       # leg A started .. its HBM back with the driver
+    ms_handover: float    # this leg's context created and armed, A reaped
+    ms_settle: float      # A reaped .. its memory back
+    ms_second: float      # leg B's time to verdict
+    first: "Optional[ScrubReport]" = None
+
+    @classmethod
+    def from_json(cls, d: dict) -> "RelayReport":
+        first = d.get("first")
+        return cls(**{**d, "first": ScrubReport.from_json(first) if first is not None else None})
+
+    def as_json(self) -> dict:
+        d = {f.name: getattr(self, f.name) for f in dataclasses.fields(self)}
+        d["first"] = self.first.as_json() if self.first is not None else None
+        return d
+
+    def summary(self) -> str:
+        """One line for an operator: the relay's coverage, where A's footprint went, what each leg left unreached and
+        how long each phase took."""
+        return (f"coverage {self.coverage:.5f} of {self.total / 2**30:.1f} GiB ({_mib(self.unreached)} unreached); "
+                f"first context's footprint {_mib(self.footprint_a)}, freed {_mib(self.freed)}, held {_mib(self.held)}, "
+                f"growth {_mib(self.growth)}; unmappable A {_mib(self.a_unreached)}, B {_mib(self.b_unreached)}"
+                + (f"; marker {_mib(self.marked)}" if self.marked else "")
+                + (f"; free memory did not settle in {self.settle_polls} reads" if not self.settled else "")
+                + f"; first leg {self.ms_first:.0f} ms, hand-over {self.ms_handover:.0f} ms, settle "
+                f"{self.ms_settle:.0f} ms, second leg {self.ms_second:.0f} ms")
+
+
+def reports_from_payload(payload: dict) -> "List[ScrubReport]":
+    """The reports of a scrub worker's JSON line.  A relayed line (ccm-scrub --relay) also holds leg A's line under
+    "first": each report's relay gets leg A's report for its GPU."""
+    reports = [ScrubReport.from_json(r) for r in payload["reports"]]
+    first = {r["bdf"]: r for r in (payload.get("first") or {}).get("reports", [])}
+    for rep in reports:
+        if rep.relay is not None and rep.bdf in first:
+            rep.relay.first = ScrubReport.from_json(first[rep.bdf])
+    return reports
+
+
 # The reports a call can carry, as (attribute of ScrubReport and GpuError, report class), in JSON order.
 _REPORTS = (("dirt", DirtReport), ("mismatch", MismatchReport), ("residue", ResidueReport), ("triage", TriageReport),
             ("mismatch_triage", TriageReport), ("cover", CoverReport), ("probe", ProbeReport),
             ("probe_cover", ProbeCoverReport), ("report_cover", ReportCoverReport), ("health", HbmHealth),
-            ("ledger", CoverLedger))
+            ("ledger", CoverLedger), ("relay", RelayReport))
 # The JSON key of a report whose attribute is not its key.
 _JSON_KEYS = {"health": "hbm_health", "ledger": "cover_ledger"}
 
@@ -1232,6 +1297,9 @@ class ScrubReport:
     # How many bytes every thread of each pass addressed on every 128 KiB slot (a CoverLedger), set for every report of
     # a proving call (prove=True) whose passes finished.  Not a dataclass field either; its JSON key is "cover_ledger".
     ledger = None
+    # What the relayed gate reached on this GPU (a RelayReport, with leg A's report as its `first`), set for every report
+    # of a relayed call (ccm-scrub --relay) whose relay was computed.  Not a dataclass field either.
+    relay = None
 
     @property
     def clean(self) -> bool:
